@@ -237,6 +237,98 @@ int sage_b200_host_log1pf_exact(void);
 /* Test hook: out[i] = the device's evaluation of log(x[i]) with `variant` (0/1), or of (double)log1pf((float)x[i]) with variant 2 — compared bit for bit with the host libm by tests/test_glibc_log.py. */
 int sage_b200_device_log(int device, int variant, const double* x, uint64_t n, double* out);
 
+/* ---------------------------------------------------------------------------------------------------------------------------------------------
+ * Label-free quantification (lfq.rs): build_feature_map (lfq.rs:94-193) and FeatureMap::quantify (lfq.rs:226-304) on the device.
+ * create -> add_ms1 (any number of batches; the result does not depend on how spectra are split) -> integrate. Calls on one handle are
+ * serialised by a per-handle mutex. Grid cells are summed in a defined order (batches in call order, spectra in input order, peaks in order,
+ * lo before hi contribution), so every cell is reproducible bit for bit; see DESIGN.md §9 for the exactness contract.
+ */
+typedef struct sage_b200_lfq sage_b200_lfq;   /* replaces FeatureMap + the DashMap<(PrecursorId, bool), Grid> of quantify */
+
+/* lfq.rs:25-37 */
+enum { SAGE_B200_PEAK_RETENTION_TIME = 0, SAGE_B200_PEAK_SPECTRAL_ANGLE = 1, SAGE_B200_PEAK_INTENSITY = 2, SAGE_B200_PEAK_HYBRID = 3 };
+enum { SAGE_B200_INTEGRATE_APEX = 0, SAGE_B200_INTEGRATE_SUM = 1 };
+
+/* LfqSettings (lfq.rs:45-54) plus Search::precursor_charge (min, max). */
+typedef struct {
+    int32_t peak_scoring;         /* SAGE_B200_PEAK_* */
+    int32_t integration;          /* SAGE_B200_INTEGRATE_* */
+    double spectral_angle;
+    float ppm_tolerance, mobility_pct_tolerance, peptide_q_value;
+    uint8_t combine_charge_states;
+    uint8_t min_precursor_charge, max_precursor_charge;
+} sage_b200_lfq_params;
+
+/* The Feature fields build_feature_map reads, n rows in the caller's confidence order (rows with peptide_q <= peptide_q_value && label == 1
+ * are kept; the first kept row of each peptide wins, lfq.rs:100-131). */
+typedef struct {
+    uint64_t n;
+    const uint32_t* peptide_idx;
+    const float* peptide_q;
+    const int32_t* label;
+    const float* aligned_rt;
+    const float* calcmass;
+    const uint32_t* file_id;      /* < n_files */
+    const float* ims;
+} sage_b200_lfq_features;
+
+/* retention_alignment.rs:87-93 (file_id is the array position) */
+typedef struct { float max_rt, slope, intercept; } sage_b200_alignment;
+
+/* One batch of MS1 ProcessedSpectrum (spectrum.rs:58-79). */
+typedef struct {
+    uint64_t n;
+    const uint64_t* peak_offsets;     /* n+1 */
+    const float* masses;              /* ProcessedSpectrum::masses (mz - PROTON), ascending */
+    const float* intensities;
+    const uint32_t* file_id;          /* < n_files */
+    const float* scan_start_time;
+    const float* mobilities;          /* per peak; NULL = no spectrum of the batch has mobilities */
+} sage_b200_ms1;
+
+/* PrecursorRange (lfq.rs:70-82) as the sorted feature map holds it. */
+typedef struct {
+    float rt, mass_lo, mass_hi, mobility_lo, mobility_hi;
+    uint32_t peptide, file_id;
+    uint8_t charge, isotope, decoy, _pad;
+} sage_b200_lfq_range;
+
+/* One entry of quantify's map: key (PrecursorId, decoy), Peak (lfq.rs:335-345); areas are returned in a separate [rows x n_files] array. */
+typedef struct {
+    uint32_t peptide;
+    uint8_t charge;                   /* PrecursorId::Charged; 0 for PrecursorId::Combined */
+    uint8_t decoy;
+    uint16_t _pad0;
+    uint32_t rt;                      /* Peak::rt, bin 0..99 */
+    uint32_t _pad1;
+    double spectral_angle, score;
+} sage_b200_lfq_row;
+
+typedef struct {
+    uint64_t n_peptides;              /* peptides that passed the filter (one PrecursorRange seed each) */
+    uint64_t n_ranges, n_pages, n_grids /* upper bound of integrate's row count */, n_files;
+    uint64_t grids_touched, ms1_spectra, ms1_peaks, contributions;
+    uint64_t device_bytes;
+    float ms_build, ms_trace, ms_integrate, ms_download;   /* CUDA events: create, summed add_ms1, last integrate's kernels and copy-back */
+} sage_b200_lfq_info;
+
+/* build_feature_map. `peptides` is the table the db was built from (only residue_offsets and sequence are read: carbon / sulfur counts,
+ * mass.rs:78-116); alignments has n_files entries. EINVAL for a file_id >= n_files or a peptide_idx outside the db; ELIMIT when the grids
+ * (n_grids * n_files * 300 f64) do not fit the device's free memory (checked before allocating). */
+int sage_b200_lfq_create(const sage_b200_db* db, const sage_b200_peptides* peptides, const sage_b200_lfq_params* params,
+                         const sage_b200_lfq_features* features, uint64_t n_files, const sage_b200_alignment* alignments, sage_b200_lfq** out);
+/* The tracing loop of quantify (lfq.rs:239-287) over one batch. EINVAL for a file_id >= n_files. */
+int sage_b200_lfq_add_ms1(sage_b200_lfq* lfq, const sage_b200_ms1* ms1);
+/* summarize_traces + integrate (lfq.rs:447-610) for every touched grid: rows ordered by (id, decoy); areas[row * n_files + file].
+ * capacity >= info.n_grids always suffices; *n_rows receives the row count. */
+int sage_b200_lfq_integrate(sage_b200_lfq* lfq, sage_b200_lfq_row* rows, double* areas, uint64_t capacity, uint64_t* n_rows);
+int sage_b200_lfq_get_info(sage_b200_lfq* lfq, sage_b200_lfq_info* info);
+/* Test hook: the sorted ranges (n_ranges), min_rts (n_pages), and optionally the raw grid matrices (n_grids * n_files * 3 * 100 f64, grid g
+ * at [g * n_files * 300], row file * 3 + isotope) and their touched flags (n_grids). Grid g is (peptide slot, [charge,] decoy) in ascending
+ * (PeptideIx, charge, decoy) order. Any pointer may be NULL. */
+int sage_b200_lfq_export(sage_b200_lfq* lfq, sage_b200_lfq_range* ranges, float* min_rts, double* grids, uint8_t* touched);
+void sage_b200_lfq_destroy(sage_b200_lfq* lfq);
+
 /* Page-locked host buffers: spectra/feature arrays placed here are copied by DMA without a staging memcpy. */
 void* sage_b200_host_alloc(size_t bytes);
 /* The same for a batch sage_b200_score_batch_multi cuts into n_devices contiguous blocks: the i-th of n equal parts of the buffer is placed on the

@@ -89,6 +89,7 @@ EXPORTED_SYMBOLS = [
     "sage_b200_batch_download", "sage_b200_score_batch_multi", "sage_b200_quick_score", "sage_b200_initial_hits", "sage_b200_counters_get",
     "sage_b200_process_spectra", "sage_b200_find_reporter_ions", "sage_b200_host_alloc", "sage_b200_host_free", "sage_b200_last_error",
     "sage_b200_host_log_variant", "sage_b200_host_log1pf_exact", "sage_b200_device_log", "sage_b200_bind_thread_to_device", "sage_b200_host_alloc_blocks",
+    "sage_b200_lfq_create", "sage_b200_lfq_add_ms1", "sage_b200_lfq_integrate", "sage_b200_lfq_get_info", "sage_b200_lfq_export", "sage_b200_lfq_destroy",
 ]
 
 _lib = None
@@ -116,6 +117,7 @@ def load_library(build: bool = True):
     lib.sage_b200_initial_hits.restype = C.c_int64
     lib.sage_b200_db_destroy.argtypes = [C.c_void_p]
     lib.sage_b200_scorer_destroy.argtypes = [C.c_void_p]
+    lib.sage_b200_lfq_destroy.argtypes = [C.c_void_p]
     _lib = lib
     return lib
 
@@ -583,6 +585,164 @@ def find_reporter_ions(peak_off, masses, intensities, labels, label_tolerance: T
     _check(load_library().sage_b200_find_reporter_ions(C.c_int(device), C.c_uint64(n), _ptr(peak_off), _ptr(masses), _ptr(intensities), _ptr(labels),
                                                        C.c_uint64(len(labels)), label_tolerance._c(), _ptr(out)))
     return out
+
+
+# ------------------------------------------------------------------------------------------------ label-free quantification (lfq.rs)
+PEAK_SCORING = {"RetentionTime": 0, "SpectralAngle": 1, "Intensity": 2, "Hybrid": 3}   # PeakScoringStrategy, lfq.rs:25-31
+INTEGRATION = {"Apex": 0, "Sum": 1}                                                   # IntegrationStrategy, lfq.rs:33-37
+
+
+class CLfqParams(C.Structure):
+    _fields_ = [("peak_scoring", C.c_int32), ("integration", C.c_int32), ("spectral_angle", C.c_double), ("ppm_tolerance", C.c_float),
+                ("mobility_pct_tolerance", C.c_float), ("peptide_q_value", C.c_float), ("combine_charge_states", C.c_uint8),
+                ("min_precursor_charge", C.c_uint8), ("max_precursor_charge", C.c_uint8)]
+
+
+class CLfqFeatures(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("peptide_idx", C.c_void_p), ("peptide_q", C.c_void_p), ("label", C.c_void_p), ("aligned_rt", C.c_void_p),
+                ("calcmass", C.c_void_p), ("file_id", C.c_void_p), ("ims", C.c_void_p)]
+
+
+class CMs1(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("peak_offsets", C.c_void_p), ("masses", C.c_void_p), ("intensities", C.c_void_p), ("file_id", C.c_void_p),
+                ("scan_start_time", C.c_void_p), ("mobilities", C.c_void_p)]
+
+
+class CLfqInfo(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("n_peptides", "n_ranges", "n_pages", "n_grids", "n_files", "grids_touched", "ms1_spectra", "ms1_peaks",
+                                          "contributions", "device_bytes")] + \
+               [(n, C.c_float) for n in ("ms_build", "ms_trace", "ms_integrate", "ms_download")]
+
+
+ALIGNMENT_DTYPE = np.dtype([("max_rt", "<f4"), ("slope", "<f4"), ("intercept", "<f4")])            # sage_b200_alignment
+LFQ_RANGE_DTYPE = np.dtype([("rt", "<f4"), ("mass_lo", "<f4"), ("mass_hi", "<f4"), ("mobility_lo", "<f4"), ("mobility_hi", "<f4"),
+                            ("peptide", "<u4"), ("file_id", "<u4"), ("charge", "u1"), ("isotope", "u1"), ("decoy", "u1"), ("_pad", "u1")])
+LFQ_ROW_DTYPE = np.dtype([("peptide", "<u4"), ("charge", "u1"), ("decoy", "u1"), ("_pad0", "<u2"), ("rt", "<u4"), ("_pad1", "<u4"),
+                          ("spectral_angle", "<f8"), ("score", "<f8")])                                 # sage_b200_lfq_row
+LFQ_FEATURE_FIELDS = ("peptide_idx", "peptide_q", "label", "aligned_rt", "calcmass", "file_id", "ims")
+_LFQ_FEATURE_TYPES = (np.uint32, np.float32, np.int32, np.float32, np.float32, np.uint32, np.float32)
+
+
+@dataclass
+class LfqSettings:
+    """LfqSettings (lfq.rs:45-68), same defaults. peak_scoring / integration take the reference's variant names."""
+    peak_scoring: str = "Hybrid"
+    integration: str = "Sum"
+    spectral_angle: float = 0.70
+    ppm_tolerance: float = 5.0
+    mobility_pct_tolerance: float = 1.0
+    combine_charge_states: bool = True
+    peptide_q_value: float = 0.01
+
+    def _c(self, precursor_charge) -> CLfqParams:
+        p = CLfqParams()
+        p.peak_scoring, p.integration = PEAK_SCORING[self.peak_scoring], INTEGRATION[self.integration]
+        p.spectral_angle, p.ppm_tolerance, p.mobility_pct_tolerance = self.spectral_angle, self.ppm_tolerance, self.mobility_pct_tolerance
+        p.peptide_q_value, p.combine_charge_states = self.peptide_q_value, int(self.combine_charge_states)
+        p.min_precursor_charge, p.max_precursor_charge = int(precursor_charge[0]), int(precursor_charge[1])
+        return p
+
+
+@dataclass
+class Ms1Batch:
+    """A batch of MS1 ProcessedSpectrum (spectrum.rs:58-79) flattened: masses are mz - PROTON, as SpectrumProcessor gives them.
+    mobilities (per peak) may be None: then no spectrum of the batch has mobility."""
+    peak_off: np.ndarray
+    masses: np.ndarray
+    intensities: np.ndarray
+    file_id: np.ndarray
+    scan_start_time: np.ndarray
+    mobilities: np.ndarray | None = None
+
+    def __len__(self):
+        return len(self.file_id)
+
+    def slice(self, a: int, b: int) -> "Ms1Batch":
+        p0, p1 = int(self.peak_off[a]), int(self.peak_off[b])
+        return Ms1Batch(self.peak_off[a:b + 1] - self.peak_off[a], self.masses[p0:p1], self.intensities[p0:p1], self.file_id[a:b], self.scan_start_time[a:b],
+                        None if self.mobilities is None else self.mobilities[p0:p1])
+
+    def _c(self, keep: list) -> CMs1:
+        def arr(x, dt):
+            if x is None:
+                return None
+            a = np.ascontiguousarray(x, dtype=dt)
+            keep.append(a)
+            return _ptr(a)
+        return CMs1(len(self), arr(self.peak_off, np.uint64), arr(self.masses, np.float32), arr(self.intensities, np.float32), arr(self.file_id, np.uint32),
+                    arr(self.scan_start_time, np.float32), arr(self.mobilities, np.float32))
+
+
+def _lfq_features(features, keep: list) -> CLfqFeatures:
+    cols = [np.ascontiguousarray(features[f], dtype=t) for f, t in zip(LFQ_FEATURE_FIELDS, _LFQ_FEATURE_TYPES)]
+    keep.extend(cols)
+    return CLfqFeatures(len(cols[0]), *[_ptr(c) for c in cols])
+
+
+class FeatureMap:
+    """build_feature_map(...) (lfq.rs:94-193) and FeatureMap::quantify (lfq.rs:226-304) on the device: build, add_ms1 any number of batches, quantify.
+    `features` is a structured array or dict with the Feature fields peptide_idx, peptide_q, label, aligned_rt, calcmass, file_id, ims, in the
+    caller's confidence order; `alignments` is ALIGNMENT_DTYPE (or [n_files, 3] float32: max_rt, slope, intercept)."""
+
+    def __init__(self, handle, n_files: int, settings: LfqSettings, precursor_charge):
+        self._h = C.c_void_p(handle)
+        self.n_files = n_files
+        self.settings = settings
+        self.precursor_charge = tuple(precursor_charge)
+
+    @staticmethod
+    def build(db: IndexedDatabase, peptides: Peptides, settings: LfqSettings, precursor_charge, features, alignments) -> "FeatureMap":
+        keep: list = []
+        cp = peptides._c(keep)
+        cf = _lfq_features(features, keep)
+        al = np.ascontiguousarray(alignments)
+        al = al.view(np.float32).reshape(-1, 3) if al.dtype.names else np.ascontiguousarray(al, np.float32).reshape(-1, 3)
+        al = np.ascontiguousarray(al)
+        params = settings._c(precursor_charge)
+        h = C.c_void_p()
+        _check(load_library().sage_b200_lfq_create(db._h, C.byref(cp), C.byref(params), C.byref(cf), C.c_uint64(len(al)), _ptr(al), C.byref(h)))
+        return FeatureMap(h.value, len(al), settings, precursor_charge)
+
+    def __del__(self):
+        try:
+            if self._h:
+                load_library().sage_b200_lfq_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def add_ms1(self, batch: Ms1Batch):
+        """The tracing loop of quantify (lfq.rs:239-287) over one batch."""
+        keep: list = []
+        cm = batch._c(keep)
+        _check(load_library().sage_b200_lfq_add_ms1(self._h, C.byref(cm)))
+
+    def info(self) -> dict:
+        ci = CLfqInfo()
+        _check(load_library().sage_b200_lfq_get_info(self._h, C.byref(ci)))
+        return {k: getattr(ci, k) for k, _ in CLfqInfo._fields_}
+
+    def quantify(self) -> dict:
+        """summarize_traces + integrate for every traced precursor. Rows are ordered by (id, decoy): id is the PeptideIx, plus the charge when
+        combine_charge_states is false (charge is 0 otherwise). Returns dict(id, charge, decoy, rt, spectral_angle, score, areas[n, n_files])."""
+        cap = max(1, int(self.info()["n_grids"]))
+        rows = np.zeros(cap, LFQ_ROW_DTYPE)
+        areas = np.zeros((cap, self.n_files), np.float64)
+        n = C.c_uint64(0)
+        _check(load_library().sage_b200_lfq_integrate(self._h, _ptr(rows), _ptr(areas), C.c_uint64(cap), C.byref(n)))
+        r = rows[:n.value]
+        return dict(id=r["peptide"].copy(), charge=r["charge"].copy(), decoy=r["decoy"].astype(bool), rt=r["rt"].copy(),
+                    spectral_angle=r["spectral_angle"].copy(), score=r["score"].copy(), areas=areas[:n.value].copy())
+
+    def export(self, grids: bool = False) -> dict:
+        """Test hook: the sorted ranges, min_rts and (grids=True) the raw grids [n_grids, n_files * 3, 100] with their touched flags."""
+        info = self.info()
+        ranges = np.zeros(info["n_ranges"], LFQ_RANGE_DTYPE)
+        min_rts = np.zeros(info["n_pages"], np.float32)
+        g = np.zeros((info["n_grids"], self.n_files * 3, 100), np.float64) if grids else None
+        t = np.zeros(info["n_grids"], np.uint8) if grids else None
+        _check(load_library().sage_b200_lfq_export(self._h, _ptr(ranges), _ptr(min_rts), _ptr(g), _ptr(t)))
+        return dict(ranges=ranges, min_rts=min_rts, grids=g, touched=t)
 
 
 Feature = FEATURE_DTYPE

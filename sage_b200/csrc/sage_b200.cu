@@ -6,7 +6,9 @@
 // sage_b200_score_batch. No CPU fallback exists: every entry point fails loudly when CUDA is unavailable.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 #include <cuda_runtime.h>
+#include <thrust/iterator/counting_iterator.h>
 
 #include <pthread.h>
 #include <sched.h>
@@ -29,6 +31,7 @@
 
 #include "../../include/sage_b200.h"
 #include "kernels.cuh"
+#include "lfq.cuh"
 
 using namespace sb;
 
@@ -2003,6 +2006,510 @@ extern "C" size_t sage_b200_last_error(char* buf, size_t cap) {
         snprintf(buf, cap, "%s", g_last_error.c_str());
     }
     return g_last_error.size();
+}
+
+// ================================================================================== label-free quantification (lfq.rs, kernels in lfq.cuh)
+// The feature map (sorted PrecursorRange pages) and one dense f64 grid per possible (PrecursorId, decoy) key stay on the device; a key's grid
+// is "touched" once a contribution reached it, which is when the reference's DashMap would have created it (lfq.rs:250-262).
+static constexpr uint32_t LFQ_MAX_FILES = 128;              // k_lfq_integrate keeps 2 x 100 f64 per file in shared memory
+static constexpr uint64_t LFQ_CHUNK_PEAKS = 1ull << 24;     // add_ms1 traces at most this many peaks per pass (results do not depend on it)
+
+struct sage_b200_lfq {
+    std::mutex mu;
+    int device = 0;
+    sage_b200_lfq_params p{};
+    uint32_t n_files = 0, n_charges = 0;
+    uint64_t n_slots = 0, n_ranges = 0, n_pages = 0, n_grids = 0;
+    void *d_ranges = nullptr, *d_grid_of = nullptr, *d_min_rts = nullptr, *d_slot_dist = nullptr, *d_slot_file = nullptr, *d_grids = nullptr,
+         *d_touched = nullptr, *d_align = nullptr, *d_consts = nullptr;
+    uint64_t fixed_bytes = 0;
+    std::vector<uint32_t> slot_pep;   // slot -> PeptideIx, ascending
+    DevBuf sp_off, sp_mass, sp_int, sp_mob, sp_file, sp_sst, counts, offsets, cell[2], value[2], tmp, ids, o_present, o_rt, o_sa, o_score, o_areas;
+    cudaStream_t st = nullptr;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    sage_b200_lfq_info info{};
+    uint64_t scratch_bytes() const {
+        uint64_t b = 0;
+        for (const DevBuf* d : {&sp_off, &sp_mass, &sp_int, &sp_mob, &sp_file, &sp_sst, &counts, &offsets, &cell[0], &cell[1], &value[0], &value[1], &tmp, &ids,
+                                &o_present, &o_rt, &o_sa, &o_score, &o_areas})
+            b += d->cap;
+        return b;
+    }
+};
+
+static int lfq_malloc(sage_b200_lfq* L, void** p, size_t bytes) {
+    CUDA_TRY(cudaMalloc(p, bytes ? bytes : 16));
+    L->fixed_bytes += bytes ? bytes : 16;
+    return 0;
+}
+
+// composition (mass.rs:78-116): carbon and sulfur count of one residue
+static void residue_composition(uint8_t aa, uint16_t& c, uint16_t& s) {
+    static const uint8_t carbon[26] = {3, 0, 3, 4, 5, 9, 2, 6, 6, 0, 6, 6, 5, 4, 12, 5, 5, 6, 3, 4, 3, 5, 11, 0, 9, 0};   // A..Z (B J X Z: 0)
+    c = 0;
+    s = 0;
+    if (aa < 'A' || aa > 'Z') return;
+    c = carbon[aa - 'A'];
+    s = (aa == 'C' || aa == 'M') ? 1 : 0;
+}
+
+// the event-timed span of one stage: ms += elapsed(ev0, ev1) after a synchronize
+static int lfq_elapsed(sage_b200_lfq* L, float& ms) {
+    CUDA_TRY(cudaEventRecord(L->ev[1], L->st));
+    CUDA_TRY(cudaEventSynchronize(L->ev[1]));
+    float t = 0.0f;
+    CUDA_TRY(cudaEventElapsedTime(&t, L->ev[0], L->ev[1]));
+    ms += t;
+    return 0;
+}
+
+extern "C" void sage_b200_lfq_destroy(sage_b200_lfq* L) {
+    if (!L) return;
+    cudaSetDevice(L->device);
+    for (void* p : {L->d_ranges, L->d_grid_of, L->d_min_rts, L->d_slot_dist, L->d_slot_file, L->d_grids, L->d_touched, L->d_align, L->d_consts})
+        if (p) cudaFree(p);
+    for (DevBuf* d : {&L->sp_off, &L->sp_mass, &L->sp_int, &L->sp_mob, &L->sp_file, &L->sp_sst, &L->counts, &L->offsets, &L->cell[0], &L->cell[1], &L->value[0],
+                      &L->value[1], &L->tmp, &L->ids, &L->o_present, &L->o_rt, &L->o_sa, &L->o_score, &L->o_areas})
+        d->release();
+    for (cudaEvent_t e : L->ev)
+        if (e) cudaEventDestroy(e);
+    if (L->st) cudaStreamDestroy(L->st);
+    delete L;
+}
+
+static int lfq_build(sage_b200_lfq* L, const sage_b200_db* db, const sage_b200_peptides* P, const sage_b200_lfq_features* F, const sage_b200_alignment* align) {
+    const uint64_t n = F->n, n_pep = db->v.n_pep;
+    cudaStream_t st = L->st;
+    CUDA_TRY(cudaEventRecord(L->ev[0], st));
+    // per-peptide first kept row (lfq.rs:100-131)
+    DevBuf d_rows[7], d_first, d_flag, d_slots, d_nsel, d_cs, d_exp;
+    const void* src[7] = {F->peptide_idx, F->peptide_q, F->label, F->aligned_rt, F->calcmass, F->file_id, F->ims};
+    auto cleanup = [&]() {
+        for (auto& d : d_rows) d.release();
+        for (DevBuf* d : {&d_first, &d_flag, &d_slots, &d_nsel, &d_cs, &d_exp}) d->release();
+    };
+    int rc = 0;
+#define LFQ_TRY(expr)                                                                                                          \
+    do {                                                                                                                       \
+        cudaError_t _e = (expr);                                                                                               \
+        if (_e != cudaSuccess) { cleanup(); return fail(SAGE_B200_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); }   \
+    } while (0)
+#define LFQ_RC(expr)              \
+    do {                          \
+        if ((rc = (expr)) != 0) { \
+            cleanup();            \
+            return rc;            \
+        }                         \
+    } while (0)
+    for (int k = 0; k < 7; k++) {
+        LFQ_RC(d_rows[k].reserve(4 * n + 16));
+        if (n) LFQ_TRY(cudaMemcpyAsync(d_rows[k].p, src[k], 4 * n, cudaMemcpyHostToDevice, st));
+    }
+    LFQ_RC(d_first.reserve(4 * n_pep + 16));
+    LFQ_RC(d_flag.reserve(n_pep + 16));
+    LFQ_RC(d_slots.reserve(4 * n_pep + 16));
+    LFQ_RC(d_nsel.reserve(16));
+    LFQ_TRY(cudaMemsetAsync(d_first.p, 0xFF, 4 * n_pep, st));
+    if (n)
+        k_lfq_first_row<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, d_rows[0].as<uint32_t>(), d_rows[1].as<float>(), d_rows[2].as<int32_t>(),
+                                                                       L->p.peptide_q_value, d_first.as<uint32_t>());
+    if (n_pep) k_lfq_flag<<<(unsigned)((n_pep + 255) / 256), 256, 0, st>>>(n_pep, d_first.as<uint32_t>(), d_flag.as<uint8_t>());
+    LFQ_TRY(cudaGetLastError());
+    {
+        size_t tb = 0;
+        thrust::counting_iterator<uint32_t> it(0);
+        LFQ_TRY(cub::DeviceSelect::Flagged(nullptr, tb, it, d_flag.as<uint8_t>(), d_slots.as<uint32_t>(), d_nsel.as<uint32_t>(), (int)n_pep, st));
+        LFQ_RC(L->tmp.reserve(tb));
+        LFQ_TRY(cub::DeviceSelect::Flagged(L->tmp.p, tb, it, d_flag.as<uint8_t>(), d_slots.as<uint32_t>(), d_nsel.as<uint32_t>(), (int)n_pep, st));
+    }
+    uint32_t n_slots = 0;
+    LFQ_TRY(cudaMemcpyAsync(&n_slots, d_nsel.p, 4, cudaMemcpyDeviceToHost, st));
+    LFQ_TRY(cudaStreamSynchronize(st));
+    std::vector<uint32_t> slot_pep(n_slots);
+    if (n_slots) LFQ_TRY(cudaMemcpyAsync(slot_pep.data(), d_slots.p, 4ull * n_slots, cudaMemcpyDeviceToHost, st));
+    LFQ_TRY(cudaStreamSynchronize(st));
+
+    L->n_slots = n_slots;
+    L->slot_pep = slot_pep;
+    L->n_ranges = (uint64_t)n_slots * L->n_charges * LFQ_ISO * 2;
+    L->n_pages = (L->n_ranges + LFQ_PAGE - 1) / LFQ_PAGE;
+    L->n_grids = (uint64_t)n_slots * (L->p.combine_charge_states ? 1 : L->n_charges) * 2;
+    if (L->n_ranges > 0x7FFFFFFFull) { cleanup(); return fail(SAGE_B200_ELIMIT, "%llu precursor ranges exceed 2^31", (unsigned long long)L->n_ranges); }
+    const uint64_t cells = L->n_grids * L->n_files * LFQ_ISO * LFQ_GRID, grid_bytes = 8 * cells;
+    {
+        size_t free_b = 0, total_b = 0;
+        LFQ_TRY(cudaMemGetInfo(&free_b, &total_b));
+        // the grids plus the map, leaving room for the tracing and integration scratch
+        const uint64_t need = grid_bytes + L->n_grids + 40 * L->n_ranges + (1ull << 28);
+        if (need > (uint64_t)free_b)
+            { cleanup(); return fail(SAGE_B200_ELIMIT, "LFQ grids need %llu bytes of device memory (%llu grids x %u files x 300 f64) but %llu are free",
+                                     (unsigned long long)need, (unsigned long long)L->n_grids, L->n_files, (unsigned long long)free_b); }
+    }
+
+    // isotope distributions: composition on the host, peptide_isotopes on the device with host-libm exp tables
+    std::vector<uint16_t> carbon(n_slots), sulfur(n_slots);
+    uint16_t max_c = 0, max_s = 0;
+    for (uint32_t s = 0; s < n_slots; s++) {
+        uint32_t c = 0, su = 0;
+        for (uint32_t r = P->residue_offsets[slot_pep[s]]; r < P->residue_offsets[slot_pep[s] + 1]; r++) {
+            uint16_t rc_, rs_;
+            residue_composition(P->sequence[r], rc_, rs_);
+            c += rc_;
+            su += rs_;
+        }
+        carbon[s] = (uint16_t)c;
+        sulfur[s] = (uint16_t)su;
+        max_c = std::max(max_c, carbon[s]);
+        max_s = std::max(max_s, sulfur[s]);
+    }
+    std::vector<float> expt((size_t)max_c + 1 + 2 * ((size_t)max_s + 1));
+    float* exp_c = expt.data();
+    float* exp_s33 = exp_c + max_c + 1;
+    float* exp_s35 = exp_s33 + max_s + 1;
+    for (uint32_t c = 0; c <= max_c; c++) exp_c[c] = std::exp(-((float)c * 0.011f));
+    for (uint32_t s = 0; s <= max_s; s++) {
+        exp_s33[s] = std::exp(-((float)s * 0.0076f));
+        exp_s35[s] = std::exp(-((float)s * 0.044f));
+    }
+    // gaussian_kernel(0.5, 10) (lfq.rs:614-628) and the RT factor of scores (lfq.rs:425, 430-431)
+    double consts[LFQ_K_WIDTH + LFQ_GRID];
+    {
+        const double sigma = 0.5, step = 2.0 / (double)(LFQ_K_WIDTH - 1), constant = 1.0 / (sigma * std::sqrt(2.0 * 3.141592653589793));
+        double sum = 0.0;
+        for (int i = 0; i < LFQ_K_WIDTH; i++) {
+            const double x = (double)i * step - 1.0, xs = x / sigma;
+            consts[i] = constant * std::exp(-0.5 * (xs * xs));
+            sum = sum + consts[i];
+        }
+        for (int i = 0; i < LFQ_K_WIDTH; i++) consts[i] = consts[i] / sum;
+        const int center = LFQ_GRID / 2;
+        for (int rt = 0; rt < LFQ_GRID; rt++) consts[LFQ_K_WIDTH + rt] = std::pow(1.0 - ((double)std::abs(rt - center) / (double)center), 0.33);
+    }
+
+    LFQ_RC(lfq_malloc(L, &L->d_ranges, sizeof(sage_b200_lfq_range) * L->n_ranges));
+    LFQ_RC(lfq_malloc(L, &L->d_grid_of, 4 * L->n_ranges));
+    LFQ_RC(lfq_malloc(L, &L->d_min_rts, 4 * L->n_pages));
+    LFQ_RC(lfq_malloc(L, &L->d_slot_dist, 12ull * n_slots));
+    LFQ_RC(lfq_malloc(L, &L->d_slot_file, 4ull * n_slots));
+    LFQ_RC(lfq_malloc(L, &L->d_touched, L->n_grids));
+    LFQ_RC(lfq_malloc(L, &L->d_align, sizeof(sage_b200_alignment) * L->n_files));
+    LFQ_RC(lfq_malloc(L, &L->d_consts, sizeof consts));
+    LFQ_RC(lfq_malloc(L, &L->d_grids, grid_bytes));
+    LFQ_TRY(cudaMemsetAsync(L->d_grids, 0, grid_bytes, st));
+    LFQ_TRY(cudaMemsetAsync(L->d_touched, 0, L->n_grids, st));
+    LFQ_TRY(cudaMemcpyAsync(L->d_align, align, sizeof(sage_b200_alignment) * L->n_files, cudaMemcpyHostToDevice, st));
+    LFQ_TRY(cudaMemcpyAsync(L->d_consts, consts, sizeof consts, cudaMemcpyHostToDevice, st));
+    if (n_slots) {
+        LFQ_RC(d_cs.reserve(4ull * n_slots));
+        LFQ_RC(d_exp.reserve(4 * expt.size()));
+        LFQ_TRY(cudaMemcpyAsync(d_cs.p, carbon.data(), 2ull * n_slots, cudaMemcpyHostToDevice, st));
+        LFQ_TRY(cudaMemcpyAsync(d_cs.as<uint16_t>() + n_slots, sulfur.data(), 2ull * n_slots, cudaMemcpyHostToDevice, st));
+        LFQ_TRY(cudaMemcpyAsync(d_exp.p, expt.data(), 4 * expt.size(), cudaMemcpyHostToDevice, st));
+        k_lfq_isotopes<<<(n_slots + 255) / 256, 256, 0, st>>>(n_slots, d_cs.as<uint16_t>(), d_cs.as<uint16_t>() + n_slots, d_exp.as<float>(),
+                                                             d_exp.as<float>() + max_c + 1, d_exp.as<float>() + max_c + 1 + max_s + 1, (float*)L->d_slot_dist);
+        LFQ_TRY(cudaGetLastError());
+
+        // expansion, stable RT sort, stable per-page mass_lo sort (lfq.rs:134-184)
+        const uint32_t nr = (uint32_t)L->n_ranges, nt = (uint32_t)(n_slots * L->n_charges * LFQ_ISO);
+        DevBuf pre, k32[2], v32[2], k64;
+        auto cleanup2 = [&]() {
+            for (DevBuf* d : {&pre, &k32[0], &k32[1], &v32[0], &v32[1], &k64}) d->release();
+        };
+        int rc2 = 0;
+        if (!rc2) rc2 = pre.reserve(sizeof(sage_b200_lfq_range) * nr);
+        for (int k = 0; k < 2 && !rc2; k++) rc2 = k32[k].reserve(4ull * nr) || v32[k].reserve(4ull * nr);
+        if (!rc2) rc2 = k64.reserve(8ull * nr);
+        if (rc2) { cleanup2(); cleanup(); return SAGE_B200_ECUDA; }
+        k_lfq_expand<<<(nt + 255) / 256, 256, 0, st>>>(n_slots, L->n_charges, L->p.min_precursor_charge, L->p.ppm_tolerance, L->p.mobility_pct_tolerance,
+                                                      d_slots.as<uint32_t>(), d_first.as<uint32_t>(), d_rows[3].as<float>(), d_rows[4].as<float>(),
+                                                      d_rows[5].as<uint32_t>(), d_rows[6].as<float>(), pre.as<sage_b200_lfq_range>(), k32[0].as<uint32_t>(),
+                                                      v32[0].as<uint32_t>(), (uint32_t*)L->d_slot_file);
+        cudaError_t e = cudaGetLastError();
+        size_t tb = 0, tb2 = 0;
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, tb, k32[0].as<uint32_t>(), k32[1].as<uint32_t>(), v32[0].as<uint32_t>(),
+                                                                  v32[1].as<uint32_t>(), (int)nr, 0, 32, st);
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, tb2, k64.as<uint64_t>(), k64.as<uint64_t>(), v32[1].as<uint32_t>(),
+                                                                  v32[0].as<uint32_t>(), (int)nr, 0, 64, st);
+        if (e == cudaSuccess && L->tmp.reserve(std::max(tb, tb2))) e = cudaErrorMemoryAllocation;
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(L->tmp.p, tb, k32[0].as<uint32_t>(), k32[1].as<uint32_t>(), v32[0].as<uint32_t>(),
+                                                                  v32[1].as<uint32_t>(), (int)nr, 0, 32, st);
+        if (e == cudaSuccess) {
+            k_lfq_page_keys<<<(nr + 255) / 256, 256, 0, st>>>(nr, v32[1].as<uint32_t>(), pre.as<sage_b200_lfq_range>(), k64.as<uint64_t>(), (float*)L->d_min_rts);
+            e = cudaGetLastError();
+        }
+        DevBuf k64o;
+        if (e == cudaSuccess && k64o.reserve(8ull * nr)) e = cudaErrorMemoryAllocation;
+        const int end_bit = 32 + (int)ceil_log2_u64(L->n_pages + 1);
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(L->tmp.p, tb2, k64.as<uint64_t>(), k64o.as<uint64_t>(), v32[1].as<uint32_t>(),
+                                                                  v32[0].as<uint32_t>(), (int)nr, 0, end_bit, st);
+        if (e == cudaSuccess) {
+            k_lfq_gather<<<(nr + 255) / 256, 256, 0, st>>>(nr, L->n_charges, L->p.combine_charge_states, v32[0].as<uint32_t>(), pre.as<sage_b200_lfq_range>(),
+                                                          (sage_b200_lfq_range*)L->d_ranges, (uint32_t*)L->d_grid_of);
+            e = cudaGetLastError();
+        }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        k64o.release();
+        cleanup2();
+        if (e != cudaSuccess) { cleanup(); return fail(SAGE_B200_ECUDA, "feature map build failed: %s", cudaGetErrorString(e)); }
+    }
+    LFQ_RC(lfq_elapsed(L, L->info.ms_build));
+    cleanup();
+#undef LFQ_TRY
+#undef LFQ_RC
+    return 0;
+}
+
+extern "C" int sage_b200_lfq_create(const sage_b200_db* db, const sage_b200_peptides* peptides, const sage_b200_lfq_params* params,
+                                    const sage_b200_lfq_features* features, uint64_t n_files, const sage_b200_alignment* alignments, sage_b200_lfq** out) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+        cudaGetLastError();
+        return fail(SAGE_B200_ECUDA, "no CUDA device available: sage_b200 has no CPU fallback");
+    }
+    if (!db || !peptides || !params || !features || !out || !alignments) return fail(SAGE_B200_EINVAL, "lfq_create: null argument");
+    if (peptides->n_peptides != db->v.n_pep || (peptides->n_peptides && (!peptides->residue_offsets || !peptides->sequence)))
+        return fail(SAGE_B200_EINVAL, "lfq_create: peptides is not the table the db was built from");
+    if (n_files == 0) return fail(SAGE_B200_EINVAL, "lfq_create: n_files must be >= 1");
+    if (n_files > LFQ_MAX_FILES) return fail(SAGE_B200_ELIMIT, "lfq_create: %llu files (at most %u supported)", (unsigned long long)n_files, LFQ_MAX_FILES);
+    if (params->peak_scoring < 0 || params->peak_scoring > 3 || params->integration < 0 || params->integration > 1)
+        return fail(SAGE_B200_EINVAL, "lfq_create: bad peak_scoring / integration");
+    if (params->min_precursor_charge == 0 || params->min_precursor_charge > params->max_precursor_charge)
+        return fail(SAGE_B200_EINVAL, "lfq_create: precursor_charge must be (min, max) with 1 <= min <= max");
+    const sage_b200_lfq_features* F = features;
+    if (F->n && (!F->peptide_idx || !F->peptide_q || !F->label || !F->aligned_rt || !F->calcmass || !F->file_id || !F->ims))
+        return fail(SAGE_B200_EINVAL, "lfq_create: null feature array");
+    if (F->n > 0xFFFFFFFEull) return fail(SAGE_B200_ELIMIT, "lfq_create: more than 2^32 - 2 features");
+    for (uint64_t i = 0; i < F->n; i++) {
+        if (!(F->peptide_q[i] <= params->peptide_q_value && F->label[i] == 1)) continue;
+        if (F->peptide_idx[i] >= db->v.n_pep)
+            return fail(SAGE_B200_EINVAL, "lfq_create: feature %llu has peptide_idx %u outside the db", (unsigned long long)i, F->peptide_idx[i]);
+        if (F->file_id[i] >= n_files)
+            return fail(SAGE_B200_EINVAL, "lfq_create: feature %llu has file_id %u >= n_files %llu", (unsigned long long)i, F->file_id[i], (unsigned long long)n_files);
+    }
+    CUDA_TRY(cudaSetDevice(db->device));
+    sage_b200_lfq* L = new sage_b200_lfq();
+    L->device = db->device;
+    L->p = *params;
+    L->n_files = (uint32_t)n_files;
+    L->n_charges = (uint32_t)params->max_precursor_charge - params->min_precursor_charge + 1;
+    if (cudaStreamCreateWithFlags(&L->st, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreate(&L->ev[0]) != cudaSuccess ||
+        cudaEventCreate(&L->ev[1]) != cudaSuccess) {
+        sage_b200_lfq_destroy(L);
+        return fail(SAGE_B200_ECUDA, "lfq_create: stream / event creation failed");
+    }
+    const int rc = lfq_build(L, db, peptides, F, alignments);
+    if (rc) {
+        std::string msg = g_last_error;
+        sage_b200_lfq_destroy(L);
+        return fail(rc, "%s", msg.c_str());
+    }
+    L->info.n_peptides = L->n_slots;
+    L->info.n_ranges = L->n_ranges;
+    L->info.n_pages = L->n_pages;
+    L->info.n_grids = L->n_grids;
+    L->info.n_files = L->n_files;
+    *out = L;
+    return 0;
+}
+
+// One pass of the tracing loop over spectra [a, b) of the batch (peaks already counted to fit LFQ_CHUNK_PEAKS unless a single spectrum is larger).
+static int lfq_trace_chunk(sage_b200_lfq* L, const sage_b200_ms1* m, uint64_t a, uint64_t b) {
+    cudaStream_t st = L->st;
+    const uint64_t ns = b - a, p0 = m->peak_offsets[a], np = m->peak_offsets[b] - p0;
+    std::vector<uint64_t> off(ns + 1);
+    for (uint64_t i = 0; i <= ns; i++) off[i] = m->peak_offsets[a + i] - p0;
+    int rc;
+    if ((rc = L->sp_off.reserve(8 * (ns + 1))) || (rc = L->sp_mass.reserve(4 * np + 16)) || (rc = L->sp_int.reserve(4 * np + 16)) ||
+        (rc = L->sp_file.reserve(4 * ns)) || (rc = L->sp_sst.reserve(4 * ns)) || (rc = L->counts.reserve(8 * np + 16)) || (rc = L->offsets.reserve(8 * np + 16)) ||
+        (m->mobilities && (rc = L->sp_mob.reserve(4 * np + 16))))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(L->sp_off.p, off.data(), 8 * (ns + 1), cudaMemcpyHostToDevice, st));
+    if (np) {
+        CUDA_TRY(cudaMemcpyAsync(L->sp_mass.p, m->masses + p0, 4 * np, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(L->sp_int.p, m->intensities + p0, 4 * np, cudaMemcpyHostToDevice, st));
+        if (m->mobilities) CUDA_TRY(cudaMemcpyAsync(L->sp_mob.p, m->mobilities + p0, 4 * np, cudaMemcpyHostToDevice, st));
+    }
+    CUDA_TRY(cudaMemcpyAsync(L->sp_file.p, m->file_id + a, 4 * ns, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(L->sp_sst.p, m->scan_start_time + a, 4 * ns, cudaMemcpyHostToDevice, st));
+    if (np == 0 || L->n_ranges == 0) return 0;
+
+    LfqTraceArgs t{};
+    t.n_spectra = (uint32_t)ns;
+    t.peak_off = L->sp_off.as<uint64_t>();
+    t.masses = L->sp_mass.as<float>();
+    t.intensities = L->sp_int.as<float>();
+    t.mobilities = m->mobilities ? L->sp_mob.as<float>() : nullptr;
+    t.file_id = L->sp_file.as<uint32_t>();
+    t.sst = L->sp_sst.as<float>();
+    t.align = (const sage_b200_alignment*)L->d_align;
+    t.ranges = (const sage_b200_lfq_range*)L->d_ranges;
+    t.grid_of = (const uint32_t*)L->d_grid_of;
+    t.n_ranges = (uint32_t)L->n_ranges;
+    t.n_pages = (uint32_t)L->n_pages;
+    t.n_files = L->n_files;
+    t.min_rts = (const float*)L->d_min_rts;
+    t.counts = L->counts.as<uint64_t>();
+    const unsigned blocks = (unsigned)((ns * 32 + LFQ_THREADS - 1) / LFQ_THREADS);
+    k_lfq_trace<false><<<blocks, LFQ_THREADS, 0, st>>>(t);
+    CUDA_TRY(cudaGetLastError());
+    size_t tb = 0;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, L->counts.as<uint64_t>(), L->offsets.as<uint64_t>(), (int)np, st));
+    if ((rc = L->tmp.reserve(tb))) return rc;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(L->tmp.p, tb, L->counts.as<uint64_t>(), L->offsets.as<uint64_t>(), (int)np, st));
+    uint64_t last[2] = {0, 0};
+    CUDA_TRY(cudaMemcpyAsync(&last[0], L->offsets.as<uint64_t>() + np - 1, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&last[1], L->counts.as<uint64_t>() + np - 1, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    const uint64_t matches = last[0] + last[1], nc = 2 * matches;
+    if (nc == 0) return 0;
+    if (nc > 0x7FFFFFFFull) return fail(SAGE_B200_ELIMIT, "one tracing pass produced %llu contributions (> 2^31): pass fewer spectra per add_ms1", (unsigned long long)nc);
+    for (int k = 0; k < 2; k++)
+        if ((rc = L->cell[k].reserve(8 * nc)) || (rc = L->value[k].reserve(8 * nc))) return rc;
+    t.offsets = L->offsets.as<uint64_t>();
+    t.cell = L->cell[0].as<uint64_t>();
+    t.value = L->value[0].as<double>();
+    k_lfq_trace<true><<<blocks, LFQ_THREADS, 0, st>>>(t);
+    CUDA_TRY(cudaGetLastError());
+    const uint64_t cells = L->n_grids * L->n_files * LFQ_ISO * LFQ_GRID;
+    const int end_bit = std::max(1, (int)ceil_log2_u64(cells));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, L->cell[0].as<uint64_t>(), L->cell[1].as<uint64_t>(), L->value[0].as<double>(), L->value[1].as<double>(),
+                                             (int)nc, 0, end_bit, st));
+    if ((rc = L->tmp.reserve(tb))) return rc;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(L->tmp.p, tb, L->cell[0].as<uint64_t>(), L->cell[1].as<uint64_t>(), L->value[0].as<double>(),
+                                             L->value[1].as<double>(), (int)nc, 0, end_bit, st));
+    k_lfq_fold<<<(unsigned)((nc + 255) / 256), 256, 0, st>>>(nc, L->cell[1].as<uint64_t>(), L->value[1].as<double>(), (double*)L->d_grids,
+                                                            (uint8_t*)L->d_touched, (uint64_t)L->n_files * LFQ_ISO * LFQ_GRID);
+    CUDA_TRY(cudaGetLastError());
+    L->info.contributions += nc;
+    return 0;
+}
+
+extern "C" int sage_b200_lfq_add_ms1(sage_b200_lfq* L, const sage_b200_ms1* m) {
+    if (!L || !m) return fail(SAGE_B200_EINVAL, "lfq_add_ms1: null argument");
+    std::lock_guard<std::mutex> lock(L->mu);
+    if (m->n == 0) return 0;
+    if (!m->peak_offsets || !m->file_id || !m->scan_start_time) return fail(SAGE_B200_EINVAL, "lfq_add_ms1: null array");
+    if (m->peak_offsets[m->n] > m->peak_offsets[0] && (!m->masses || !m->intensities)) return fail(SAGE_B200_EINVAL, "lfq_add_ms1: null peak arrays");
+    for (uint64_t i = 0; i < m->n; i++) {
+        if (m->file_id[i] >= L->n_files)
+            return fail(SAGE_B200_EINVAL, "lfq_add_ms1: spectrum %llu has file_id %u >= n_files %u", (unsigned long long)i, m->file_id[i], L->n_files);
+        if (m->peak_offsets[i + 1] < m->peak_offsets[i]) return fail(SAGE_B200_EINVAL, "lfq_add_ms1: peak_offsets not monotone at spectrum %llu", (unsigned long long)i);
+    }
+    CUDA_TRY(cudaSetDevice(L->device));
+    CUDA_TRY(cudaEventRecord(L->ev[0], L->st));
+    for (uint64_t a = 0; a < m->n;) {
+        uint64_t b = a + 1;
+        while (b < m->n && b - a < 0x7FFFFFull && m->peak_offsets[b + 1] - m->peak_offsets[a] <= LFQ_CHUNK_PEAKS) b++;
+        const int rc = lfq_trace_chunk(L, m, a, b);
+        if (rc) return rc;
+        a = b;
+    }
+    L->info.ms1_spectra += m->n;
+    L->info.ms1_peaks += m->peak_offsets[m->n] - m->peak_offsets[0];
+    return lfq_elapsed(L, L->info.ms_trace);
+}
+
+extern "C" int sage_b200_lfq_integrate(sage_b200_lfq* L, sage_b200_lfq_row* rows, double* areas, uint64_t capacity, uint64_t* n_rows) {
+    if (!L || !n_rows) return fail(SAGE_B200_EINVAL, "lfq_integrate: null argument");
+    std::lock_guard<std::mutex> lock(L->mu);
+    CUDA_TRY(cudaSetDevice(L->device));
+    cudaStream_t st = L->st;
+    const uint32_t F = L->n_files;
+    *n_rows = 0;
+    if (L->n_grids == 0) return 0;
+    int rc;
+    CUDA_TRY(cudaEventRecord(L->ev[0], st));
+    if ((rc = L->ids.reserve(4 * L->n_grids + 16)) || (rc = L->o_present.reserve(4 * L->n_grids + 16))) return rc;
+    size_t tb = 0;
+    thrust::counting_iterator<uint32_t> it(0);
+    uint32_t* d_n = L->o_present.as<uint32_t>() + L->n_grids;   // the selected count lives behind the present flags' room
+    CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, it, (const uint8_t*)L->d_touched, L->ids.as<uint32_t>(), d_n, (int)L->n_grids, st));
+    if ((rc = L->tmp.reserve(tb))) return rc;
+    CUDA_TRY(cub::DeviceSelect::Flagged(L->tmp.p, tb, it, (const uint8_t*)L->d_touched, L->ids.as<uint32_t>(), d_n, (int)L->n_grids, st));
+    uint32_t nt = 0;
+    CUDA_TRY(cudaMemcpyAsync(&nt, d_n, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    L->info.grids_touched = nt;
+    if (nt == 0) { L->info.ms_integrate = 0.0f; return lfq_elapsed(L, L->info.ms_integrate); }
+    if ((rc = L->o_rt.reserve(4ull * nt)) || (rc = L->o_sa.reserve(8ull * nt)) || (rc = L->o_score.reserve(8ull * nt)) || (rc = L->o_areas.reserve(8ull * nt * F)))
+        return rc;
+    const size_t smem = lfq_integrate_smem(F);
+    CUDA_TRY(cudaFuncSetAttribute(k_lfq_integrate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    LfqIntegrateArgs a{};
+    a.n = nt;
+    a.grid_ids = L->ids.as<uint32_t>();
+    a.grids = (const double*)L->d_grids;
+    a.slot_dist = (const float*)L->d_slot_dist;
+    a.slot_file = (const uint32_t*)L->d_slot_file;
+    a.consts = (const double*)L->d_consts;
+    a.n_files = F;
+    a.n_charges = L->n_charges;
+    a.combine = L->p.combine_charge_states;
+    a.peak_scoring = L->p.peak_scoring;
+    a.integration = L->p.integration;
+    a.spectral_angle = L->p.spectral_angle;
+    a.present = L->o_present.as<uint8_t>();
+    a.rt = L->o_rt.as<uint32_t>();
+    a.sa = L->o_sa.as<double>();
+    a.score = L->o_score.as<double>();
+    a.areas = L->o_areas.as<double>();
+    k_lfq_integrate<<<nt, LFQ_THREADS, smem, st>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    L->info.ms_integrate = 0.0f;
+    if ((rc = lfq_elapsed(L, L->info.ms_integrate))) return rc;
+
+    // copy back and keep the grids that produced a peak, in grid order == (PrecursorId, decoy) order
+    CUDA_TRY(cudaEventRecord(L->ev[0], st));
+    std::vector<uint32_t> ids(nt), rt(nt);
+    std::vector<uint8_t> present(nt);
+    std::vector<double> sa(nt), score(nt), ar((size_t)nt * F);
+    CUDA_TRY(cudaMemcpyAsync(ids.data(), L->ids.p, 4ull * nt, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(present.data(), L->o_present.p, nt, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(rt.data(), L->o_rt.p, 4ull * nt, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(sa.data(), L->o_sa.p, 8ull * nt, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(score.data(), L->o_score.p, 8ull * nt, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ar.data(), L->o_areas.p, 8ull * nt * F, cudaMemcpyDeviceToHost, st));
+    L->info.ms_download = 0.0f;
+    if ((rc = lfq_elapsed(L, L->info.ms_download))) return rc;
+    uint64_t k = 0;
+    for (uint32_t i = 0; i < nt; i++) {
+        if (!present[i]) continue;
+        if (k >= capacity) return fail(SAGE_B200_ELIMIT, "lfq_integrate: capacity %llu too small (at most n_grids = %llu rows)", (unsigned long long)capacity,
+                                       (unsigned long long)L->n_grids);
+        const uint32_t g = ids[i], slot = L->p.combine_charge_states ? g / 2 : g / 2 / L->n_charges;
+        sage_b200_lfq_row r{};
+        r.peptide = L->slot_pep[slot];
+        r.charge = L->p.combine_charge_states ? 0 : (uint8_t)(L->p.min_precursor_charge + (g / 2) % L->n_charges);
+        r.decoy = (uint8_t)(g & 1);
+        r.rt = rt[i];
+        r.spectral_angle = sa[i];
+        r.score = score[i];
+        if (rows) rows[k] = r;
+        if (areas) memcpy(areas + k * F, ar.data() + (size_t)i * F, 8ull * F);
+        k++;
+    }
+    *n_rows = k;
+    return 0;
+}
+
+extern "C" int sage_b200_lfq_get_info(sage_b200_lfq* L, sage_b200_lfq_info* info) {
+    if (!L || !info) return fail(SAGE_B200_EINVAL, "lfq_get_info: null argument");
+    std::lock_guard<std::mutex> lock(L->mu);
+    *info = L->info;
+    info->device_bytes = L->fixed_bytes + L->scratch_bytes();
+    return 0;
+}
+
+extern "C" int sage_b200_lfq_export(sage_b200_lfq* L, sage_b200_lfq_range* ranges, float* min_rts, double* grids, uint8_t* touched) {
+    if (!L) return fail(SAGE_B200_EINVAL, "lfq_export: null handle");
+    std::lock_guard<std::mutex> lock(L->mu);
+    CUDA_TRY(cudaSetDevice(L->device));
+    CUDA_TRY(cudaStreamSynchronize(L->st));
+    if (ranges && L->n_ranges) CUDA_TRY(cudaMemcpy(ranges, L->d_ranges, sizeof(sage_b200_lfq_range) * L->n_ranges, cudaMemcpyDeviceToHost));
+    if (min_rts && L->n_pages) CUDA_TRY(cudaMemcpy(min_rts, L->d_min_rts, 4 * L->n_pages, cudaMemcpyDeviceToHost));
+    if (grids && L->n_grids) CUDA_TRY(cudaMemcpy(grids, L->d_grids, 8 * L->n_grids * L->n_files * LFQ_ISO * LFQ_GRID, cudaMemcpyDeviceToHost));
+    if (touched && L->n_grids) CUDA_TRY(cudaMemcpy(touched, L->d_touched, L->n_grids, cudaMemcpyDeviceToHost));
+    return 0;
 }
 
 #if SAGE_B200_PHASE_CLOCKS

@@ -288,3 +288,94 @@ def make_spectra(pep: Peptides, n: int = 50_000, seed: int = 0xB202, n_peaks: in
     return SpectraBatch(peak_off=peak_off, masses=masses.ravel(), intensities=intens.ravel(), prec_mz=prec_mz, prec_charge=chg,
                         iso_lo=np.full(n, np.nan, np.float32), iso_hi=np.full(n, np.nan, np.float32), tic=tic, level=np.full(n, 2, np.uint8),
                         rt=(np.arange(n, dtype=np.float32) * np.float32(0.01)), ims=np.full(n, np.nan, np.float32))
+
+
+NEUTRON = np.float32(1.00335)
+# carbon count per residue (mass.rs:78-104), for an approximate isotope envelope
+_CARBON = np.zeros(256, np.int64)
+for _aa, _c in zip("ACDEFGHIKLMNPQRSTVWYUO", [3, 3, 4, 5, 9, 2, 6, 6, 6, 6, 5, 4, 5, 5, 6, 3, 4, 5, 11, 9, 3, 12]):
+    _CARBON[ord(_aa)] = _c
+
+
+def make_ms1_runs(pep: Peptides, n_ids: int = 30_000, n_files: int = 4, spectra_per_file: int = 3000, peaks_per_spectrum: int = 1500, seed: int = 0x1F0,
+                  mobility: bool = False, charges=(2, 3), absent_fraction: float = 0.15, ppm_jitter: float = 2.0, sigma: float = 0.0015):
+    """Synthetic label-free quantification input: `n_ids` target peptides "identified" at an aligned RT (normalized run time, 0..1), a charge
+    and a file; per-file linear RT distortion (returned as the alignments that undo it); Gaussian elution profiles (sd `sigma` in aligned RT) of
+    3-isotope envelopes from each peptide's carbon count, with ppm jitter; every peptide absent from a random `absent_fraction` of the other
+    files; noise peaks up to `peaks_per_spectrum`; optionally per-peak mobilities. The Feature rows also hold filtered-out rows (q-value too
+    high, decoys) and lower-confidence repeats of identified peptides, as a real confidence-sorted Feature table does.
+    Returns dict(features, alignments, batch: Ms1Batch of every file's spectra in acquisition order, file by file)."""
+    from .api import ALIGNMENT_DTYPE, Ms1Batch
+    rng = np.random.default_rng(seed)
+    targets = np.nonzero(pep.decoy == 0)[0]
+    decoys = np.nonzero(pep.decoy != 0)[0]
+    ids = rng.choice(targets, size=min(n_ids, len(targets)), replace=False).astype(np.uint32)
+    n = len(ids)
+    t_rt = rng.uniform(0.05, 0.95, n).astype(np.float32)
+    charge = rng.choice(np.asarray(charges), n).astype(np.int64)
+    file_of = rng.integers(0, n_files, n).astype(np.uint32)
+    ims = rng.uniform(0.7, 1.3, n).astype(np.float32) if mobility else np.zeros(n, np.float32)
+    mono = pep.mono[ids].astype(np.float32)
+    off = pep.seq_off.astype(np.int64)
+    carbon = np.add.reduceat(_CARBON[pep.seq], off[:-1])[ids] if len(pep.seq) else np.zeros(n, np.int64)
+    lam = carbon * 0.011
+    env = np.stack([np.ones(n), lam, lam * lam / 2.0], axis=1)
+    env /= env.max(axis=1, keepdims=True)
+    present = rng.random((n_files, n)) >= absent_fraction
+    present[file_of, np.arange(n)] = True
+    abundance = np.exp(rng.normal(13.0, 1.5, n))
+
+    # features: identified rows, then lower-confidence repeats, rows above the q-value cut and decoy rows, shuffled after the first block
+    n_rep, n_bad, n_dec = n // 5, n // 10, n // 10
+    rep = rng.choice(n, n_rep)
+    bad = rng.choice(targets, n_bad).astype(np.uint32)
+    dec = rng.choice(decoys, n_dec).astype(np.uint32) if len(decoys) else np.zeros(0, np.uint32)
+    tail_pep = np.concatenate([ids[rep], bad, dec])
+    m = len(tail_pep)
+    feats = np.zeros(n + m, dtype=[("peptide_idx", "<u4"), ("peptide_q", "<f4"), ("label", "<i4"), ("aligned_rt", "<f4"), ("calcmass", "<f4"),
+                                   ("file_id", "<u4"), ("ims", "<f4")])
+    feats["peptide_idx"] = np.concatenate([ids, tail_pep])
+    feats["peptide_q"] = np.concatenate([rng.uniform(0, 0.01, n), rng.uniform(0, 0.01, n_rep), rng.uniform(0.0101, 0.5, n_bad), rng.uniform(0, 0.01, n_dec)])
+    feats["label"] = np.concatenate([np.ones(n + n_rep + n_bad, np.int32), -np.ones(n_dec, np.int32)])
+    feats["aligned_rt"] = np.concatenate([t_rt + rng.normal(0, sigma / 4, n).astype(np.float32), rng.uniform(0, 1, m).astype(np.float32)])
+    feats["calcmass"] = pep.mono[feats["peptide_idx"]]
+    feats["file_id"] = np.concatenate([file_of, rng.integers(0, n_files, m).astype(np.uint32)])
+    feats["ims"] = np.concatenate([ims, rng.uniform(0.7, 1.3, m).astype(np.float32) if mobility else np.zeros(m, np.float32)])
+    tail = n + rng.permutation(m)
+    feats = np.concatenate([feats[:n], feats[tail]])
+
+    align = np.zeros(n_files, ALIGNMENT_DTYPE)
+    align["max_rt"] = rng.uniform(60.0, 120.0, n_files)
+    align["slope"] = rng.uniform(0.95, 1.05, n_files)
+    align["intercept"] = rng.uniform(-0.02, 0.02, n_files)
+
+    offs, masses, intens, fids, ssts, mobs = [np.zeros(1, np.uint64)], [], [], [], [], []
+    total = 0
+    for f in range(n_files):
+        sel = np.nonzero(present[f])[0]
+        sel = sel[np.argsort(t_rt[sel])]
+        sst = (np.arange(spectra_per_file, dtype=np.float64) + 0.5) / spectra_per_file * float(align["max_rt"][f])
+        arts = (sst / float(align["max_rt"][f])) * float(align["slope"][f]) + float(align["intercept"][f])
+        for s in range(spectra_per_file):
+            a, b = np.searchsorted(t_rt[sel], [arts[s] - 4 * sigma, arts[s] + 4 * sigma])
+            el = sel[a:b]
+            prof = abundance[el] * np.exp(-0.5 * ((arts[s] - t_rt[el]) / sigma) ** 2)
+            sig_m = ((mono[el, None] + np.arange(3)[None, :] * NEUTRON) / charge[el, None]).ravel()
+            sig_m = sig_m * (1.0 + rng.normal(0, ppm_jitter * 1e-6, len(sig_m)))
+            sig_i = (prof[:, None] * env[el]).ravel()
+            sig_mob = np.repeat(ims[el], 3) * (1.0 + rng.normal(0, 0.002, 3 * len(el)))
+            k = max(peaks_per_spectrum - len(sig_m), 0)
+            mm = np.concatenate([sig_m, rng.uniform(300.0, 1500.0, k)]).astype(np.float32)
+            ii = np.concatenate([sig_i, np.exp(rng.normal(9.0, 1.0, k))]).astype(np.float32)
+            mo = np.concatenate([sig_mob, rng.uniform(0.7, 1.3, k)]).astype(np.float32)
+            order = np.argsort(mm, kind="stable")
+            masses.append(mm[order])
+            intens.append(ii[order])
+            mobs.append(mo[order])
+            total += len(mm)
+            offs.append(np.array([total], np.uint64))
+            fids.append(f)
+            ssts.append(sst[s])
+    batch = Ms1Batch(np.concatenate(offs), np.concatenate(masses), np.concatenate(intens), np.array(fids, np.uint32), np.array(ssts, np.float32),
+                     np.concatenate(mobs) if mobility else None)
+    return dict(features=feats, alignments=align, batch=batch, ids=ids, charge=charge)
