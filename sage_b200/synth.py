@@ -298,12 +298,19 @@ for _aa, _c in zip("ACDEFGHIKLMNPQRSTVWYUO", [3, 3, 4, 5, 9, 2, 6, 6, 6, 6, 5, 4
 
 
 def make_ms1_runs(pep: Peptides, n_ids: int = 30_000, n_files: int = 4, spectra_per_file: int = 3000, peaks_per_spectrum: int = 1500, seed: int = 0x1F0,
-                  mobility: bool = False, charges=(2, 3), absent_fraction: float = 0.15, ppm_jitter: float = 2.0, sigma: float = 0.0015):
-    """Synthetic label-free quantification input: `n_ids` target peptides "identified" at an aligned RT (normalized run time, 0..1), a charge
-    and a file; per-file linear RT distortion (returned as the alignments that undo it); Gaussian elution profiles (sd `sigma` in aligned RT) of
-    3-isotope envelopes from each peptide's carbon count, with ppm jitter; every peptide absent from a random `absent_fraction` of the other
-    files; noise peaks up to `peaks_per_spectrum`; optionally per-peak mobilities. The Feature rows also hold filtered-out rows (q-value too
-    high, decoys) and lower-confidence repeats of identified peptides, as a real confidence-sorted Feature table does.
+                  mobility: bool = False, charges=(2, 3), absent_fraction: float = 0.15, ppm_jitter: float = 2.0, sigma: float = 0.0015,
+                  rt_range=(0.05, 0.95), scan_range=None, rt_offset_bins=None, distort: bool = True, ref_file=None, silent_files=()):
+    """Synthetic label-free quantification input: `n_ids` target peptides "identified" at an aligned RT (normalized run time, uniform in
+    `rt_range`), a charge and a file; per-file linear RT distortion (returned as the alignments that undo it); Gaussian elution profiles (sd
+    `sigma` in aligned RT) of 3-isotope envelopes from each peptide's carbon count, with ppm jitter; every peptide absent from a random
+    `absent_fraction` of the other files; noise peaks up to `peaks_per_spectrum`; optionally per-peak mobilities. The Feature rows also hold
+    filtered-out rows (q-value too high, decoys) and lower-confidence repeats of identified peptides, as a real confidence-sorted Feature table does.
+    Options that shape the time warps quantification finds (the defaults leave the output unchanged):
+      scan_range      (lo, hi): the spectra sample this aligned-RT interval evenly instead of the whole run;
+      rt_offset_bins  one int per file: that file's elution is late by this many grid bins (RT_TOL * 2 / 100 = 1e-4 of aligned RT each);
+      distort=False   identity alignments (max_rt 100, slope 1, intercept 0): every file samples the same aligned RTs;
+      ref_file        every identified peptide's best PSM is in this file (the grid's reference file);
+      silent_files    files with no peptide signal at all.
     Returns dict(features, alignments, batch: Ms1Batch of every file's spectra in acquisition order, file by file)."""
     from .api import ALIGNMENT_DTYPE, Ms1Batch
     rng = np.random.default_rng(seed)
@@ -311,9 +318,12 @@ def make_ms1_runs(pep: Peptides, n_ids: int = 30_000, n_files: int = 4, spectra_
     decoys = np.nonzero(pep.decoy != 0)[0]
     ids = rng.choice(targets, size=min(n_ids, len(targets)), replace=False).astype(np.uint32)
     n = len(ids)
-    t_rt = rng.uniform(0.05, 0.95, n).astype(np.float32)
+    t_rt = rng.uniform(rt_range[0], rt_range[1], n).astype(np.float32)
     charge = rng.choice(np.asarray(charges), n).astype(np.int64)
     file_of = rng.integers(0, n_files, n).astype(np.uint32)
+    if ref_file is not None:
+        file_of[:] = ref_file
+    shift = np.zeros(n_files) if rt_offset_bins is None else np.asarray(rt_offset_bins, np.float64) * 1e-4
     ims = rng.uniform(0.7, 1.3, n).astype(np.float32) if mobility else np.zeros(n, np.float32)
     mono = pep.mono[ids].astype(np.float32)
     off = pep.seq_off.astype(np.int64)
@@ -323,6 +333,7 @@ def make_ms1_runs(pep: Peptides, n_ids: int = 30_000, n_files: int = 4, spectra_
     env /= env.max(axis=1, keepdims=True)
     present = rng.random((n_files, n)) >= absent_fraction
     present[file_of, np.arange(n)] = True
+    present[list(silent_files)] = False
     abundance = np.exp(rng.normal(13.0, 1.5, n))
 
     # features: identified rows, then lower-confidence repeats, rows above the q-value cut and decoy rows, shuffled after the first block
@@ -348,18 +359,24 @@ def make_ms1_runs(pep: Peptides, n_ids: int = 30_000, n_files: int = 4, spectra_
     align["max_rt"] = rng.uniform(60.0, 120.0, n_files)
     align["slope"] = rng.uniform(0.95, 1.05, n_files)
     align["intercept"] = rng.uniform(-0.02, 0.02, n_files)
+    if not distort:
+        align["max_rt"], align["slope"], align["intercept"] = 100.0, 1.0, 0.0
 
     offs, masses, intens, fids, ssts, mobs = [np.zeros(1, np.uint64)], [], [], [], [], []
     total = 0
     for f in range(n_files):
         sel = np.nonzero(present[f])[0]
         sel = sel[np.argsort(t_rt[sel])]
-        sst = (np.arange(spectra_per_file, dtype=np.float64) + 0.5) / spectra_per_file * float(align["max_rt"][f])
+        if scan_range is None:
+            sst = (np.arange(spectra_per_file, dtype=np.float64) + 0.5) / spectra_per_file * float(align["max_rt"][f])
+        else:
+            want = scan_range[0] + (np.arange(spectra_per_file, dtype=np.float64) + 0.5) / spectra_per_file * (scan_range[1] - scan_range[0])
+            sst = (want - float(align["intercept"][f])) / float(align["slope"][f]) * float(align["max_rt"][f])
         arts = (sst / float(align["max_rt"][f])) * float(align["slope"][f]) + float(align["intercept"][f])
         for s in range(spectra_per_file):
-            a, b = np.searchsorted(t_rt[sel], [arts[s] - 4 * sigma, arts[s] + 4 * sigma])
+            a, b = np.searchsorted(t_rt[sel], [arts[s] - shift[f] - 4 * sigma, arts[s] - shift[f] + 4 * sigma])
             el = sel[a:b]
-            prof = abundance[el] * np.exp(-0.5 * ((arts[s] - t_rt[el]) / sigma) ** 2)
+            prof = abundance[el] * np.exp(-0.5 * ((arts[s] - shift[f] - t_rt[el]) / sigma) ** 2)
             sig_m = ((mono[el, None] + np.arange(3)[None, :] * NEUTRON) / charge[el, None]).ravel()
             sig_m = sig_m * (1.0 + rng.normal(0, ppm_jitter * 1e-6, len(sig_m)))
             sig_i = (prof[:, None] * env[el]).ravel()

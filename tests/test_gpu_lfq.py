@@ -4,6 +4,8 @@ decisions are not near-ties; score and spectral_angle within 1e-12 relative)."""
 import numpy as np
 import pytest
 
+import lfq_cases
+from lfq_reference import LfqReference
 from oracle_lfq import lfq_oracle as LO
 from sage_b200 import FeatureMap, IndexedDatabase, LfqSettings, Ms1Batch, SageB200Error, synth
 from sage_b200.api import ALIGNMENT_DTYPE
@@ -16,7 +18,7 @@ NEAR_TIE = 1e-9
 
 @pytest.fixture(scope="module")
 def pep():
-    return synth.make_peptides(20000, seed=41)
+    return lfq_cases.peptides()   # synth.make_peptides(20000, seed=41), the table of the edge workloads
 
 
 @pytest.fixture(scope="module")
@@ -182,3 +184,72 @@ def test_bench_sized_workload(db, pep):
     rows, near = assert_integration_matches(fm, orc, threads=16)
     assert n > 30000 and rows > 20000
     print(f"bench-sized: {n} grids, {rows} rows, {near} near-tie grids not compared")
+
+
+# ---------------------------------------------------------------------------------------------------- edge workloads (tests/lfq_cases.py)
+def _build_case(db, c):
+    fm = FeatureMap.build(db, c["peptides"], c["settings"], c["charges"], c["features"], c["alignments"])
+    orc = LO.LfqOracle(c["peptides"], c["settings"], c["charges"], c["features"], c["alignments"])
+    return fm, orc
+
+
+@pytest.mark.parametrize("name", lfq_cases.NAMES)
+def test_edge_workloads(db, name):
+    """Device against the oracle on every edge workload, and against the restatement without the oracle: the contribution count (two per
+    add_entry), the touched set; and quantify twice gives identical bytes."""
+    c = lfq_cases.case(name)
+    combine = c["settings"].combine_charge_states
+    fm, orc = _build_case(db, c)
+    ref = LfqReference(c["peptides"], c["settings"], c["charges"], c["features"], c["alignments"])
+    for b in c["batches"]:
+        fm.add_ms1(b)
+        orc.add_ms1(b)
+        ref.add_ms1(b)
+    n = assert_map_and_grids_equal(fm, orc, combine, c["charges"])
+    assert fm.info()["contributions"] == 2 * ref.matches
+    ex = fm.export(grids=True)
+    assert grid_keys(fm, ex, combine, c["charges"])[ex["touched"].astype(bool)].tolist() == ref.export_grids()[0].tolist()
+    rows, near = assert_integration_matches(fm, orc)
+    a, b = fm.quantify(), fm.quantify()
+    for k in a:
+        assert a[k].tobytes() == b[k].tobytes(), f"second quantify differs in {k}"
+    if name != "no_kept_feature":
+        assert rows > 0
+    print(f"{name}: {n} grids compared, {rows} rows, {near} near-tie grids not compared")
+
+
+def test_add_ms1_after_quantify(db):
+    """Tracing more spectra after quantify adds to the same grids: the result equals the oracle fed every batch before integrating."""
+    c = lfq_cases.case("files9")
+    fm, orc = _build_case(db, c)
+    b = c["batches"][0]
+    half = len(b) // 2
+    fm.add_ms1(b.slice(0, half))
+    fm.quantify()
+    fm.add_ms1(b.slice(half, len(b)))
+    orc.add_ms1(b)
+    assert assert_map_and_grids_equal(fm, orc, True, c["charges"]) > 100
+    assert_integration_matches(fm, orc)
+
+
+def test_big_batch_equals_small_calls(db):
+    """One add_ms1 of 2^24 + 2^20 peaks (two tracing passes) gives the grids of the same spectra fed in calls of at most 2^22 peaks."""
+    c = lfq_cases.case("big_batch")
+    b = c["batches"][0]
+    fm_big, _ = _build_case(db, dict(c, batches=[]))
+    fm_big.add_ms1(b)
+    fm_small = FeatureMap.build(db, c["peptides"], c["settings"], c["charges"], c["features"], c["alignments"])
+    off = b.peak_off.astype(np.int64)
+    a = 0
+    calls = 0
+    while a < len(b):
+        z = int(np.searchsorted(off, off[a] + (1 << 22), side="right")) - 1
+        z = max(z, a + 1)
+        fm_small.add_ms1(b.slice(a, z))
+        a = z
+        calls += 1
+    assert calls >= 5
+    g1, g2 = fm_big.export(grids=True), fm_small.export(grids=True)
+    assert g1["touched"].tobytes() == g2["touched"].tobytes() and g1["touched"].any()
+    assert g1["grids"].tobytes() == g2["grids"].tobytes()
+    assert fm_big.info()["contributions"] == fm_small.info()["contributions"]
