@@ -329,6 +329,37 @@ int sage_b200_lfq_get_info(sage_b200_lfq* lfq, sage_b200_lfq_info* info);
 int sage_b200_lfq_export(sage_b200_lfq* lfq, sage_b200_lfq_range* ranges, float* min_rts, double* grids, uint8_t* touched);
 void sage_b200_lfq_destroy(sage_b200_lfq* lfq);
 
+/* ---------------------------------------------------------------------------------------------------------------------------------------------
+ * PSM rescoring (runner.rs:280-291 spectrum_fdr): linear_discriminant::score_psms (mass-error KDE, 20-feature LDA, discriminant KDE and
+ * posterior errors), the heuristic fallback when it returns None, the descending sort and qvalue::spectrum_q_value. Every output is
+ * reproducible bit for bit under the orders of DESIGN.md §10.
+ */
+typedef struct { sage_b200_tolerance precursor_tol; } sage_b200_fdr_params;   /* Ppm or Da; Pct -> EINVAL (linear_discriminant.rs:142) */
+typedef struct {
+    float* discriminant_score;       /* [n], indexed like the input rows */
+    float* posterior_error;          /* [n] log10(PEP) as f32, -324 for PEP 0; 1.0 when the LDA was not fitted (scoring.rs:577) */
+    float* spectrum_q;               /* [n] */
+    uint32_t* order;                 /* [n] input row at each sorted position (descending discriminant, ties by ascending input row) */
+    uint64_t passing;                /* spectrum_q_value's return: rows with q <= 0.01 (targets and decoys) */
+    int32_t lda_fitted;              /* 0: score_psms returned None and the heuristic was used */
+    double coef[20];                 /* the LDA weights when Gauss::solve succeeded (also when they are not finite, which falls back); else 0 */
+    double eps;                      /* the Gauss::solve ridge that succeeded; 0 when none did or the LDA was not trained */
+    float ms_mass_kde, ms_features, ms_lda, ms_discriminant_kde, ms_sort_q, ms_total;   /* CUDA-event stage times of the call */
+} sage_b200_fdr_out;
+/* rows: the Feature rows the search returned, in the caller's order. aligned_rt / delta_rt_model / delta_ims_model: [n] each, or NULL for the
+ * Feature defaults (scoring.rs:583-585: aligned_rt = rt, 0.999 for both deltas). EINVAL for a Pct or unknown tolerance; ELIMIT beyond
+ * 65535 * 4096 rows (the KDE's chunk grid), for a tolerance span of 2^24 or more mass-error bins, or when the work buffers do not fit the device's
+ * free memory (checked before allocating). */
+int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p, const sage_b200_feature* rows, uint64_t n, const float* aligned_rt,
+                           const float* delta_rt_model, const float* delta_ims_model, sage_b200_fdr_out* out);
+/* White-box hook: kde::Builder::build (kde.rs:83-136) with bins, monotonic and bw_adjust = x * bw_factor; scores f64[n], decoy u8[n] (nonzero =
+ * decoy). out_bins[bins] is the PEP per bin; *min_score and *score_step place the bins. ELIMIT beyond 2^31 - 1 scores or 2^24 bins. */
+int sage_b200_kde_build(int device, const double* scores, const uint8_t* decoy, uint64_t n, uint64_t bins, int monotonic, double bw_factor,
+                        double* out_bins, double* min_score, double* score_step);
+/* Test hook: out[i] = the device's evaluation of glibc's exp (function 0), log1p (1) or log10 (2) at x[i]; variant 0 = the FMA builds,
+ * 1 = the uncontracted builds, -1 = the variant the library selected for this host's libm. */
+int sage_b200_device_math(int device, int function, int variant, const double* x, uint64_t n, double* out);
+
 /* Page-locked host buffers: spectra/feature arrays placed here are copied by DMA without a staging memcpy. */
 void* sage_b200_host_alloc(size_t bytes);
 /* The same for a batch sage_b200_score_batch_multi cuts into n_devices contiguous blocks: the i-th of n equal parts of the buffer is placed on the

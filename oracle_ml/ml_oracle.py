@@ -1,0 +1,90 @@
+"""ctypes binding of the CPU oracle of PSM rescoring (oracle_ml/ml_oracle.cpp).
+
+TEST INFRASTRUCTURE ONLY: imported by tests/, __graft_entry__ and tools/bench_rescore.py. Never imported by the sage_b200 package.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import os
+import subprocess
+
+import numpy as np
+
+_HERE = os.path.dirname(os.path.abspath(__file__))
+_SRC = os.path.join(_HERE, "ml_oracle.cpp")
+_SO = os.path.join(_HERE, "_build", "libml_oracle.so")
+# no FMA contraction, no fast-math: every f32/f64 operation stays separately rounded, as rustc emits it
+CXXFLAGS = ["-O2", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-shared", "-pthread", "-Wall"]
+
+_lib = None
+
+
+def build(force: bool = False) -> str:
+    if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(_SRC):
+        os.makedirs(os.path.dirname(_SO), exist_ok=True)
+        env = dict(os.environ)
+        env.pop("CXX", None)
+        subprocess.check_call(["/usr/bin/g++"] + CXXFLAGS + ["-o", _SO, _SRC], env=env)
+    return _SO
+
+
+def lib():
+    global _lib
+    if _lib is None:
+        build()
+        _lib = C.CDLL(_SO)
+        _lib.mo_spectrum_fdr.restype = C.c_double
+        _lib.mo_spectrum_fdr.argtypes = [C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_uint64] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 9
+        _lib.mo_kde_build.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int, C.c_double, C.c_int] + [C.c_void_p] * 3
+        _lib.mo_lda_train.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_void_p]
+    return _lib
+
+
+def _p(a):
+    return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def default_threads() -> int:
+    return max(1, len(os.sched_getaffinity(0)))
+
+
+def kde_build(scores, decoy, bins=1000, monotonic=True, bw_factor=1.0, threads=None):
+    """kde::Builder::build: (PEP per bin, min_score, score_step)."""
+    s = np.ascontiguousarray(scores, np.float64)
+    d = np.ascontiguousarray(decoy, np.uint8)
+    out = np.zeros(int(bins))
+    lo, step = C.c_double(), C.c_double()
+    lib().mo_kde_build(_p(s), _p(d), len(s), int(bins), int(monotonic), float(bw_factor), int(threads or default_threads()), _p(out), C.byref(lo), C.byref(step))
+    return out, lo.value, step.value
+
+
+def lda_train(X, decoy):
+    """LinearDiscriminantAnalysis::train on any [n, D] matrix: (coef, eps), or None when the reference returns None."""
+    X = np.ascontiguousarray(X, np.float64)
+    d = np.ascontiguousarray(decoy, np.uint8)
+    coef = np.zeros(X.shape[1])
+    eps = C.c_double()
+    if not lib().mo_lda_train(_p(X), _p(d), X.shape[0], X.shape[1], _p(coef), C.byref(eps)):
+        return None
+    return coef, eps.value
+
+
+def spectrum_fdr(features, precursor_tol, aligned_rt=None, delta_rt_model=None, delta_ims_model=None, threads=None, with_features=False) -> dict:
+    """runner.rs spectrum_fdr on the CPU; the same keys as sage_b200.spectrum_fdr, plus `seconds` (wall time) and `threads`."""
+    rows = np.ascontiguousarray(features)
+    assert rows.dtype.itemsize == 128
+    n = len(rows)
+    cols = [None if c is None else np.ascontiguousarray(c, np.float32) for c in (aligned_rt, delta_rt_model, delta_ims_model)]
+    disc, pep, q = np.zeros(n, np.float32), np.zeros(n, np.float32), np.zeros(n, np.float32)
+    order = np.zeros(n, np.uint32)
+    passing, fitted = C.c_uint64(), C.c_int32()
+    coef, eps = np.zeros(20), C.c_double()
+    feats = np.zeros((n, 20)) if with_features else None
+    threads = int(threads or default_threads())
+    secs = lib().mo_spectrum_fdr(precursor_tol.kind, precursor_tol.lo, precursor_tol.hi, _p(rows), n, *[_p(c) for c in cols], threads, _p(disc), _p(pep),
+                                 _p(q), _p(order), C.byref(passing), C.byref(fitted), _p(coef), C.byref(eps), _p(feats))
+    res = dict(discriminant_score=disc, posterior_error=pep, spectrum_q=q, order=order, passing=passing.value, lda_fitted=bool(fitted.value), coef=coef,
+               eps=eps.value, seconds=secs, threads=threads)
+    if with_features:
+        res["features"] = feats
+    return res

@@ -90,6 +90,7 @@ EXPORTED_SYMBOLS = [
     "sage_b200_process_spectra", "sage_b200_find_reporter_ions", "sage_b200_host_alloc", "sage_b200_host_free", "sage_b200_last_error",
     "sage_b200_host_log_variant", "sage_b200_host_log1pf_exact", "sage_b200_device_log", "sage_b200_bind_thread_to_device", "sage_b200_host_alloc_blocks",
     "sage_b200_lfq_create", "sage_b200_lfq_add_ms1", "sage_b200_lfq_integrate", "sage_b200_lfq_get_info", "sage_b200_lfq_export", "sage_b200_lfq_destroy",
+    "sage_b200_spectrum_fdr", "sage_b200_kde_build", "sage_b200_device_math",
 ]
 
 _lib = None
@@ -746,3 +747,61 @@ class FeatureMap:
 
 
 Feature = FEATURE_DTYPE
+
+
+# ------------------------------------------------------------------------------------------------ rescoring (spectrum_fdr)
+class CFdrParams(C.Structure):
+    _fields_ = [("precursor_tol", CTol)]
+
+
+FDR_STAGES = ["ms_mass_kde", "ms_features", "ms_lda", "ms_discriminant_kde", "ms_sort_q", "ms_total"]
+
+
+class CFdrOut(C.Structure):
+    _fields_ = [("discriminant_score", C.c_void_p), ("posterior_error", C.c_void_p), ("spectrum_q", C.c_void_p), ("order", C.c_void_p),
+                ("passing", C.c_uint64), ("lda_fitted", C.c_int32), ("coef", C.c_double * 20), ("eps", C.c_double)] + [(s, C.c_float) for s in FDR_STAGES]
+
+
+def spectrum_fdr(features: np.ndarray, precursor_tol: Tolerance, aligned_rt=None, delta_rt_model=None, delta_ims_model=None, device: int = 0) -> dict:
+    """The runner's spectrum_fdr (runner.rs:280-291) on the device: linear_discriminant::score_psms, the heuristic fallback when it fails, the
+    descending sort and spectrum_q_value. `features` are FEATURE_DTYPE rows as Scorer.score_batch returns them; the three optional f32 columns
+    default to the Feature defaults (aligned_rt = rt, 0.999). Returns discriminant_score, posterior_error, spectrum_q (indexed like the rows),
+    order (row at each sorted position), passing, lda_fitted, coef, eps and the stage times (ms_*)."""
+    rows = np.ascontiguousarray(features)
+    if rows.dtype != FEATURE_DTYPE:
+        raise TypeError("features must have FEATURE_DTYPE")
+    n = len(rows)
+    cols = [None if c is None else np.ascontiguousarray(c, np.float32) for c in (aligned_rt, delta_rt_model, delta_ims_model)]
+    for c in cols:
+        if c is not None and len(c) != n:
+            raise ValueError("optional columns must have one value per row")
+    res = dict(discriminant_score=np.zeros(n, np.float32), posterior_error=np.zeros(n, np.float32), spectrum_q=np.zeros(n, np.float32),
+               order=np.zeros(n, np.uint32))
+    out = CFdrOut(_ptr(res["discriminant_score"]), _ptr(res["posterior_error"]), _ptr(res["spectrum_q"]), _ptr(res["order"]))
+    params = CFdrParams(precursor_tol._c())
+    _check(load_library().sage_b200_spectrum_fdr(C.c_int(device), C.byref(params), _ptr(rows), C.c_uint64(n), *[_ptr(c) for c in cols], C.byref(out)))
+    res.update(passing=int(out.passing), lda_fitted=bool(out.lda_fitted), coef=np.array(out.coef[:], np.float64), eps=float(out.eps))
+    res.update({s: float(getattr(out, s)) for s in FDR_STAGES})
+    return res
+
+
+def kde_build(scores: np.ndarray, decoy: np.ndarray, bins: int = 1000, monotonic: bool = True, bw_factor: float = 1.0, device: int = 0):
+    """kde::Builder::build (kde.rs:83-136) on the device with bw_adjust = x * bw_factor: (PEP per bin, min_score, score_step)."""
+    s = np.ascontiguousarray(scores, np.float64)
+    d = np.ascontiguousarray(decoy, np.uint8)
+    out = np.zeros(int(bins), np.float64)
+    lo, step = C.c_double(), C.c_double()
+    _check(load_library().sage_b200_kde_build(C.c_int(device), _ptr(s), _ptr(d), C.c_uint64(len(s)), C.c_uint64(int(bins)), C.c_int(int(monotonic)),
+                                              C.c_double(bw_factor), _ptr(out), C.byref(lo), C.byref(step)))
+    return out, lo.value, step.value
+
+
+MATH_FUNCTIONS = {"exp": 0, "log1p": 1, "log10": 2}
+
+
+def device_math(function: str, x: np.ndarray, variant: int = -1, device: int = 0) -> np.ndarray:
+    """The device's evaluation of glibc's exp / log1p / log10 (variant 0 FMA builds, 1 uncontracted, -1 the one selected for this host)."""
+    x = np.ascontiguousarray(x, np.float64)
+    out = np.zeros_like(x)
+    _check(load_library().sage_b200_device_math(C.c_int(device), C.c_int(MATH_FUNCTIONS[function]), C.c_int(variant), _ptr(x), C.c_uint64(len(x)), _ptr(out)))
+    return out

@@ -7,6 +7,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
+#include <cub/device/device_reduce.cuh>
 #include <cuda_runtime.h>
 #include <thrust/iterator/counting_iterator.h>
 
@@ -32,6 +33,7 @@
 #include "../../include/sage_b200.h"
 #include "kernels.cuh"
 #include "lfq.cuh"
+#include "fdr.cuh"
 
 using namespace sb;
 
@@ -2511,6 +2513,376 @@ extern "C" int sage_b200_lfq_export(sage_b200_lfq* L, sage_b200_lfq_range* range
     if (touched && L->n_grids) CUDA_TRY(cudaMemcpy(touched, L->d_touched, L->n_grids, cudaMemcpyDeviceToHost));
     return 0;
 }
+
+// ================================================================================== rescoring (linear_discriminant.rs, kde.rs, qvalue.rs; kernels in fdr.cuh)
+// Which build of glibc's exp / log1p / log10 is the host libm (glibc_math.cuh)? Both variants are compared with the host functions bit for bit on
+// a few thousand inputs each, of the kinds rescoring feeds them. 0 = the FMA builds, 1 = the uncontracted ones, -1 = neither matched (the device
+// then uses variant 0 and agrees with the host to about 1e-12 relative).
+static int host_math_variant() {
+    static const int variant = []() {   // initialised once, thread-safe
+        uint64_t st = 0x853C49E6748FEA9Bull;
+        auto next = [&]() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return st; };
+        bool ok[2] = {true, true};
+        for (int i = 0; i < 9000; i++) {
+            const uint64_t u = next();
+            const double unit = (double)(u >> 11) * 0x1p-53;
+            const int f = i % 3;
+            const double x = f == 0 ? -0.5 * (unit * 40.0) * (unit * 40.0) : f == 1 ? unit * 200.0 - 0.5 : unit * (1.0 + (double)(u & 7));
+            volatile double vx = x;
+            const double ref = f == 0 ? std::exp(vx) : f == 1 ? std::log1p(vx) : std::log10(vx);
+            for (int v = 0; v < 2; v++) {
+                const double got = gmath::eval(f, v, x);
+                if (memcmp(&got, &ref, 8)) ok[v] = false;
+            }
+        }
+        return ok[0] ? 0 : (ok[1] ? 1 : -1);
+    }();
+    return variant;
+}
+
+// gauss.rs + the matrix.rs subset it uses, on the host (20 x 20). Row-major.
+struct HostMat {
+    int rows = 0, cols = 0;
+    std::vector<double> a;
+    HostMat(int r, int c) : rows(r), cols(c), a((size_t)r * c, 0.0) {}
+    double& operator()(int i, int j) { return a[(size_t)i * cols + j]; }
+    void swap_rows(int i, int j) { for (int k = 0; k < cols; k++) std::swap((*this)(i, k), (*this)(j, k)); }
+};
+static bool gauss_solve_inner(HostMat left, HostMat right, double eps, std::vector<double>* x) {
+    const int m = left.rows, n = left.cols;
+    for (int i = 0; i < n; i++) left(i, i) += eps;   // fill_zero
+    for (int h = 0, k = 0; h < m && k < n;) {        // echelon
+        int imax = 0;
+        double vmax = -1.7976931348623157e308;
+        for (int i = h; i < m; i++)
+            if (left(i, k) >= vmax) { imax = i; vmax = left(i, k); }
+        if (left(imax, k) == 0.0) { k++; continue; }
+        if (h != imax) { left.swap_rows(h, imax); right.swap_rows(h, imax); }
+        for (int i = h + 1; i < m; i++) {
+            const double factor = left(i, k) / left(h, k);
+            left(i, k) = 0.0;
+            for (int j = k + 1; j < n; j++) left(i, j) -= left(h, j) * factor;
+            for (int j = 0; j < right.cols; j++) right(i, j) -= right(h, j) * factor;
+        }
+        h++;
+        k++;
+    }
+    for (int i = left.rows - 1; i >= 0; i--)          // reduce
+        for (int j = 0; j < left.cols; j++) {
+            const double v = left(i, j);
+            if (v == 0.0) continue;
+            for (int k = j; k < left.cols; k++) left(i, k) /= v;
+            for (int k = 0; k < right.cols; k++) right(i, k) /= v;
+            break;
+        }
+    for (int i = left.rows - 1; i >= 0; i--)          // backfill
+        for (int j = 0; j < left.cols; j++) {
+            if (left(i, j) == 0.0) continue;
+            for (int k = 0; k < i; k++) {
+                const double factor = left(k, j) / left(i, j);
+                for (int h = 0; h < left.cols; h++) left(k, h) -= left(i, h) * factor;
+                for (int h = 0; h < right.cols; h++) right(k, h) -= right(i, h) * factor;
+            }
+            break;
+        }
+    for (int i = 0; i < n; i++)                       // left_solved
+        for (int j = 0; j < n; j++) {
+            const double v = left(i, j);
+            if (i == j ? (v != 1.0 && v != 0.0) : v > 1e-8) return false;
+        }
+    *x = right.a;
+    return true;
+}
+static bool gauss_solve(const HostMat& left, const HostMat& right, std::vector<double>* x, double* eps_used) {
+    for (double eps = 1e-8; eps <= 1.0; eps *= 10.0)
+        if (gauss_solve_inner(left, right, eps, x)) { *eps_used = eps; return true; }
+    return false;
+}
+
+// Device allocations of one rescoring call, released together.
+struct FdrArena {
+    std::vector<void*> ps;
+    ~FdrArena() { for (void* p : ps) cudaFree(p); }
+    template <class T>
+    cudaError_t alloc(T** out, size_t count) {
+        void* p = nullptr;
+        cudaError_t e = cudaMalloc(&p, count ? count * sizeof(T) : 16);
+        if (e == cudaSuccess) { ps.push_back(p); *out = (T*)p; }
+        return e;
+    }
+};
+#define FDR_TRY(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) return fail(SAGE_B200_ECUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); } while (0)
+
+// kde::Builder::build (kde.rs:83-136) with bw_adjust = x * bw_factor, on device scores; d_out_bins[bins], d_moments[4] = std_d, std_t, min, max.
+static int fdr_kde(cudaStream_t st, FdrArena& A, const double* d_scores, const uint8_t* d_decoy, const uint8_t* d_target, uint64_t n, uint32_t bins,
+                   bool monotonic, double bw_factor, bool fma, double* d_out_bins, double* d_moments) {
+    double *d_sel = nullptr, *part[2] = {nullptr, nullptr};
+    uint64_t* d_nsel = nullptr;
+    void* tmp = nullptr;
+    size_t tb = 0;
+    FDR_TRY(A.alloc(&d_sel, 2 * n));
+    FDR_TRY(A.alloc(&d_nsel, 2));
+    FDR_TRY(cub::DeviceSelect::Flagged(nullptr, tb, d_scores, d_decoy, d_sel, d_nsel, (int64_t)n, st));
+    FDR_TRY(A.alloc((char**)&tmp, tb));
+    FDR_TRY(cub::DeviceSelect::Flagged(tmp, tb, d_scores, d_decoy, d_sel, d_nsel, (int64_t)n, st));           // decoys in row order
+    FDR_TRY(cub::DeviceSelect::Flagged(tmp, tb, d_scores, d_target, d_sel + n, d_nsel + 1, (int64_t)n, st));  // targets in row order
+    uint64_t m[2];
+    FDR_TRY(cudaMemcpyAsync(m, d_nsel, 16, cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaStreamSynchronize(st));
+    k_fdr_kde_moments<<<1, 256, 0, st>>>(d_sel, m[0], d_sel + n, m[1], d_scores, n, d_moments);
+    FDR_TRY(cudaGetLastError());
+    double mom[2];
+    FDR_TRY(cudaMemcpyAsync(mom, d_moments, 16, cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaStreamSynchronize(st));
+    double cst[2];
+    uint32_t chunks[2];
+    for (int c = 0; c < 2; c++) {   // Kde::new (kde.rs:21-32): the bandwidth and normalising constant, host libm pow / sqrt
+        const double bw = (mom[c] * std::pow((4.0 / 3.0) / (double)m[c], 1.0 / 5.0)) * bw_factor;
+        cst[c] = std::sqrt(2.0 * M_PI) * bw * (double)m[c];
+        chunks[c] = (uint32_t)((m[c] + KDE_CHUNK - 1) / KDE_CHUNK);
+        if (chunks[c] > 65535) return fail(SAGE_B200_ELIMIT, "kde: %llu samples exceed the %d-chunk grid", (unsigned long long)m[c], 65535);
+        FDR_TRY(A.alloc(&part[c], (size_t)bins * chunks[c]));
+        if (chunks[c]) {
+            const dim3 grid((bins + 127) / 128, chunks[c]);
+            if (fma) k_fdr_kde_bins<true><<<grid, 128, 0, st>>>(d_sel + c * n, m[c], bins, chunks[c], d_moments, bw, part[c]);
+            else k_fdr_kde_bins<false><<<grid, 128, 0, st>>>(d_sel + c * n, m[c], bins, chunks[c], d_moments, bw, part[c]);
+            FDR_TRY(cudaGetLastError());
+        }
+    }
+    const double pi = (double)m[0] / (double)n;
+    k_fdr_kde_pep<<<(bins + 127) / 128, 128, 0, st>>>(part[0], chunks[0], part[1], chunks[1], bins, cst[0], cst[1], pi, monotonic, d_out_bins);
+    FDR_TRY(cudaGetLastError());
+    if (monotonic) k_fdr_kde_monotone<<<1, 1, 0, st>>>(d_out_bins, bins);
+    FDR_TRY(cudaGetLastError());
+    return 0;
+}
+
+static int fdr_device(int device) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(SAGE_B200_ECUDA, "no CUDA device available: sage_b200 has no CPU fallback");
+    if (device < 0 || device >= ndev) return fail(SAGE_B200_EINVAL, "device out of range");
+    FDR_TRY(cudaSetDevice(device));
+    return 0;
+}
+
+extern "C" int sage_b200_kde_build(int device, const double* scores, const uint8_t* decoy, uint64_t n, uint64_t bins, int monotonic, double bw_factor,
+                                   double* out_bins, double* min_score, double* score_step) {
+    if (n == 0 || !scores || !decoy || !out_bins || !min_score || !score_step || bins < 2) return fail(SAGE_B200_EINVAL, "kde_build: bad argument");
+    if (n > (uint64_t)INT32_MAX || bins > (1u << 24)) return fail(SAGE_B200_ELIMIT, "kde_build: n or bins too large");
+    if (int rc = fdr_device(device)) return rc;
+    FdrArena A;
+    double *d_s = nullptr, *d_bins = nullptr, *d_mom = nullptr;
+    uint8_t* d_flags = nullptr;
+    FDR_TRY(A.alloc(&d_s, n));
+    FDR_TRY(A.alloc(&d_flags, 2 * n));
+    FDR_TRY(A.alloc(&d_bins, bins));
+    FDR_TRY(A.alloc(&d_mom, 4));
+    std::vector<uint8_t> flags(2 * n);
+    for (uint64_t i = 0; i < n; i++) { flags[i] = decoy[i] != 0; flags[n + i] = decoy[i] == 0; }
+    FDR_TRY(cudaMemcpy(d_s, scores, 8 * n, cudaMemcpyHostToDevice));
+    FDR_TRY(cudaMemcpy(d_flags, flags.data(), 2 * n, cudaMemcpyHostToDevice));
+    const int v = host_math_variant();
+    if (int rc = fdr_kde(0, A, d_s, d_flags, d_flags + n, n, (uint32_t)bins, monotonic != 0, bw_factor, v != 1, d_bins, d_mom)) return rc;
+    double mom[4];
+    FDR_TRY(cudaMemcpy(out_bins, d_bins, 8 * bins, cudaMemcpyDeviceToHost));
+    FDR_TRY(cudaMemcpy(mom, d_mom, 32, cudaMemcpyDeviceToHost));
+    *min_score = mom[2];
+    *score_step = (mom[3] - mom[2]) / (double)(bins - 1);
+    return 0;
+}
+
+extern "C" int sage_b200_device_math(int device, int function, int variant, const double* x, uint64_t n, double* out) {
+    if (function < 0 || function > 2 || variant < -1 || variant > 1 || (n && (!x || !out))) return fail(SAGE_B200_EINVAL, "device_math: bad argument");
+    if (n == 0) return 0;
+    if (int rc = fdr_device(device)) return rc;
+    if (variant == -1) variant = host_math_variant() == 1 ? 1 : 0;
+    FdrArena A;
+    double *dx = nullptr, *dy = nullptr;
+    FDR_TRY(A.alloc(&dx, n));
+    FDR_TRY(A.alloc(&dy, n));
+    FDR_TRY(cudaMemcpy(dx, x, 8 * n, cudaMemcpyHostToDevice));
+    const unsigned g = (unsigned)((n + 255) / 256);
+    if (variant == 0) k_device_math<true><<<g, 256>>>(function, dx, n, dy);
+    else k_device_math<false><<<g, 256>>>(function, dx, n, dy);
+    FDR_TRY(cudaGetLastError());
+    FDR_TRY(cudaMemcpy(out, dy, 8 * n, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+struct MinF {
+    __device__ float operator()(float a, float b) const { return fminf(a, b); }
+};
+
+// spectrum_fdr (runner.rs:280-291): score_psms, the heuristic fallback when it returns None, the descending sort and spectrum_q_value.
+extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p, const sage_b200_feature* rows, uint64_t n, const float* aligned_rt,
+                                      const float* delta_rt_model, const float* delta_ims_model, sage_b200_fdr_out* out) {
+    if (!p || !out || (n && (!rows || !out->discriminant_score || !out->posterior_error || !out->spectrum_q || !out->order)))
+        return fail(SAGE_B200_EINVAL, "spectrum_fdr: null argument");
+    const int kind = p->precursor_tol.kind;
+    if (kind == SAGE_B200_TOL_PCT) return fail(SAGE_B200_EINVAL, "spectrum_fdr: Pct tolerance is never used on precursor m/z (linear_discriminant.rs:142)");
+    if (kind != SAGE_B200_TOL_PPM && kind != SAGE_B200_TOL_DA) return fail(SAGE_B200_EINVAL, "spectrum_fdr: unknown tolerance kind %d", kind);
+    if (n > (uint64_t)INT32_MAX) return fail(SAGE_B200_ELIMIT, "spectrum_fdr: more than 2^31 - 1 rows (qvalue.rs counts in i32)");
+    out->passing = 0;
+    out->lda_fitted = 0;
+    memset(out->coef, 0, sizeof out->coef);
+    out->eps = 0.0;
+    out->ms_mass_kde = out->ms_features = out->ms_lda = out->ms_discriminant_kde = out->ms_sort_q = out->ms_total = 0.0f;
+    if (n == 0) return 0;
+    if (int rc = fdr_device(device)) return rc;
+    if (n > (uint64_t)65535 * KDE_CHUNK) return fail(SAGE_B200_ELIMIT, "spectrum_fdr: more than 65535 KDE chunks of %d rows", KDE_CHUNK);
+    const int variant = host_math_variant();
+    const bool fma = variant != 1;
+    // linear_discriminant.rs:146-150: bandwidth factor and bin count of the mass-error KDE, in the tolerance's f32
+    const float lo = p->precursor_tol.lo, hi = p->precursor_tol.hi;
+    const float span = std::ceil(std::fmax(hi - lo, kind == SAGE_B200_TOL_PPM ? 100.0f : 1000.0f));
+    const double bw_factor = kind == SAGE_B200_TOL_PPM ? 2.0 : 0.1;
+    const float span_abs = std::fabs(span);
+    if (!(span_abs < 16777216.0f)) return fail(SAGE_B200_ELIMIT, "spectrum_fdr: tolerance span gives too many mass-error bins");
+    const uint32_t mbins = (uint32_t)span_abs;
+    {   // everything below stays allocated until the call returns: fail with ELIMIT before allocating when it cannot fit
+        size_t free_b = 0, total_b = 0;
+        FDR_TRY(cudaMemGetInfo(&free_b, &total_b));
+        // per row: the rows, mass errors, flags, feature matrix, f64 discriminants, five f32 and six u32 work columns, the three optional
+        // columns, the class-compacted samples of both KDEs (16 bytes each) and the radix sort's temporary storage; then both KDEs' partial sums
+        const uint64_t per_row = sizeof(sage_b200_feature) + 8 + 2 + 8 * FDR_FEATURES + 8 + 4 * 5 + 4 * 6 + 4 * 3 + 16 * 2 + 16;
+        const uint64_t partial = 8ull * ((uint64_t)mbins + 1000) * (n / KDE_CHUNK + 2);
+        const uint64_t need = n * per_row + partial + (64ull << 20);
+        if (need > free_b) return fail(SAGE_B200_ELIMIT, "spectrum_fdr: %llu rows need about %llu bytes of device memory, %llu free", (unsigned long long)n,
+                                       (unsigned long long)need, (unsigned long long)free_b);
+    }
+
+    FdrArena A;
+    cudaStream_t st = 0;
+    cudaEvent_t ev[6] = {};
+    struct EvFree { cudaEvent_t* e; ~EvFree() { for (int i = 0; i < 6; i++) if (e[i]) cudaEventDestroy(e[i]); } } ev_free{ev};
+    for (auto& e : ev) FDR_TRY(cudaEventCreate(&e));
+    sage_b200_feature* d_rows = nullptr;
+    double *d_mass = nullptr, *d_mbins = nullptr, *d_mmom = nullptr, *d_X = nullptr, *d_means = nullptr, *d_scatter = nullptr, *d_coef = nullptr,
+           *d_disc = nullptr, *d_dbins = nullptr, *d_dmom = nullptr;
+    uint8_t* d_flags = nullptr;
+    uint64_t* d_counts = nullptr;
+    float *d_disc32 = nullptr, *d_pep = nullptr, *d_q = nullptr, *d_rq = nullptr, *d_rqmin = nullptr, *d_cols[3] = {nullptr, nullptr, nullptr};
+    uint32_t *d_key = nullptr, *d_key2 = nullptr, *d_idx = nullptr, *d_order = nullptr, *d_isdec = nullptr, *d_dscan = nullptr;
+    unsigned long long* d_passing = nullptr;
+    FDR_TRY(A.alloc(&d_rows, n));
+    FDR_TRY(A.alloc(&d_mass, n));
+    FDR_TRY(A.alloc(&d_flags, 2 * n));
+    FDR_TRY(A.alloc(&d_mbins, mbins));
+    FDR_TRY(A.alloc(&d_mmom, 4));
+    FDR_TRY(A.alloc(&d_X, n * FDR_FEATURES));
+    FDR_TRY(A.alloc(&d_means, 2 * FDR_FEATURES));
+    FDR_TRY(A.alloc(&d_scatter, 2 * FDR_FEATURES * FDR_FEATURES));
+    FDR_TRY(A.alloc(&d_counts, 2));
+    FDR_TRY(A.alloc(&d_coef, FDR_FEATURES));
+    FDR_TRY(A.alloc(&d_disc, n));
+    FDR_TRY(A.alloc(&d_dbins, 1000));
+    FDR_TRY(A.alloc(&d_dmom, 4));
+    FDR_TRY(A.alloc(&d_disc32, n));
+    FDR_TRY(A.alloc(&d_pep, n));
+    FDR_TRY(A.alloc(&d_q, n));
+    FDR_TRY(A.alloc(&d_rq, n));
+    FDR_TRY(A.alloc(&d_rqmin, n));
+    FDR_TRY(A.alloc(&d_key, n));
+    FDR_TRY(A.alloc(&d_key2, n));
+    FDR_TRY(A.alloc(&d_idx, n));
+    FDR_TRY(A.alloc(&d_order, n));
+    FDR_TRY(A.alloc(&d_isdec, n));
+    FDR_TRY(A.alloc(&d_dscan, n));
+    FDR_TRY(A.alloc(&d_passing, 1));
+    const float* cols_h[3] = {aligned_rt, delta_rt_model, delta_ims_model};
+    for (int c = 0; c < 3; c++)
+        if (cols_h[c]) {
+            FDR_TRY(A.alloc(&d_cols[c], n));
+            FDR_TRY(cudaMemcpy(d_cols[c], cols_h[c], 4 * n, cudaMemcpyHostToDevice));
+        }
+    FDR_TRY(cudaMemcpy(d_rows, rows, sizeof(sage_b200_feature) * n, cudaMemcpyHostToDevice));
+    const unsigned g = (unsigned)((n + 255) / 256);
+
+    // 1. mass-error KDE (linear_discriminant.rs:140-158)
+    FDR_TRY(cudaEventRecord(ev[0], st));
+    k_fdr_mass<<<g, 256, 0, st>>>(d_rows, n, kind, d_mass, d_flags, d_flags + n);
+    FDR_TRY(cudaGetLastError());
+    if (int rc = fdr_kde(st, A, d_mass, d_flags, d_flags + n, n, mbins, false, bw_factor, fma, d_mbins, d_mmom)) return rc;
+    FDR_TRY(cudaEventRecord(ev[1], st));
+    // 2. feature rows (linear_discriminant.rs:162-193)
+    const FdrColumns cols{d_cols[0], d_cols[1], d_cols[2]};
+    if (fma) k_fdr_features<true><<<g, 256, 0, st>>>(d_rows, n, cols, d_mass, d_mbins, mbins, d_mmom, d_X);
+    else k_fdr_features<false><<<g, 256, 0, st>>>(d_rows, n, cols, d_mass, d_mbins, mbins, d_mmom, d_X);
+    FDR_TRY(cudaGetLastError());
+    FDR_TRY(cudaEventRecord(ev[2], st));
+    // 3. LDA class sums and scatter on the device, Gauss::solve on the host (linear_discriminant.rs:63-124, 195-208)
+    k_fdr_lda<<<2, 256, 0, st>>>(d_X, d_flags, n, d_means, d_scatter, d_counts);
+    FDR_TRY(cudaGetLastError());
+    std::vector<double> means(2 * FDR_FEATURES), scatter(2 * FDR_FEATURES * FDR_FEATURES);
+    uint64_t counts[2];
+    FDR_TRY(cudaMemcpyAsync(means.data(), d_means, 8 * means.size(), cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaMemcpyAsync(scatter.data(), d_scatter, 8 * scatter.size(), cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaMemcpyAsync(counts, d_counts, 16, cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaStreamSynchronize(st));
+    bool fitted = false;
+    if (counts[0] != 0 && counts[1] != 0) {
+        HostMat sw(FDR_FEATURES, FDR_FEATURES), rhs(FDR_FEATURES, 1);
+        for (int c = 0; c < 2; c++)   // scatter_within = (0 + S_decoy / n_decoy) + S_target / n_target
+            for (int e = 0; e < FDR_FEATURES * FDR_FEATURES; e++) sw.a[e] += scatter[(size_t)c * FDR_FEATURES * FDR_FEATURES + e] / (double)counts[c];
+        for (int j = 0; j < FDR_FEATURES; j++) rhs.a[j] = means[FDR_FEATURES + j] - means[j];
+        std::vector<double> coef;
+        double eps = 0.0;
+        if (gauss_solve(sw, rhs, &coef, &eps)) {
+            for (int j = 0; j < FDR_FEATURES; j++) out->coef[j] = coef[j];
+            out->eps = eps;
+            fitted = true;
+            for (double w : coef) fitted = fitted && std::isfinite(w);   // linear_discriminant.rs:196-208
+        }
+    }
+    FDR_TRY(cudaEventRecord(ev[3], st));
+    // 4. projection, discriminant KDE and posterior errors (linear_discriminant.rs:209-228), or the fallback (runner.rs:284-287)
+    if (fitted) {
+        FDR_TRY(cudaMemcpyAsync(d_coef, out->coef, 8 * FDR_FEATURES, cudaMemcpyHostToDevice, st));
+        k_fdr_project<<<g, 256, 0, st>>>(d_X, n, d_coef, d_disc, d_disc32);
+        FDR_TRY(cudaGetLastError());
+        if (int rc = fdr_kde(st, A, d_disc, d_flags, d_flags + n, n, 1000, true, 1.0, fma, d_dbins, d_dmom)) return rc;
+        if (fma) k_fdr_pep<true><<<g, 256, 0, st>>>(d_disc, n, d_dbins, 1000, d_dmom, d_pep);
+        else k_fdr_pep<false><<<g, 256, 0, st>>>(d_disc, n, d_dbins, 1000, d_dmom, d_pep);
+    } else {
+        k_fdr_fallback<<<g, 256, 0, st>>>(d_rows, n, d_disc32, d_pep);
+    }
+    FDR_TRY(cudaGetLastError());
+    FDR_TRY(cudaEventRecord(ev[4], st));
+    // 5. stable descending sort (ties by input row) and spectrum_q_value (qvalue.rs)
+    k_fdr_sort_key<<<g, 256, 0, st>>>(d_disc32, n, d_key, d_idx);
+    FDR_TRY(cudaGetLastError());
+    size_t tb = 0, tb2 = 0, tb3 = 0;
+    FDR_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key2, d_idx, d_order, (int)n, 0, 32, st));
+    FDR_TRY(cub::DeviceScan::InclusiveSum(nullptr, tb2, d_isdec, d_dscan, (int)n, st));
+    FDR_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
+    char* tmp = nullptr;
+    FDR_TRY(A.alloc(&tmp, std::max(tb, std::max(tb2, tb3))));
+    FDR_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, d_key, d_key2, d_idx, d_order, (int)n, 0, 32, st));
+    k_fdr_sorted_decoy<<<g, 256, 0, st>>>(d_rows, d_order, n, d_isdec);
+    FDR_TRY(cudaGetLastError());
+    FDR_TRY(cub::DeviceScan::InclusiveSum(tmp, tb2, d_isdec, d_dscan, (int)n, st));
+    k_fdr_q_raw<<<g, 256, 0, st>>>(d_dscan, n, d_rq);
+    FDR_TRY(cudaGetLastError());
+    FDR_TRY(cub::DeviceScan::InclusiveScan(tmp, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
+    FDR_TRY(cudaMemsetAsync(d_passing, 0, 8, st));
+    k_fdr_q_out<<<g, 256, 0, st>>>(d_rqmin, d_order, n, d_q, d_passing);
+    FDR_TRY(cudaGetLastError());
+    FDR_TRY(cudaEventRecord(ev[5], st));
+    unsigned long long passing = 0;
+    FDR_TRY(cudaMemcpyAsync(out->discriminant_score, d_disc32, 4 * n, cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaMemcpyAsync(out->posterior_error, d_pep, 4 * n, cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaMemcpyAsync(out->spectrum_q, d_q, 4 * n, cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaMemcpyAsync(out->order, d_order, 4 * n, cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaMemcpyAsync(&passing, d_passing, 8, cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaStreamSynchronize(st));
+    out->passing = passing;
+    out->lda_fitted = fitted ? 1 : 0;
+    float* ms[5] = {&out->ms_mass_kde, &out->ms_features, &out->ms_lda, &out->ms_discriminant_kde, &out->ms_sort_q};
+    for (int i = 0; i < 5; i++) FDR_TRY(cudaEventElapsedTime(ms[i], ev[i], ev[i + 1]));
+    FDR_TRY(cudaEventElapsedTime(&out->ms_total, ev[0], ev[5]));
+    return 0;
+}
+#undef FDR_TRY
 
 #if SAGE_B200_PHASE_CLOCKS
 // variant builds only (not declared in the header): cycles per k_score phase summed over CTAs since the last reset

@@ -396,3 +396,49 @@ def make_ms1_runs(pep: Peptides, n_ids: int = 30_000, n_files: int = 4, spectra_
     batch = Ms1Batch(np.concatenate(offs), np.concatenate(masses), np.concatenate(intens), np.array(fids, np.uint32), np.array(ssts, np.float32),
                      np.concatenate(mobs) if mobility else None)
     return dict(features=feats, alignments=align, batch=batch, ids=ids, charge=charge)
+
+
+def make_psms(n: int, seed: int = 0x0FD2, decoy_fraction: float = 0.3, true_fraction: float = 0.5, ppm: float = 20.0, ims: bool = False,
+              rt_range: float = 60.0) -> np.ndarray:
+    """Seeded Feature rows (FEATURE_DTYPE) shaped like a search's output, for rescoring (spectrum_fdr). A `decoy_fraction` of the rows are decoys;
+    the targets are a mix of true matches (`true_fraction` of them: higher hyperscore, more matched peaks, a mass error centred on 0) and
+    false matches drawn like decoys. Mass errors are within +-`ppm`; `ims` fills the mobility column (else 0, as without mobility data)."""
+    from .api import FEATURE_DTYPE
+    rng = np.random.default_rng(seed)
+    out = np.zeros(n, FEATURE_DTYPE)
+    decoy = rng.random(n) < decoy_fraction
+    true = ~decoy & (rng.random(n) < true_fraction)
+    plen = rng.integers(7, 31, n).astype(np.uint32)
+    matched = np.where(true, rng.integers(6, 30, n), rng.integers(1, 12, n)).astype(np.uint32)
+    longest_b = np.minimum(rng.integers(0, 10, n) + true * rng.integers(0, 8, n), plen - 1).astype(np.uint32)
+    longest_y = np.minimum(rng.integers(0, 10, n) + true * rng.integers(0, 12, n), plen - 1).astype(np.uint32)
+    hyper = np.where(true, rng.normal(40.0, 8.0, n), rng.normal(18.0, 6.0, n)).clip(0.5, None)
+    delta_next = (hyper * np.where(true, rng.uniform(0.05, 0.6, n), rng.uniform(0.0, 0.15, n)))
+    charge = rng.integers(2, 5, n).astype(np.uint32)
+    calc = rng.uniform(700.0, 4000.0, n).astype(np.float32)
+    dppm = np.where(true, rng.normal(0.0, ppm / 8.0, n), rng.uniform(-ppm, ppm, n)).clip(-ppm, ppm).astype(np.float32)
+    exp = (calc.astype(np.float64) * (1.0 + dppm.astype(np.float64) * 1e-6)).astype(np.float32)
+    out["spectrum"] = np.arange(n, dtype=np.uint32)
+    out["peptide_idx"] = rng.integers(0, 1 << 20, n).astype(np.uint32)
+    out["peptide_len"] = plen
+    out["rank"] = np.where(rng.random(n) < 0.8, 1, 2).astype(np.uint32)
+    out["label"] = np.where(decoy, -1, 1).astype(np.int32)
+    out["expmass"], out["calcmass"] = exp, calc
+    out["charge"] = charge
+    out["rt"] = rng.uniform(0.0, rt_range, n).astype(np.float32)
+    out["ims"] = rng.uniform(0.6, 1.4, n).astype(np.float32) if ims else np.float32(0)
+    out["delta_mass"] = np.abs(dppm)
+    out["isotope_error"] = np.where(rng.random(n) < 0.05, 1.0, 0.0).astype(np.float32)
+    out["average_ppm"] = np.abs(np.where(true, rng.normal(0.0, 3.0, n), rng.uniform(-10.0, 10.0, n))).astype(np.float32)
+    out["hyperscore"] = hyper
+    out["delta_next"] = delta_next
+    out["delta_best"] = np.where(out["rank"] == 1, 0.0, delta_next * 0.5)
+    out["matched_peaks"] = matched
+    out["longest_b"], out["longest_y"] = longest_b, longest_y
+    out["longest_y_pct"] = (longest_y.astype(np.float32) / plen.astype(np.float32)).astype(np.float32)
+    out["missed_cleavages"] = rng.integers(0, 2, n).astype(np.uint32)
+    out["matched_intensity_pct"] = np.where(true, rng.uniform(20.0, 80.0, n), rng.uniform(1.0, 30.0, n)).astype(np.float32)
+    out["scored_candidates"] = rng.integers(1, 5000, n).astype(np.uint32)
+    out["ms2_intensity"] = rng.uniform(1e3, 1e6, n).astype(np.float32)
+    out["poisson"] = np.where(true, -rng.uniform(5.0, 20.0, n), -rng.uniform(0.0, 4.0, n))
+    return out
