@@ -360,6 +360,35 @@ int sage_b200_kde_build(int device, const double* scores, const uint8_t* decoy, 
  * 1 = the uncontracted builds, -1 = the variant the library selected for this host's libm. */
 int sage_b200_device_math(int device, int function, int variant, const double* x, uint64_t n, double* out);
 
+/* ---------------------------------------------------------------------------------------------------------------------------------------------
+ * Retention-time alignment and RT / mobility prediction (runner.rs:513-531 predict_rt): the ascending poisson sort and interim
+ * qvalue::spectrum_q_value, retention_alignment::global_alignment, retention_model::predict and mobility_model::predict (regression.rs's
+ * LinearRegression::fit). Every output is reproducible bit for bit under the orders of DESIGN.md §11. The rows are not reordered.
+ */
+typedef struct {
+    float* aligned_rt;                /* [n] Feature::aligned_rt */
+    float* predicted_rt;              /* [n] clamp(0, 1); 0.0 when the RT model was not fitted */
+    float* delta_rt_model;            /* [n] |aligned_rt - predicted_rt|; 0.999 when the RT model was not fitted */
+    float* predicted_ims;             /* [n] clamp(0, 2); 0.0 when the mobility model was not fitted */
+    float* delta_ims_model;           /* [n] |ims - predicted_ims|; 0.999 when the mobility model was not fitted */
+    float* spectrum_q;                /* [n] or NULL: the interim q-values, computed over the ascending-poisson order, indexed like the rows */
+    sage_b200_alignment* alignments;  /* [n_files] global_alignment's result, file_id = position; the input of sage_b200_lfq_create */
+    uint64_t training_rows;           /* rows with label == 1 && q <= 0.01 */
+    uint64_t aligned_peptides;        /* matrix rows kept (peptides whose mean normalised RT is_normal) */
+    int32_t rt_fitted;                /* 0: LinearRegression::fit returned None (no training rows, or Gauss::solve failed at every eps) */
+    double rt_r2, rt_eps, rt_beta[69];/* r2 = 1 - sse / y_var, the Gauss::solve ridge that succeeded, the coefficients; 0 when not fitted */
+    int32_t ims_fitted;
+    double ims_r2, ims_eps, ims_beta[100];
+    float ms_sort_q, ms_alignment, ms_rt_model, ms_ims_model, ms_total;   /* CUDA-event stage times of the call (the host solves included) */
+} sage_b200_rt_out;
+/* rows: the Feature rows in the caller's order; file_id[n] < n_files; peptides: the table the db was built from (residue_offsets, sequence and
+ * monoisotopic are read). EINVAL for a file_id >= n_files, a peptide_idx outside the db, n_files == 0 with rows, a peptide table of another size
+ * than the db's, or a residue byte outside 'A'..'Z' in a referenced peptide; ELIMIT beyond 2^31 - 1 rows or when the work buffers (the
+ * peptide x file matrix the largest) do not fit the device's free memory (checked before allocating). n == 0: every alignment is
+ * {0, 1, 0} and nothing is fitted. */
+int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_peptides* peptides, const sage_b200_feature* rows, const uint32_t* file_id, uint64_t n,
+                         uint64_t n_files, sage_b200_rt_out* out);
+
 /* Page-locked host buffers: spectra/feature arrays placed here are copied by DMA without a staging memcpy. */
 void* sage_b200_host_alloc(size_t bytes);
 /* The same for a batch sage_b200_score_batch_multi cuts into n_devices contiguous blocks: the i-th of n equal parts of the buffer is placed on the

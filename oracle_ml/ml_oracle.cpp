@@ -10,11 +10,20 @@
 // with host libm (exp, log1p, log10, log1pf, pow, sqrt) and -ffp-contract=off, in the orders DESIGN.md §10 defines where the reference leaves
 // them to rayon: Kde::pdf folds chunks of KDE_CHUNK samples from 0.0 and adds the chunk sums in order from -0.0; the unstable sort breaks ties
 // by input row. f64 Sum starts from -0.0 (the neutral element of current Rust's `impl Sum for f64`). Shares no code with the library.
+//
+// Also restates the runner's predict_rt stage (runner.rs:513-531), the authority for sage_b200/csrc/rt.cuh:
+//   retention_alignment.rs  global_alignment
+//   regression.rs           LinearRegression::fit
+//   retention_model.rs      RetentionModel::embed / fit / predict
+//   mobility_model.rs       MobilityModel::embed / fit / predict
+// in the orders DESIGN.md §11 defines: poisson ties by input row, ordered maps (ascending PeptideIx, ascending file), fit chunks of RT_CHUNK
+// training rows merged in order.
 #include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
+#include <map>
 #include <thread>
 #include <vector>
 
@@ -224,6 +233,169 @@ double clamp_sqrt(double v) {   // f64::clamp(0.001, 0.999).sqrt()
 
 }  // namespace
 
+namespace {
+
+constexpr uint64_t RT_CHUNK = 1024;
+const char VALID_AA[] = "ACDEFGHIKLMNPQRSTVWYUO";   // mass.rs:59-62
+constexpr size_t N_AA = 22;
+constexpr int RT_D = 22 * 3 + 3, IMS_D = 22 * 4 + 12;
+
+struct AaMap {   // retention_model.rs:64-67: letters outside VALID_AA keep the map's initial 0
+    size_t m[26];
+    AaMap() {
+        for (size_t& v : m) v = 0;
+        for (size_t i = 0; i < N_AA; i++) m[VALID_AA[i] - 'A'] = i;
+    }
+};
+const AaMap AA;
+
+// retention_model.rs:42-59
+void rt_embed(const uint8_t* seq, size_t len, float mono, double* e) {
+    const size_t NT = N_AA, CT = N_AA * 2, LEN = RT_D - 3, MASS = RT_D - 2, ICPT = RT_D - 1;
+    std::fill(e, e + RT_D, 0.0);
+    const size_t cterm = len >= 3 ? len - 3 : 0;
+    for (size_t i = 0; i < len; i++) {
+        const size_t idx = AA.m[seq[i] - 'A'];
+        e[idx] += 1.0;
+        if (i == 0 || i == 1) e[NT + idx] += 1.0;
+        else if (i == cterm || i == cterm + 1) e[CT + idx] += 1.0;
+    }
+    e[LEN] = (double)len;
+    e[MASS] = std::log1p((double)mono);
+    e[ICPT] = 1.0;
+}
+
+bool contains(const size_t* set, size_t n, size_t x) {
+    for (size_t i = 0; i < n; i++)
+        if (set[i] == x) return true;
+    return false;
+}
+
+// mobility_model.rs:97-149, the group constants as letter offsets compared with the VALID_AA position, as written
+void ims_embed(const uint8_t* seq, size_t len, float mono, uint8_t charge, double* e) {
+    const size_t F = IMS_D, PCT = N_AA, NT = N_AA * 2, CT = N_AA * 3;
+    const size_t BULKY[6] = {'L' - 'A', 'V' - 'A', 'I' - 'A', 'F' - 'A', 'W' - 'A', 'Y' - 'A'};
+    const size_t UC_POLAR[4] = {'S' - 'A', 'T' - 'A', 'N' - 'A', 'Q' - 'A'};
+    const size_t POSITIVE[3] = {'R' - 'A', 'K' - 'A', 'H' - 'A'};
+    const size_t NEGATIVE[2] = {'D' - 'A', 'E' - 'A'};
+    const size_t TINY[3] = {'G' - 'A', 'A' - 'A', 'S' - 'A'};
+    const size_t BRANCHED[3] = {'L' - 'A', 'I' - 'A', 'V' - 'A'};
+    std::fill(e, e + IMS_D, 0.0);
+    const size_t cterm = len >= 3 ? len - 3 : 0;
+    const double pep_length = (double)len;
+    for (size_t i = 0; i < len; i++) {
+        const size_t idx = AA.m[seq[i] - 'A'];
+        e[idx] += 1.0;
+        if (i == 0 || i == 1) e[NT + idx] += 1.0;
+        else if (i > cterm) e[CT + idx] += 1.0;
+        if (contains(BULKY, 6, idx)) e[F - 9] += 1.0;
+        if (contains(UC_POLAR, 4, idx)) e[F - 10] += 1.0;
+        if (contains(POSITIVE, 3, idx)) e[F - 8] += 1.0;
+        if (contains(NEGATIVE, 2, idx)) e[F - 7] += 1.0;
+        if (contains(TINY, 3, idx)) e[F - 11] += 1.0;
+        if (contains(BRANCHED, 3, idx)) e[F - 12] += 1.0;
+    }
+    for (size_t idx = 0; idx < N_AA; idx++) e[PCT + idx] = e[idx] / pep_length;
+    const double z = (double)charge;
+    e[F - 5] = z;
+    e[F - 6] = 1. / z;
+    e[F - 3] = (double)len;
+    e[F - 2] = (double)mono / 1000.0;
+    e[F - 4] = ((double)mono / z) / 1000.0;
+    e[F - 1] = 1.0;
+}
+
+struct Fit {
+    bool ok = false;
+    std::vector<double> beta;
+    double r2 = 0, eps = 0;
+};
+
+// regression.rs:72-117 over items 0..n (already filtered), embed(i, row) and target(i). The rayon fold/reduce is chunks of RT_CHUNK items, each
+// from Acc::zero, merged as ((0 + A_0) + A_1) + ...; the SSE sum is chunk sums from -0.0 added in order from -0.0. Chunks run on `threads`.
+template <class Embed, class Target>
+Fit linreg_fit(uint64_t n, int d, Embed embed, Target target, int threads) {
+    Fit out;
+    if (n == 0) return out;
+    const uint64_t chunks = (n + RT_CHUNK - 1) / RT_CHUNK;
+    const size_t acc_len = (size_t)d * d + d + 2;
+    std::vector<double> part(chunks * acc_len, 0.0);
+    auto run = [&](auto&& body) {
+        std::vector<std::thread> pool;
+        for (int w = 0; w < threads; w++)
+            pool.emplace_back([&, w]() {
+                for (uint64_t c = (uint64_t)w; c < chunks; c += (uint64_t)threads) body(c);
+            });
+        for (auto& t : pool) t.join();
+    };
+    run([&](uint64_t c) {   // Acc::add_row over the chunk, the full d x d product as written
+        double* acc = &part[c * acc_len];
+        double *cov = acc, *b = acc + (size_t)d * d;
+        std::vector<double> row(d);
+        for (uint64_t i = c * RT_CHUNK; i < std::min(n, (c + 1) * RT_CHUNK); i++) {
+            embed(i, row.data());
+            const double y = target(i);
+            for (int j = 0; j < d; j++) {
+                const double rj = row[j];
+                b[j] += rj * y;
+                for (int k = 0; k < d; k++) cov[(size_t)j * d + k] += rj * row[k];
+            }
+            acc[acc_len - 2] += y;
+            acc[acc_len - 1] += y * y;
+        }
+    });
+    std::vector<double> tot(acc_len, 0.0);
+    for (uint64_t c = 0; c < chunks; c++)
+        for (size_t a = 0; a < acc_len; a++) tot[a] += part[c * acc_len + a];
+    const double nf = (double)n, y_mean = tot[acc_len - 2] / nf, y_var = tot[acc_len - 1] - nf * y_mean * y_mean;
+    Mat cov(d, d), rhs(d, 1);
+    std::copy(tot.begin(), tot.begin() + (size_t)d * d, cov.a.begin());
+    std::copy(tot.begin() + (size_t)d * d, tot.begin() + (size_t)d * d + d, rhs.a.begin());
+    std::vector<double> beta;
+    for (double eps = 1e-8; eps <= 1.0; eps *= 10.0)   // Gauss::solve
+        if (solve_inner(cov, rhs, eps, &beta)) {
+            out.ok = true;
+            out.eps = eps;
+            break;
+        }
+    if (!out.ok) return out;
+    std::vector<double> csse(chunks);
+    run([&](uint64_t c) {
+        std::vector<double> row(d);
+        double s = -0.0;
+        for (uint64_t i = c * RT_CHUNK; i < std::min(n, (c + 1) * RT_CHUNK); i++) {
+            embed(i, row.data());
+            double pred = -0.0;
+            for (int j = 0; j < d; j++) pred += row[j] * beta[j];
+            const double diff = pred - target(i);
+            s += diff * diff;
+        }
+        csse[c] = s;
+    });
+    double sse = -0.0;
+    for (double v : csse) sse += v;
+    out.r2 = 1.0 - sse / y_var;
+    out.beta = beta;
+    return out;
+}
+
+double rust_min(double a, double b) {   // f64::min; -0.0 kept over +0.0
+    if (std::isnan(a)) return b;
+    if (std::isnan(b)) return a;
+    if (a < b) return a;
+    if (b < a) return b;
+    return std::signbit(a) ? a : b;
+}
+
+uint32_t ceil_as_u32(float rt) {   // `rt.ceil() as u32`, saturating
+    const float c = std::ceil(rt);
+    if (!(c >= 0.0f)) return 0;
+    if (c >= 4294967296.0f) return UINT32_MAX;
+    return (uint32_t)c;
+}
+
+}  // namespace
+
 extern "C" {
 
 int mo_kde_build(const double* scores, const uint8_t* decoy, uint64_t n, uint64_t bins, int monotonic, double bw_factor, int threads, double* out_bins,
@@ -337,6 +509,172 @@ double mo_spectrum_fdr(int kind, float lo, float hi, const void* rows_v, uint64_
     }
     *passing = pass;
     std::copy(idx.begin(), idx.end(), order);
+    return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+}
+
+
+// RetentionModel::embed (model 0, charge ignored) or MobilityModel::embed (model 1) of one peptide into out[69] / out[100].
+void mo_rt_embed(int model, const uint8_t* seq, uint64_t len, float mono, uint32_t charge, double* out) {
+    if (model == 0) rt_embed(seq, len, mono, out);
+    else ims_embed(seq, len, mono, (uint8_t)charge, out);
+}
+
+// LinearRegression::fit on a given row-major [n][d] matrix and targets: 1 with beta[d], r2 and eps, or 0 for None.
+int mo_linreg_fit(const double* X, const double* y, uint64_t n, int d, int threads, double* beta, double* r2, double* eps) {
+    const Fit f = linreg_fit(n, d, [&](uint64_t i, double* row) { std::copy(X + i * d, X + (i + 1) * d, row); }, [&](uint64_t i) { return y[i]; },
+                             std::max(1, threads));
+    if (!f.ok) return 0;
+    std::copy(f.beta.begin(), f.beta.end(), beta);
+    *r2 = f.r2;
+    *eps = f.eps;
+    return 1;
+}
+
+// runner.rs:513-531 predict_rt. Peptides: off[n_pep + 1], seq, mono. cols: aligned_rt, predicted_rt, delta_rt_model, predicted_ims,
+// delta_ims_model, spectrum_q (indexed like the rows, each [n]). align[n_files][3] = max_rt, slope, intercept. stats = training rows, matrix rows
+// kept. fitted / r2 / eps: [2] (RT, mobility). Returns the wall time in seconds.
+double mo_predict_rt(const uint32_t* off, const uint8_t* seq, const float* mono, const void* rows_v, const uint32_t* file_id, uint64_t n, uint64_t n_files,
+                     int threads, float* aligned_rt, float* predicted_rt, float* delta_rt, float* predicted_ims, float* delta_ims, float* spectrum_q, float* align,
+                     uint64_t* stats, int32_t* fitted, double* r2, double* eps, double* rt_beta, double* ims_beta) {
+    const auto t0 = std::chrono::steady_clock::now();
+    const Row* rows = (const Row*)rows_v;
+    threads = std::max(1, threads);
+    // par_sort_unstable_by(|a, b| a.poisson.total_cmp(&b.poisson)), ties by input row
+    auto total_key = [&](uint64_t i) {
+        int64_t b;
+        memcpy(&b, &rows[i].poisson, 8);
+        return b ^ (int64_t)((uint64_t)(b >> 63) >> 1);
+    };
+    std::vector<uint32_t> order(n);
+    for (uint64_t i = 0; i < n; i++) order[i] = (uint32_t)i;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return total_key(a) < total_key(b); });
+    // spectrum_q_value over that order
+    std::vector<float> qs(n), q(n);
+    int32_t dec = 1, tar = 0;
+    for (uint64_t p = 0; p < n; p++) {
+        if (rows[order[p]].label == -1) dec++;
+        else tar++;
+        qs[p] = (float)dec / (float)tar;
+    }
+    float q_min = 1.0f;
+    for (uint64_t p = n; p-- > 0;) {
+        q_min = std::fmin(q_min, qs[p]);
+        q[order[p]] = q_min;
+    }
+    if (spectrum_q) std::copy(q.begin(), q.end(), spectrum_q);
+    std::vector<uint32_t> train;   // the training filter, in poisson order
+    for (uint64_t p = 0; p < n; p++)
+        if (rows[order[p]].label == 1 && q[order[p]] <= 0.01f) train.push_back(order[p]);
+
+    // global_alignment
+    std::vector<uint32_t> max_u(n_files, 0);
+    for (uint64_t i = 0; i < n; i++) max_u[file_id[i]] = std::max(max_u[file_id[i]], ceil_as_u32(rows[i].rt));
+    std::vector<double> max_rt(n_files);
+    for (uint64_t f = 0; f < n_files; f++) max_rt[f] = (double)max_u[f];
+    std::map<uint32_t, std::map<uint64_t, double>> rts;
+    for (uint32_t r : train) {
+        auto& files = rts[rows[r].peptide_idx];
+        auto it = files.find(file_id[r]);
+        if (it == files.end()) files[file_id[r]] = (double)rows[r].rt;
+        else it->second = rust_min(it->second, (double)rows[r].rt);
+    }
+    std::vector<std::vector<double>> mat;
+    for (auto& [pep, files] : rts) {
+        std::vector<double> v(n_files, NAN);
+        double sum = 0.0, len = 0.0;
+        for (auto& [f, rt0] : files) {
+            const double rt = rt0 / max_rt[f];
+            v[f] = rt;
+            sum += rt;
+            len += 1.0;
+        }
+        if (std::isnormal(sum / len)) mat.push_back(std::move(v));
+    }
+    std::vector<double> mean_rts(mat.size());
+    for (size_t r = 0; r < mat.size(); r++) {
+        uint64_t len = 0;
+        double sum = 0.0;
+        for (double x : mat[r])
+            if (std::isfinite(x)) { len++; sum += x; }
+        mean_rts[r] = sum / (double)len;
+    }
+    std::vector<float> al(3 * n_files);
+    for (uint64_t f = 0; f < n_files; f++) {
+        uint64_t len = 0;
+        double dot = 0.0, sum_x = 0.0, sum_y = 0.0;
+        for (size_t r = 0; r < mat.size(); r++) {
+            const double x = mat[r][f], y = mean_rts[r];
+            if (!std::isfinite(x)) continue;
+            len++;
+            dot += x * y;
+            sum_x += x;
+            sum_y += y;
+        }
+        const double x_mean = sum_x / (double)len, y_mean = sum_y / (double)len;
+        const double ssxy = dot - (double)len * x_mean * y_mean;
+        double sx2 = 1E-8;
+        for (size_t r = 0; r < mat.size(); r++)
+            if (std::isfinite(mat[r][f])) sx2 += (mat[r][f] - x_mean) * (mat[r][f] - x_mean);
+        double slope = ssxy / sx2, intercept = y_mean - slope * x_mean;
+        if (!std::isfinite(slope)) slope = 1.0;
+        if (!std::isfinite(intercept)) intercept = 0.0;
+        al[3 * f] = (float)max_rt[f];
+        al[3 * f + 1] = (float)slope;
+        al[3 * f + 2] = (float)intercept;
+    }
+    std::copy(al.begin(), al.end(), align);
+    for (uint64_t i = 0; i < n; i++) {
+        const float* a = &al[3 * file_id[i]];
+        aligned_rt[i] = (rows[i].rt / a[0]) * a[1] + a[2];
+    }
+    stats[0] = train.size();
+    stats[1] = mat.size();
+
+    // retention_model::predict, mobility_model::predict
+    auto pep_of = [&](uint32_t r, const uint8_t** s, uint64_t* len) {
+        const uint32_t p = rows[r].peptide_idx;
+        *s = seq + off[p];
+        *len = off[p + 1] - off[p];
+        return p;
+    };
+    for (int model = 0; model < 2; model++) {
+        const int d = model == 0 ? RT_D : IMS_D;
+        auto embed_row = [&](uint32_t r, double* e) {
+            const uint8_t* s;
+            uint64_t len;
+            const uint32_t p = pep_of(r, &s, &len);
+            if (model == 0) rt_embed(s, len, mono[p], e);
+            else ims_embed(s, len, mono[p], (uint8_t)rows[r].charge, e);
+        };
+        const Fit fit = linreg_fit(
+            train.size(), d, [&](uint64_t i, double* e) { embed_row(train[i], e); },
+            [&](uint64_t i) { return model == 0 ? (double)aligned_rt[train[i]] : (double)rows[train[i]].ims; }, threads);
+        float* pred = model == 0 ? predicted_rt : predicted_ims;
+        float* delta = model == 0 ? delta_rt : delta_ims;
+        fitted[model] = fit.ok;
+        r2[model] = fit.ok ? fit.r2 : 0.0;
+        eps[model] = fit.ok ? fit.eps : 0.0;
+        double* beta_out = model == 0 ? rt_beta : ims_beta;
+        std::fill(beta_out, beta_out + d, 0.0);
+        if (!fit.ok) {
+            std::fill(pred, pred + n, 0.0f);
+            std::fill(delta, delta + n, 0.999f);
+            continue;
+        }
+        std::copy(fit.beta.begin(), fit.beta.end(), beta_out);
+        std::vector<double> e(d);
+        const double hi = model == 0 ? 1.0 : 2.0;
+        for (uint64_t i = 0; i < n; i++) {   // predict_peptide: fold from 0.0, then clamp (NaN passes) as f32
+            embed_row((uint32_t)i, e.data());
+            double v = 0.0;
+            for (int j = 0; j < d; j++) v = v + e[j] * fit.beta[j];
+            if (v < 0.0) v = 0.0;
+            if (v > hi) v = hi;
+            const float bounded = (float)v;
+            pred[i] = bounded;
+            delta[i] = std::fabs((model == 0 ? aligned_rt[i] : rows[i].ims) - bounded);
+        }
+    }
     return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 }
 

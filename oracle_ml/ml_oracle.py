@@ -37,6 +37,10 @@ def lib():
         _lib.mo_spectrum_fdr.argtypes = [C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_uint64] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 9
         _lib.mo_kde_build.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int, C.c_double, C.c_int] + [C.c_void_p] * 3
         _lib.mo_lda_train.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_void_p]
+        _lib.mo_rt_embed.argtypes = [C.c_int, C.c_void_p, C.c_uint64, C.c_float, C.c_uint32, C.c_void_p]
+        _lib.mo_linreg_fit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.mo_predict_rt.restype = C.c_double
+        _lib.mo_predict_rt.argtypes = [C.c_void_p] * 5 + [C.c_uint64, C.c_uint64, C.c_int] + [C.c_void_p] * 13
     return _lib
 
 
@@ -87,4 +91,43 @@ def spectrum_fdr(features, precursor_tol, aligned_rt=None, delta_rt_model=None, 
                eps=eps.value, seconds=secs, threads=threads)
     if with_features:
         res["features"] = feats
+    return res
+
+
+def rt_embed(model: int, sequence, monoisotopic: float, charge: int = 2) -> np.ndarray:
+    """RetentionModel::embed (model 0, 69 features) or MobilityModel::embed (model 1, 100 features) of one peptide."""
+    seq = np.frombuffer(sequence.encode() if isinstance(sequence, str) else bytes(sequence), np.uint8).copy()
+    out = np.zeros(69 if model == 0 else 100)
+    lib().mo_rt_embed(int(model), _p(seq), len(seq), float(monoisotopic), int(charge), _p(out))
+    return out
+
+
+def linreg_fit(X, y, threads=None):
+    """LinearRegression::fit over a given [n, d] matrix (every row passes the filter): (beta, r2, eps), or None when the reference returns None."""
+    X = np.ascontiguousarray(X, np.float64)
+    y = np.ascontiguousarray(y, np.float64)
+    beta, r2, eps = np.zeros(X.shape[1]), C.c_double(), C.c_double()
+    if not lib().mo_linreg_fit(_p(X), _p(y), len(y), X.shape[1], int(threads or default_threads()), _p(beta), C.byref(r2), C.byref(eps)):
+        return None
+    return beta, r2.value, eps.value
+
+
+def predict_rt(peptides, features, file_id, n_files, threads=None) -> dict:
+    """runner.rs:513-531 on the CPU; the same keys as sage_b200.predict_rt (stage times aside), plus `seconds` (wall time) and `threads`."""
+    rows = np.ascontiguousarray(features)
+    assert rows.dtype.itemsize == 128
+    n = len(rows)
+    fid = np.ascontiguousarray(file_id, np.uint32)
+    off, seq, mono = (np.ascontiguousarray(a, t) for a, t in ((peptides.seq_off, np.uint32), (peptides.seq, np.uint8), (peptides.mono, np.float32)))
+    cols = {c: np.zeros(n, np.float32) for c in ("aligned_rt", "predicted_rt", "delta_rt_model", "predicted_ims", "delta_ims_model", "spectrum_q")}
+    align = np.zeros((int(n_files), 3), np.float32)
+    stats, fitted = np.zeros(2, np.uint64), np.zeros(2, np.int32)
+    r2, eps, rt_beta, ims_beta = np.zeros(2), np.zeros(2), np.zeros(69), np.zeros(100)
+    threads = int(threads or default_threads())
+    secs = lib().mo_predict_rt(_p(off), _p(seq), _p(mono), _p(rows), _p(fid), n, int(n_files), threads, *[_p(cols[c]) for c in cols], _p(align), _p(stats),
+                               _p(fitted), _p(r2), _p(eps), _p(rt_beta), _p(ims_beta))
+    from sage_b200.api import ALIGNMENT_DTYPE
+    res = dict(cols, alignments=align.view(ALIGNMENT_DTYPE).reshape(-1), training_rows=int(stats[0]), aligned_peptides=int(stats[1]),
+               rt_fitted=bool(fitted[0]), rt_r2=float(r2[0]), rt_eps=float(eps[0]), rt_beta=rt_beta, ims_fitted=bool(fitted[1]), ims_r2=float(r2[1]),
+               ims_eps=float(eps[1]), ims_beta=ims_beta, seconds=secs, threads=threads)
     return res

@@ -90,7 +90,7 @@ EXPORTED_SYMBOLS = [
     "sage_b200_process_spectra", "sage_b200_find_reporter_ions", "sage_b200_host_alloc", "sage_b200_host_free", "sage_b200_last_error",
     "sage_b200_host_log_variant", "sage_b200_host_log1pf_exact", "sage_b200_device_log", "sage_b200_bind_thread_to_device", "sage_b200_host_alloc_blocks",
     "sage_b200_lfq_create", "sage_b200_lfq_add_ms1", "sage_b200_lfq_integrate", "sage_b200_lfq_get_info", "sage_b200_lfq_export", "sage_b200_lfq_destroy",
-    "sage_b200_spectrum_fdr", "sage_b200_kde_build", "sage_b200_device_math",
+    "sage_b200_spectrum_fdr", "sage_b200_kde_build", "sage_b200_device_math", "sage_b200_predict_rt",
 ]
 
 _lib = None
@@ -805,3 +805,44 @@ def device_math(function: str, x: np.ndarray, variant: int = -1, device: int = 0
     out = np.zeros_like(x)
     _check(load_library().sage_b200_device_math(C.c_int(device), C.c_int(MATH_FUNCTIONS[function]), C.c_int(variant), _ptr(x), C.c_uint64(len(x)), _ptr(out)))
     return out
+
+
+# ------------------------------------------------------------------------------------------------ predict_rt (runner.rs:513-531)
+RT_STAGES = ["ms_sort_q", "ms_alignment", "ms_rt_model", "ms_ims_model", "ms_total"]
+RT_FEATURES, IMS_FEATURES = 69, 100
+RT_COLUMNS = ("aligned_rt", "predicted_rt", "delta_rt_model", "predicted_ims", "delta_ims_model", "spectrum_q")
+
+
+class CRtOut(C.Structure):
+    _fields_ = [(c, C.c_void_p) for c in RT_COLUMNS] + [("alignments", C.c_void_p), ("training_rows", C.c_uint64), ("aligned_peptides", C.c_uint64),
+                                                         ("rt_fitted", C.c_int32), ("rt_r2", C.c_double), ("rt_eps", C.c_double),
+                                                         ("rt_beta", C.c_double * RT_FEATURES), ("ims_fitted", C.c_int32), ("ims_r2", C.c_double),
+                                                         ("ims_eps", C.c_double), ("ims_beta", C.c_double * IMS_FEATURES)] + [(s, C.c_float) for s in RT_STAGES]
+
+
+def predict_rt(db: IndexedDatabase, peptides: Peptides, features: np.ndarray, file_id, n_files: int) -> dict:
+    """The runner's predict_rt stage (runner.rs:513-531) on the device: the ascending poisson sort and interim spectrum q-values,
+    global_alignment, retention_model::predict and mobility_model::predict. `features` are FEATURE_DTYPE rows, `file_id` one file per row
+    (< n_files), `peptides` the table `db` was built from. The rows are not reordered. Returns aligned_rt, predicted_rt, delta_rt_model,
+    predicted_ims, delta_ims_model and the interim spectrum_q (f32, indexed like the rows), alignments (ALIGNMENT_DTYPE[n_files], the input of
+    FeatureMap.build), training_rows, aligned_peptides, rt_fitted / rt_r2 / rt_eps / rt_beta, the same for ims, and the stage times (ms_*).
+    aligned_rt, delta_rt_model and delta_ims_model feed spectrum_fdr's optional columns."""
+    rows = np.ascontiguousarray(features)
+    if rows.dtype != FEATURE_DTYPE:
+        raise TypeError("features must have FEATURE_DTYPE")
+    n = len(rows)
+    fid = np.ascontiguousarray(file_id, np.uint32)
+    if len(fid) != n:
+        raise ValueError("file_id must have one value per row")
+    res = {c: np.zeros(n, np.float32) for c in RT_COLUMNS}
+    res["alignments"] = np.zeros(int(n_files), ALIGNMENT_DTYPE)
+    out = CRtOut(*[_ptr(res[c]) for c in RT_COLUMNS], _ptr(res["alignments"]))
+    keep: list = []
+    cp = peptides._c(keep)
+    _check(load_library().sage_b200_predict_rt(db._h, C.byref(cp), _ptr(rows), _ptr(fid), C.c_uint64(n), C.c_uint64(int(n_files)), C.byref(out)))
+    res.update(training_rows=int(out.training_rows), aligned_peptides=int(out.aligned_peptides))
+    for m, d in (("rt", RT_FEATURES), ("ims", IMS_FEATURES)):
+        res.update({f"{m}_fitted": bool(getattr(out, f"{m}_fitted")), f"{m}_r2": float(getattr(out, f"{m}_r2")),
+                    f"{m}_eps": float(getattr(out, f"{m}_eps")), f"{m}_beta": np.array(getattr(out, f"{m}_beta")[:d], np.float64)})
+    res.update({s: float(getattr(out, s)) for s in RT_STAGES})
+    return res

@@ -34,6 +34,7 @@
 #include "kernels.cuh"
 #include "lfq.cuh"
 #include "fdr.cuh"
+#include "rt.cuh"
 
 using namespace sb;
 
@@ -2880,6 +2881,296 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
     float* ms[5] = {&out->ms_mass_kde, &out->ms_features, &out->ms_lda, &out->ms_discriminant_kde, &out->ms_sort_q};
     for (int i = 0; i < 5; i++) FDR_TRY(cudaEventElapsedTime(ms[i], ev[i], ev[i + 1]));
     FDR_TRY(cudaEventElapsedTime(&out->ms_total, ev[0], ev[5]));
+    return 0;
+}
+
+// ================================================================================== predict_rt (runner.rs:513-531; kernels in rt.cuh)
+// LinearRegression::fit (regression.rs:72-117) for one model over the training list: chunk accumulators on the device, merged in chunk order,
+// Gauss::solve on the host, the SSE pass chunked the same way; then predict for every row (or the Feature defaults when the fit is None).
+template <int MODEL>
+static int rt_model(cudaStream_t st, FdrArena& A, bool fma, const RtPeptides& P, const sage_b200_feature* d_rows, uint64_t n, const uint32_t* d_train,
+                    uint64_t n_train, const float* d_ycol, const float* d_aligned, float* d_pred, float* d_delta, int32_t* fitted, double* r2, double* eps,
+                    double* beta_out) {
+    using Dm = RtDims<MODEL>;
+    constexpr int D = Dm::D;
+    *fitted = 0;
+    *r2 = 0.0;
+    *eps = 0.0;
+    std::fill(beta_out, beta_out + D, 0.0);
+    std::vector<double> beta;
+    if (n_train) {
+        const uint64_t n_chunks = (n_train + RT_CHUNK - 1) / RT_CHUNK;
+        double *d_part = nullptr, *d_acc = nullptr, *d_sse = nullptr, *d_beta = nullptr;
+        FDR_TRY(A.alloc(&d_part, n_chunks * Dm::NACC));
+        FDR_TRY(A.alloc(&d_acc, Dm::NACC));
+        const dim3 grid((unsigned)n_chunks, (Dm::NACC + 255) / 256);
+        if (fma) k_rt_accumulate<MODEL, true><<<grid, 256, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_part);
+        else k_rt_accumulate<MODEL, false><<<grid, 256, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_part);
+        FDR_TRY(cudaGetLastError());
+        k_rt_merge<<<(Dm::NACC + 255) / 256, 256, 0, st>>>(d_part, n_chunks, Dm::NACC, d_acc);
+        FDR_TRY(cudaGetLastError());
+        std::vector<double> acc(Dm::NACC);
+        FDR_TRY(cudaMemcpyAsync(acc.data(), d_acc, 8 * Dm::NACC, cudaMemcpyDeviceToHost, st));
+        FDR_TRY(cudaStreamSynchronize(st));
+        HostMat cov(D, D), b(D, 1);
+        for (int j = 0, a = 0; j < D; j++)
+            for (int k = j; k < D; k++, a++) cov(j, k) = cov(k, j) = acc[a];
+        for (int j = 0; j < D; j++) b.a[j] = acc[Dm::NCOV + j];
+        const double sum_y = acc[Dm::NCOV + D], sum_y2 = acc[Dm::NCOV + D + 1];
+        const double nf = (double)n_train, y_mean = sum_y / nf, y_var = sum_y2 - nf * y_mean * y_mean;
+        if (gauss_solve(cov, b, &beta, eps)) {
+            FDR_TRY(A.alloc(&d_beta, D));
+            FDR_TRY(A.alloc(&d_sse, n_chunks));
+            FDR_TRY(cudaMemcpyAsync(d_beta, beta.data(), 8 * D, cudaMemcpyHostToDevice, st));
+            if (fma) k_rt_sse<MODEL, true><<<(unsigned)n_chunks, 32, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_beta, d_sse);
+            else k_rt_sse<MODEL, false><<<(unsigned)n_chunks, 32, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_beta, d_sse);
+            FDR_TRY(cudaGetLastError());
+            std::vector<double> chunk_sse(n_chunks);
+            FDR_TRY(cudaMemcpyAsync(chunk_sse.data(), d_sse, 8 * n_chunks, cudaMemcpyDeviceToHost, st));
+            FDR_TRY(cudaStreamSynchronize(st));
+            double sse = -0.0;   // f64 Sum of the chunk sums, in chunk order
+            for (double s : chunk_sse) sse = sse + s;
+            *r2 = 1.0 - sse / y_var;
+            *fitted = 1;
+            std::copy(beta.begin(), beta.end(), beta_out);
+            const unsigned g = (unsigned)((n + RT_TILE - 1) / RT_TILE);
+            if (fma) k_rt_predict<MODEL, true><<<g, 32, 0, st>>>(P, d_rows, n, d_beta, d_aligned, d_pred, d_delta);
+            else k_rt_predict<MODEL, false><<<g, 32, 0, st>>>(P, d_rows, n, d_beta, d_aligned, d_pred, d_delta);
+            FDR_TRY(cudaGetLastError());
+            return 0;
+        }
+        *eps = 0.0;
+    }
+    k_rt_defaults<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, d_pred, d_delta);
+    FDR_TRY(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_peptides* P, const sage_b200_feature* rows, const uint32_t* file_id, uint64_t n,
+                                    uint64_t n_files, sage_b200_rt_out* out) {
+    if (!db || !P || !out || (n_files && !out->alignments) ||
+        (n && (!rows || !file_id || !out->aligned_rt || !out->predicted_rt || !out->delta_rt_model || !out->predicted_ims || !out->delta_ims_model)))
+        return fail(SAGE_B200_EINVAL, "predict_rt: null argument");
+    if (P->n_peptides != db->v.n_pep) return fail(SAGE_B200_EINVAL, "predict_rt: the peptide table has %llu peptides, the db %u",
+                                                  (unsigned long long)P->n_peptides, db->v.n_pep);
+    const uint64_t n_pep = P->n_peptides;
+    if (n_pep && (!P->residue_offsets || !P->sequence || !P->monoisotopic)) return fail(SAGE_B200_EINVAL, "predict_rt: null peptide array");
+    if (n && n_files == 0) return fail(SAGE_B200_EINVAL, "predict_rt: rows but no files");
+    if (n > (uint64_t)INT32_MAX) return fail(SAGE_B200_ELIMIT, "predict_rt: more than 2^31 - 1 rows (qvalue.rs counts in i32)");
+    out->training_rows = out->aligned_peptides = 0;
+    out->rt_fitted = out->ims_fitted = 0;
+    out->rt_r2 = out->rt_eps = out->ims_r2 = out->ims_eps = 0.0;
+    memset(out->rt_beta, 0, sizeof out->rt_beta);
+    memset(out->ims_beta, 0, sizeof out->ims_beta);
+    out->ms_sort_q = out->ms_alignment = out->ms_rt_model = out->ms_ims_model = out->ms_total = 0.0f;
+    // argument checks: the reference indexes out of bounds (file_id, peptide_idx) or panics (residue - b'A') on these
+    std::vector<uint8_t> referenced(n_pep, 0);
+    for (uint64_t i = 0; i < n; i++) {
+        if (file_id[i] >= n_files) return fail(SAGE_B200_EINVAL, "predict_rt: row %llu has file_id %u >= n_files %llu", (unsigned long long)i, file_id[i],
+                                               (unsigned long long)n_files);
+        if (rows[i].peptide_idx >= n_pep) return fail(SAGE_B200_EINVAL, "predict_rt: row %llu has peptide_idx %u outside the db (%llu peptides)",
+                                                      (unsigned long long)i, rows[i].peptide_idx, (unsigned long long)n_pep);
+        referenced[rows[i].peptide_idx] = 1;
+    }
+    for (uint64_t p = 0; p < n_pep; p++)
+        if (referenced[p])
+            for (uint64_t r = P->residue_offsets[p]; r < P->residue_offsets[p + 1]; r++)
+                if (P->sequence[r] < 'A' || P->sequence[r] > 'Z')
+                    return fail(SAGE_B200_EINVAL, "predict_rt: peptide %llu has residue byte 0x%02x outside 'A'..'Z'", (unsigned long long)p, P->sequence[r]);
+    if (n == 0) {
+        for (uint64_t f = 0; f < n_files; f++) out->alignments[f] = sage_b200_alignment{0.0f, 1.0f, 0.0f};
+        return 0;
+    }
+    FDR_TRY(cudaSetDevice(db->device));
+    const uint64_t nres = P->residue_offsets[n_pep];
+    const uint64_t n_chunks = (n + RT_CHUNK - 1) / RT_CHUNK + 1;
+    {   // everything below stays allocated until the call returns: fail with ELIMIT before allocating when it cannot fit
+        size_t free_b = 0, total_b = 0;
+        FDR_TRY(cudaMemGetInfo(&free_b, &total_b));
+        // per row: the rows, file ids, sort keys / values / order, the q-value work columns, flags, training list, (peptide, file) keys and
+        // values, segment arrays, the five outputs and the sort's temporary storage; the peptide table; per file the maxima and alignments;
+        // both models' chunk partials; and the peptide x file matrix, at most one row per referenced peptide
+        const double per_row = sizeof(sage_b200_feature) + 4 + 8 * 2 + 4 * 2 + 4 * 5 + 1 + 4 + 8 * 2 + 4 * 2 + 1 + 4 + 8 + 1 + 4 + 4 + 4 + 4 * 5 + 48;
+        uint64_t n_ref = 0;
+        for (uint8_t r : referenced) n_ref += r;
+        const double need = (double)n * per_row + (double)nres + 8.0 * (double)n_pep + 24.0 * (double)n_files +
+                            8.0 * (double)n_chunks * (RtDims<0>::NACC + RtDims<1>::NACC + 2) + 8.0 * (double)n_ref * ((double)n_files + 1) + (double)(64ull << 20);
+        if (need > (double)free_b)
+            return fail(SAGE_B200_ELIMIT, "predict_rt: %llu rows over %llu files need about %.0f bytes of device memory, %llu free", (unsigned long long)n,
+                        (unsigned long long)n_files, need, (unsigned long long)free_b);
+    }
+    const bool fma = host_math_variant() != 1;
+    FdrArena A;
+    cudaStream_t st = 0;
+    cudaEvent_t ev[5] = {};
+    struct EvFree { cudaEvent_t* e; ~EvFree() { for (int i = 0; i < 5; i++) if (e[i]) cudaEventDestroy(e[i]); } } ev_free{ev};
+    for (auto& e : ev) FDR_TRY(cudaEventCreate(&e));
+    sage_b200_feature* d_rows = nullptr;
+    uint32_t *d_file = nullptr, *d_off = nullptr, *d_idx = nullptr, *d_order = nullptr, *d_isdec = nullptr, *d_dscan = nullptr, *d_train = nullptr,
+             *d_val = nullptr, *d_val2 = nullptr, *d_seg = nullptr, *d_prow = nullptr, *d_keep = nullptr, *d_mrow = nullptr, *d_count = nullptr;
+    uint8_t *d_seq = nullptr, *d_flag = nullptr;
+    float *d_mono = nullptr, *d_q = nullptr, *d_rq = nullptr, *d_rqmin = nullptr, *d_out[5] = {};
+    uint64_t *d_key = nullptr, *d_key2 = nullptr;
+    unsigned* d_maxrt = nullptr;
+    unsigned long long* d_passing = nullptr;
+    double *d_segmin = nullptr, *d_mat = nullptr, *d_mean = nullptr;
+    sage_b200_alignment* d_align = nullptr;
+    FDR_TRY(A.alloc(&d_rows, n));
+    FDR_TRY(A.alloc(&d_file, n));
+    FDR_TRY(A.alloc(&d_off, n_pep + 1));
+    FDR_TRY(A.alloc(&d_seq, nres));
+    FDR_TRY(A.alloc(&d_mono, n_pep));
+    FDR_TRY(A.alloc(&d_key, n));
+    FDR_TRY(A.alloc(&d_key2, n));
+    FDR_TRY(A.alloc(&d_idx, n));
+    FDR_TRY(A.alloc(&d_order, n));
+    FDR_TRY(A.alloc(&d_isdec, n));
+    FDR_TRY(A.alloc(&d_dscan, n));
+    FDR_TRY(A.alloc(&d_q, n));
+    FDR_TRY(A.alloc(&d_rq, n));
+    FDR_TRY(A.alloc(&d_rqmin, n));
+    FDR_TRY(A.alloc(&d_flag, n));
+    FDR_TRY(A.alloc(&d_train, n));
+    FDR_TRY(A.alloc(&d_val, n));
+    FDR_TRY(A.alloc(&d_val2, n));
+    FDR_TRY(A.alloc(&d_seg, n));
+    FDR_TRY(A.alloc(&d_segmin, n));
+    FDR_TRY(A.alloc(&d_prow, n));
+    FDR_TRY(A.alloc(&d_keep, n));
+    FDR_TRY(A.alloc(&d_mrow, n));
+    FDR_TRY(A.alloc(&d_count, 4));
+    FDR_TRY(A.alloc(&d_passing, 1));
+    FDR_TRY(A.alloc(&d_maxrt, n_files));
+    FDR_TRY(A.alloc(&d_align, n_files));
+    for (auto& o : d_out) FDR_TRY(A.alloc(&o, n));
+    FDR_TRY(cudaMemcpyAsync(d_rows, rows, sizeof(sage_b200_feature) * n, cudaMemcpyHostToDevice, st));
+    FDR_TRY(cudaMemcpyAsync(d_file, file_id, 4 * n, cudaMemcpyHostToDevice, st));
+    FDR_TRY(cudaMemcpyAsync(d_off, P->residue_offsets, 4 * (n_pep + 1), cudaMemcpyHostToDevice, st));
+    if (nres) FDR_TRY(cudaMemcpyAsync(d_seq, P->sequence, nres, cudaMemcpyHostToDevice, st));
+    FDR_TRY(cudaMemcpyAsync(d_mono, P->monoisotopic, 4 * n_pep, cudaMemcpyHostToDevice, st));
+    const RtPeptides pk{d_off, d_seq, d_mono};
+    const unsigned g = (unsigned)((n + 255) / 256);
+    thrust::counting_iterator<uint32_t> count_it(0);
+    char* tmp = nullptr;
+    size_t tmp_bytes = 0;
+    auto ensure_tmp = [&](size_t b) -> int {   // one temporary buffer for every cub call, grown when a call needs more
+        if (b <= tmp_bytes) return 0;
+        FDR_TRY(A.alloc(&tmp, b));
+        tmp_bytes = b;
+        return 0;
+    };
+    auto read_count = [&](uint64_t* v) -> int {
+        uint32_t c = 0;
+        FDR_TRY(cudaMemcpyAsync(&c, d_count, 4, cudaMemcpyDeviceToHost, st));
+        FDR_TRY(cudaStreamSynchronize(st));
+        *v = c;
+        return 0;
+    };
+
+    // 1. par_sort_unstable_by(poisson.total_cmp), ties by input row, then spectrum_q_value (runner.rs:517-520)
+    FDR_TRY(cudaEventRecord(ev[0], st));
+    k_rt_poisson_key<<<g, 256, 0, st>>>(d_rows, n, d_key, d_idx);
+    FDR_TRY(cudaGetLastError());
+    {
+        size_t tb = 0, tb2 = 0, tb3 = 0;
+        FDR_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key2, d_idx, d_order, (int)n, 0, 64, st));
+        FDR_TRY(cub::DeviceScan::InclusiveSum(nullptr, tb2, d_isdec, d_dscan, (int)n, st));
+        FDR_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
+        if (int rc = ensure_tmp(std::max(tb, std::max(tb2, tb3)))) return rc;
+        FDR_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, d_key, d_key2, d_idx, d_order, (int)n, 0, 64, st));
+        k_fdr_sorted_decoy<<<g, 256, 0, st>>>(d_rows, d_order, n, d_isdec);
+        FDR_TRY(cudaGetLastError());
+        FDR_TRY(cub::DeviceScan::InclusiveSum(tmp, tb2, d_isdec, d_dscan, (int)n, st));
+        k_fdr_q_raw<<<g, 256, 0, st>>>(d_dscan, n, d_rq);
+        FDR_TRY(cudaGetLastError());
+        FDR_TRY(cub::DeviceScan::InclusiveScan(tmp, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
+        FDR_TRY(cudaMemsetAsync(d_passing, 0, 8, st));
+        k_fdr_q_out<<<g, 256, 0, st>>>(d_rqmin, d_order, n, d_q, d_passing);
+        FDR_TRY(cudaGetLastError());
+    }
+    // the training rows (label == 1 && spectrum_q <= 0.01) in poisson order
+    k_rt_train_flag<<<g, 256, 0, st>>>(d_rows, d_order, d_q, n, d_flag);
+    FDR_TRY(cudaGetLastError());
+    uint64_t n_train = 0;
+    {
+        size_t tb = 0;
+        FDR_TRY(cub::DeviceSelect::Flagged(nullptr, tb, d_order, d_flag, d_train, d_count, (int)n, st));
+        if (int rc = ensure_tmp(tb)) return rc;
+        FDR_TRY(cub::DeviceSelect::Flagged(tmp, tb, d_order, d_flag, d_train, d_count, (int)n, st));
+        if (int rc = read_count(&n_train)) return rc;
+    }
+    FDR_TRY(cudaEventRecord(ev[1], st));
+
+    // 2. global_alignment (retention_alignment.rs:95-173)
+    FDR_TRY(cudaMemsetAsync(d_maxrt, 0, 4 * n_files, st));
+    k_rt_max_rt<<<g, 256, 0, st>>>(d_rows, d_file, n, d_maxrt);
+    FDR_TRY(cudaGetLastError());
+    uint64_t n_seg = 0, n_pr = 0, n_rows = 0;
+    if (n_train) {
+        const unsigned gt = (unsigned)((n_train + 255) / 256);
+        k_rt_pf_key<<<gt, 256, 0, st>>>(d_rows, d_file, d_train, n_train, d_key);
+        FDR_TRY(cudaGetLastError());
+        size_t tb = 0;
+        FDR_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key2, d_train, d_val, (int)n_train, 0, 64, st));
+        if (int rc = ensure_tmp(tb)) return rc;
+        FDR_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, d_key, d_key2, d_train, d_val, (int)n_train, 0, 64, st));   // stable: poisson order kept
+        k_rt_heads<<<gt, 256, 0, st>>>(d_key2, n_train, d_flag);
+        FDR_TRY(cudaGetLastError());
+        FDR_TRY(cub::DeviceSelect::Flagged(nullptr, tb, count_it, d_flag, d_seg, d_count, (int)n_train, st));
+        if (int rc = ensure_tmp(tb)) return rc;
+        FDR_TRY(cub::DeviceSelect::Flagged(tmp, tb, count_it, d_flag, d_seg, d_count, (int)n_train, st));
+        if (int rc = read_count(&n_seg)) return rc;
+        const unsigned gs = (unsigned)((n_seg + 255) / 256);
+        k_rt_seg_min<<<gs, 256, 0, st>>>(d_rows, d_key2, d_val, d_seg, n_seg, n_train, d_segmin, d_flag);
+        FDR_TRY(cudaGetLastError());
+        FDR_TRY(cub::DeviceSelect::Flagged(nullptr, tb, count_it, d_flag, d_prow, d_count, (int)n_seg, st));
+        if (int rc = ensure_tmp(tb)) return rc;
+        FDR_TRY(cub::DeviceSelect::Flagged(tmp, tb, count_it, d_flag, d_prow, d_count, (int)n_seg, st));
+        if (int rc = read_count(&n_pr)) return rc;
+        const unsigned gp = (unsigned)((n_pr + 255) / 256);
+        k_rt_row_mean<<<gp, 256, 0, st>>>(d_key2, d_seg, d_segmin, d_prow, n_pr, n_seg, d_maxrt, d_keep);
+        FDR_TRY(cudaGetLastError());
+        FDR_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_keep, d_mrow, (int)n_pr, st));
+        if (int rc = ensure_tmp(tb)) return rc;
+        FDR_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, d_keep, d_mrow, (int)n_pr, st));
+        uint32_t last[2] = {0, 0};
+        FDR_TRY(cudaMemcpyAsync(&last[0], d_mrow + n_pr - 1, 4, cudaMemcpyDeviceToHost, st));
+        FDR_TRY(cudaMemcpyAsync(&last[1], d_keep + n_pr - 1, 4, cudaMemcpyDeviceToHost, st));
+        FDR_TRY(cudaStreamSynchronize(st));
+        n_rows = (uint64_t)last[0] + last[1];
+        FDR_TRY(A.alloc(&d_mat, n_rows * n_files));
+        FDR_TRY(A.alloc(&d_mean, n_rows));
+        FDR_TRY(cudaMemsetAsync(d_mat, 0xFF, 8 * n_rows * n_files, st));   // NaN where a peptide was not seen in a file
+        k_rt_fill<<<gp, 256, 0, st>>>(d_key2, d_seg, d_segmin, d_prow, n_pr, n_seg, d_maxrt, d_keep, d_mrow, n_files, d_mat, d_mean);
+        FDR_TRY(cudaGetLastError());
+    }
+    k_rt_align<<<(unsigned)((n_files + 127) / 128), 128, 0, st>>>(d_mat, d_mean, n_rows, n_files, d_maxrt, d_align);
+    FDR_TRY(cudaGetLastError());
+    float* d_aligned = d_out[0];
+    k_rt_aligned<<<g, 256, 0, st>>>(d_rows, d_file, n, d_align, d_aligned);
+    FDR_TRY(cudaGetLastError());
+    FDR_TRY(cudaEventRecord(ev[2], st));
+
+    // 3. retention_model::predict, 4. mobility_model::predict
+    if (int rc = rt_model<0>(st, A, fma, pk, d_rows, n, d_train, n_train, d_aligned, d_aligned, d_out[1], d_out[2], &out->rt_fitted, &out->rt_r2,
+                             &out->rt_eps, out->rt_beta))
+        return rc;
+    FDR_TRY(cudaEventRecord(ev[3], st));
+    if (int rc = rt_model<1>(st, A, fma, pk, d_rows, n, d_train, n_train, nullptr, d_aligned, d_out[3], d_out[4], &out->ims_fitted, &out->ims_r2,
+                             &out->ims_eps, out->ims_beta))
+        return rc;
+    FDR_TRY(cudaEventRecord(ev[4], st));
+
+    float* dst[5] = {out->aligned_rt, out->predicted_rt, out->delta_rt_model, out->predicted_ims, out->delta_ims_model};
+    for (int c = 0; c < 5; c++) FDR_TRY(cudaMemcpyAsync(dst[c], d_out[c], 4 * n, cudaMemcpyDeviceToHost, st));
+    if (out->spectrum_q) FDR_TRY(cudaMemcpyAsync(out->spectrum_q, d_q, 4 * n, cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaMemcpyAsync(out->alignments, d_align, sizeof(sage_b200_alignment) * n_files, cudaMemcpyDeviceToHost, st));
+    FDR_TRY(cudaStreamSynchronize(st));
+    out->training_rows = n_train;
+    out->aligned_peptides = n_rows;
+    float* ms[4] = {&out->ms_sort_q, &out->ms_alignment, &out->ms_rt_model, &out->ms_ims_model};
+    for (int i = 0; i < 4; i++) FDR_TRY(cudaEventElapsedTime(ms[i], ev[i], ev[i + 1]));
+    FDR_TRY(cudaEventElapsedTime(&out->ms_total, ev[0], ev[4]));
     return 0;
 }
 #undef FDR_TRY

@@ -442,3 +442,48 @@ def make_psms(n: int, seed: int = 0x0FD2, decoy_fraction: float = 0.3, true_frac
     out["ms2_intensity"] = rng.uniform(1e3, 1e6, n).astype(np.float32)
     out["poisson"] = np.where(true, -rng.uniform(5.0, 20.0, n), -rng.uniform(0.0, 4.0, n))
     return out
+
+
+def make_rt_psms(pep: Peptides, n: int, n_files: int, seed: int = 0x5E7, mobility: bool = False, with_truth: bool = False):
+    """Seeded Feature rows (FEATURE_DTYPE) and their file ids for the predict_rt stage (runner.rs:513-531). A quarter of the rows are decoys; 60 %
+    of the targets are true matches (poisson -20 .. -5) and the rest false (poisson -4 .. 0, like the decoys). A true match's normalised RT is a
+    hidden linear function of its peptide's residue counts and length (the RT model's features) plus noise; file f then applies its own linear
+    distortion x = (rt - b_f) / a_f and scale rt = x * T_f (T_f uniform in 60 .. 120). False matches and decoys get uniform RTs. With
+    `mobility`, every row's ims is linear in the mobility model's features (residue fractions, 1 / charge, mass) plus noise; otherwise 0.
+    Returns (rows, file_id), plus a dict of the hidden values (rt_true, is_true, T, a, b per file) when `with_truth`."""
+    from .api import FEATURE_DTYPE
+    rng = np.random.default_rng(seed)
+    rows = make_psms(n, seed=seed)
+    decoy = rng.random(n) < 0.25
+    true = ~decoy & (rng.random(n) < 0.6)
+    targets, decoys = np.nonzero(pep.decoy == 0)[0], np.nonzero(pep.decoy != 0)[0]
+    pidx = rng.choice(targets, n).astype(np.uint32)
+    if len(decoys):
+        pidx[decoy] = rng.choice(decoys, int(decoy.sum())).astype(np.uint32)
+    off = pep.seq_off.astype(np.int64)
+    lens = np.diff(off)
+    coef = np.zeros(256)
+    coef[np.frombuffer(b"ACDEFGHIKLMNPQRSTVWYUO", np.uint8)] = rng.uniform(-0.02, 0.04, 22)
+    raw = np.add.reduceat(coef[pep.seq], off[:-1]) + 0.004 * lens if len(pep.seq) else np.zeros(len(lens))
+    lo, hi = raw.min(), raw.max()
+    pep_rt = 0.05 + 0.9 * (raw - lo) / max(hi - lo, 1e-12)
+    rt_true = pep_rt[pidx] + rng.normal(0.0, 0.004, n)
+    fid = rng.integers(0, n_files, n).astype(np.uint32)
+    T, a, b = rng.uniform(60.0, 120.0, n_files), rng.uniform(0.9, 1.1, n_files), rng.uniform(-0.05, 0.05, n_files)
+    x = np.where(true, (rt_true - b[fid]) / a[fid], rng.uniform(0.0, 1.0, n))
+    rows["peptide_idx"] = pidx
+    rows["peptide_len"] = lens[pidx].astype(np.uint32)
+    rows["label"] = np.where(decoy, -1, 1).astype(np.int32)
+    rows["poisson"] = np.where(true, -rng.uniform(5.0, 20.0, n), -rng.uniform(0.0, 4.0, n))
+    rows["rt"] = (x * T[fid]).astype(np.float32)
+    charge = rows["charge"].astype(np.float64)
+    if mobility:
+        cim = np.zeros(256)
+        cim[np.frombuffer(b"ACDEFGHIKLMNPQRSTVWYUO", np.uint8)] = rng.uniform(-0.3, 0.3, 22)
+        pep_ims = (np.add.reduceat(cim[pep.seq], off[:-1]) / lens if len(pep.seq) else np.zeros(len(lens))) + 0.1 * pep.mono.astype(np.float64) / 1000.0
+        rows["ims"] = (0.6 + pep_ims[pidx] + 0.6 / charge + rng.normal(0.0, 0.003, n)).astype(np.float32)
+    else:
+        rows["ims"] = np.float32(0)
+    if with_truth:
+        return rows, fid, dict(rt_true=rt_true, is_true=true, T=T, a=a, b=b)
+    return rows, fid
