@@ -170,7 +170,7 @@ void sage_b200_scorer_destroy(sage_b200_scorer* scorer);
  *   "mass_parts"      1..4 (default 2): the peak-mass copy of a chunk from PINNED caller memory is cut into this many runs of spectra and the
  *                     counting kernel is queued once per run, so it starts while the rest of the copy is in flight
  *   "wide_tile", "wide_lmax", "worklist_reset", "narrow_block"   test hooks (tile size / survivor-list size of the open-search kernel; forget learned
- *                     list sizes; peptides per block of the narrow-search copy, 0 = sized by the average precursor window) */
+ *                     list sizes; peptides per block of the narrow-search copy, 0 = sized by the average precursor window, else 64..65536) */
 int sage_b200_scorer_set_option(sage_b200_scorer* scorer, const char* name, int64_t value);
 
 /* Scorer::score over a batch (runner.rs:311-325 `par_iter().flat_map(|s| scorer.score(s))`).

@@ -12,6 +12,7 @@ namespace sb {
 constexpr int K_MAX = 128;            // max preliminary candidates kept per spectrum: max(50, 2*report_psms)
 constexpr uint32_t NARROW_CAP = 8192; // precursor windows up to this many peptides are counted in shared memory
 constexpr int PRELIM_THREADS = 256;
+constexpr int PRELIM_CTAS = 6;              // CTAs per SM of k_prelim_narrow (a persistent grid over its work list)
 constexpr int SCORE_THREADS = 128;  // chosen by A/B on cfg2 against 64 and 256; must stay >= K_MAX for the rank sort
 #ifndef SAGE_B200_SCORE_MIN_CTAS
 #define SAGE_B200_SCORE_MIN_CTAS 10
@@ -218,10 +219,29 @@ struct DbView {
 // shared-memory count tile) and sorted by m/z inside a block, so the entries matching one (peak, charge) probe inside one tile are a single
 // contiguous run found through a per-block m/z LUT — instead of filtering every entry of the page slices (database.rs:514-534 visits ~9x more
 // entries than match). Built lazily per db the first time a scorer meets a window wider than NARROW_CAP (sage_b200.cu: db_wide_index).
+// Blocks hold ~2 M entries here, so a 2^18-cell u32 LUT per block is small next to them; narrow windows use NarrowIndexView instead.
 struct WideIndexView {
     const uint2* frag;        // {PeptideIx, m/z bits}, block-major, ascending m/z inside a block; nullptr = not built (page-slice streaming is used)
     const uint64_t* blk_off;  // [n_block + 1]
     const uint32_t* lut;      // [n_block][cells + 1]: #{entries of the block with m/z < base + c / inv_w}
+    uint32_t block, n_block, cells;
+    float base, inv_w;
+};
+
+// Index copy for narrow precursor windows (k_prelim_narrow_warp<true>, k_prelim_narrow): the fragments grouped by blocks of `block` (<= 65536)
+// consecutive PeptideIx, ascending m/z inside a block, as two parallel arrays — the m/z values alone (a run walk compares only these, 8 per
+// 32-byte sector) and the PeptideIx offset within the block (read only for entries inside the probe's m/z bounds). Per block an m/z directory
+// of `cells` u16 cells, about one per entry, so that the part of the directory that the resident queries touch stays in L2. Built lazily by
+// the first narrow-search chunk (sage_b200.cu: db_narrow_index).
+constexpr uint32_t NARROW_GROUP = 64;   // directory cells per u32 group base
+struct NarrowIndexView {
+    const float* mz;          // block-major, ascending m/z inside a block; nullptr = not built (the page index is probed instead)
+    const uint16_t* pep;      // PeptideIx - block index * block, parallel to mz
+    const uint64_t* blk_off;  // [n_block + 1]
+    // start of the run of m/z >= edge(c), edge(c) = base + c / inv_w, as an entry of the block: grp[c / NARROW_GROUP] + dir[c]. Both count the
+    // block's entries with m/z < the edge (grp at the group's first cell); dir is clamped to 65535, which can only move a start earlier.
+    const uint16_t* dir;      // [n_block][cells]
+    const uint32_t* grp;      // [n_block][cells / NARROW_GROUP]
     uint32_t block, n_block, cells;
     float base, inv_w;
 };

@@ -328,44 +328,68 @@ __device__ __forceinline__ void index_probe(const DbView& db, const QueryDesc& q
 }
 
 // The same probe against the NARROW BLOCK INDEX (a second copy of the fragments: blocks of `nv.block` consecutive PeptideIx, ascending m/z inside
-// a block, one m/z LUT per block — the open-search layout with small blocks). A precursor window of a few hundred peptides lies in one or two
-// blocks, so a probe is: LUT cell of `flo` (one cell early: float rounding) -> walk the block's entries until m/z > fhi, counting those inside
-// [flo, fhi] whose PeptideIx is in the window. Same matched set as index_probe by construction (every index entry with PeptideIx in the window
-// lies in these blocks); two dependent loads before the walk instead of five, no page loop, no bisection.
+// a block, device_common.cuh: NarrowIndexView). A precursor window of a few hundred peptides lies in one or two blocks, so a probe is: directory
+// cell of `flo` (one cell early: float rounding) -> walk the block's m/z values until one is > fhi; an entry inside [flo, fhi] reads its
+// PeptideIx offset and counts when the PeptideIx is in the window. Same matched set as index_probe by construction (every index entry with
+// PeptideIx in the window lies in these blocks); two dependent loads before the walk instead of five, no page loop, no bisection.
 //
 // One warp = 32 probes of one query. Most walks are one or two entries, but a peak at a fragment mass that MANY peptides share (y1 of K / R, b2
 // of frequent dipeptides) matches a run of up to a few hundred entries: walked by its own lane that run set the trip count of the whole warp
 // (CPU statistics of cfg2: mean 3.5 loads per probe, mean of the per-warp maximum 24). So a lane walks at most WALK_SOLO entries alone; runs
-// still open after that are finished by the whole warp, 32 consecutive entries per step (coalesced 256-byte reads). Counting kernel on cfg2 (ms):
-// every lane walks alone 0.546 | WALK_SOLO 2 0.698 | 4 0.588 | 8 0.494 | 16 0.500 | 32 0.520; finishing four runs at a time with 8-lane groups
-// 0.52-0.53 at WALK_SOLO 4-12 (each cooperative step costs a full memory latency, so only the genuinely long runs should get there).
-// The reference's page / entry work counters are not produced on this path (sage_b200.cu: option "narrow_index"). Measured slower and dropped: fetching a
-// 32-byte sector (4 entries) per step.
+// still open after that are finished by the whole warp, 32 consecutive entries per step (coalesced 128-byte reads of m/z).
+// The reference's page / entry work counters are not produced on this path (sage_b200.cu: option "narrow_index").
 #ifndef SAGE_B200_WALK_SOLO
 #define SAGE_B200_WALK_SOLO 8
 #endif
 constexpr uint32_t WALK_SOLO = SAGE_B200_WALK_SOLO;
-__device__ __forceinline__ void block_probe_warp(const WideIndexView& nv, const QueryDesc& q, uint32_t b0, uint32_t b1, bool act, float flo, float fhi,
+// A lane's walk is a chain of dependent loads (each entry decides whether the next is needed), so it issues the loads of WALK_STEP entries, m/z
+// and PeptideIx offset, at once. Counting kernel, H100 SXM at 700 W (ms, cfg2): WALK_STEP 1: 0.638; 2: 0.595; 4: 0.582 but 28 bytes of register
+// spills at the 40 registers WARPQ_MIN_CTAS allows. Reading the offset only for entries inside [flo, fhi] (one more dependent load per match)
+// measured slower: 0.630 on cfg2 at WALK_STEP 3, 12.24 against 11.55 ms on cfg3; in the warp-wide walk as well (cfg3 12.53 ms), so both
+// walks read the offset with the m/z value. WALK_SOLO re-measured with the batched walk: 4: 0.699, 8: 0.630, 16: 0.639.
+constexpr uint32_t WALK_STEP = 2;
+// Directory cell a probe starts from: one cell before the cell of `flo`, so that edge(c) <= flo despite the rounding of both computations
+// (tests/test_narrow_directory.py restates them on the CPU).
+__device__ __forceinline__ uint32_t narrow_start_cell(const NarrowIndexView& nv, float flo) {
+    const float tt = (flo - nv.base) * nv.inv_w;
+    return tt > 1.0f ? (uint32_t)((int)fminf(tt, (float)(nv.cells - 1)) - 1) : 0u;
+}
+__device__ __forceinline__ void block_probe_warp(const NarrowIndexView& nv, const QueryDesc& q, uint32_t b0, uint32_t b1, bool act, float flo, float fhi,
                                                  uint32_t* cnt32, uint32_t& matched) {
     const uint32_t lane = threadIdx.x & 31;
-    const float tt = (flo - nv.base) * nv.inv_w;
-    const int c = tt > 1.0f ? (int)fminf(tt, (float)(nv.cells - 1)) - 1 : 0;
+    const uint32_t c = narrow_start_cell(nv, flo);
     for (uint32_t blk = b0; blk <= b1; blk++) {   // warp-uniform: b0, b1 belong to the query
-        const uint64_t base = __ldg(nv.blk_off + blk);
-        const uint32_t cnt = (uint32_t)(__ldg(nv.blk_off + blk + 1) - base);
-        const uint2* fr = nv.frag + base;
+        const uint32_t base = (uint32_t)__ldg(nv.blk_off + blk);   // < 2^31 fragments (db_narrow_index)
+        const uint32_t cnt = (uint32_t)__ldg(nv.blk_off + blk + 1) - base;
+        const float* mz = nv.mz + base;
+        const uint16_t* off = nv.pep + base;
+        const uint32_t pep0 = blk * nv.block;
         uint32_t e = cnt;
         if (act) {
-            e = __ldg(nv.lut + (size_t)blk * (nv.cells + 1) + c);
-            for (uint32_t k = 0; k < WALK_SOLO && e < cnt; k++, e++) {
-                const uint2 f = __ldg(fr + e);
-                const float fmz = __uint_as_float(f.y);
-                if (fmz > fhi) { e = cnt; break; }
-                if (fmz >= flo && f.x >= q.eff_lo && f.x <= q.eff_hi) {
-                    const uint32_t idx = f.x - q.pre_lo;
-                    atomicAdd(&cnt32[idx >> 1], 1u << ((idx & 1) * 16));
-                    matched++;
+            e = __ldg(nv.grp + (size_t)blk * (nv.cells / NARROW_GROUP) + c / NARROW_GROUP) + __ldg(nv.dir + (size_t)blk * nv.cells + c);
+            // WALK_STEP entries per step, their loads issued together (one memory latency per step instead of one per entry); past the block
+            // end an entry reads as +inf, which ends the run like an m/z above fhi
+            for (uint32_t k = 0; k < WALK_SOLO && e < cnt; k += WALK_STEP, e += WALK_STEP) {
+                float m[WALK_STEP];
+                uint32_t o[WALK_STEP];
+#pragma unroll
+                for (uint32_t j = 0; j < WALK_STEP; j++) {
+                    const bool in = e + j < cnt;
+                    m[j] = in ? __ldg(mz + e + j) : __int_as_float(0x7f800000);
+                    o[j] = in ? __ldg(off + e + j) : 0u;
                 }
+                bool stop = false;
+#pragma unroll
+                for (uint32_t j = 0; j < WALK_STEP; j++) {
+                    stop |= m[j] > fhi;
+                    const uint32_t pid = pep0 + o[j];
+                    if (!stop && m[j] >= flo && pid >= q.eff_lo && pid <= q.eff_hi) {
+                        const uint32_t idx = pid - q.pre_lo;
+                        atomicAdd(&cnt32[idx >> 1], 1u << ((idx & 1) * 16));
+                        matched++;
+                    }
+                }
+                if (stop) { e = cnt; break; }
             }
         }
         uint32_t pend = __ballot_sync(0xffffffffu, e < cnt);   // runs still open
@@ -378,13 +402,15 @@ __device__ __forceinline__ void block_probe_warp(const WideIndexView& nv, const 
                 const uint32_t i = pos + lane;
                 bool stop = i >= cnt;
                 if (!stop) {
-                    const uint2 f = __ldg(fr + i);
-                    const float fmz = __uint_as_float(f.y);
+                    const float fmz = __ldg(mz + i);
+                    const uint32_t pid = pep0 + __ldg(off + i);
                     stop = fmz > hi_s;
-                    if (!stop && fmz >= lo_s && f.x >= q.eff_lo && f.x <= q.eff_hi) {
-                        const uint32_t idx = f.x - q.pre_lo;
-                        atomicAdd(&cnt32[idx >> 1], 1u << ((idx & 1) * 16));
-                        matched++;   // counted on the lane that saw the entry: the warp sums `matched` afterwards
+                    if (!stop && fmz >= lo_s) {
+                        if (pid >= q.eff_lo && pid <= q.eff_hi) {
+                            const uint32_t idx = pid - q.pre_lo;
+                            atomicAdd(&cnt32[idx >> 1], 1u << ((idx & 1) * 16));
+                            matched++;   // counted on the lane that saw the entry: the warp sums `matched` afterwards
+                        }
                     }
                 }
                 if (__any_sync(0xffffffffu, stop)) break;
@@ -405,7 +431,7 @@ __device__ __forceinline__ void block_probe_warp(const WideIndexView& nv, const 
 //    (bounds computed with the reference's f32 ops; both arrays are monotone in the peak mass, which is verified per
 //    spectrum — otherwise the CTA falls back to the index path).
 __device__ __forceinline__ void narrow_cta_query(const DbView& db, const ScorerView& sc, const BatchView& b, uint32_t pmax, uint64_t* nlist, uint32_t item,
-                                                 float* bounds_smem, const WideIndexView& nv) {
+                                                 float* bounds_smem, const NarrowIndexView& nv) {
     __shared__ uint32_t cnt32[NARROW_CAP / 2 + 1];
     __shared__ uint32_t s_warp[40];
     ReplaySlot* const nslots = b.nslots;
@@ -499,7 +525,7 @@ __device__ __forceinline__ void narrow_cta_query(const DbView& db, const ScorerV
                 }
             }
         }
-    } else if (nv.frag != nullptr) {
+    } else if (nv.mz != nullptr) {
         // small-block copy of the index: every warp takes 32 probes at a time (block_probe_warp finishes long runs warp-wide)
         const uint32_t blk0 = q.pre_lo / nv.block, blk1 = min(q.pre_hi, db.n_pep - 1) / nv.block;
         for (uint32_t t0 = warp * 32; t0 < ntask; t0 += PRELIM_THREADS) {
@@ -613,7 +639,8 @@ __device__ __forceinline__ void narrow_cta_query(const DbView& db, const ScorerV
 
 // Queries counted by a whole CTA (windows of WARPQ_CAP+1..NARROW_CAP peptides, and the peptide-centric path): a fixed-size grid walks the
 // compacted list k_setup_queries wrote.
-__global__ void __launch_bounds__(PRELIM_THREADS) k_prelim_narrow(DbView db, ScorerView sc, BatchView b, uint32_t pmax, uint64_t* nlist, WideIndexView nv) {
+// The register budget holds the PRELIM_CTAS CTAs per SM the grid is sized for (without it ptxas picked a budget that spilled).
+__global__ void __launch_bounds__(PRELIM_THREADS, PRELIM_CTAS) k_prelim_narrow(DbView db, ScorerView sc, BatchView b, uint32_t pmax, uint64_t* nlist, NarrowIndexView nv) {
     extern __shared__ float bounds_smem[];  // LO[nfc][np] then HI[nfc][np] (peptide-centric path only)
     const uint32_t total = (uint32_t)min(b.counters[C_NCTA], (unsigned long long)b.n * sc.qmax);
     for (uint32_t i = blockIdx.x; i < total; i += gridDim.x) {
@@ -629,7 +656,7 @@ __global__ void __launch_bounds__(PRELIM_THREADS) k_prelim_narrow(DbView db, Sco
 // (e.g. the charge fold of known-charge spectra) sit at the end of the grid and leave after one cached load.
 template <bool BLK>
 __global__ void __launch_bounds__(WARPQ_WARPS * 32, WARPQ_MIN_CTAS) k_prelim_narrow_warp(DbView db, ScorerView sc, BatchView b, uint64_t* nlist, uint32_t s_lo,
-                                                                                                uint32_t s_hi, WideIndexView nv) {
+                                                                                                uint32_t s_hi, NarrowIndexView nv) {
     __shared__ uint32_t cnt_all[WARPQ_WARPS][WARPQ_CAP / 2];
     if (b.counters[C_COUNT + blockIdx.y] == 0ull) return;
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -2824,12 +2851,22 @@ __global__ void k_wide_keys(uint64_t n_frag, const uint2* frag, uint32_t block, 
     key64[i] = ((uint64_t)(f.x / block) << 32) | (uint32_t)((uint32_t)f32_key(__uint_as_float(f.y)) ^ 0x80000000u);   // unsigned order == total_cmp order
     pep[i] = f.x;
 }
+__device__ __forceinline__ uint32_t mz_bits_of_key(uint64_t key) {
+    const uint32_t u = (uint32_t)key ^ 0x80000000u;                    // back to the signed total_cmp key ...
+    return u ^ (((uint32_t)((int)u >> 31)) >> 1);                       // ... and to the float's bit pattern (f32_key is an involution)
+}
 __global__ void k_wide_pack(uint64_t n_frag, const uint64_t* key64, const uint32_t* pep, uint2* out) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_frag) return;
-    const uint32_t u = (uint32_t)key64[i] ^ 0x80000000u;               // back to the signed total_cmp key ...
-    const uint32_t bits = u ^ (((uint32_t)((int)u >> 31)) >> 1);        // ... and to the float's bit pattern (f32_key is an involution)
-    out[i] = make_uint2(pep[i], bits);
+    out[i] = make_uint2(pep[i], mz_bits_of_key(key64[i]));
+}
+// the narrow copy: the same sorted keys as two parallel arrays, m/z and PeptideIx relative to its block
+__global__ void k_narrow_pack(uint64_t n_frag, const uint64_t* key64, const uint32_t* pep, uint32_t block, float* mz, uint16_t* off) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_frag) return;
+    const uint64_t k = key64[i];
+    mz[i] = __uint_as_float(mz_bits_of_key(k));
+    off[i] = (uint16_t)(pep[i] - (uint32_t)(k >> 32) * block);
 }
 __global__ void k_wide_block_offsets(uint64_t n_frag, const uint64_t* key64, uint32_t n_block, uint64_t* blk_off) {
     const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2875,6 +2912,27 @@ __global__ void k_wide_lut(WideIndexView w, uint32_t* lut) {
         while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if (__uint_as_float(e[m].y) < edge) lo = m + 1; else hi = m; }
     }
     lut[j] = lo;
+}
+// One thread per (block, directory cell): #{entries with m/z < edge(c)}, split into the group base (written by the group's first cell) and the
+// u16 remainder. A remainder above 65535 (> 65535 entries between two edges of one group: near-degenerate m/z) is clamped, i.e. the walk
+// starts earlier than it could; inv_w == 0 (degenerate m/z range) leaves every start at the block start.
+__global__ void k_narrow_dir(NarrowIndexView v, uint16_t* dir, uint32_t* grp) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= (uint64_t)v.n_block * v.cells) return;
+    const uint32_t b = (uint32_t)(j / v.cells), c = (uint32_t)(j - (uint64_t)b * v.cells);
+    const float* m = v.mz + v.blk_off[b];
+    const uint32_t n = (uint32_t)(v.blk_off[b + 1] - v.blk_off[b]);
+    auto below = [&](uint32_t cc) -> uint32_t {
+        if (cc == 0 || !(v.inv_w > 0.0f)) return 0;
+        const float edge = v.base + (float)cc * (1.0f / v.inv_w);
+        uint32_t lo = 0, hi = n;
+        while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (m[mid] < edge) lo = mid + 1; else hi = mid; }
+        return lo;
+    };
+    const uint32_t g = c / NARROW_GROUP;
+    const uint32_t at = below(c), gb = below(g * NARROW_GROUP);
+    if (c == g * NARROW_GROUP) grp[(uint64_t)b * (v.cells / NARROW_GROUP) + g] = at;
+    dir[j] = (uint16_t)min(at - gb, 65535u);
 }
 
 __global__ void k_build_bucket_lut(DbView db, float base, float inv_w, uint32_t* lut) {

@@ -206,26 +206,31 @@ static bool is_pinned(const void* p) {
 }
 
 // ------------------------------------------------------------------------------------------------ db
+// One lazily built block-major copy of the fragments: its view and the device arrays behind it.
+template <class View>
 struct BlockIndexSlot {
-    WideIndexView v{};
-    void *d_frag = nullptr, *d_blk = nullptr, *d_lut = nullptr;
+    View v{};
+    void* d[5] = {};   // the arrays of the current build
     int failed = 0;
     uint64_t bytes = 0;
     std::vector<void*> retired;   // arrays of earlier builds: another scorer of the same db may still hold a view of them (freed with the db)
     uint64_t retired_bytes = 0;
+    void free_current() {
+        for (void*& p : d) { if (p) cudaFree(p); p = nullptr; }
+        v = View{};
+        bytes = 0;
+    }
     void release() {
-        for (void** p : {&d_frag, &d_blk, &d_lut}) { if (*p) cudaFree(*p); *p = nullptr; }
+        free_current();
         for (void* p : retired) cudaFree(p);
         retired.clear();
         retired_bytes = 0;
-        v = WideIndexView{};
-        bytes = 0;
     }
     // A rebuild with another block size keeps the old arrays alive: a chunk of another scorer, queued with the old view, may still run.
     void retire() {
-        for (void** p : {&d_frag, &d_blk, &d_lut}) { if (*p) retired.push_back(*p); *p = nullptr; }
+        for (void*& p : d) { if (p) retired.push_back(p); p = nullptr; }
         retired_bytes += bytes;
-        v = WideIndexView{};
+        v = View{};
         bytes = 0;
     }
 };
@@ -238,10 +243,12 @@ struct sage_b200_db {
          *d_pep_flags = nullptr, *d_pep_missed = nullptr;
     uint64_t total_residues = 0, device_bytes = 0;
     int sm_count = 132;   // H100 SXM; replaced by the device's multiProcessorCount in db_new
-    // secondary copies of the fragments in peptide-block-major order (WideIndexView), built lazily and guarded by wmu: `wide` (blocks = the
-    // open-search count tile, built by the first scorer that meets a wide window) and `narrow` (small blocks, built by the first narrow chunk)
+    // secondary copies of the fragments in peptide-block-major order, built lazily and guarded by wmu: `wide` (WideIndexView: blocks = the
+    // open-search count tile, built by the first scorer that meets a wide window) and `narrow` (NarrowIndexView: small blocks, built by the
+    // first narrow chunk)
     mutable std::mutex wmu;
-    mutable BlockIndexSlot wide, narrow;
+    mutable BlockIndexSlot<WideIndexView> wide;
+    mutable BlockIndexSlot<NarrowIndexView> narrow;
 };
 
 static int dmalloc(sage_b200_db* db, void** p, size_t bytes) {
@@ -605,59 +612,75 @@ extern "C" int sage_b200_db_export_index(const sage_b200_db* db, uint32_t* fragm
     return 0;
 }
 
-// Secondary index for open search (device_common.cuh: WideIndexView): fragments keyed by (PeptideIx / block, m/z), one LSD radix sort, block
-// offsets and a per-block m/z LUT. `block` = the scorer's count-tile size. Returns a view with frag == nullptr when the index cannot be built
-// (out of memory, SAGE_B200_NO_WIDE_INDEX=1): k_prelim_wide then streams the page slices as the reference does.
-// Builds (or returns) one block-major copy of the fragments. `cells_for(entries per block)` picks the LUT resolution; wmu must be held.
-static WideIndexView build_block_index(const sage_b200_db* db, BlockIndexSlot& slot, uint32_t block, uint32_t cells) {
-    WideIndexView none{};
-    if (slot.v.frag != nullptr && slot.v.block == block) return slot.v;
-    if (slot.failed || block == 0 || db->v.n_frag == 0 || db->v.n_pep == 0) return none;
+// Both block-major copies of the fragments start alike: fragments keyed by (PeptideIx / block, m/z), one LSD radix sort, block offsets, and
+// the m/z range of the index. On success *keys / *peps hold the sorted keys and PeptideIx (freed by the caller, as is everything in `tmp`).
+static bool sort_block_major(const sage_b200_db* db, uint32_t block, uint32_t n_block, uint64_t* blk_off, void** keys, void** peps, void* (&tmp)[4],
+                             float& lo, float& hi) {
     const uint64_t nf = db->v.n_frag;
-    slot.retire();   // a rebuild with another block size (tests, scorers with very different tolerances): see BlockIndexSlot::retire
-    void *k_a = nullptr, *k_b = nullptr, *p_a = nullptr, *p_b = nullptr, *tmp = nullptr, *d_rng = nullptr;
-    auto cleanup = [&]() { for (void* p : {k_a, k_b, p_a, p_b, tmp, d_rng}) if (p) cudaFree(p); };
-    auto give_up = [&]() { cleanup(); for (void** p : {&slot.d_frag, &slot.d_blk, &slot.d_lut}) { if (*p) cudaFree(*p); *p = nullptr; } slot.v = WideIndexView{}; slot.bytes = 0; cudaGetLastError(); slot.failed = 1; return WideIndexView{}; };
-    const uint32_t n_block = (db->v.n_pep + block - 1) / block;
-    while (cells > 256 && (uint64_t)n_block * (cells + 1) * 4 > (1024ull << 20)) cells >>= 1;   // at most 1 GB of LUT
-    if (cudaMalloc(&slot.d_frag, 8 * nf + 64) != cudaSuccess || cudaMalloc(&slot.d_blk, 8 * ((size_t)n_block + 1)) != cudaSuccess ||
-        cudaMalloc(&slot.d_lut, 4 * (size_t)n_block * (cells + 1)) != cudaSuccess)
-        return give_up();
-    if (cudaMalloc(&k_a, 8 * nf) != cudaSuccess || cudaMalloc(&k_b, 8 * nf) != cudaSuccess || cudaMalloc(&p_a, 4 * nf) != cudaSuccess ||
-        cudaMalloc(&p_b, 4 * nf) != cudaSuccess || cudaMalloc(&d_rng, 8) != cudaSuccess)
-        return give_up();
+    if (nf > 0x7FFFFFFFull) return false;
+    void *&k_a = tmp[0], *&p_a = tmp[1], *&sort_tmp = tmp[2], *&d_rng = tmp[3];
+    if (cudaMalloc(&k_a, 8 * nf) != cudaSuccess || cudaMalloc(keys, 8 * nf) != cudaSuccess || cudaMalloc(&p_a, 4 * nf) != cudaSuccess ||
+        cudaMalloc(peps, 4 * nf) != cudaSuccess || cudaMalloc(&d_rng, 8) != cudaSuccess)
+        return false;
     k_wide_keys<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, block, (uint64_t*)k_a, (uint32_t*)p_a);
     int nb_bits = 1;
     while (nb_bits < 32 && (n_block >> nb_bits)) nb_bits++;
     size_t tb = 0;
-    if (nf > 0x7FFFFFFFull) return give_up();
-    if (cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)k_a, (uint64_t*)k_b, (const uint32_t*)p_a, (uint32_t*)p_b, (int)nf, 0, 32 + nb_bits) != cudaSuccess ||
-        cudaMalloc(&tmp, tb + 16) != cudaSuccess ||
-        cub::DeviceRadixSort::SortPairs(tmp, tb, (const uint64_t*)k_a, (uint64_t*)k_b, (const uint32_t*)p_a, (uint32_t*)p_b, (int)nf, 0, 32 + nb_bits) != cudaSuccess)
-        return give_up();
-    k_wide_pack<<<(unsigned)((nf + 255) / 256), 256>>>(nf, (const uint64_t*)k_b, (const uint32_t*)p_b, (uint2*)slot.d_frag);
-    k_wide_block_offsets<<<(n_block + 1 + 255) / 256, 256>>>(nf, (const uint64_t*)k_b, n_block, (uint64_t*)slot.d_blk);
+    if (cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)k_a, (uint64_t*)*keys, (const uint32_t*)p_a, (uint32_t*)*peps, (int)nf, 0, 32 + nb_bits) != cudaSuccess ||
+        cudaMalloc(&sort_tmp, tb + 16) != cudaSuccess ||
+        cub::DeviceRadixSort::SortPairs(sort_tmp, tb, (const uint64_t*)k_a, (uint64_t*)*keys, (const uint32_t*)p_a, (uint32_t*)*peps, (int)nf, 0, 32 + nb_bits) != cudaSuccess)
+        return false;
+    k_wide_block_offsets<<<(n_block + 1 + 255) / 256, 256>>>(nf, (const uint64_t*)*keys, n_block, blk_off);
     // m/z range of the index (positive floats order like their bit patterns)
     const uint32_t rng0[2] = {0xFFFFFFFFu, 0u};
-    if (cudaMemcpy(d_rng, rng0, 8, cudaMemcpyHostToDevice) != cudaSuccess) return give_up();
+    if (cudaMemcpy(d_rng, rng0, 8, cudaMemcpyHostToDevice) != cudaSuccess) return false;
     k_frag_mz_range<<<(unsigned)std::min<uint64_t>((nf + 255) / 256, 4096), 256>>>(nf, db->v.frag, (uint32_t*)d_rng);
     uint32_t rng[2];
-    if (cudaMemcpy(rng, d_rng, 8, cudaMemcpyDeviceToHost) != cudaSuccess) return give_up();
-    cleanup();
-    k_a = k_b = p_a = p_b = tmp = d_rng = nullptr;
-    float lo, hi;
+    if (cudaMemcpy(rng, d_rng, 8, cudaMemcpyDeviceToHost) != cudaSuccess) return false;
     memcpy(&lo, &rng[0], 4); memcpy(&hi, &rng[1], 4);
-    WideIndexView w{};
-    w.frag = (const uint2*)slot.d_frag; w.blk_off = (const uint64_t*)slot.d_blk; w.lut = (const uint32_t*)slot.d_lut;
-    w.block = block; w.n_block = n_block; w.cells = cells;
+    return true;
+}
+
+// Directory cells of `cells` equal m/z steps over [lo, hi] (the same for every block): base and inverse width, or inv_w = 0 (every walk
+// starts at the block start) when the range is degenerate.
+template <class View>
+static void set_mz_cells(View& v, float lo, float hi, uint32_t cells) {
+    v.cells = cells;
     const float width = (hi - lo) / (float)cells;
-    w.base = (std::isfinite(lo) && lo > 0.0f) ? lo : 0.0f;
-    w.inv_w = (std::isfinite(width) && width > 0.0f && lo > 0.0f) ? 1.0f / width : 0.0f;
+    v.base = (std::isfinite(lo) && lo > 0.0f) ? lo : 0.0f;
+    v.inv_w = (std::isfinite(width) && width > 0.0f && lo > 0.0f) ? 1.0f / width : 0.0f;
+}
+
+// Secondary index for open search (device_common.cuh: WideIndexView): the sorted fragments as {PeptideIx, m/z} and a per-block u32 m/z LUT.
+// `block` = the scorer's count-tile size. Returns a view with frag == nullptr when the index cannot be built (out of memory,
+// SAGE_B200_NO_WIDE_INDEX=1): k_prelim_wide then streams the page slices as the reference does. wmu must be held.
+static WideIndexView build_wide_index(const sage_b200_db* db, BlockIndexSlot<WideIndexView>& slot, uint32_t block, uint32_t cells) {
+    if (slot.v.frag != nullptr && slot.v.block == block) return slot.v;
+    if (slot.failed || block == 0 || db->v.n_frag == 0 || db->v.n_pep == 0) return WideIndexView{};
+    const uint64_t nf = db->v.n_frag;
+    slot.retire();   // a rebuild with another block size (tests, scorers with very different tolerances): see BlockIndexSlot::retire
+    void *keys = nullptr, *peps = nullptr, *tmp[4] = {};
+    auto cleanup = [&]() { for (void* p : {keys, peps, tmp[0], tmp[1], tmp[2], tmp[3]}) if (p) cudaFree(p); };
+    auto give_up = [&]() { cleanup(); slot.free_current(); cudaGetLastError(); slot.failed = 1; return WideIndexView{}; };
+    const uint32_t n_block = (db->v.n_pep + block - 1) / block;
+    while (cells > 256 && (uint64_t)n_block * (cells + 1) * 4 > (1024ull << 20)) cells >>= 1;   // at most 1 GB of LUT
+    void *&d_frag = slot.d[0], *&d_blk = slot.d[1], *&d_lut = slot.d[2];
+    if (cudaMalloc(&d_frag, 8 * nf + 64) != cudaSuccess || cudaMalloc(&d_blk, 8 * ((size_t)n_block + 1)) != cudaSuccess ||
+        cudaMalloc(&d_lut, 4 * (size_t)n_block * (cells + 1)) != cudaSuccess)
+        return give_up();
+    float lo, hi;
+    if (!sort_block_major(db, block, n_block, (uint64_t*)d_blk, &keys, &peps, tmp, lo, hi)) return give_up();
+    k_wide_pack<<<(unsigned)((nf + 255) / 256), 256>>>(nf, (const uint64_t*)keys, (const uint32_t*)peps, (uint2*)d_frag);
+    WideIndexView w{};
+    w.frag = (const uint2*)d_frag; w.blk_off = (const uint64_t*)d_blk; w.lut = (const uint32_t*)d_lut;
+    w.block = block; w.n_block = n_block;
+    set_mz_cells(w, lo, hi, cells);
     if (w.inv_w > 0.0f) {
         const uint64_t total = (uint64_t)n_block * (cells + 1);
-        k_wide_lut<<<(unsigned)((total + 255) / 256), 256>>>(w, (uint32_t*)slot.d_lut);
-    } else if (cudaMemset(slot.d_lut, 0, 4 * (size_t)n_block * (cells + 1)) != cudaSuccess) return give_up();   // degenerate range: every walk starts at the block start
+        k_wide_lut<<<(unsigned)((total + 255) / 256), 256>>>(w, (uint32_t*)d_lut);
+    } else if (cudaMemset(d_lut, 0, 4 * (size_t)n_block * (cells + 1)) != cudaSuccess) return give_up();   // degenerate range: every walk starts at the block start
     if (cudaDeviceSynchronize() != cudaSuccess) return give_up();
+    cleanup();
     slot.v = w;
     slot.bytes = 8 * nf + 8 * ((uint64_t)n_block + 1) + 4ull * n_block * (cells + 1);
     return w;
@@ -668,20 +691,58 @@ static WideIndexView db_wide_index(const sage_b200_db* db, uint32_t block) {
     if (const char* e = getenv("SAGE_B200_NO_WIDE_INDEX")) if (e[0] == '1') return WideIndexView{};   // A/B + tests: stream the page slices instead
     // ~2 M entries per 80 k-peptide block, most of them inside a third of the m/z range: 2^18 cells leave a few dozen entries per cell there,
     // so the conservative (one cell early) start of a walk costs about one extra 32-entry fetch (measured: 2^16 cells -> ~8 extra fetches)
-    return build_block_index(db, db->wide, block, 1u << 18);
+    return build_wide_index(db, db->wide, block, 1u << 18);
 }
 
-// The narrow-search copy: blocks of `block` peptides (a +-20 ppm window holds a few hundred), LUT cells ~ `cells_x` per block entry.
-static WideIndexView db_narrow_index(const sage_b200_db* db, uint32_t block, uint32_t cells_x, bool exact) {
-    std::lock_guard<std::mutex> lock(db->wmu);
-    // an automatically sized request accepts an existing copy whose blocks are within a factor of two (scorers with different tolerances
-    // sharing one index must not rebuild it in turns)
-    if (!exact && db->narrow.v.frag != nullptr && db->narrow.v.block * 2 >= block && db->narrow.v.block <= block * 2) return db->narrow.v;
-    const uint32_t n_block = (db->v.n_pep + block - 1) / std::max(block, 1u);
-    const uint64_t per_block = n_block ? db->v.n_frag / n_block : 0;
+// Directory cells of the narrow copy: the power of two at or above twice the mean block's entries, 1024..32768 (cfg2: 16384 cells for 6 660
+// entries per 256-peptide block; cfg3: 85 k entries per 2048-peptide block, capped at 32768 = 0.5 GB of directory). Measured on cfg2 (H100
+// SXM, 700 W; counting kernel, ms): 1 cell per entry 0.638, 2 cells 0.582, 4 cells 0.615 — a start one coarse cell early walks more entries.
+// The directory is held to 1 GB (halving the cells), which only small blocks over a large index reach: e.g. cfg3's 678 M fragments in blocks
+// of 256 peptides get 8192 cells per block (1.0 GB) instead of 32768 (4.2 GB).
+constexpr uint64_t NARROW_CELLS_PER_ENTRY = 2;
+static uint32_t narrow_dir_cells(uint64_t n_frag, uint32_t n_block) {
+    const uint64_t per_block = n_block ? n_frag / n_block : 0;
     uint32_t cells = 1024;
-    while (cells < (1u << 18) && (uint64_t)cells < per_block * cells_x) cells <<= 1;
-    return build_block_index(db, db->narrow, block, cells);
+    while (cells < 32768u && (uint64_t)cells < per_block * NARROW_CELLS_PER_ENTRY) cells <<= 1;
+    while (cells > 1024u && 2ull * n_block * cells > (1024ull << 20)) cells >>= 1;
+    return cells;
+}
+
+// The narrow-search copy (device_common.cuh: NarrowIndexView), blocks of `block` peptides (a +-20 ppm window holds a few hundred). Returns a
+// view with mz == nullptr when it cannot be built (out of memory): the narrow kernels then probe the page index. An automatically sized
+// request (!exact) accepts an existing copy whose blocks are within a factor of two (scorers with different tolerances sharing one index must
+// not rebuild it in turns).
+static NarrowIndexView db_narrow_index(const sage_b200_db* db, uint32_t block, bool exact) {
+    std::lock_guard<std::mutex> lock(db->wmu);
+    BlockIndexSlot<NarrowIndexView>& slot = db->narrow;
+    if (slot.v.mz != nullptr && (slot.v.block == block || (!exact && slot.v.block * 2 >= block && slot.v.block <= block * 2))) return slot.v;
+    if (slot.failed || block == 0 || block > 65536 || db->v.n_frag == 0 || db->v.n_pep == 0) return NarrowIndexView{};
+    const uint64_t nf = db->v.n_frag;
+    slot.retire();
+    void *keys = nullptr, *peps = nullptr, *tmp[4] = {};
+    auto cleanup = [&]() { for (void* p : {keys, peps, tmp[0], tmp[1], tmp[2], tmp[3]}) if (p) cudaFree(p); };
+    auto give_up = [&]() { cleanup(); slot.free_current(); cudaGetLastError(); slot.failed = 1; return NarrowIndexView{}; };
+    const uint32_t n_block = (db->v.n_pep + block - 1) / block;
+    const uint32_t cells = narrow_dir_cells(nf, n_block), ngrp = cells / NARROW_GROUP;
+    void *&d_mz = slot.d[0], *&d_pep = slot.d[1], *&d_blk = slot.d[2], *&d_dir = slot.d[3], *&d_grp = slot.d[4];
+    if (cudaMalloc(&d_mz, 4 * nf + 64) != cudaSuccess || cudaMalloc(&d_pep, 2 * nf + 64) != cudaSuccess ||
+        cudaMalloc(&d_blk, 8 * ((size_t)n_block + 1)) != cudaSuccess || cudaMalloc(&d_dir, 2 * (size_t)n_block * cells) != cudaSuccess ||
+        cudaMalloc(&d_grp, 4 * (size_t)n_block * ngrp) != cudaSuccess)
+        return give_up();
+    float lo, hi;
+    if (!sort_block_major(db, block, n_block, (uint64_t*)d_blk, &keys, &peps, tmp, lo, hi)) return give_up();
+    k_narrow_pack<<<(unsigned)((nf + 255) / 256), 256>>>(nf, (const uint64_t*)keys, (const uint32_t*)peps, block, (float*)d_mz, (uint16_t*)d_pep);
+    NarrowIndexView v{};
+    v.mz = (const float*)d_mz; v.pep = (const uint16_t*)d_pep; v.blk_off = (const uint64_t*)d_blk; v.dir = (const uint16_t*)d_dir;
+    v.grp = (const uint32_t*)d_grp; v.block = block; v.n_block = n_block;
+    set_mz_cells(v, lo, hi, cells);
+    const uint64_t total = (uint64_t)n_block * cells;
+    k_narrow_dir<<<(unsigned)((total + 255) / 256), 256>>>(v, (uint16_t*)d_dir, (uint32_t*)d_grp);
+    if (cudaDeviceSynchronize() != cudaSuccess) return give_up();
+    cleanup();
+    slot.v = v;
+    slot.bytes = 6 * nf + 128 + 8 * ((uint64_t)n_block + 1) + 2 * total + 4ull * n_block * ngrp;
+    return v;
 }
 
 // Dynamic shared-memory opt-in of the kernels that need more than 48 KB: set ONCE per device to the device maximum (the attribute is per-function,
@@ -844,8 +905,7 @@ struct sage_b200_scorer {
     int narrow_index = 1;
     uint32_t narrow_block_auto = 0;   // block size narrow_block_for chose for this scorer's precursor tolerance
     int narrow_cta = 1;   // windows of WARPQ_CAP+1..NARROW_CAP peptides (one CTA per query) use the copy too
-    uint32_t narrow_block = 0 /* 0 = sized by the average precursor window, see narrow_block_for */, narrow_cells_x = 4;   // chosen by A/B on cfg2 over blocks of
-                                                       // 128..1024 peptides and 2..8 LUT cells per block entry
+    uint32_t narrow_block = 0;   // 0 = sized by the average precursor window, see narrow_block_for
     int mass_parts = 2;        // chosen by A/B on cfg2 (e2e) against 1, 3 and 4 parts
     int first_chunk_pct = 0;   // chosen by A/B on cfg2 (e2e) against 10..35 %
     // SAGE_B200_TRACE=1: per-chunk device timeline (ms since the start of the call) on stderr
@@ -922,8 +982,8 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
     if (const char* e = getenv("SAGE_B200_SCORE_SPLIT")) s->score_split = atoi(e) != 0;
     if (const char* e = getenv("SAGE_B200_NARROW_INDEX")) s->narrow_index = atoi(e) != 0;
     if (const char* e = getenv("SAGE_B200_NARROW_CTA")) s->narrow_cta = atoi(e) != 0;
-    if (const char* e = getenv("SAGE_B200_NARROW_BLOCK")) s->narrow_block = (uint32_t)std::max(0, atoi(e));
-    if (const char* e = getenv("SAGE_B200_NARROW_CELLS_X")) s->narrow_cells_x = (uint32_t)std::max(1, atoi(e));
+    if (const char* e = getenv("SAGE_B200_NARROW_BLOCK")) s->narrow_block = (uint32_t)std::min(65536, std::max(0, atoi(e)));   // 0 or 64..65536 (u16 offsets)
+    if (s->narrow_block != 0 && s->narrow_block < 64) s->narrow_block = 64;
     if (const char* e = getenv("SAGE_B200_MASS_PARTS")) s->mass_parts = std::min(MASS_PARTS, std::max(1, atoi(e)));
     if (const char* e = getenv("SAGE_B200_FIRST_CHUNK_PCT")) s->first_chunk_pct = std::min(50, std::max(0, atoi(e)));
     CUDA_TRY(cudaEventCreate(&s->ev_base));
@@ -939,7 +999,7 @@ extern "C" int sage_b200_scorer_set_option(sage_b200_scorer* s, const char* name
     if (!strcmp(name, "score_split")) { s->score_split = value != 0; return 0; }
     if (!strcmp(name, "narrow_index")) { s->narrow_index = value != 0; return 0; }
     if (!strcmp(name, "narrow_block")) {   // test hook: peptides per block of the narrow-search copy (rebuilds it on the next batch)
-        if (value != 0 && (value < 64 || value > (1 << 20))) return fail(SAGE_B200_EINVAL, "narrow_block must be 0 (automatic) or 64..1048576");
+        if (value != 0 && (value < 64 || value > 65536)) return fail(SAGE_B200_EINVAL, "narrow_block must be 0 (automatic) or 64..65536");
         s->narrow_block = (uint32_t)value;
         return 0;
     }
@@ -1268,22 +1328,22 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
     // (nor for open-search tolerances, whose windows exceed the warp kernel's cap: the copy would only cost memory)
     const float ptol_span = std::max(std::fabs(sv.precursor_tol.lo), std::fabs(sv.precursor_tol.hi));
     const bool narrow_tol = ptol_span <= (sv.precursor_tol.kind == 0 ? 2000.0f : sv.precursor_tol.kind == 1 ? 0.2f : 5.0f);   // ppm / percent / Da
-    WideIndexView nv{};
+    NarrowIndexView nv{};
     if (S->narrow_index && !sv.wide_window && narrow_tol) {
         if (S->narrow_block == 0 && (rc = narrow_block_for(S))) return rc;
-        nv = db_narrow_index(db, S->narrow_block ? S->narrow_block : S->narrow_block_auto, S->narrow_cells_x, S->narrow_block != 0);
+        nv = db_narrow_index(db, S->narrow_block ? S->narrow_block : S->narrow_block_auto, S->narrow_block != 0);
     }
     for (uint32_t q = 0; q < C.nparts; q++) {   // one launch per part of the masses copy (a resident batch has one part)
         if (C.nparts > 1) CUDA_TRY(cudaStreamWaitEvent(st, L.ev_part[q], 0));
         const dim3 wgrid((n + WARPQ_WARPS - 1) / WARPQ_WARPS, sv.qmax);
-        if (nv.frag != nullptr) k_prelim_narrow_warp<true><<<wgrid, WARPQ_WARPS * 32, 0, st>>>(db->v, svq, bv, L.d_nlist.as<uint64_t>(), C.part_lo[q], C.part_lo[q + 1], nv);
+        if (nv.mz != nullptr) k_prelim_narrow_warp<true><<<wgrid, WARPQ_WARPS * 32, 0, st>>>(db->v, svq, bv, L.d_nlist.as<uint64_t>(), C.part_lo[q], C.part_lo[q + 1], nv);
         else k_prelim_narrow_warp<false><<<wgrid, WARPQ_WARPS * 32, 0, st>>>(db->v, svq, bv, L.d_nlist.as<uint64_t>(), C.part_lo[q], C.part_lo[q + 1], nv);
         CUDA_TRY(cudaGetLastError());
         launches += q > 0;
     }
     if (C.nparts > 1) CUDA_TRY(cudaStreamWaitEvent(st, L.ev_masses, 0));
-    k_prelim_narrow<<<(unsigned)std::min<uint64_t>(C.nitems, (uint64_t)db->sm_count * 6), PRELIM_THREADS, pep_smem, st>>>(db->v, svq, bv, C.pmax, L.d_nlist.as<uint64_t>(),
-                                                                                                                         S->narrow_cta ? nv : WideIndexView{});
+    k_prelim_narrow<<<(unsigned)std::min<uint64_t>(C.nitems, (uint64_t)db->sm_count * PRELIM_CTAS), PRELIM_THREADS, pep_smem, st>>>(db->v, svq, bv, C.pmax, L.d_nlist.as<uint64_t>(),
+                                                                                                                         S->narrow_cta ? nv : NarrowIndexView{});
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(L.ev[8], st));   // narrow counting kernels done (the open-search kernel, when present, is timed with the replays)
     // narrow windows (<= NARROW_CAP peptides): 32-bit heap keys, half the shared memory
