@@ -4,7 +4,7 @@ import numpy as np
 
 from sage_b200 import Peptides, synth
 
-RT_CHUNK = 1024   # rt.cuh / ml_oracle.cpp
+RT_CHUNK = 1024   # rt.cuh / ml_oracle.cpp / ml_reference.py
 
 
 def peptides_from(seqs, mono=None) -> Peptides:
@@ -93,4 +93,51 @@ def cases():
     rows, fid = synth.make_rt_psms(cpep, 20_000, 3, seed=29, mobility=True)
     rows["charge"] = 2                                                                # one charge, one length: a collinear design; the
     out["collinear"] = _case(cpep, rows, fid, 3)                                      # m/z column is half the mass column, bit for bit
+    out.update(edge_cases())
+    return out
+
+
+def _all_targets(pep, n, n_files, seed, mobility=True):
+    """n rows, every one a target in training (q = 1/n <= 0.01 needs n >= 100)."""
+    rows, fid = synth.make_rt_psms(pep, n, n_files, seed=seed, mobility=mobility)
+    rows["label"] = 1
+    return rows, fid
+
+
+def edge_cases():
+    """Peptide lengths around the embedding's 32-lane stride, u8 charges, clamped predictions and targets, k_rt_predict's RT_TILE edges and a
+    single (peptide, file) training set."""
+    out = {}
+    rng = np.random.default_rng(31)
+    valid = np.array(list("ACDEFGHIKLMNPQRSTVWYUO"))
+    seqs = ["".join(rng.choice(valid, n)) for n in (31, 32, 33, 64, 65, 255) for _ in range(20)]
+    lpep = peptides_from(seqs, rng.uniform(3000.0, 30000.0, len(seqs)))
+    rows, fid = synth.make_rt_psms(lpep, 6000, 3, seed=32, mobility=True)
+    out["lengths_31_to_255"] = _case(lpep, rows, fid, 3)
+    pep = base_peptides()
+    rows, fid = synth.make_rt_psms(pep, 8000, 3, seed=33, mobility=True)
+    rows["charge"] = np.array([1, 255, 257])[np.arange(8000) % 3]                     # the low byte: 257 reads as 1
+    dec = rows["label"] == -1
+    rows["charge"][dec] = np.array([0, 256])[np.arange(int(dec.sum())) % 2]           # decoys (never trained on) at z = 0: 1/z and m/z inf
+    out["charges_u8"] = _case(pep, rows, fid, 3)
+    rows, fid = synth.make_rt_psms(pep, 4000, 3, seed=34, mobility=True)
+    rows["charge"] = np.array([0, 1, 255, 256, 257])[np.arange(4000) % 5]              # z = 0 among the training rows: the mobility fit fails
+    out["charges_zero_trained"] = _case(pep, rows, fid, 3)
+    rows, fid = synth.make_rt_psms(pep, 8000, 3, seed=35, mobility=True)
+    odd = np.nonzero(rows["label"] == -1)[0]
+    cpep = peptides_from([pep.sequence(i) for i in range(len(pep.mono))] + [a * 255 for a in "ACDEFGHIKLMNPQRSTVWYUO"] + ["G"],
+                         np.concatenate([pep.mono, np.full(22, 28000.0), [57.0]]))
+    rows["peptide_idx"][odd[1::2]] = len(pep.mono) + np.arange(len(odd[1::2])) % 23    # untrained outliers: predictions past both clamps
+    rows["ims"][np.nonzero(rows["label"] == 1)[0][::4]] *= 4.0                         # mobility targets past 2 and below 0
+    rows["ims"][np.nonzero(rows["label"] == 1)[0][1::9]] *= -1.0
+    out["clamps"] = _case(cpep, rows, fid, 3)
+    rows, fid = synth.make_rt_psms(pep, 4000, 3, seed=36, mobility=True)
+    rows["ims"][np.argsort(rows["poisson"])[5]] = np.nan                                # a NaN mobility target: NaN coefficients
+    out["ims_nan_target"] = _case(pep, rows, fid, 3)
+    for n in (127, 128, 129):                                                          # RT_TILE = 32 rows per k_rt_predict warp
+        out[f"predict_rows_{n}"] = _case(pep, *_all_targets(pep, n, 1, seed=n), 1)
+    rows, fid = _all_targets(pep, 150, 2, seed=37)
+    rows["peptide_idx"] = rows["peptide_idx"][0]
+    fid[:] = 1
+    out["one_segment"] = _case(pep, rows, fid, 2)                                      # one (peptide, file) pair: one matrix row, one entry
     return out

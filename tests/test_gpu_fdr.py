@@ -4,12 +4,15 @@ import ctypes
 import numpy as np
 import pytest
 
-from fdr_cases import cases, q_reference
+import ml_reference
+from fdr_cases import cases, kde_samples
+from ml_reference import q_reference
 from oracle_ml import ml_oracle
 from sage_b200 import Tolerance, api, synth
 
 pytestmark = pytest.mark.gpu
 KEYS = ("discriminant_score", "posterior_error", "spectrum_q", "order")
+RESTATED_ROWS = 100_000   # the numpy restatement (tests/ml_reference.py) is checked up to this size
 
 
 def same_bits(a, b):
@@ -38,6 +41,8 @@ def test_edge_workloads(name):
     rows, tol = c.pop("rows"), c.pop("tol")
     got = api.spectrum_fdr(rows, tol, **c)
     assert_same(got, ml_oracle.spectrum_fdr(rows, tol, **c), name)
+    if len(rows) <= RESTATED_ROWS:
+        assert_same(got, ml_reference.spectrum_fdr(rows, tol, **c), name + " (restatement)")
     if name in ("no_decoys", "no_targets", "nan_delta_next"):
         assert not got["lda_fitted"] and (got["posterior_error"] == 1.0).all()
     if name == "psms_100000":
@@ -78,6 +83,29 @@ def test_kde_build_hook(monotonic, bw):
     got = api.kde_build(s, d, 1000, monotonic, bw)
     want = ml_oracle.kde_build(s, d, 1000, monotonic, bw)
     assert same_bits(got[0], want[0]).all() and got[1:] == want[1:]
+
+
+@pytest.mark.parametrize("monotonic,bw", [(True, 1.0), (False, 2.0)])
+@pytest.mark.parametrize("sample", sorted(kde_samples()))
+def test_kde_build_samples(sample, monotonic, bw):
+    """Scores exactly on the 1000 bin points (min_score and max_score repeated), and one decoy (bandwidth 0): against the oracle and the
+    restatement."""
+    s, d = kde_samples()[sample]
+    got = api.kde_build(s, d, 1000, monotonic, bw)
+    for want in (ml_oracle.kde_build(s, d, 1000, monotonic, bw), ml_reference.kde_build(s, d, 1000, monotonic, lambda x: x * bw)):
+        assert same_bits(got[0], want[0]).all() and got[1:] == want[1:]
+
+
+def test_mass_bins_limit():
+    """A tolerance span of 2^24 - 1 mass-error bins runs and equals the oracle; 2^24 bins is refused with ELIMIT, Ppm and Da alike."""
+    rows = synth.make_psms(4, seed=42)
+    rows["label"] = [-1, 1, -1, 1]
+    tol = Tolerance.ppm(-8388608, 8388607)
+    assert_same(api.spectrum_fdr(rows, tol), ml_oracle.spectrum_fdr(rows, tol), "2^24 - 1 bins")
+    for tol in (Tolerance.ppm(-8388608, 8388608), Tolerance.da(0, 1 << 24), Tolerance.ppm(0, 1 << 30)):
+        with pytest.raises(api.SageB200Error) as e:
+            api.spectrum_fdr(rows, tol)
+        assert e.value.code == -5, tol
 
 
 def test_kde_build_all_scores_equal():

@@ -2,6 +2,7 @@
 import numpy as np
 import pytest
 
+import ml_reference
 from oracle_ml import ml_oracle
 from rt_cases import base_peptides, cases
 from sage_b200 import FeatureMap, IndexedDatabase, LfqSettings, Tolerance, api, synth
@@ -9,6 +10,7 @@ from sage_b200 import FeatureMap, IndexedDatabase, LfqSettings, Tolerance, api, 
 pytestmark = pytest.mark.gpu
 COLUMNS = ("aligned_rt", "predicted_rt", "delta_rt_model", "predicted_ims", "delta_ims_model", "spectrum_q")
 SCALARS = ("training_rows", "aligned_peptides", "rt_fitted", "rt_eps", "ims_fitted", "ims_eps")
+RESTATED_ROWS = 100_000   # the numpy restatement (tests/ml_reference.py) is checked up to this size
 
 
 def same_bits(a, b):
@@ -52,6 +54,8 @@ def test_edge_workloads(name):
     c = _CASES[name]
     got, want = run_both(c)
     assert_same(got, want, name)
+    if len(c["rows"]) <= RESTATED_ROWS:
+        assert_same(got, ml_reference.predict_rt(c["pep"], c["rows"], c["file_id"], c["n_files"]), name + " (restatement)")
     if name.startswith("train_"):
         assert got["training_rows"] == int(name.split("_")[1]) and got["rt_fitted"] and got["ims_fitted"]
     if name in ("no_training", "rows_1_files_1"):

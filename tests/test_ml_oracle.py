@@ -5,7 +5,7 @@ import subprocess
 
 import numpy as np
 
-from fdr_cases import q_reference
+from ml_reference import q_reference
 from oracle_ml import ml_oracle
 from sage_b200 import Tolerance, synth
 

@@ -1,12 +1,12 @@
 """CPU checks of the predict_rt oracle (oracle_ml/ml_oracle.cpp): the reference's own known answers (regression.rs, mobility_model.rs), the
 embedding quirks it keeps, global_alignment against a pure-Python restatement, the fit against numpy, and the C header against ctypes."""
 import ctypes as C
-import math
 import os
 import subprocess
 
 import numpy as np
 
+from ml_reference import py_alignment
 from oracle_ml import ml_oracle
 from rt_cases import base_peptides, peptides_from
 from sage_b200 import synth
@@ -60,69 +60,6 @@ def test_short_peptides_terminal_rules_and_groups():
     bulky = ml_oracle.rt_embed(1, "NOKGLVIFWY", 900.0, 2)
     assert bulky[91] == 4                                                    # N, O, K, G; none of L V I F W Y
     assert ml_oracle.rt_embed(1, "BJXZ", 900.0, 2)[0] == 4                    # letters outside VALID_AA land in A's column
-
-
-def py_alignment(rows, fid, n_files):
-    """retention_alignment.rs restated in Python floats, with the orders DESIGN.md §11 defines."""
-    key = rows["poisson"].view(np.int64)
-    key = key ^ ((key >> 63).astype(np.uint64) >> np.uint64(1)).astype(np.int64)
-    order = np.argsort(key, kind="stable")
-    dec, tar, qs = 1, 0, []
-    for r in order:
-        if rows["label"][r] == -1:
-            dec += 1
-        else:
-            tar += 1
-        qs.append(np.float32(dec) / np.float32(tar))
-    q = np.zeros(len(rows), np.float32)
-    qm = np.float32(1.0)
-    for p in range(len(order) - 1, -1, -1):
-        qm = min(qm, qs[p])
-        q[order[p]] = qm
-    max_rt = [0.0] * n_files
-    for i in range(len(rows)):
-        c = math.ceil(float(rows["rt"][i])) if not math.isnan(rows["rt"][i]) else 0
-        max_rt[fid[i]] = float(max(max_rt[fid[i]], min(max(c, 0), 2**32 - 1)))
-    mins = {}
-    for r in order:
-        if rows["label"][r] == 1 and q[r] <= np.float32(0.01):
-            k = (int(rows["peptide_idx"][r]), int(fid[r]))
-            x = float(rows["rt"][r])
-            mins[k] = x if k not in mins else (mins[k] if math.isnan(x) else (x if math.isnan(mins[k]) else min(mins[k], x)))
-    mat = []
-    for pep in sorted({p for p, _ in mins}):
-        v = [math.nan] * n_files
-        s, n = 0.0, 0.0
-        for f in sorted(f for p, f in mins if p == pep):
-            v[f] = mins[(pep, f)] / max_rt[f] if max_rt[f] else (math.copysign(math.inf, mins[(pep, f)]) if mins[(pep, f)] else math.nan)
-            s += v[f]
-            n += 1.0
-        m = s / n
-        if math.isfinite(m) and abs(m) >= 2.2250738585072014e-308:
-            mat.append(v)
-    means = []
-    for v in mat:
-        xs = [x for x in v if math.isfinite(x)]
-        means.append(sum(xs, 0.0) / len(xs))
-    out = []
-    for f in range(n_files):
-        n, dot, sx, sy = 0, 0.0, 0.0, 0.0
-        for v, y in zip(mat, means):
-            if math.isfinite(v[f]):
-                n, dot, sx, sy = n + 1, dot + v[f] * y, sx + v[f], sy + y
-        xm = sx / n if n else math.nan
-        ym = sy / n if n else math.nan
-        ssxy = dot - n * xm * ym
-        sx2 = 1e-8
-        for v in mat:
-            if math.isfinite(v[f]):
-                sx2 += (v[f] - xm) ** 2
-        slope = ssxy / sx2 if sx2 else math.nan
-        icpt = ym - slope * xm
-        slope = slope if math.isfinite(slope) else 1.0
-        icpt = icpt if math.isfinite(icpt) else 0.0
-        out.append((np.float32(max_rt[f]), np.float32(slope), np.float32(icpt)))
-    return out
 
 
 def test_alignment_against_python():
