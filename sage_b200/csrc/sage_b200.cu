@@ -60,10 +60,28 @@ static const float kResidueMass[26] = {71.03711f, 0.0f,      103.00919f, 115.026
                                        0.0f,      128.09496f, 113.08406f, 131.0405f,  114.04293f, 237.14774f, 97.05276f, 128.05858f, 156.1011f,
                                        87.03203f, 101.04768f, 150.95363f, 99.06841f,  186.07932f, 0.0f,       163.06332f, 0.0f};
 
+// Every entry point that takes a device: one must exist (there is no CPU fallback) and the index must name one; then it is selected.
+static int select_device(int device) {
+    int ndev = 0;
+    const cudaError_t e = cudaGetDeviceCount(&ndev);
+    if (e != cudaSuccess || ndev == 0) {
+        cudaGetLastError();
+        return fail(SAGE_B200_ECUDA, "no CUDA device available (%s): sage_b200 has no CPU fallback", e == cudaSuccess ? "device count 0" : cudaGetErrorString(e));
+    }
+    if (device < 0 || device >= ndev) return fail(SAGE_B200_EINVAL, "device %d out of range (0..%d)", device, ndev - 1);
+    CUDA_TRY(cudaSetDevice(device));
+    return 0;
+}
+
 // ------------------------------------------------------------------------------------------- device buffers
+// A growable buffer (25 % + 256 B of headroom) that lives as long as its owner.
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
     int reserve(size_t bytes) {
         if (bytes <= cap) return 0;
         if (p) cudaFree(p);
@@ -75,17 +93,16 @@ struct DevBuf {
         cap = want;
         return 0;
     }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
     template <class T>
     T* as() const { return reinterpret_cast<T*>(p); }
 };
 struct PinBuf {
     void* p = nullptr;
     size_t cap = 0;
+    PinBuf() = default;
+    PinBuf(const PinBuf&) = delete;
+    PinBuf& operator=(const PinBuf&) = delete;
+    ~PinBuf() { if (p) cudaFreeHost(p); }
     int reserve(size_t bytes) {
         if (bytes <= cap) return 0;
         if (p) cudaFreeHost(p);
@@ -97,11 +114,50 @@ struct PinBuf {
         cap = want;
         return 0;
     }
-    void release() {
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
+};
+
+// Exact-size device allocations freed together when the arena goes (the temporaries of one call, or arrays that live as long as their
+// owner), and one growable buffer for the temporary storage of cub's two-phase calls.
+struct DevArena {
+    std::vector<void*> ps;
+    uint64_t bytes = 0;
+    void* tmp = nullptr;
+    size_t tmp_bytes = 0;
+    DevArena() = default;
+    DevArena(const DevArena&) = delete;
+    DevArena& operator=(const DevArena&) = delete;
+    ~DevArena() { for (void* p : ps) cudaFree(p); }
+    template <class T>
+    cudaError_t alloc(T** out, size_t count) {
+        const size_t b = count ? count * sizeof(T) : 16;
+        void* p = nullptr;
+        cudaError_t e = cudaMalloc(&p, b);
+        if (e == cudaSuccess) { ps.push_back(p); bytes += b; *out = (T*)p; }
+        return e;
     }
+    // A larger request allocates a new buffer; the old one stays until the arena goes (work queued on a stream may still use it).
+    cudaError_t reserve_tmp(size_t b) {
+        if (tmp && b <= tmp_bytes) return cudaSuccess;
+        cudaError_t e = alloc((char**)&tmp, b);
+        if (e == cudaSuccess) tmp_bytes = b;
+        return e;
+    }
+};
+
+// The events that time the stages of one call.
+template <int N>
+struct StageEvents {
+    cudaEvent_t ev[N] = {};
+    StageEvents() = default;
+    StageEvents(const StageEvents&) = delete;
+    StageEvents& operator=(const StageEvents&) = delete;
+    ~StageEvents() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+    cudaError_t create() {
+        for (cudaEvent_t& e : ev)
+            if (cudaError_t r = cudaEventCreate(&e)) return r;
+        return cudaSuccess;
+    }
+    cudaEvent_t operator[](int i) const { return ev[i]; }
 };
 
 // Host -> device copy of a PAGEABLE array (a Rust Vec<f32>, a numpy array) through a pinned staging buffer: a few pool threads copy 2 MB pieces
@@ -306,16 +362,15 @@ static int db_upload_peptides(sage_b200_db* db, const sage_b200_peptides* P, con
     CUDA_TRY(cudaMemcpy(db->d_pep_missed, P->missed_cleavages, n, cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(db->d_ion_off, ion_off.data(), 4 * (n + 1), cudaMemcpyHostToDevice));
     // temporaries for ion generation
-    void *t_off = nullptr, *t_seq = nullptr, *t_mods = nullptr, *t_nterm = nullptr, *t_res = nullptr;
-    struct Temps {   // freed on every exit of this function
-        void **a, **b, **c, **d, **e;
-        ~Temps() { for (void** p : {a, b, c, d, e}) if (*p) cudaFree(*p); }
-    } temps{&t_off, &t_seq, &t_mods, &t_nterm, &t_res};
-    CUDA_TRY(cudaMalloc(&t_off, 4 * (n + 1) + 16));
-    CUDA_TRY(cudaMalloc(&t_seq, nres + 16));
-    CUDA_TRY(cudaMalloc(&t_mods, 4 * nres + 16));
-    CUDA_TRY(cudaMalloc(&t_nterm, 4 * n + 16));
-    CUDA_TRY(cudaMalloc(&t_res, sizeof kResidueMass));
+    DevArena A;
+    uint32_t* t_off = nullptr;
+    uint8_t* t_seq = nullptr;
+    float *t_mods = nullptr, *t_nterm = nullptr, *t_res = nullptr;
+    CUDA_TRY(A.alloc(&t_off, n + 5));
+    CUDA_TRY(A.alloc(&t_seq, nres + 16));
+    CUDA_TRY(A.alloc(&t_mods, nres + 4));
+    CUDA_TRY(A.alloc(&t_nterm, n + 4));
+    CUDA_TRY(A.alloc(&t_res, sizeof kResidueMass / sizeof(float)));
     if (n) {
         CUDA_TRY(cudaMemcpy(t_off, P->residue_offsets, 4 * (n + 1), cudaMemcpyHostToDevice));
         CUDA_TRY(cudaMemcpy(t_seq, P->sequence, nres, cudaMemcpyHostToDevice));
@@ -330,27 +385,23 @@ static int db_upload_peptides(sage_b200_db* db, const sage_b200_peptides* P, con
     db->v.ion_off = (const uint32_t*)db->d_ion_off;
     db->v.ions = (const float*)db->d_ions;
     if (n) {
-        k_build_ions<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, (const uint32_t*)t_off, (const uint8_t*)t_seq, (const float*)t_mods,
-                                                           (const float*)t_nterm, (const float*)db->d_pep_mono, (const uint32_t*)db->d_ion_off,
-                                                           (uint32_t)n_kinds, db->v, (float*)db->d_ions, (const float*)t_res);
+        k_build_ions<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, t_off, t_seq, t_mods, t_nterm, (const float*)db->d_pep_mono, (const uint32_t*)db->d_ion_off,
+                                                           (uint32_t)n_kinds, db->v, (float*)db->d_ions, t_res);
         CUDA_TRY(cudaGetLastError());
     }
     CUDA_TRY(cudaDeviceSynchronize());
     return 0;
 }
 
-static int db_new(int device, sage_b200_db** out) {
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0)
-        return fail(SAGE_B200_ECUDA, "no CUDA device available (%s): sage_b200 has no CPU fallback", e == cudaSuccess ? "device count 0" : cudaGetErrorString(e));
-    if (device < 0 || device >= ndev) return fail(SAGE_B200_EINVAL, "device %d out of range (0..%d)", device, ndev - 1);
-    CUDA_TRY(cudaSetDevice(device));
-    sage_b200_db* db = new sage_b200_db();
-    db->device = device;
+// A db under construction: destroyed unless released to the caller.
+using DbGuard = std::unique_ptr<sage_b200_db, void (*)(sage_b200_db*)>;
+
+static int db_new(int device, DbGuard& out) {
+    if (int rc = select_device(device)) return rc;
+    out.reset(new sage_b200_db());
+    out->device = device;
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) db->sm_count = prop.multiProcessorCount;
-    *out = db;
+    if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) out->sm_count = prop.multiProcessorCount;
     return 0;
 }
 
@@ -414,13 +465,13 @@ static int db_build_directories(sage_b200_db* db) {
     const float pw = (pe[1] - pe[0]) / (float)PEP_LUT_CELLS;
     bool plut_ok = pe[0] > 0.0f && std::isfinite(pe[1]) && pw > 0.0f && pw < 3.0e38f;
     if (plut_ok) {   // only for a table the reference's binary search is well defined on: ascending, positive, finite
+        DevArena A;
         uint32_t* d_bad = nullptr;
         uint32_t h_bad = 1;
-        CUDA_TRY(cudaMalloc(&d_bad, 4));
+        CUDA_TRY(A.alloc(&d_bad, 1));
         cudaMemset(d_bad, 0, 4);
         k_check_ascending<<<(v.n_pep + 255) / 256, 256>>>(v.n_pep, (const float*)db->d_pep_mono, d_bad);
         cudaMemcpy(&h_bad, d_bad, 4, cudaMemcpyDeviceToHost);
-        cudaFree(d_bad);
         plut_ok = h_bad == 0;
     }
     if (plut_ok) {
@@ -442,32 +493,31 @@ extern "C" int sage_b200_db_create(const sage_b200_peptides* peptides, const sag
     if (index->n_fragments && (!index->fragment_peptide || !index->fragment_mz || !index->bucket_min)) return fail(SAGE_B200_EINVAL, "index: null array");
     const uint64_t nb_expect = (index->n_fragments + index->bucket_size - 1) / index->bucket_size;
     if (index->n_buckets != nb_expect) return fail(SAGE_B200_EINVAL, "n_buckets %llu != ceil(n_fragments/bucket_size) %llu", (unsigned long long)index->n_buckets, (unsigned long long)nb_expect);
-    sage_b200_db* db = nullptr;
-    int rc = db_new(device, &db);
-    if (rc) return rc;
-    if ((rc = db_upload_peptides(db, peptides, index->ion_kinds, index->n_ion_kinds))) { sage_b200_db_destroy(db); return rc; }
+    DbGuard guard(nullptr, sage_b200_db_destroy);
+    if (int rc = db_new(device, guard)) return rc;
+    sage_b200_db* db = guard.get();
+    if (int rc = db_upload_peptides(db, peptides, index->ion_kinds, index->n_ion_kinds)) return rc;
     const uint64_t nf = index->n_fragments;
     db->v.n_frag = nf;
     db->v.n_bucket = (uint32_t)index->n_buckets;
     db->v.bucket_size = (uint32_t)index->bucket_size;
-    if ((rc = dmalloc(db, &db->d_frag, 8 * nf + 64))) { sage_b200_db_destroy(db); return rc; }
-    if ((rc = dmalloc(db, &db->d_bucket_min, 4 * index->n_buckets))) { sage_b200_db_destroy(db); return rc; }
-    void *t_pep = nullptr, *t_mz = nullptr;
-    auto cleanup = [&]() { if (t_pep) cudaFree(t_pep); if (t_mz) cudaFree(t_mz); };
-    if (nf) {
-        if (cudaMalloc(&t_pep, 4 * nf) != cudaSuccess || cudaMalloc(&t_mz, 4 * nf) != cudaSuccess) { cleanup(); sage_b200_db_destroy(db); return fail(SAGE_B200_ECUDA, "cudaMalloc of upload temporaries failed"); }
-        cudaError_t ce = cudaMemcpy(t_pep, index->fragment_peptide, 4 * nf, cudaMemcpyHostToDevice);
-        if (ce == cudaSuccess) ce = cudaMemcpy(t_mz, index->fragment_mz, 4 * nf, cudaMemcpyHostToDevice);
-        if (ce == cudaSuccess) ce = cudaMemcpy(db->d_bucket_min, index->bucket_min, 4 * index->n_buckets, cudaMemcpyHostToDevice);
-        if (ce != cudaSuccess) {   // these errors are not sticky: a later synchronize would not report them and the index would be garbage
-            cleanup(); sage_b200_db_destroy(db);
-            return fail(SAGE_B200_ECUDA, "index upload failed: %s", cudaGetErrorString(ce));
+    if (int rc = dmalloc(db, &db->d_frag, 8 * nf + 64)) return rc;
+    if (int rc = dmalloc(db, &db->d_bucket_min, 4 * index->n_buckets)) return rc;
+    {
+        DevArena A;
+        if (nf) {
+            uint32_t* t_pep = nullptr;
+            float* t_mz = nullptr;
+            CUDA_TRY(A.alloc(&t_pep, nf));
+            CUDA_TRY(A.alloc(&t_mz, nf));
+            // these errors are not sticky: a later synchronize would not report them and the index would be garbage
+            CUDA_TRY(cudaMemcpy(t_pep, index->fragment_peptide, 4 * nf, cudaMemcpyHostToDevice));
+            CUDA_TRY(cudaMemcpy(t_mz, index->fragment_mz, 4 * nf, cudaMemcpyHostToDevice));
+            CUDA_TRY(cudaMemcpy(db->d_bucket_min, index->bucket_min, 4 * index->n_buckets, cudaMemcpyHostToDevice));
+            k_pack_fragments_soa<<<(unsigned)((nf + 255) / 256), 256>>>(nf, t_pep, t_mz, (uint2*)db->d_frag);
         }
-        k_pack_fragments_soa<<<(unsigned)((nf + 255) / 256), 256>>>(nf, (const uint32_t*)t_pep, (const float*)t_mz, (uint2*)db->d_frag);
+        CUDA_TRY(cudaDeviceSynchronize());
     }
-    cudaError_t e = cudaDeviceSynchronize();
-    cleanup();
-    if (e != cudaSuccess) { sage_b200_db_destroy(db); return fail(SAGE_B200_ECUDA, "index upload failed: %s", cudaGetErrorString(e)); }
     db->v.frag = (const uint2*)db->d_frag;
     db->v.bucket_min = (const float*)db->d_bucket_min;
     // IndexedDatabase does not carry min_ion_index (it lives in Parameters, database.rs:128): infer it from the fragment count and
@@ -486,24 +536,23 @@ extern "C" int sage_b200_db_create(const sage_b200_peptides* peptides, const sag
             if (tot == nf) found = (int)m;
             if (tot < nf) break;
         }
-        if (found >= 0) {
-            void *acc = nullptr, *mis = nullptr;
+        if (found >= 0) {   // any failure here only leaves the peptide-centric path off
+            DevArena A;
+            uint32_t *acc = nullptr, *mis = nullptr;
             uint32_t mismatch = 1;
-            if (cudaMalloc(&acc, 8 * n) == cudaSuccess && cudaMalloc(&mis, 4) == cudaSuccess && cudaMemset(acc, 0, 8 * n) == cudaSuccess &&
+            if (A.alloc(&acc, 2 * n) == cudaSuccess && A.alloc(&mis, 1) == cudaSuccess && cudaMemset(acc, 0, 8 * n) == cudaSuccess &&
                 cudaMemset(mis, 0, 4) == cudaSuccess) {
-                k_index_signature<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, (uint32_t)n, (uint32_t*)acc);
+                k_index_signature<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, (uint32_t)n, acc);
                 k_index_verify<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, db->v.pep_len, db->v.ion_off, db->v.ions, db->v.n_kinds, db->v, (uint32_t)found,
-                                                                    (const uint32_t*)acc, (uint32_t*)mis);
+                                                                    acc, mis);
                 if (cudaMemcpy(&mismatch, mis, 4, cudaMemcpyDeviceToHost) != cudaSuccess) mismatch = 1;
             }
-            if (acc) cudaFree(acc);
-            if (mis) cudaFree(mis);
             cudaGetLastError();
             if (mismatch == 0) { db->v.min_ion_index = (uint32_t)found; db->v.pep_centric_ok = 1; }
         }
     }
-    if ((rc = db_build_directories(db))) { sage_b200_db_destroy(db); return rc; }
-    *out = db;
+    if (int rc = db_build_directories(db)) return rc;
+    *out = guard.release();
     return 0;
 }
 
@@ -512,10 +561,10 @@ extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t b
     if (!out || !peptides || !ion_kinds) return fail(SAGE_B200_EINVAL, "db_build: null argument");
     if (bucket_size == 0 || (bucket_size & (bucket_size - 1)) || bucket_size > (1ull << 30))
         return fail(SAGE_B200_EINVAL, "bucket_size must be a power of two (Builder::make_parameters rounds up, database.rs:97)");
-    sage_b200_db* db = nullptr;
-    int rc = db_new(device, &db);
-    if (rc) return rc;
-    if ((rc = db_upload_peptides(db, peptides, ion_kinds, n_ion_kinds))) { sage_b200_db_destroy(db); return rc; }
+    DbGuard guard(nullptr, sage_b200_db_destroy);
+    if (int rc = db_new(device, guard)) return rc;
+    sage_b200_db* db = guard.get();
+    if (int rc = db_upload_peptides(db, peptides, ion_kinds, n_ion_kinds)) return rc;
     const uint64_t n = peptides->n_peptides;
     // fragments kept per peptide: n_kinds * max(0, L-1-min_ion_index)   (database.rs:281-291)
     std::vector<uint64_t> frag_off(n + 1);
@@ -529,56 +578,57 @@ extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t b
     frag_off[n] = nf;
     const uint32_t shift = ceil_log2_u64(bucket_size);
     const uint64_t nb = (nf + bucket_size - 1) / bucket_size;
-    if (nb > 0xFFFFFFFFull) { sage_b200_db_destroy(db); return fail(SAGE_B200_ELIMIT, "too many buckets"); }
+    if (nb > 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "too many buckets");
     db->v.n_frag = nf;
     db->v.n_bucket = (uint32_t)nb;
     db->v.bucket_size = (uint32_t)bucket_size;
     db->v.min_ion_index = (uint32_t)std::min<uint64_t>(min_ion_index, 0xFFFFFFFFull);
     db->v.pep_centric_ok = 1;  // the index is generated from the ion table with this filter by construction
-    if ((rc = dmalloc(db, &db->d_frag, 8 * nf + 64))) { sage_b200_db_destroy(db); return rc; }
-    if ((rc = dmalloc(db, &db->d_bucket_min, 4 * nb))) { sage_b200_db_destroy(db); return rc; }
+    if (int rc = dmalloc(db, &db->d_frag, 8 * nf + 64)) return rc;
+    if (int rc = dmalloc(db, &db->d_bucket_min, 4 * nb)) return rc;
     db->v.frag = (const uint2*)db->d_frag;
     db->v.bucket_min = (const float*)db->d_bucket_min;
-    if (nf == 0) { *out = db; return 0; }
+    if (nf == 0) { *out = guard.release(); return 0; }
 
-    void *d_off = nullptr, *k32a = nullptr, *k32b = nullptr, *pa = nullptr, *pb = nullptr, *k64a = nullptr, *k64b = nullptr, *mza = nullptr, *mzb = nullptr, *tmp = nullptr;
-    auto cleanup = [&]() { for (void* p : {d_off, k32a, k32b, pa, pb, k64a, k64b, mza, mzb, tmp}) if (p) cudaFree(p); };
-#define TRY_BUILD(expr)                                                                                                    \
-    do {                                                                                                                   \
-        cudaError_t _e = (expr);                                                                                           \
-        if (_e != cudaSuccess) { cleanup(); sage_b200_db_destroy(db); return fail(SAGE_B200_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); } \
-    } while (0)
-    TRY_BUILD(cudaMalloc(&d_off, 8 * (n + 1)));
-    TRY_BUILD(cudaMemcpy(d_off, frag_off.data(), 8 * (n + 1), cudaMemcpyHostToDevice));
-    TRY_BUILD(cudaMalloc(&k32a, 4 * nf)); TRY_BUILD(cudaMalloc(&k32b, 4 * nf));
-    TRY_BUILD(cudaMalloc(&pa, 4 * nf)); TRY_BUILD(cudaMalloc(&pb, 4 * nf));
-    k_gen_fragments<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, db->v.pep_len, db->v.ion_off, db->v.ions, db->v.n_kinds, db->v, (uint32_t)std::min<uint64_t>(min_ion_index, 0xFFFFFFFFull),
-                                                          nullptr, (const uint64_t*)d_off, (uint32_t*)k32a, (uint32_t*)pa);
-    TRY_BUILD(cudaGetLastError());
-    // (1) stable LSD radix sort by fragment m/z (par_sort_unstable_by fragment_mz, database.rs:301; ties keep PeptideIx order)
-    size_t tb = 0;
-    if (nf > 0x7FFFFFFFull) { cleanup(); sage_b200_db_destroy(db); return fail(SAGE_B200_ELIMIT, "more than 2^31 fragments: sort in slabs not implemented"); }
-    TRY_BUILD(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint32_t*)k32a, (uint32_t*)k32b, (const uint32_t*)pa, (uint32_t*)pb, (int)nf));
-    TRY_BUILD(cudaMalloc(&tmp, tb + 16));
-    TRY_BUILD(cub::DeviceRadixSort::SortPairs(tmp, tb, (const uint32_t*)k32a, (uint32_t*)k32b, (const uint32_t*)pa, (uint32_t*)pb, (int)nf));
-    cudaFree(tmp); tmp = nullptr;
-    cudaFree(k32a); k32a = nullptr; cudaFree(pa); pa = nullptr;
-    // (2) bucket minima + (bucket, PeptideIx) keys, then a stable sort inside buckets (database.rs:337-346)
-    TRY_BUILD(cudaMalloc(&k64a, 8 * nf)); TRY_BUILD(cudaMalloc(&k64b, 8 * nf));
-    TRY_BUILD(cudaMalloc(&mza, 4 * nf)); TRY_BUILD(cudaMalloc(&mzb, 4 * nf));
-    k_bucket_keys<<<(unsigned)((nf + 255) / 256), 256>>>(nf, shift, (const uint32_t*)k32b, (const uint32_t*)pb, (uint64_t*)k64a, (uint32_t*)mza, (float*)db->d_bucket_min);
-    TRY_BUILD(cudaGetLastError());
-    const int end_bit = std::min<int>(64, 32 + (int)ceil_log2_u64(nb + 1) + 1);
-    TRY_BUILD(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)k64a, (uint64_t*)k64b, (const uint32_t*)mza, (uint32_t*)mzb, (int)nf, 0, end_bit));
-    TRY_BUILD(cudaMalloc(&tmp, tb + 16));
-    TRY_BUILD(cub::DeviceRadixSort::SortPairs(tmp, tb, (const uint64_t*)k64a, (uint64_t*)k64b, (const uint32_t*)mza, (uint32_t*)mzb, (int)nf, 0, end_bit));
-    k_pack_fragments<<<(unsigned)((nf + 255) / 256), 256>>>(nf, (const uint64_t*)k64b, (const uint32_t*)mzb, (uint2*)db->d_frag);
-    TRY_BUILD(cudaGetLastError());
-    TRY_BUILD(cudaDeviceSynchronize());
-    cleanup();
-#undef TRY_BUILD
-    if ((rc = db_build_directories(db))) { sage_b200_db_destroy(db); return rc; }
-    *out = db;
+    {
+        DevArena A;   // freed before the directories are built
+        uint32_t *k32b = nullptr, *pb = nullptr;
+        CUDA_TRY(A.alloc(&k32b, nf)); CUDA_TRY(A.alloc(&pb, nf));
+        {   // (1) stable LSD radix sort by fragment m/z (par_sort_unstable_by fragment_mz, database.rs:301; ties keep PeptideIx order); its
+            // inputs are freed before step (2) allocates
+            DevArena S;
+            uint64_t* d_off = nullptr;
+            uint32_t *k32a = nullptr, *pa = nullptr;
+            CUDA_TRY(S.alloc(&d_off, n + 1));
+            CUDA_TRY(cudaMemcpy(d_off, frag_off.data(), 8 * (n + 1), cudaMemcpyHostToDevice));
+            CUDA_TRY(S.alloc(&k32a, nf)); CUDA_TRY(S.alloc(&pa, nf));
+            k_gen_fragments<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, db->v.pep_len, db->v.ion_off, db->v.ions, db->v.n_kinds, db->v, (uint32_t)std::min<uint64_t>(min_ion_index, 0xFFFFFFFFull),
+                                                                  nullptr, d_off, k32a, pa);
+            CUDA_TRY(cudaGetLastError());
+            if (nf > 0x7FFFFFFFull) return fail(SAGE_B200_ELIMIT, "more than 2^31 fragments: sort in slabs not implemented");
+            size_t tb = 0;
+            CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint32_t*)k32a, k32b, (const uint32_t*)pa, pb, (int)nf));
+            CUDA_TRY(S.reserve_tmp(tb + 16));
+            CUDA_TRY(cub::DeviceRadixSort::SortPairs(S.tmp, tb, (const uint32_t*)k32a, k32b, (const uint32_t*)pa, pb, (int)nf));
+        }
+        // (2) bucket minima + (bucket, PeptideIx) keys, then a stable sort inside buckets (database.rs:337-346)
+        uint64_t *k64a = nullptr, *k64b = nullptr;
+        uint32_t *mza = nullptr, *mzb = nullptr;
+        CUDA_TRY(A.alloc(&k64a, nf)); CUDA_TRY(A.alloc(&k64b, nf));
+        CUDA_TRY(A.alloc(&mza, nf)); CUDA_TRY(A.alloc(&mzb, nf));
+        k_bucket_keys<<<(unsigned)((nf + 255) / 256), 256>>>(nf, shift, k32b, pb, k64a, mza, (float*)db->d_bucket_min);
+        CUDA_TRY(cudaGetLastError());
+        const int end_bit = std::min<int>(64, 32 + (int)ceil_log2_u64(nb + 1) + 1);
+        size_t tb = 0;
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)k64a, k64b, (const uint32_t*)mza, mzb, (int)nf, 0, end_bit));
+        CUDA_TRY(A.reserve_tmp(tb + 16));
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, (const uint64_t*)k64a, k64b, (const uint32_t*)mza, mzb, (int)nf, 0, end_bit));
+        k_pack_fragments<<<(unsigned)((nf + 255) / 256), 256>>>(nf, k64b, mzb, (uint2*)db->d_frag);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaDeviceSynchronize());
+    }
+    if (int rc = db_build_directories(db)) return rc;
+    *out = guard.release();
     return 0;
 }
 
@@ -598,43 +648,44 @@ extern "C" int sage_b200_db_export_index(const sage_b200_db* db, uint32_t* fragm
     CUDA_TRY(cudaSetDevice(db->device));
     const uint64_t nf = db->v.n_frag;
     if (nf && (fragment_peptide || fragment_mz)) {
-        void *t_pep = nullptr, *t_mz = nullptr;
-        CUDA_TRY(cudaMalloc(&t_pep, 4 * nf));
-        CUDA_TRY(cudaMalloc(&t_mz, 4 * nf));
-        k_unpack_fragments<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, (uint32_t*)t_pep, (float*)t_mz);
-        cudaError_t e = cudaDeviceSynchronize();
-        if (e == cudaSuccess && fragment_peptide) e = cudaMemcpy(fragment_peptide, t_pep, 4 * nf, cudaMemcpyDeviceToHost);
-        if (e == cudaSuccess && fragment_mz) e = cudaMemcpy(fragment_mz, t_mz, 4 * nf, cudaMemcpyDeviceToHost);
-        cudaFree(t_pep); cudaFree(t_mz);
-        if (e != cudaSuccess) return fail(SAGE_B200_ECUDA, "export failed: %s", cudaGetErrorString(e));
+        DevArena A;
+        uint32_t* t_pep = nullptr;
+        float* t_mz = nullptr;
+        CUDA_TRY(A.alloc(&t_pep, nf));
+        CUDA_TRY(A.alloc(&t_mz, nf));
+        k_unpack_fragments<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, t_pep, t_mz);
+        CUDA_TRY(cudaDeviceSynchronize());
+        if (fragment_peptide) CUDA_TRY(cudaMemcpy(fragment_peptide, t_pep, 4 * nf, cudaMemcpyDeviceToHost));
+        if (fragment_mz) CUDA_TRY(cudaMemcpy(fragment_mz, t_mz, 4 * nf, cudaMemcpyDeviceToHost));
     }
     if (bucket_min && db->v.n_bucket) CUDA_TRY(cudaMemcpy(bucket_min, db->d_bucket_min, 4ull * db->v.n_bucket, cudaMemcpyDeviceToHost));
     return 0;
 }
 
 // Both block-major copies of the fragments start alike: fragments keyed by (PeptideIx / block, m/z), one LSD radix sort, block offsets, and
-// the m/z range of the index. On success *keys / *peps hold the sorted keys and PeptideIx (freed by the caller, as is everything in `tmp`).
-static bool sort_block_major(const sage_b200_db* db, uint32_t block, uint32_t n_block, uint64_t* blk_off, void** keys, void** peps, void* (&tmp)[4],
+// the m/z range of the index. On success *keys / *peps hold the sorted keys and PeptideIx; every temporary is in A.
+static bool sort_block_major(const sage_b200_db* db, DevArena& A, uint32_t block, uint32_t n_block, uint64_t* blk_off, uint64_t** keys, uint32_t** peps,
                              float& lo, float& hi) {
     const uint64_t nf = db->v.n_frag;
     if (nf > 0x7FFFFFFFull) return false;
-    void *&k_a = tmp[0], *&p_a = tmp[1], *&sort_tmp = tmp[2], *&d_rng = tmp[3];
-    if (cudaMalloc(&k_a, 8 * nf) != cudaSuccess || cudaMalloc(keys, 8 * nf) != cudaSuccess || cudaMalloc(&p_a, 4 * nf) != cudaSuccess ||
-        cudaMalloc(peps, 4 * nf) != cudaSuccess || cudaMalloc(&d_rng, 8) != cudaSuccess)
+    uint64_t* k_a = nullptr;
+    uint32_t *p_a = nullptr, *d_rng = nullptr;
+    if (A.alloc(&k_a, nf) != cudaSuccess || A.alloc(keys, nf) != cudaSuccess || A.alloc(&p_a, nf) != cudaSuccess || A.alloc(peps, nf) != cudaSuccess ||
+        A.alloc(&d_rng, 2) != cudaSuccess)
         return false;
-    k_wide_keys<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, block, (uint64_t*)k_a, (uint32_t*)p_a);
+    k_wide_keys<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, block, k_a, p_a);
     int nb_bits = 1;
     while (nb_bits < 32 && (n_block >> nb_bits)) nb_bits++;
     size_t tb = 0;
-    if (cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)k_a, (uint64_t*)*keys, (const uint32_t*)p_a, (uint32_t*)*peps, (int)nf, 0, 32 + nb_bits) != cudaSuccess ||
-        cudaMalloc(&sort_tmp, tb + 16) != cudaSuccess ||
-        cub::DeviceRadixSort::SortPairs(sort_tmp, tb, (const uint64_t*)k_a, (uint64_t*)*keys, (const uint32_t*)p_a, (uint32_t*)*peps, (int)nf, 0, 32 + nb_bits) != cudaSuccess)
+    if (cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)k_a, *keys, (const uint32_t*)p_a, *peps, (int)nf, 0, 32 + nb_bits) != cudaSuccess ||
+        A.reserve_tmp(tb + 16) != cudaSuccess ||
+        cub::DeviceRadixSort::SortPairs(A.tmp, tb, (const uint64_t*)k_a, *keys, (const uint32_t*)p_a, *peps, (int)nf, 0, 32 + nb_bits) != cudaSuccess)
         return false;
-    k_wide_block_offsets<<<(n_block + 1 + 255) / 256, 256>>>(nf, (const uint64_t*)*keys, n_block, blk_off);
+    k_wide_block_offsets<<<(n_block + 1 + 255) / 256, 256>>>(nf, *keys, n_block, blk_off);
     // m/z range of the index (positive floats order like their bit patterns)
     const uint32_t rng0[2] = {0xFFFFFFFFu, 0u};
     if (cudaMemcpy(d_rng, rng0, 8, cudaMemcpyHostToDevice) != cudaSuccess) return false;
-    k_frag_mz_range<<<(unsigned)std::min<uint64_t>((nf + 255) / 256, 4096), 256>>>(nf, db->v.frag, (uint32_t*)d_rng);
+    k_frag_mz_range<<<(unsigned)std::min<uint64_t>((nf + 255) / 256, 4096), 256>>>(nf, db->v.frag, d_rng);
     uint32_t rng[2];
     if (cudaMemcpy(rng, d_rng, 8, cudaMemcpyDeviceToHost) != cudaSuccess) return false;
     memcpy(&lo, &rng[0], 4); memcpy(&hi, &rng[1], 4);
@@ -659,9 +710,10 @@ static WideIndexView build_wide_index(const sage_b200_db* db, BlockIndexSlot<Wid
     if (slot.failed || block == 0 || db->v.n_frag == 0 || db->v.n_pep == 0) return WideIndexView{};
     const uint64_t nf = db->v.n_frag;
     slot.retire();   // a rebuild with another block size (tests, scorers with very different tolerances): see BlockIndexSlot::retire
-    void *keys = nullptr, *peps = nullptr, *tmp[4] = {};
-    auto cleanup = [&]() { for (void* p : {keys, peps, tmp[0], tmp[1], tmp[2], tmp[3]}) if (p) cudaFree(p); };
-    auto give_up = [&]() { cleanup(); slot.free_current(); cudaGetLastError(); slot.failed = 1; return WideIndexView{}; };
+    DevArena A;
+    uint64_t* keys = nullptr;
+    uint32_t* peps = nullptr;
+    auto give_up = [&]() { slot.free_current(); cudaGetLastError(); slot.failed = 1; return WideIndexView{}; };
     const uint32_t n_block = (db->v.n_pep + block - 1) / block;
     while (cells > 256 && (uint64_t)n_block * (cells + 1) * 4 > (1024ull << 20)) cells >>= 1;   // at most 1 GB of LUT
     void *&d_frag = slot.d[0], *&d_blk = slot.d[1], *&d_lut = slot.d[2];
@@ -669,8 +721,8 @@ static WideIndexView build_wide_index(const sage_b200_db* db, BlockIndexSlot<Wid
         cudaMalloc(&d_lut, 4 * (size_t)n_block * (cells + 1)) != cudaSuccess)
         return give_up();
     float lo, hi;
-    if (!sort_block_major(db, block, n_block, (uint64_t*)d_blk, &keys, &peps, tmp, lo, hi)) return give_up();
-    k_wide_pack<<<(unsigned)((nf + 255) / 256), 256>>>(nf, (const uint64_t*)keys, (const uint32_t*)peps, (uint2*)d_frag);
+    if (!sort_block_major(db, A, block, n_block, (uint64_t*)d_blk, &keys, &peps, lo, hi)) return give_up();
+    k_wide_pack<<<(unsigned)((nf + 255) / 256), 256>>>(nf, keys, peps, (uint2*)d_frag);
     WideIndexView w{};
     w.frag = (const uint2*)d_frag; w.blk_off = (const uint64_t*)d_blk; w.lut = (const uint32_t*)d_lut;
     w.block = block; w.n_block = n_block;
@@ -680,7 +732,6 @@ static WideIndexView build_wide_index(const sage_b200_db* db, BlockIndexSlot<Wid
         k_wide_lut<<<(unsigned)((total + 255) / 256), 256>>>(w, (uint32_t*)d_lut);
     } else if (cudaMemset(d_lut, 0, 4 * (size_t)n_block * (cells + 1)) != cudaSuccess) return give_up();   // degenerate range: every walk starts at the block start
     if (cudaDeviceSynchronize() != cudaSuccess) return give_up();
-    cleanup();
     slot.v = w;
     slot.bytes = 8 * nf + 8 * ((uint64_t)n_block + 1) + 4ull * n_block * (cells + 1);
     return w;
@@ -719,9 +770,10 @@ static NarrowIndexView db_narrow_index(const sage_b200_db* db, uint32_t block, b
     if (slot.failed || block == 0 || block > 65536 || db->v.n_frag == 0 || db->v.n_pep == 0) return NarrowIndexView{};
     const uint64_t nf = db->v.n_frag;
     slot.retire();
-    void *keys = nullptr, *peps = nullptr, *tmp[4] = {};
-    auto cleanup = [&]() { for (void* p : {keys, peps, tmp[0], tmp[1], tmp[2], tmp[3]}) if (p) cudaFree(p); };
-    auto give_up = [&]() { cleanup(); slot.free_current(); cudaGetLastError(); slot.failed = 1; return NarrowIndexView{}; };
+    DevArena A;
+    uint64_t* keys = nullptr;
+    uint32_t* peps = nullptr;
+    auto give_up = [&]() { slot.free_current(); cudaGetLastError(); slot.failed = 1; return NarrowIndexView{}; };
     const uint32_t n_block = (db->v.n_pep + block - 1) / block;
     const uint32_t cells = narrow_dir_cells(nf, n_block), ngrp = cells / NARROW_GROUP;
     void *&d_mz = slot.d[0], *&d_pep = slot.d[1], *&d_blk = slot.d[2], *&d_dir = slot.d[3], *&d_grp = slot.d[4];
@@ -730,8 +782,8 @@ static NarrowIndexView db_narrow_index(const sage_b200_db* db, uint32_t block, b
         cudaMalloc(&d_grp, 4 * (size_t)n_block * ngrp) != cudaSuccess)
         return give_up();
     float lo, hi;
-    if (!sort_block_major(db, block, n_block, (uint64_t*)d_blk, &keys, &peps, tmp, lo, hi)) return give_up();
-    k_narrow_pack<<<(unsigned)((nf + 255) / 256), 256>>>(nf, (const uint64_t*)keys, (const uint32_t*)peps, block, (float*)d_mz, (uint16_t*)d_pep);
+    if (!sort_block_major(db, A, block, n_block, (uint64_t*)d_blk, &keys, &peps, lo, hi)) return give_up();
+    k_narrow_pack<<<(unsigned)((nf + 255) / 256), 256>>>(nf, keys, peps, block, (float*)d_mz, (uint16_t*)d_pep);
     NarrowIndexView v{};
     v.mz = (const float*)d_mz; v.pep = (const uint16_t*)d_pep; v.blk_off = (const uint64_t*)d_blk; v.dir = (const uint16_t*)d_dir;
     v.grp = (const uint32_t*)d_grp; v.block = block; v.n_block = n_block;
@@ -739,7 +791,6 @@ static NarrowIndexView db_narrow_index(const sage_b200_db* db, uint32_t block, b
     const uint64_t total = (uint64_t)n_block * cells;
     k_narrow_dir<<<(unsigned)((total + 255) / 256), 256>>>(v, (uint16_t*)d_dir, (uint32_t*)d_grp);
     if (cudaDeviceSynchronize() != cudaSuccess) return give_up();
-    cleanup();
     slot.v = v;
     slot.bytes = 6 * nf + 128 + 8 * ((uint64_t)n_block + 1) + 2 * total + 4ull * n_block * ngrp;
     return v;
@@ -867,9 +918,6 @@ struct Lane {
     char stager_msg[256] = {0};
     void release() {
         if (stager.joinable()) stager.join();
-        for (DevBuf* b : {&d_small, &d_masses, &d_intens, &d_queries, &d_hits, &d_keys, &d_features, &d_counts, &d_counters, &d_dbgk, &d_dbgm, &d_sort, &d_sorttmp,
-                          &d_wlist, &d_wslots, &d_witems, &d_citems, &d_nlist, &d_nslots, &d_frags, &d_cand, &d_meta, &d_recs, &d_hkey, &d_emit, &d_hitk, &d_hiti, &d_hitt}) b->release();
-        for (PinBuf* b : {&h_small, &h_masses, &h_intens, &h_features, &h_counts, &h_counters}) b->release();
         for (auto& e : ev) if (e) cudaEventDestroy(e);
         if (ev_masses) cudaEventDestroy(ev_masses);
         if (ev_intens) cudaEventDestroy(ev_intens);
@@ -922,7 +970,7 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
     if (p->precursor_tol.kind < 0 || p->precursor_tol.kind > 2 || p->fragment_tol.kind < 0 || p->fragment_tol.kind > 2) return fail(SAGE_B200_EINVAL, "bad tolerance kind");
     if (p->score_type > 1) return fail(SAGE_B200_EINVAL, "bad score_type");
     CUDA_TRY(cudaSetDevice(db->device));
-    { int rc_attr = ensure_kernel_attributes(db->device); if (rc_attr) return rc_attr; }
+    if (int rc = ensure_kernel_attributes(db->device)) return rc;
     sage_b200_scorer* s = new sage_b200_scorer();
     s->db = db;
     s->device = db->device;
@@ -957,8 +1005,7 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
             const double x = (double)n;
             tab[n] = x * std::log(x) - x + 0.5 * std::log(x) + 0.5 * std::log(3.14159265358979323846 * 2.0 * x);
         }
-        int rc2 = s->d_lnfact.reserve(8 * N);
-        if (rc2) { delete s; return rc2; }
+        if (int rc = s->d_lnfact.reserve(8 * N)) { delete s; return rc; }
         CUDA_TRY(cudaMemcpy(s->d_lnfact.p, tab.data(), 8 * N, cudaMemcpyHostToDevice));
         v.lnfact_tab = s->d_lnfact.as<double>();
         v.lnfact_n = N;
@@ -1047,8 +1094,6 @@ extern "C" void sage_b200_scorer_destroy(sage_b200_scorer* s) {
     cudaSetDevice(s->device);
     for (Lane& L : s->lanes) L.release();
     if (s->ev_base) cudaEventDestroy(s->ev_base);
-    s->d_lnfact.release();
-    s->d_keep.release();
     delete s;
 }
 
@@ -1060,16 +1105,13 @@ static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static int narrow_block_for(sage_b200_scorer* S) {
     if (S->narrow_block_auto) return 0;
     const uint32_t samples = 4096;
+    DevArena A;
     unsigned long long* d_sum = nullptr;
     unsigned long long sum = 0;
-    CUDA_TRY(cudaMalloc(&d_sum, 8));
-    cudaError_t e = cudaMemset(d_sum, 0, 8);
-    if (e == cudaSuccess) {
-        k_window_sample<<<(samples + 255) / 256, 256>>>(S->db->v, S->sv.precursor_tol, samples, d_sum);
-        e = cudaMemcpy(&sum, d_sum, 8, cudaMemcpyDeviceToHost);
-    }
-    cudaFree(d_sum);
-    if (e != cudaSuccess) return fail(SAGE_B200_ECUDA, "window sampling failed: %s", cudaGetErrorString(e));
+    CUDA_TRY(A.alloc(&d_sum, 1));
+    CUDA_TRY(cudaMemset(d_sum, 0, 8));
+    k_window_sample<<<(samples + 255) / 256, 256>>>(S->db->v, S->sv.precursor_tol, samples, d_sum);
+    CUDA_TRY(cudaMemcpy(&sum, d_sum, 8, cudaMemcpyDeviceToHost));
     const double avg = (double)sum / samples;
     uint32_t block = 128;
     while (block < 4096 && (double)block < avg) block <<= 1;
@@ -1893,10 +1935,7 @@ extern "C" int64_t sage_b200_initial_hits(sage_b200_scorer* S, const sage_b200_s
 extern "C" int sage_b200_process_spectra(int device, const sage_b200_processor_params* pr, const sage_b200_raw_spectra* raw, uint64_t* out_peak_offsets,
                                          float* out_masses, float* out_intensities, float* out_tic) {
     if (!pr || !raw || !out_peak_offsets || !out_tic) return fail(SAGE_B200_EINVAL, "process_spectra: null argument");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(SAGE_B200_ECUDA, "no CUDA device available: sage_b200 has no CPU fallback");
-    if (device < 0 || device >= ndev) return fail(SAGE_B200_EINVAL, "device out of range");
-    CUDA_TRY(cudaSetDevice(device));
+    if (int rc = select_device(device)) return rc;
     cudaGetLastError();   // a stale non-sticky error left by another user of the runtime must not be blamed on the launches below
     const uint64_t n = raw->n;
     out_peak_offsets[0] = 0;
@@ -1916,26 +1955,24 @@ extern "C" int sage_b200_process_spectra(int device, const sage_b200_processor_p
     while (p2 < pmax) p2 <<= 1;
     const size_t smem = (size_t)p2 * 12 + (size_t)pmax * (5 * 4 + 2) + 32;
     if (smem > 200 * 1024) return fail(SAGE_B200_ELIMIT, "spectrum with %u raw peaks exceeds the shared-memory budget of the preprocessing kernel", pmax);
-    void *d_off = nullptr, *d_mz = nullptr, *d_int = nullptr, *d_chg = nullptr, *d_om = nullptr, *d_oi = nullptr, *d_cnt = nullptr, *d_tic = nullptr;
-    auto cleanup = [&]() { for (void* p : {d_off, d_mz, d_int, d_chg, d_om, d_oi, d_cnt, d_tic}) if (p) cudaFree(p); };
-#define TRY_P(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { cleanup(); return fail(SAGE_B200_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); } } while (0)
-    TRY_P(cudaMalloc(&d_off, 4 * (n + 1))); TRY_P(cudaMalloc(&d_mz, 4 * npk + 16)); TRY_P(cudaMalloc(&d_int, 4 * npk + 16)); TRY_P(cudaMalloc(&d_chg, n));
-    TRY_P(cudaMalloc(&d_om, 4 * npk + 16)); TRY_P(cudaMalloc(&d_oi, 4 * npk + 16)); TRY_P(cudaMalloc(&d_cnt, 4 * n)); TRY_P(cudaMalloc(&d_tic, 4 * n));
-    TRY_P(cudaMemcpy(d_off, off.data(), 4 * (n + 1), cudaMemcpyHostToDevice));
-    if (npk) { TRY_P(cudaMemcpy(d_mz, raw->mz + pk0, 4 * npk, cudaMemcpyHostToDevice)); TRY_P(cudaMemcpy(d_int, raw->intensity + pk0, 4 * npk, cudaMemcpyHostToDevice)); }
-    TRY_P(cudaMemcpy(d_chg, raw->precursor_charge, n, cudaMemcpyHostToDevice));
+    DevArena A;
+    uint32_t *d_off = nullptr, *d_cnt = nullptr;
+    float *d_mz = nullptr, *d_int = nullptr, *d_om = nullptr, *d_oi = nullptr, *d_tic = nullptr;
+    uint8_t* d_chg = nullptr;
+    CUDA_TRY(A.alloc(&d_off, n + 1)); CUDA_TRY(A.alloc(&d_mz, npk + 4)); CUDA_TRY(A.alloc(&d_int, npk + 4)); CUDA_TRY(A.alloc(&d_chg, n));
+    CUDA_TRY(A.alloc(&d_om, npk + 4)); CUDA_TRY(A.alloc(&d_oi, npk + 4)); CUDA_TRY(A.alloc(&d_cnt, n)); CUDA_TRY(A.alloc(&d_tic, n));
+    CUDA_TRY(cudaMemcpy(d_off, off.data(), 4 * (n + 1), cudaMemcpyHostToDevice));
+    if (npk) { CUDA_TRY(cudaMemcpy(d_mz, raw->mz + pk0, 4 * npk, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(d_int, raw->intensity + pk0, 4 * npk, cudaMemcpyHostToDevice)); }
+    CUDA_TRY(cudaMemcpy(d_chg, raw->precursor_charge, n, cudaMemcpyHostToDevice));
     ProcParams pp{(uint32_t)std::min<uint64_t>(pr->take_top_n, 0xFFFFFFFFull), pr->deisotope ? 1u : 0u, pr->min_deisotope_mz};
-    { int rc_attr = ensure_kernel_attributes(device); if (rc_attr) { cleanup(); return rc_attr; } }
-    k_process_ms2<<<(unsigned)n, 32, smem>>>(pp, (uint32_t)n, (const uint32_t*)d_off, (const float*)d_mz, (const float*)d_int, (const uint8_t*)d_chg, pmax, p2,
-                                            (float*)d_om, (float*)d_oi, (uint32_t*)d_cnt, (float*)d_tic);
-    TRY_P(cudaGetLastError());
+    if (int rc = ensure_kernel_attributes(device)) return rc;
+    k_process_ms2<<<(unsigned)n, 32, smem>>>(pp, (uint32_t)n, d_off, d_mz, d_int, d_chg, pmax, p2, d_om, d_oi, d_cnt, d_tic);
+    CUDA_TRY(cudaGetLastError());
     std::vector<uint32_t> cnt(n);
     std::vector<float> om(npk), oi(npk);
-    TRY_P(cudaMemcpy(cnt.data(), d_cnt, 4 * n, cudaMemcpyDeviceToHost));
-    TRY_P(cudaMemcpy(out_tic, d_tic, 4 * n, cudaMemcpyDeviceToHost));
-    if (npk) { TRY_P(cudaMemcpy(om.data(), d_om, 4 * npk, cudaMemcpyDeviceToHost)); TRY_P(cudaMemcpy(oi.data(), d_oi, 4 * npk, cudaMemcpyDeviceToHost)); }
-#undef TRY_P
-    cleanup();
+    CUDA_TRY(cudaMemcpy(cnt.data(), d_cnt, 4 * n, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(out_tic, d_tic, 4 * n, cudaMemcpyDeviceToHost));
+    if (npk) { CUDA_TRY(cudaMemcpy(om.data(), d_om, 4 * npk, cudaMemcpyDeviceToHost)); CUDA_TRY(cudaMemcpy(oi.data(), d_oi, 4 * npk, cudaMemcpyDeviceToHost)); }
     uint64_t w = 0;   // compact: spectrum i keeps cnt[i] <= raw count peaks
     for (uint64_t i = 0; i < n; i++) {
         memcpy(out_masses + w, om.data() + off[i], 4 * (size_t)cnt[i]);
@@ -1951,31 +1988,26 @@ extern "C" int sage_b200_find_reporter_ions(int device, uint64_t n, const uint64
                                             uint64_t n_labels, sage_b200_tolerance label_tolerance, float* out) {
     if (n == 0 || n_labels == 0) return 0;
     if (!peak_offsets || !labels || !out) return fail(SAGE_B200_EINVAL, "find_reporter_ions: null argument");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(SAGE_B200_ECUDA, "no CUDA device available: sage_b200 has no CPU fallback");
-    if (device < 0 || device >= ndev) return fail(SAGE_B200_EINVAL, "device out of range");
+    if (int rc = select_device(device)) return rc;
     if (label_tolerance.kind < 0 || label_tolerance.kind > 2) return fail(SAGE_B200_EINVAL, "bad tolerance kind");
-    CUDA_TRY(cudaSetDevice(device));
     const uint64_t pk0 = peak_offsets[0], npk = peak_offsets[n] - pk0;
     if (npk && (!masses || !intensities)) return fail(SAGE_B200_EINVAL, "find_reporter_ions: null peak arrays");
     if (n > 0x7FFFFFFFull || npk > 0xFFFFFFF0ull || n_labels > 4096) return fail(SAGE_B200_ELIMIT, "find_reporter_ions: batch too large");
     std::vector<uint32_t> off(n + 1);
     for (uint64_t i = 0; i <= n; i++) off[i] = (uint32_t)(peak_offsets[i] - pk0);
-    void *d_off = nullptr, *d_m = nullptr, *d_i = nullptr, *d_l = nullptr, *d_o = nullptr;
-    auto cleanup = [&]() { for (void* p : {d_off, d_m, d_i, d_l, d_o}) if (p) cudaFree(p); };
-#define TRY_R(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { cleanup(); return fail(SAGE_B200_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); } } while (0)
-    TRY_R(cudaMalloc(&d_off, 4 * (n + 1))); TRY_R(cudaMalloc(&d_m, 4 * npk + 16)); TRY_R(cudaMalloc(&d_i, 4 * npk + 16));
-    TRY_R(cudaMalloc(&d_l, 4 * n_labels)); TRY_R(cudaMalloc(&d_o, 4 * n * n_labels));
-    TRY_R(cudaMemcpy(d_off, off.data(), 4 * (n + 1), cudaMemcpyHostToDevice));
-    if (npk) { TRY_R(cudaMemcpy(d_m, masses + pk0, 4 * npk, cudaMemcpyHostToDevice)); TRY_R(cudaMemcpy(d_i, intensities + pk0, 4 * npk, cudaMemcpyHostToDevice)); }
-    TRY_R(cudaMemcpy(d_l, labels, 4 * n_labels, cudaMemcpyHostToDevice));
+    DevArena A;
+    uint32_t* d_off = nullptr;
+    float *d_m = nullptr, *d_i = nullptr, *d_l = nullptr, *d_o = nullptr;
+    CUDA_TRY(A.alloc(&d_off, n + 1)); CUDA_TRY(A.alloc(&d_m, npk + 4)); CUDA_TRY(A.alloc(&d_i, npk + 4));
+    CUDA_TRY(A.alloc(&d_l, n_labels)); CUDA_TRY(A.alloc(&d_o, n * n_labels));
+    CUDA_TRY(cudaMemcpy(d_off, off.data(), 4 * (n + 1), cudaMemcpyHostToDevice));
+    if (npk) { CUDA_TRY(cudaMemcpy(d_m, masses + pk0, 4 * npk, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(d_i, intensities + pk0, 4 * npk, cudaMemcpyHostToDevice)); }
+    CUDA_TRY(cudaMemcpy(d_l, labels, 4 * n_labels, cudaMemcpyHostToDevice));
     const uint64_t total = n * n_labels;
-    k_find_reporter_ions<<<(unsigned)((total + 255) / 256), 256>>>((uint32_t)n, (uint32_t)n_labels, (const uint32_t*)d_off, (const float*)d_m, (const float*)d_i,
-                                                                  (const float*)d_l, Tol{label_tolerance.kind, label_tolerance.lo, label_tolerance.hi}, (float*)d_o);
-    TRY_R(cudaGetLastError());
-    TRY_R(cudaMemcpy(out, d_o, 4 * total, cudaMemcpyDeviceToHost));
-#undef TRY_R
-    cleanup();
+    k_find_reporter_ions<<<(unsigned)((total + 255) / 256), 256>>>((uint32_t)n, (uint32_t)n_labels, d_off, d_m, d_i, d_l,
+                                                                  Tol{label_tolerance.kind, label_tolerance.lo, label_tolerance.hi}, d_o);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpy(out, d_o, 4 * total, cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -1986,20 +2018,14 @@ __global__ void k_device_log(int variant, const double* x, uint64_t n, double* o
 extern "C" int sage_b200_device_log(int device, int variant, const double* x, uint64_t n, double* out) {
     if (n == 0) return 0;
     if (!x || !out || variant < 0 || variant > 2) return fail(SAGE_B200_EINVAL, "device_log: bad argument");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(SAGE_B200_ECUDA, "no CUDA device available: sage_b200 has no CPU fallback");
-    if (device < 0 || device >= ndev) return fail(SAGE_B200_EINVAL, "device out of range");
-    CUDA_TRY(cudaSetDevice(device));
+    if (int rc = select_device(device)) return rc;
+    DevArena A;
     double *dx = nullptr, *dy = nullptr;
-    CUDA_TRY(cudaMalloc(&dx, 8 * n));
-    if (cudaMalloc(&dy, 8 * n) != cudaSuccess) { cudaFree(dx); return fail(SAGE_B200_ECUDA, "device_log: cudaMalloc failed"); }
-    cudaError_t e = cudaMemcpy(dx, x, 8 * n, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        k_device_log<<<(unsigned)((n + 255) / 256), 256>>>(variant, dx, n, dy);
-        e = cudaMemcpy(out, dy, 8 * n, cudaMemcpyDeviceToHost);
-    }
-    cudaFree(dx); cudaFree(dy);
-    if (e != cudaSuccess) return fail(SAGE_B200_ECUDA, "device_log failed: %s", cudaGetErrorString(e));
+    CUDA_TRY(A.alloc(&dx, n));
+    CUDA_TRY(A.alloc(&dy, n));
+    CUDA_TRY(cudaMemcpy(dx, x, 8 * n, cudaMemcpyHostToDevice));
+    k_device_log<<<(unsigned)((n + 255) / 256), 256>>>(variant, dx, n, dy);
+    CUDA_TRY(cudaMemcpy(out, dy, 8 * n, cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -2083,9 +2109,13 @@ struct sage_b200_lfq {
     sage_b200_lfq_params p{};
     uint32_t n_files = 0, n_charges = 0;
     uint64_t n_slots = 0, n_ranges = 0, n_pages = 0, n_grids = 0;
-    void *d_ranges = nullptr, *d_grid_of = nullptr, *d_min_rts = nullptr, *d_slot_dist = nullptr, *d_slot_file = nullptr, *d_grids = nullptr,
-         *d_touched = nullptr, *d_align = nullptr, *d_consts = nullptr;
-    uint64_t fixed_bytes = 0;
+    DevArena fixed;   // the arrays below, exact-size
+    sage_b200_lfq_range* d_ranges = nullptr;
+    uint32_t *d_grid_of = nullptr, *d_slot_file = nullptr;
+    float *d_min_rts = nullptr, *d_slot_dist = nullptr;
+    double *d_grids = nullptr, *d_consts = nullptr;
+    uint8_t* d_touched = nullptr;
+    sage_b200_alignment* d_align = nullptr;
     std::vector<uint32_t> slot_pep;   // slot -> PeptideIx, ascending
     DevBuf sp_off, sp_mass, sp_int, sp_mob, sp_file, sp_sst, counts, offsets, cell[2], value[2], tmp, ids, o_present, o_rt, o_sa, o_score, o_areas;
     cudaStream_t st = nullptr;
@@ -2099,12 +2129,6 @@ struct sage_b200_lfq {
         return b;
     }
 };
-
-static int lfq_malloc(sage_b200_lfq* L, void** p, size_t bytes) {
-    CUDA_TRY(cudaMalloc(p, bytes ? bytes : 16));
-    L->fixed_bytes += bytes ? bytes : 16;
-    return 0;
-}
 
 // composition (mass.rs:78-116): carbon and sulfur count of one residue
 static void residue_composition(uint8_t aa, uint16_t& c, uint16_t& s) {
@@ -2129,11 +2153,6 @@ static int lfq_elapsed(sage_b200_lfq* L, float& ms) {
 extern "C" void sage_b200_lfq_destroy(sage_b200_lfq* L) {
     if (!L) return;
     cudaSetDevice(L->device);
-    for (void* p : {L->d_ranges, L->d_grid_of, L->d_min_rts, L->d_slot_dist, L->d_slot_file, L->d_grids, L->d_touched, L->d_align, L->d_consts})
-        if (p) cudaFree(p);
-    for (DevBuf* d : {&L->sp_off, &L->sp_mass, &L->sp_int, &L->sp_mob, &L->sp_file, &L->sp_sst, &L->counts, &L->offsets, &L->cell[0], &L->cell[1], &L->value[0],
-                      &L->value[1], &L->tmp, &L->ids, &L->o_present, &L->o_rt, &L->o_sa, &L->o_score, &L->o_areas})
-        d->release();
     for (cudaEvent_t e : L->ev)
         if (e) cudaEventDestroy(e);
     if (L->st) cudaStreamDestroy(L->st);
@@ -2145,68 +2164,53 @@ static int lfq_build(sage_b200_lfq* L, const sage_b200_db* db, const sage_b200_p
     cudaStream_t st = L->st;
     CUDA_TRY(cudaEventRecord(L->ev[0], st));
     // per-peptide first kept row (lfq.rs:100-131)
-    DevBuf d_rows[7], d_first, d_flag, d_slots, d_nsel, d_cs, d_exp;
+    DevArena A;
+    uint32_t *d_rows[7] = {}, *d_first = nullptr, *d_slots = nullptr, *d_nsel = nullptr;   // d_rows: the feature columns, 4 bytes per row each
+    uint8_t* d_flag = nullptr;
     const void* src[7] = {F->peptide_idx, F->peptide_q, F->label, F->aligned_rt, F->calcmass, F->file_id, F->ims};
-    auto cleanup = [&]() {
-        for (auto& d : d_rows) d.release();
-        for (DevBuf* d : {&d_first, &d_flag, &d_slots, &d_nsel, &d_cs, &d_exp}) d->release();
-    };
-    int rc = 0;
-#define LFQ_TRY(expr)                                                                                                          \
-    do {                                                                                                                       \
-        cudaError_t _e = (expr);                                                                                               \
-        if (_e != cudaSuccess) { cleanup(); return fail(SAGE_B200_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); }   \
-    } while (0)
-#define LFQ_RC(expr)              \
-    do {                          \
-        if ((rc = (expr)) != 0) { \
-            cleanup();            \
-            return rc;            \
-        }                         \
-    } while (0)
     for (int k = 0; k < 7; k++) {
-        LFQ_RC(d_rows[k].reserve(4 * n + 16));
-        if (n) LFQ_TRY(cudaMemcpyAsync(d_rows[k].p, src[k], 4 * n, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(A.alloc(&d_rows[k], n + 4));
+        if (n) CUDA_TRY(cudaMemcpyAsync(d_rows[k], src[k], 4 * n, cudaMemcpyHostToDevice, st));
     }
-    LFQ_RC(d_first.reserve(4 * n_pep + 16));
-    LFQ_RC(d_flag.reserve(n_pep + 16));
-    LFQ_RC(d_slots.reserve(4 * n_pep + 16));
-    LFQ_RC(d_nsel.reserve(16));
-    LFQ_TRY(cudaMemsetAsync(d_first.p, 0xFF, 4 * n_pep, st));
+    CUDA_TRY(A.alloc(&d_first, n_pep + 4));
+    CUDA_TRY(A.alloc(&d_flag, n_pep + 16));
+    CUDA_TRY(A.alloc(&d_slots, n_pep + 4));
+    CUDA_TRY(A.alloc(&d_nsel, 4));
+    CUDA_TRY(cudaMemsetAsync(d_first, 0xFF, 4 * n_pep, st));
     if (n)
-        k_lfq_first_row<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, d_rows[0].as<uint32_t>(), d_rows[1].as<float>(), d_rows[2].as<int32_t>(),
-                                                                       L->p.peptide_q_value, d_first.as<uint32_t>());
-    if (n_pep) k_lfq_flag<<<(unsigned)((n_pep + 255) / 256), 256, 0, st>>>(n_pep, d_first.as<uint32_t>(), d_flag.as<uint8_t>());
-    LFQ_TRY(cudaGetLastError());
+        k_lfq_first_row<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, d_rows[0], (const float*)d_rows[1], (const int32_t*)d_rows[2], L->p.peptide_q_value,
+                                                                       d_first);
+    if (n_pep) k_lfq_flag<<<(unsigned)((n_pep + 255) / 256), 256, 0, st>>>(n_pep, d_first, d_flag);
+    CUDA_TRY(cudaGetLastError());
     {
         size_t tb = 0;
         thrust::counting_iterator<uint32_t> it(0);
-        LFQ_TRY(cub::DeviceSelect::Flagged(nullptr, tb, it, d_flag.as<uint8_t>(), d_slots.as<uint32_t>(), d_nsel.as<uint32_t>(), (int)n_pep, st));
-        LFQ_RC(L->tmp.reserve(tb));
-        LFQ_TRY(cub::DeviceSelect::Flagged(L->tmp.p, tb, it, d_flag.as<uint8_t>(), d_slots.as<uint32_t>(), d_nsel.as<uint32_t>(), (int)n_pep, st));
+        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, it, d_flag, d_slots, d_nsel, (int)n_pep, st));
+        if (int rc = L->tmp.reserve(tb)) return rc;
+        CUDA_TRY(cub::DeviceSelect::Flagged(L->tmp.p, tb, it, d_flag, d_slots, d_nsel, (int)n_pep, st));
     }
     uint32_t n_slots = 0;
-    LFQ_TRY(cudaMemcpyAsync(&n_slots, d_nsel.p, 4, cudaMemcpyDeviceToHost, st));
-    LFQ_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaMemcpyAsync(&n_slots, d_nsel, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     std::vector<uint32_t> slot_pep(n_slots);
-    if (n_slots) LFQ_TRY(cudaMemcpyAsync(slot_pep.data(), d_slots.p, 4ull * n_slots, cudaMemcpyDeviceToHost, st));
-    LFQ_TRY(cudaStreamSynchronize(st));
+    if (n_slots) CUDA_TRY(cudaMemcpyAsync(slot_pep.data(), d_slots, 4ull * n_slots, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
 
     L->n_slots = n_slots;
     L->slot_pep = slot_pep;
     L->n_ranges = (uint64_t)n_slots * L->n_charges * LFQ_ISO * 2;
     L->n_pages = (L->n_ranges + LFQ_PAGE - 1) / LFQ_PAGE;
     L->n_grids = (uint64_t)n_slots * (L->p.combine_charge_states ? 1 : L->n_charges) * 2;
-    if (L->n_ranges > 0x7FFFFFFFull) { cleanup(); return fail(SAGE_B200_ELIMIT, "%llu precursor ranges exceed 2^31", (unsigned long long)L->n_ranges); }
+    if (L->n_ranges > 0x7FFFFFFFull) return fail(SAGE_B200_ELIMIT, "%llu precursor ranges exceed 2^31", (unsigned long long)L->n_ranges);
     const uint64_t cells = L->n_grids * L->n_files * LFQ_ISO * LFQ_GRID, grid_bytes = 8 * cells;
     {
         size_t free_b = 0, total_b = 0;
-        LFQ_TRY(cudaMemGetInfo(&free_b, &total_b));
+        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
         // the grids plus the map, leaving room for the tracing and integration scratch
         const uint64_t need = grid_bytes + L->n_grids + 40 * L->n_ranges + (1ull << 28);
         if (need > (uint64_t)free_b)
-            { cleanup(); return fail(SAGE_B200_ELIMIT, "LFQ grids need %llu bytes of device memory (%llu grids x %u files x 300 f64) but %llu are free",
-                                     (unsigned long long)need, (unsigned long long)L->n_grids, L->n_files, (unsigned long long)free_b); }
+            return fail(SAGE_B200_ELIMIT, "LFQ grids need %llu bytes of device memory (%llu grids x %u files x 300 f64) but %llu are free",
+                        (unsigned long long)need, (unsigned long long)L->n_grids, L->n_files, (unsigned long long)free_b);
     }
 
     // isotope distributions: composition on the host, peptide_isotopes on the device with host-libm exp tables
@@ -2249,86 +2253,66 @@ static int lfq_build(sage_b200_lfq* L, const sage_b200_db* db, const sage_b200_p
         for (int rt = 0; rt < LFQ_GRID; rt++) consts[LFQ_K_WIDTH + rt] = std::pow(1.0 - ((double)std::abs(rt - center) / (double)center), 0.33);
     }
 
-    LFQ_RC(lfq_malloc(L, &L->d_ranges, sizeof(sage_b200_lfq_range) * L->n_ranges));
-    LFQ_RC(lfq_malloc(L, &L->d_grid_of, 4 * L->n_ranges));
-    LFQ_RC(lfq_malloc(L, &L->d_min_rts, 4 * L->n_pages));
-    LFQ_RC(lfq_malloc(L, &L->d_slot_dist, 12ull * n_slots));
-    LFQ_RC(lfq_malloc(L, &L->d_slot_file, 4ull * n_slots));
-    LFQ_RC(lfq_malloc(L, &L->d_touched, L->n_grids));
-    LFQ_RC(lfq_malloc(L, &L->d_align, sizeof(sage_b200_alignment) * L->n_files));
-    LFQ_RC(lfq_malloc(L, &L->d_consts, sizeof consts));
-    LFQ_RC(lfq_malloc(L, &L->d_grids, grid_bytes));
-    LFQ_TRY(cudaMemsetAsync(L->d_grids, 0, grid_bytes, st));
-    LFQ_TRY(cudaMemsetAsync(L->d_touched, 0, L->n_grids, st));
-    LFQ_TRY(cudaMemcpyAsync(L->d_align, align, sizeof(sage_b200_alignment) * L->n_files, cudaMemcpyHostToDevice, st));
-    LFQ_TRY(cudaMemcpyAsync(L->d_consts, consts, sizeof consts, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(L->fixed.alloc(&L->d_ranges, L->n_ranges));
+    CUDA_TRY(L->fixed.alloc(&L->d_grid_of, L->n_ranges));
+    CUDA_TRY(L->fixed.alloc(&L->d_min_rts, L->n_pages));
+    CUDA_TRY(L->fixed.alloc(&L->d_slot_dist, 3ull * n_slots));
+    CUDA_TRY(L->fixed.alloc(&L->d_slot_file, n_slots));
+    CUDA_TRY(L->fixed.alloc(&L->d_touched, L->n_grids));
+    CUDA_TRY(L->fixed.alloc(&L->d_align, L->n_files));
+    CUDA_TRY(L->fixed.alloc(&L->d_consts, LFQ_K_WIDTH + LFQ_GRID));
+    CUDA_TRY(L->fixed.alloc(&L->d_grids, cells));
+    CUDA_TRY(cudaMemsetAsync(L->d_grids, 0, grid_bytes, st));
+    CUDA_TRY(cudaMemsetAsync(L->d_touched, 0, L->n_grids, st));
+    CUDA_TRY(cudaMemcpyAsync(L->d_align, align, sizeof(sage_b200_alignment) * L->n_files, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(L->d_consts, consts, sizeof consts, cudaMemcpyHostToDevice, st));
     if (n_slots) {
-        LFQ_RC(d_cs.reserve(4ull * n_slots));
-        LFQ_RC(d_exp.reserve(4 * expt.size()));
-        LFQ_TRY(cudaMemcpyAsync(d_cs.p, carbon.data(), 2ull * n_slots, cudaMemcpyHostToDevice, st));
-        LFQ_TRY(cudaMemcpyAsync(d_cs.as<uint16_t>() + n_slots, sulfur.data(), 2ull * n_slots, cudaMemcpyHostToDevice, st));
-        LFQ_TRY(cudaMemcpyAsync(d_exp.p, expt.data(), 4 * expt.size(), cudaMemcpyHostToDevice, st));
-        k_lfq_isotopes<<<(n_slots + 255) / 256, 256, 0, st>>>(n_slots, d_cs.as<uint16_t>(), d_cs.as<uint16_t>() + n_slots, d_exp.as<float>(),
-                                                             d_exp.as<float>() + max_c + 1, d_exp.as<float>() + max_c + 1 + max_s + 1, (float*)L->d_slot_dist);
-        LFQ_TRY(cudaGetLastError());
+        uint16_t* d_cs = nullptr;
+        float* d_exp = nullptr;
+        CUDA_TRY(A.alloc(&d_cs, 2ull * n_slots));
+        CUDA_TRY(A.alloc(&d_exp, expt.size()));
+        CUDA_TRY(cudaMemcpyAsync(d_cs, carbon.data(), 2ull * n_slots, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_cs + n_slots, sulfur.data(), 2ull * n_slots, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_exp, expt.data(), 4 * expt.size(), cudaMemcpyHostToDevice, st));
+        k_lfq_isotopes<<<(n_slots + 255) / 256, 256, 0, st>>>(n_slots, d_cs, d_cs + n_slots, d_exp, d_exp + max_c + 1, d_exp + max_c + 1 + max_s + 1, L->d_slot_dist);
+        CUDA_TRY(cudaGetLastError());
 
         // expansion, stable RT sort, stable per-page mass_lo sort (lfq.rs:134-184)
         const uint32_t nr = (uint32_t)L->n_ranges, nt = (uint32_t)(n_slots * L->n_charges * LFQ_ISO);
-        DevBuf pre, k32[2], v32[2], k64;
-        auto cleanup2 = [&]() {
-            for (DevBuf* d : {&pre, &k32[0], &k32[1], &v32[0], &v32[1], &k64}) d->release();
-        };
-        int rc2 = 0;
-        if (!rc2) rc2 = pre.reserve(sizeof(sage_b200_lfq_range) * nr);
-        for (int k = 0; k < 2 && !rc2; k++) rc2 = k32[k].reserve(4ull * nr) || v32[k].reserve(4ull * nr);
-        if (!rc2) rc2 = k64.reserve(8ull * nr);
-        if (rc2) { cleanup2(); cleanup(); return SAGE_B200_ECUDA; }
+        DevArena B;   // freed before the call returns
+        sage_b200_lfq_range* pre = nullptr;
+        uint32_t *k32[2] = {}, *v32[2] = {};
+        uint64_t *k64 = nullptr, *k64o = nullptr;
+        CUDA_TRY(B.alloc(&pre, nr));
+        for (int k = 0; k < 2; k++) {
+            CUDA_TRY(B.alloc(&k32[k], nr));
+            CUDA_TRY(B.alloc(&v32[k], nr));
+        }
+        CUDA_TRY(B.alloc(&k64, nr));
         k_lfq_expand<<<(nt + 255) / 256, 256, 0, st>>>(n_slots, L->n_charges, L->p.min_precursor_charge, L->p.ppm_tolerance, L->p.mobility_pct_tolerance,
-                                                      d_slots.as<uint32_t>(), d_first.as<uint32_t>(), d_rows[3].as<float>(), d_rows[4].as<float>(),
-                                                      d_rows[5].as<uint32_t>(), d_rows[6].as<float>(), pre.as<sage_b200_lfq_range>(), k32[0].as<uint32_t>(),
-                                                      v32[0].as<uint32_t>(), (uint32_t*)L->d_slot_file);
-        cudaError_t e = cudaGetLastError();
+                                                      d_slots, d_first, (const float*)d_rows[3], (const float*)d_rows[4], d_rows[5], (const float*)d_rows[6], pre,
+                                                      k32[0], v32[0], L->d_slot_file);
+        CUDA_TRY(cudaGetLastError());
         size_t tb = 0, tb2 = 0;
-        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, tb, k32[0].as<uint32_t>(), k32[1].as<uint32_t>(), v32[0].as<uint32_t>(),
-                                                                  v32[1].as<uint32_t>(), (int)nr, 0, 32, st);
-        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, tb2, k64.as<uint64_t>(), k64.as<uint64_t>(), v32[1].as<uint32_t>(),
-                                                                  v32[0].as<uint32_t>(), (int)nr, 0, 64, st);
-        if (e == cudaSuccess && L->tmp.reserve(std::max(tb, tb2))) e = cudaErrorMemoryAllocation;
-        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(L->tmp.p, tb, k32[0].as<uint32_t>(), k32[1].as<uint32_t>(), v32[0].as<uint32_t>(),
-                                                                  v32[1].as<uint32_t>(), (int)nr, 0, 32, st);
-        if (e == cudaSuccess) {
-            k_lfq_page_keys<<<(nr + 255) / 256, 256, 0, st>>>(nr, v32[1].as<uint32_t>(), pre.as<sage_b200_lfq_range>(), k64.as<uint64_t>(), (float*)L->d_min_rts);
-            e = cudaGetLastError();
-        }
-        DevBuf k64o;
-        if (e == cudaSuccess && k64o.reserve(8ull * nr)) e = cudaErrorMemoryAllocation;
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, k32[0], k32[1], v32[0], v32[1], (int)nr, 0, 32, st));
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb2, k64, k64, v32[1], v32[0], (int)nr, 0, 64, st));
+        if (int rc = L->tmp.reserve(std::max(tb, tb2))) return rc;
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(L->tmp.p, tb, k32[0], k32[1], v32[0], v32[1], (int)nr, 0, 32, st));
+        k_lfq_page_keys<<<(nr + 255) / 256, 256, 0, st>>>(nr, v32[1], pre, k64, L->d_min_rts);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(B.alloc(&k64o, nr));
         const int end_bit = 32 + (int)ceil_log2_u64(L->n_pages + 1);
-        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(L->tmp.p, tb2, k64.as<uint64_t>(), k64o.as<uint64_t>(), v32[1].as<uint32_t>(),
-                                                                  v32[0].as<uint32_t>(), (int)nr, 0, end_bit, st);
-        if (e == cudaSuccess) {
-            k_lfq_gather<<<(nr + 255) / 256, 256, 0, st>>>(nr, L->n_charges, L->p.combine_charge_states, v32[0].as<uint32_t>(), pre.as<sage_b200_lfq_range>(),
-                                                          (sage_b200_lfq_range*)L->d_ranges, (uint32_t*)L->d_grid_of);
-            e = cudaGetLastError();
-        }
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        k64o.release();
-        cleanup2();
-        if (e != cudaSuccess) { cleanup(); return fail(SAGE_B200_ECUDA, "feature map build failed: %s", cudaGetErrorString(e)); }
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(L->tmp.p, tb2, k64, k64o, v32[1], v32[0], (int)nr, 0, end_bit, st));
+        k_lfq_gather<<<(nr + 255) / 256, 256, 0, st>>>(nr, L->n_charges, L->p.combine_charge_states, v32[0], pre, L->d_ranges, L->d_grid_of);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaStreamSynchronize(st));
     }
-    LFQ_RC(lfq_elapsed(L, L->info.ms_build));
-    cleanup();
-#undef LFQ_TRY
-#undef LFQ_RC
-    return 0;
+    return lfq_elapsed(L, L->info.ms_build);
 }
 
 extern "C" int sage_b200_lfq_create(const sage_b200_db* db, const sage_b200_peptides* peptides, const sage_b200_lfq_params* params,
                                     const sage_b200_lfq_features* features, uint64_t n_files, const sage_b200_alignment* alignments, sage_b200_lfq** out) {
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        return fail(SAGE_B200_ECUDA, "no CUDA device available: sage_b200 has no CPU fallback");
-    }
+    if (int rc = select_device(db ? db->device : 0)) return rc;
     if (!db || !peptides || !params || !features || !out || !alignments) return fail(SAGE_B200_EINVAL, "lfq_create: null argument");
     if (peptides->n_peptides != db->v.n_pep || (peptides->n_peptides && (!peptides->residue_offsets || !peptides->sequence)))
         return fail(SAGE_B200_EINVAL, "lfq_create: peptides is not the table the db was built from");
@@ -2349,7 +2333,6 @@ extern "C" int sage_b200_lfq_create(const sage_b200_db* db, const sage_b200_pept
         if (F->file_id[i] >= n_files)
             return fail(SAGE_B200_EINVAL, "lfq_create: feature %llu has file_id %u >= n_files %llu", (unsigned long long)i, F->file_id[i], (unsigned long long)n_files);
     }
-    CUDA_TRY(cudaSetDevice(db->device));
     sage_b200_lfq* L = new sage_b200_lfq();
     L->device = db->device;
     L->p = *params;
@@ -2360,11 +2343,9 @@ extern "C" int sage_b200_lfq_create(const sage_b200_db* db, const sage_b200_pept
         sage_b200_lfq_destroy(L);
         return fail(SAGE_B200_ECUDA, "lfq_create: stream / event creation failed");
     }
-    const int rc = lfq_build(L, db, peptides, F, alignments);
-    if (rc) {
-        std::string msg = g_last_error;
+    if (int rc = lfq_build(L, db, peptides, F, alignments)) {
         sage_b200_lfq_destroy(L);
-        return fail(rc, "%s", msg.c_str());
+        return rc;
     }
     L->info.n_peptides = L->n_slots;
     L->info.n_ranges = L->n_ranges;
@@ -2559,7 +2540,7 @@ extern "C" int sage_b200_lfq_get_info(sage_b200_lfq* L, sage_b200_lfq_info* info
     if (!L || !info) return fail(SAGE_B200_EINVAL, "lfq_get_info: null argument");
     std::lock_guard<std::mutex> lock(L->mu);
     *info = L->info;
-    info->device_bytes = L->fixed_bytes + L->scratch_bytes();
+    info->device_bytes = L->fixed.bytes + L->scratch_bytes();
     return 0;
 }
 
@@ -2660,41 +2641,26 @@ static bool gauss_solve(const HostMat& left, const HostMat& right, std::vector<d
     return false;
 }
 
-// Device allocations of one rescoring call, released together.
-struct FdrArena {
-    std::vector<void*> ps;
-    ~FdrArena() { for (void* p : ps) cudaFree(p); }
-    template <class T>
-    cudaError_t alloc(T** out, size_t count) {
-        void* p = nullptr;
-        cudaError_t e = cudaMalloc(&p, count ? count * sizeof(T) : 16);
-        if (e == cudaSuccess) { ps.push_back(p); *out = (T*)p; }
-        return e;
-    }
-};
-#define FDR_TRY(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) return fail(SAGE_B200_ECUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); } while (0)
-
 // kde::Builder::build (kde.rs:83-136) with bw_adjust = x * bw_factor, on device scores; d_out_bins[bins], d_moments[4] = std_d, std_t, min, max.
-static int fdr_kde(cudaStream_t st, FdrArena& A, const double* d_scores, const uint8_t* d_decoy, const uint8_t* d_target, uint64_t n, uint32_t bins,
+static int fdr_kde(cudaStream_t st, DevArena& A, const double* d_scores, const uint8_t* d_decoy, const uint8_t* d_target, uint64_t n, uint32_t bins,
                    bool monotonic, double bw_factor, bool fma, double* d_out_bins, double* d_moments) {
     double *d_sel = nullptr, *part[2] = {nullptr, nullptr};
     uint64_t* d_nsel = nullptr;
-    void* tmp = nullptr;
     size_t tb = 0;
-    FDR_TRY(A.alloc(&d_sel, 2 * n));
-    FDR_TRY(A.alloc(&d_nsel, 2));
-    FDR_TRY(cub::DeviceSelect::Flagged(nullptr, tb, d_scores, d_decoy, d_sel, d_nsel, (int64_t)n, st));
-    FDR_TRY(A.alloc((char**)&tmp, tb));
-    FDR_TRY(cub::DeviceSelect::Flagged(tmp, tb, d_scores, d_decoy, d_sel, d_nsel, (int64_t)n, st));           // decoys in row order
-    FDR_TRY(cub::DeviceSelect::Flagged(tmp, tb, d_scores, d_target, d_sel + n, d_nsel + 1, (int64_t)n, st));  // targets in row order
+    CUDA_TRY(A.alloc(&d_sel, 2 * n));
+    CUDA_TRY(A.alloc(&d_nsel, 2));
+    CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, d_scores, d_decoy, d_sel, d_nsel, (int64_t)n, st));
+    CUDA_TRY(A.reserve_tmp(tb));
+    CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, d_scores, d_decoy, d_sel, d_nsel, (int64_t)n, st));           // decoys in row order
+    CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, d_scores, d_target, d_sel + n, d_nsel + 1, (int64_t)n, st));  // targets in row order
     uint64_t m[2];
-    FDR_TRY(cudaMemcpyAsync(m, d_nsel, 16, cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaMemcpyAsync(m, d_nsel, 16, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     k_fdr_kde_moments<<<1, 256, 0, st>>>(d_sel, m[0], d_sel + n, m[1], d_scores, n, d_moments);
-    FDR_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     double mom[2];
-    FDR_TRY(cudaMemcpyAsync(mom, d_moments, 16, cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaMemcpyAsync(mom, d_moments, 16, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     double cst[2];
     uint32_t chunks[2];
     for (int c = 0; c < 2; c++) {   // Kde::new (kde.rs:21-32): the bandwidth and normalising constant, host libm pow / sqrt
@@ -2702,27 +2668,19 @@ static int fdr_kde(cudaStream_t st, FdrArena& A, const double* d_scores, const u
         cst[c] = std::sqrt(2.0 * M_PI) * bw * (double)m[c];
         chunks[c] = (uint32_t)((m[c] + KDE_CHUNK - 1) / KDE_CHUNK);
         if (chunks[c] > 65535) return fail(SAGE_B200_ELIMIT, "kde: %llu samples exceed the %d-chunk grid", (unsigned long long)m[c], 65535);
-        FDR_TRY(A.alloc(&part[c], (size_t)bins * chunks[c]));
+        CUDA_TRY(A.alloc(&part[c], (size_t)bins * chunks[c]));
         if (chunks[c]) {
             const dim3 grid((bins + 127) / 128, chunks[c]);
             if (fma) k_fdr_kde_bins<true><<<grid, 128, 0, st>>>(d_sel + c * n, m[c], bins, chunks[c], d_moments, bw, part[c]);
             else k_fdr_kde_bins<false><<<grid, 128, 0, st>>>(d_sel + c * n, m[c], bins, chunks[c], d_moments, bw, part[c]);
-            FDR_TRY(cudaGetLastError());
+            CUDA_TRY(cudaGetLastError());
         }
     }
     const double pi = (double)m[0] / (double)n;
     k_fdr_kde_pep<<<(bins + 127) / 128, 128, 0, st>>>(part[0], chunks[0], part[1], chunks[1], bins, cst[0], cst[1], pi, monotonic, d_out_bins);
-    FDR_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     if (monotonic) k_fdr_kde_monotone<<<1, 1, 0, st>>>(d_out_bins, bins);
-    FDR_TRY(cudaGetLastError());
-    return 0;
-}
-
-static int fdr_device(int device) {
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(SAGE_B200_ECUDA, "no CUDA device available: sage_b200 has no CPU fallback");
-    if (device < 0 || device >= ndev) return fail(SAGE_B200_EINVAL, "device out of range");
-    FDR_TRY(cudaSetDevice(device));
+    CUDA_TRY(cudaGetLastError());
     return 0;
 }
 
@@ -2730,23 +2688,23 @@ extern "C" int sage_b200_kde_build(int device, const double* scores, const uint8
                                    double* out_bins, double* min_score, double* score_step) {
     if (n == 0 || !scores || !decoy || !out_bins || !min_score || !score_step || bins < 2) return fail(SAGE_B200_EINVAL, "kde_build: bad argument");
     if (n > (uint64_t)INT32_MAX || bins > (1u << 24)) return fail(SAGE_B200_ELIMIT, "kde_build: n or bins too large");
-    if (int rc = fdr_device(device)) return rc;
-    FdrArena A;
+    if (int rc = select_device(device)) return rc;
+    DevArena A;
     double *d_s = nullptr, *d_bins = nullptr, *d_mom = nullptr;
     uint8_t* d_flags = nullptr;
-    FDR_TRY(A.alloc(&d_s, n));
-    FDR_TRY(A.alloc(&d_flags, 2 * n));
-    FDR_TRY(A.alloc(&d_bins, bins));
-    FDR_TRY(A.alloc(&d_mom, 4));
+    CUDA_TRY(A.alloc(&d_s, n));
+    CUDA_TRY(A.alloc(&d_flags, 2 * n));
+    CUDA_TRY(A.alloc(&d_bins, bins));
+    CUDA_TRY(A.alloc(&d_mom, 4));
     std::vector<uint8_t> flags(2 * n);
     for (uint64_t i = 0; i < n; i++) { flags[i] = decoy[i] != 0; flags[n + i] = decoy[i] == 0; }
-    FDR_TRY(cudaMemcpy(d_s, scores, 8 * n, cudaMemcpyHostToDevice));
-    FDR_TRY(cudaMemcpy(d_flags, flags.data(), 2 * n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(d_s, scores, 8 * n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(d_flags, flags.data(), 2 * n, cudaMemcpyHostToDevice));
     const int v = host_math_variant();
     if (int rc = fdr_kde(0, A, d_s, d_flags, d_flags + n, n, (uint32_t)bins, monotonic != 0, bw_factor, v != 1, d_bins, d_mom)) return rc;
     double mom[4];
-    FDR_TRY(cudaMemcpy(out_bins, d_bins, 8 * bins, cudaMemcpyDeviceToHost));
-    FDR_TRY(cudaMemcpy(mom, d_mom, 32, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(out_bins, d_bins, 8 * bins, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(mom, d_mom, 32, cudaMemcpyDeviceToHost));
     *min_score = mom[2];
     *score_step = (mom[3] - mom[2]) / (double)(bins - 1);
     return 0;
@@ -2755,24 +2713,50 @@ extern "C" int sage_b200_kde_build(int device, const double* scores, const uint8
 extern "C" int sage_b200_device_math(int device, int function, int variant, const double* x, uint64_t n, double* out) {
     if (function < 0 || function > 2 || variant < -1 || variant > 1 || (n && (!x || !out))) return fail(SAGE_B200_EINVAL, "device_math: bad argument");
     if (n == 0) return 0;
-    if (int rc = fdr_device(device)) return rc;
+    if (int rc = select_device(device)) return rc;
     if (variant == -1) variant = host_math_variant() == 1 ? 1 : 0;
-    FdrArena A;
+    DevArena A;
     double *dx = nullptr, *dy = nullptr;
-    FDR_TRY(A.alloc(&dx, n));
-    FDR_TRY(A.alloc(&dy, n));
-    FDR_TRY(cudaMemcpy(dx, x, 8 * n, cudaMemcpyHostToDevice));
+    CUDA_TRY(A.alloc(&dx, n));
+    CUDA_TRY(A.alloc(&dy, n));
+    CUDA_TRY(cudaMemcpy(dx, x, 8 * n, cudaMemcpyHostToDevice));
     const unsigned g = (unsigned)((n + 255) / 256);
     if (variant == 0) k_device_math<true><<<g, 256>>>(function, dx, n, dy);
     else k_device_math<false><<<g, 256>>>(function, dx, n, dy);
-    FDR_TRY(cudaGetLastError());
-    FDR_TRY(cudaMemcpy(out, dy, 8 * n, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpy(out, dy, 8 * n, cudaMemcpyDeviceToHost));
     return 0;
 }
 
 struct MinF {
     __device__ float operator()(float a, float b) const { return fminf(a, b); }
 };
+
+// qvalue::spectrum_q_value over the rows in ascending (key, row) order: d_key / d_idx hold each row's sort key and index. d_key_sorted,
+// d_isdec, d_dscan, d_rq and d_rqmin are n-element work columns (allocated by the caller with its other arrays: an allocation here would
+// stall the stage). Returns the row at each sorted position (d_order), each row's q-value (d_q) and the count at q <= 0.01 (d_passing).
+template <class Key>
+static int spectrum_q_values(cudaStream_t st, DevArena& A, const sage_b200_feature* d_rows, uint64_t n, const Key* d_key, Key* d_key_sorted,
+                             const uint32_t* d_idx, uint32_t* d_isdec, uint32_t* d_dscan, float* d_rq, float* d_rqmin, uint32_t* d_order, float* d_q,
+                             unsigned long long* d_passing) {
+    const unsigned g = (unsigned)((n + 255) / 256);
+    size_t tb = 0, tb2 = 0, tb3 = 0;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key_sorted, d_idx, d_order, (int)n, 0, 8 * (int)sizeof(Key), st));
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, tb2, d_isdec, d_dscan, (int)n, st));
+    CUDA_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
+    CUDA_TRY(A.reserve_tmp(std::max(tb, std::max(tb2, tb3))));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, d_key, d_key_sorted, d_idx, d_order, (int)n, 0, 8 * (int)sizeof(Key), st));
+    k_fdr_sorted_decoy<<<g, 256, 0, st>>>(d_rows, d_order, n, d_isdec);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(A.tmp, tb2, d_isdec, d_dscan, (int)n, st));
+    k_fdr_q_raw<<<g, 256, 0, st>>>(d_dscan, n, d_rq);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceScan::InclusiveScan(A.tmp, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
+    CUDA_TRY(cudaMemsetAsync(d_passing, 0, 8, st));
+    k_fdr_q_out<<<g, 256, 0, st>>>(d_rqmin, d_order, n, d_q, d_passing);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
 
 // spectrum_fdr (runner.rs:280-291): score_psms, the heuristic fallback when it returns None, the descending sort and spectrum_q_value.
 extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p, const sage_b200_feature* rows, uint64_t n, const float* aligned_rt,
@@ -2789,7 +2773,7 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
     out->eps = 0.0;
     out->ms_mass_kde = out->ms_features = out->ms_lda = out->ms_discriminant_kde = out->ms_sort_q = out->ms_total = 0.0f;
     if (n == 0) return 0;
-    if (int rc = fdr_device(device)) return rc;
+    if (int rc = select_device(device)) return rc;
     if (n > (uint64_t)65535 * KDE_CHUNK) return fail(SAGE_B200_ELIMIT, "spectrum_fdr: more than 65535 KDE chunks of %d rows", KDE_CHUNK);
     const int variant = host_math_variant();
     const bool fma = variant != 1;
@@ -2802,7 +2786,7 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
     const uint32_t mbins = (uint32_t)span_abs;
     {   // everything below stays allocated until the call returns: fail with ELIMIT before allocating when it cannot fit
         size_t free_b = 0, total_b = 0;
-        FDR_TRY(cudaMemGetInfo(&free_b, &total_b));
+        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
         // per row: the rows, mass errors, flags, feature matrix, f64 discriminants, five f32 and six u32 work columns, the three optional
         // columns, the class-compacted samples of both KDEs (16 bytes each) and the radix sort's temporary storage; then both KDEs' partial sums
         const uint64_t per_row = sizeof(sage_b200_feature) + 8 + 2 + 8 * FDR_FEATURES + 8 + 4 * 5 + 4 * 6 + 4 * 3 + 16 * 2 + 16;
@@ -2812,11 +2796,10 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
                                        (unsigned long long)need, (unsigned long long)free_b);
     }
 
-    FdrArena A;
+    DevArena A;
     cudaStream_t st = 0;
-    cudaEvent_t ev[6] = {};
-    struct EvFree { cudaEvent_t* e; ~EvFree() { for (int i = 0; i < 6; i++) if (e[i]) cudaEventDestroy(e[i]); } } ev_free{ev};
-    for (auto& e : ev) FDR_TRY(cudaEventCreate(&e));
+    StageEvents<6> ev;
+    CUDA_TRY(ev.create());
     sage_b200_feature* d_rows = nullptr;
     double *d_mass = nullptr, *d_mbins = nullptr, *d_mmom = nullptr, *d_X = nullptr, *d_means = nullptr, *d_scatter = nullptr, *d_coef = nullptr,
            *d_disc = nullptr, *d_dbins = nullptr, *d_dmom = nullptr;
@@ -2825,61 +2808,61 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
     float *d_disc32 = nullptr, *d_pep = nullptr, *d_q = nullptr, *d_rq = nullptr, *d_rqmin = nullptr, *d_cols[3] = {nullptr, nullptr, nullptr};
     uint32_t *d_key = nullptr, *d_key2 = nullptr, *d_idx = nullptr, *d_order = nullptr, *d_isdec = nullptr, *d_dscan = nullptr;
     unsigned long long* d_passing = nullptr;
-    FDR_TRY(A.alloc(&d_rows, n));
-    FDR_TRY(A.alloc(&d_mass, n));
-    FDR_TRY(A.alloc(&d_flags, 2 * n));
-    FDR_TRY(A.alloc(&d_mbins, mbins));
-    FDR_TRY(A.alloc(&d_mmom, 4));
-    FDR_TRY(A.alloc(&d_X, n * FDR_FEATURES));
-    FDR_TRY(A.alloc(&d_means, 2 * FDR_FEATURES));
-    FDR_TRY(A.alloc(&d_scatter, 2 * FDR_FEATURES * FDR_FEATURES));
-    FDR_TRY(A.alloc(&d_counts, 2));
-    FDR_TRY(A.alloc(&d_coef, FDR_FEATURES));
-    FDR_TRY(A.alloc(&d_disc, n));
-    FDR_TRY(A.alloc(&d_dbins, 1000));
-    FDR_TRY(A.alloc(&d_dmom, 4));
-    FDR_TRY(A.alloc(&d_disc32, n));
-    FDR_TRY(A.alloc(&d_pep, n));
-    FDR_TRY(A.alloc(&d_q, n));
-    FDR_TRY(A.alloc(&d_rq, n));
-    FDR_TRY(A.alloc(&d_rqmin, n));
-    FDR_TRY(A.alloc(&d_key, n));
-    FDR_TRY(A.alloc(&d_key2, n));
-    FDR_TRY(A.alloc(&d_idx, n));
-    FDR_TRY(A.alloc(&d_order, n));
-    FDR_TRY(A.alloc(&d_isdec, n));
-    FDR_TRY(A.alloc(&d_dscan, n));
-    FDR_TRY(A.alloc(&d_passing, 1));
+    CUDA_TRY(A.alloc(&d_rows, n));
+    CUDA_TRY(A.alloc(&d_mass, n));
+    CUDA_TRY(A.alloc(&d_flags, 2 * n));
+    CUDA_TRY(A.alloc(&d_mbins, mbins));
+    CUDA_TRY(A.alloc(&d_mmom, 4));
+    CUDA_TRY(A.alloc(&d_X, n * FDR_FEATURES));
+    CUDA_TRY(A.alloc(&d_means, 2 * FDR_FEATURES));
+    CUDA_TRY(A.alloc(&d_scatter, 2 * FDR_FEATURES * FDR_FEATURES));
+    CUDA_TRY(A.alloc(&d_counts, 2));
+    CUDA_TRY(A.alloc(&d_coef, FDR_FEATURES));
+    CUDA_TRY(A.alloc(&d_disc, n));
+    CUDA_TRY(A.alloc(&d_dbins, 1000));
+    CUDA_TRY(A.alloc(&d_dmom, 4));
+    CUDA_TRY(A.alloc(&d_disc32, n));
+    CUDA_TRY(A.alloc(&d_pep, n));
+    CUDA_TRY(A.alloc(&d_q, n));
+    CUDA_TRY(A.alloc(&d_rq, n));
+    CUDA_TRY(A.alloc(&d_rqmin, n));
+    CUDA_TRY(A.alloc(&d_key, n));
+    CUDA_TRY(A.alloc(&d_key2, n));
+    CUDA_TRY(A.alloc(&d_idx, n));
+    CUDA_TRY(A.alloc(&d_order, n));
+    CUDA_TRY(A.alloc(&d_isdec, n));
+    CUDA_TRY(A.alloc(&d_dscan, n));
+    CUDA_TRY(A.alloc(&d_passing, 1));
     const float* cols_h[3] = {aligned_rt, delta_rt_model, delta_ims_model};
     for (int c = 0; c < 3; c++)
         if (cols_h[c]) {
-            FDR_TRY(A.alloc(&d_cols[c], n));
-            FDR_TRY(cudaMemcpy(d_cols[c], cols_h[c], 4 * n, cudaMemcpyHostToDevice));
+            CUDA_TRY(A.alloc(&d_cols[c], n));
+            CUDA_TRY(cudaMemcpy(d_cols[c], cols_h[c], 4 * n, cudaMemcpyHostToDevice));
         }
-    FDR_TRY(cudaMemcpy(d_rows, rows, sizeof(sage_b200_feature) * n, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(d_rows, rows, sizeof(sage_b200_feature) * n, cudaMemcpyHostToDevice));
     const unsigned g = (unsigned)((n + 255) / 256);
 
     // 1. mass-error KDE (linear_discriminant.rs:140-158)
-    FDR_TRY(cudaEventRecord(ev[0], st));
+    CUDA_TRY(cudaEventRecord(ev[0], st));
     k_fdr_mass<<<g, 256, 0, st>>>(d_rows, n, kind, d_mass, d_flags, d_flags + n);
-    FDR_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     if (int rc = fdr_kde(st, A, d_mass, d_flags, d_flags + n, n, mbins, false, bw_factor, fma, d_mbins, d_mmom)) return rc;
-    FDR_TRY(cudaEventRecord(ev[1], st));
+    CUDA_TRY(cudaEventRecord(ev[1], st));
     // 2. feature rows (linear_discriminant.rs:162-193)
     const FdrColumns cols{d_cols[0], d_cols[1], d_cols[2]};
     if (fma) k_fdr_features<true><<<g, 256, 0, st>>>(d_rows, n, cols, d_mass, d_mbins, mbins, d_mmom, d_X);
     else k_fdr_features<false><<<g, 256, 0, st>>>(d_rows, n, cols, d_mass, d_mbins, mbins, d_mmom, d_X);
-    FDR_TRY(cudaGetLastError());
-    FDR_TRY(cudaEventRecord(ev[2], st));
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(ev[2], st));
     // 3. LDA class sums and scatter on the device, Gauss::solve on the host (linear_discriminant.rs:63-124, 195-208)
     k_fdr_lda<<<2, 256, 0, st>>>(d_X, d_flags, n, d_means, d_scatter, d_counts);
-    FDR_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     std::vector<double> means(2 * FDR_FEATURES), scatter(2 * FDR_FEATURES * FDR_FEATURES);
     uint64_t counts[2];
-    FDR_TRY(cudaMemcpyAsync(means.data(), d_means, 8 * means.size(), cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaMemcpyAsync(scatter.data(), d_scatter, 8 * scatter.size(), cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaMemcpyAsync(counts, d_counts, 16, cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaMemcpyAsync(means.data(), d_means, 8 * means.size(), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(scatter.data(), d_scatter, 8 * scatter.size(), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(counts, d_counts, 16, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     bool fitted = false;
     if (counts[0] != 0 && counts[1] != 0) {
         HostMat sw(FDR_FEATURES, FDR_FEATURES), rhs(FDR_FEATURES, 1);
@@ -2895,52 +2878,37 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
             for (double w : coef) fitted = fitted && std::isfinite(w);   // linear_discriminant.rs:196-208
         }
     }
-    FDR_TRY(cudaEventRecord(ev[3], st));
+    CUDA_TRY(cudaEventRecord(ev[3], st));
     // 4. projection, discriminant KDE and posterior errors (linear_discriminant.rs:209-228), or the fallback (runner.rs:284-287)
     if (fitted) {
-        FDR_TRY(cudaMemcpyAsync(d_coef, out->coef, 8 * FDR_FEATURES, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_coef, out->coef, 8 * FDR_FEATURES, cudaMemcpyHostToDevice, st));
         k_fdr_project<<<g, 256, 0, st>>>(d_X, n, d_coef, d_disc, d_disc32);
-        FDR_TRY(cudaGetLastError());
+        CUDA_TRY(cudaGetLastError());
         if (int rc = fdr_kde(st, A, d_disc, d_flags, d_flags + n, n, 1000, true, 1.0, fma, d_dbins, d_dmom)) return rc;
         if (fma) k_fdr_pep<true><<<g, 256, 0, st>>>(d_disc, n, d_dbins, 1000, d_dmom, d_pep);
         else k_fdr_pep<false><<<g, 256, 0, st>>>(d_disc, n, d_dbins, 1000, d_dmom, d_pep);
     } else {
         k_fdr_fallback<<<g, 256, 0, st>>>(d_rows, n, d_disc32, d_pep);
     }
-    FDR_TRY(cudaGetLastError());
-    FDR_TRY(cudaEventRecord(ev[4], st));
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(ev[4], st));
     // 5. stable descending sort (ties by input row) and spectrum_q_value (qvalue.rs)
     k_fdr_sort_key<<<g, 256, 0, st>>>(d_disc32, n, d_key, d_idx);
-    FDR_TRY(cudaGetLastError());
-    size_t tb = 0, tb2 = 0, tb3 = 0;
-    FDR_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key2, d_idx, d_order, (int)n, 0, 32, st));
-    FDR_TRY(cub::DeviceScan::InclusiveSum(nullptr, tb2, d_isdec, d_dscan, (int)n, st));
-    FDR_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
-    char* tmp = nullptr;
-    FDR_TRY(A.alloc(&tmp, std::max(tb, std::max(tb2, tb3))));
-    FDR_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, d_key, d_key2, d_idx, d_order, (int)n, 0, 32, st));
-    k_fdr_sorted_decoy<<<g, 256, 0, st>>>(d_rows, d_order, n, d_isdec);
-    FDR_TRY(cudaGetLastError());
-    FDR_TRY(cub::DeviceScan::InclusiveSum(tmp, tb2, d_isdec, d_dscan, (int)n, st));
-    k_fdr_q_raw<<<g, 256, 0, st>>>(d_dscan, n, d_rq);
-    FDR_TRY(cudaGetLastError());
-    FDR_TRY(cub::DeviceScan::InclusiveScan(tmp, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
-    FDR_TRY(cudaMemsetAsync(d_passing, 0, 8, st));
-    k_fdr_q_out<<<g, 256, 0, st>>>(d_rqmin, d_order, n, d_q, d_passing);
-    FDR_TRY(cudaGetLastError());
-    FDR_TRY(cudaEventRecord(ev[5], st));
+    CUDA_TRY(cudaGetLastError());
+    if (int rc = spectrum_q_values(st, A, d_rows, n, d_key, d_key2, d_idx, d_isdec, d_dscan, d_rq, d_rqmin, d_order, d_q, d_passing)) return rc;
+    CUDA_TRY(cudaEventRecord(ev[5], st));
     unsigned long long passing = 0;
-    FDR_TRY(cudaMemcpyAsync(out->discriminant_score, d_disc32, 4 * n, cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaMemcpyAsync(out->posterior_error, d_pep, 4 * n, cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaMemcpyAsync(out->spectrum_q, d_q, 4 * n, cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaMemcpyAsync(out->order, d_order, 4 * n, cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaMemcpyAsync(&passing, d_passing, 8, cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaMemcpyAsync(out->discriminant_score, d_disc32, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->posterior_error, d_pep, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->spectrum_q, d_q, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->order, d_order, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&passing, d_passing, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     out->passing = passing;
     out->lda_fitted = fitted ? 1 : 0;
     float* ms[5] = {&out->ms_mass_kde, &out->ms_features, &out->ms_lda, &out->ms_discriminant_kde, &out->ms_sort_q};
-    for (int i = 0; i < 5; i++) FDR_TRY(cudaEventElapsedTime(ms[i], ev[i], ev[i + 1]));
-    FDR_TRY(cudaEventElapsedTime(&out->ms_total, ev[0], ev[5]));
+    for (int i = 0; i < 5; i++) CUDA_TRY(cudaEventElapsedTime(ms[i], ev[i], ev[i + 1]));
+    CUDA_TRY(cudaEventElapsedTime(&out->ms_total, ev[0], ev[5]));
     return 0;
 }
 
@@ -2948,7 +2916,7 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
 // LinearRegression::fit (regression.rs:72-117) for one model over the training list: chunk accumulators on the device, merged in chunk order,
 // Gauss::solve on the host, the SSE pass chunked the same way; then predict for every row (or the Feature defaults when the fit is None).
 template <int MODEL>
-static int rt_model(cudaStream_t st, FdrArena& A, bool fma, const RtPeptides& P, const sage_b200_feature* d_rows, uint64_t n, const uint32_t* d_train,
+static int rt_model(cudaStream_t st, DevArena& A, bool fma, const RtPeptides& P, const sage_b200_feature* d_rows, uint64_t n, const uint32_t* d_train,
                     uint64_t n_train, const float* d_ycol, const float* d_aligned, float* d_pred, float* d_delta, int32_t* fitted, double* r2, double* eps,
                     double* beta_out) {
     using Dm = RtDims<MODEL>;
@@ -2961,17 +2929,17 @@ static int rt_model(cudaStream_t st, FdrArena& A, bool fma, const RtPeptides& P,
     if (n_train) {
         const uint64_t n_chunks = (n_train + RT_CHUNK - 1) / RT_CHUNK;
         double *d_part = nullptr, *d_acc = nullptr, *d_sse = nullptr, *d_beta = nullptr;
-        FDR_TRY(A.alloc(&d_part, n_chunks * Dm::NACC));
-        FDR_TRY(A.alloc(&d_acc, Dm::NACC));
+        CUDA_TRY(A.alloc(&d_part, n_chunks * Dm::NACC));
+        CUDA_TRY(A.alloc(&d_acc, Dm::NACC));
         const dim3 grid((unsigned)n_chunks, (Dm::NACC + 255) / 256);
         if (fma) k_rt_accumulate<MODEL, true><<<grid, 256, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_part);
         else k_rt_accumulate<MODEL, false><<<grid, 256, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_part);
-        FDR_TRY(cudaGetLastError());
+        CUDA_TRY(cudaGetLastError());
         k_rt_merge<<<(Dm::NACC + 255) / 256, 256, 0, st>>>(d_part, n_chunks, Dm::NACC, d_acc);
-        FDR_TRY(cudaGetLastError());
+        CUDA_TRY(cudaGetLastError());
         std::vector<double> acc(Dm::NACC);
-        FDR_TRY(cudaMemcpyAsync(acc.data(), d_acc, 8 * Dm::NACC, cudaMemcpyDeviceToHost, st));
-        FDR_TRY(cudaStreamSynchronize(st));
+        CUDA_TRY(cudaMemcpyAsync(acc.data(), d_acc, 8 * Dm::NACC, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
         HostMat cov(D, D), b(D, 1);
         for (int j = 0, a = 0; j < D; j++)
             for (int k = j; k < D; k++, a++) cov(j, k) = cov(k, j) = acc[a];
@@ -2979,15 +2947,15 @@ static int rt_model(cudaStream_t st, FdrArena& A, bool fma, const RtPeptides& P,
         const double sum_y = acc[Dm::NCOV + D], sum_y2 = acc[Dm::NCOV + D + 1];
         const double nf = (double)n_train, y_mean = sum_y / nf, y_var = sum_y2 - nf * y_mean * y_mean;
         if (gauss_solve(cov, b, &beta, eps)) {
-            FDR_TRY(A.alloc(&d_beta, D));
-            FDR_TRY(A.alloc(&d_sse, n_chunks));
-            FDR_TRY(cudaMemcpyAsync(d_beta, beta.data(), 8 * D, cudaMemcpyHostToDevice, st));
+            CUDA_TRY(A.alloc(&d_beta, D));
+            CUDA_TRY(A.alloc(&d_sse, n_chunks));
+            CUDA_TRY(cudaMemcpyAsync(d_beta, beta.data(), 8 * D, cudaMemcpyHostToDevice, st));
             if (fma) k_rt_sse<MODEL, true><<<(unsigned)n_chunks, 32, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_beta, d_sse);
             else k_rt_sse<MODEL, false><<<(unsigned)n_chunks, 32, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_beta, d_sse);
-            FDR_TRY(cudaGetLastError());
+            CUDA_TRY(cudaGetLastError());
             std::vector<double> chunk_sse(n_chunks);
-            FDR_TRY(cudaMemcpyAsync(chunk_sse.data(), d_sse, 8 * n_chunks, cudaMemcpyDeviceToHost, st));
-            FDR_TRY(cudaStreamSynchronize(st));
+            CUDA_TRY(cudaMemcpyAsync(chunk_sse.data(), d_sse, 8 * n_chunks, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaStreamSynchronize(st));
             double sse = -0.0;   // f64 Sum of the chunk sums, in chunk order
             for (double s : chunk_sse) sse = sse + s;
             *r2 = 1.0 - sse / y_var;
@@ -2996,13 +2964,13 @@ static int rt_model(cudaStream_t st, FdrArena& A, bool fma, const RtPeptides& P,
             const unsigned g = (unsigned)((n + RT_TILE - 1) / RT_TILE);
             if (fma) k_rt_predict<MODEL, true><<<g, 32, 0, st>>>(P, d_rows, n, d_beta, d_aligned, d_pred, d_delta);
             else k_rt_predict<MODEL, false><<<g, 32, 0, st>>>(P, d_rows, n, d_beta, d_aligned, d_pred, d_delta);
-            FDR_TRY(cudaGetLastError());
+            CUDA_TRY(cudaGetLastError());
             return 0;
         }
         *eps = 0.0;
     }
     k_rt_defaults<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, d_pred, d_delta);
-    FDR_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     return 0;
 }
 
@@ -3041,12 +3009,12 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
         for (uint64_t f = 0; f < n_files; f++) out->alignments[f] = sage_b200_alignment{0.0f, 1.0f, 0.0f};
         return 0;
     }
-    FDR_TRY(cudaSetDevice(db->device));
+    CUDA_TRY(cudaSetDevice(db->device));
     const uint64_t nres = P->residue_offsets[n_pep];
     const uint64_t n_chunks = (n + RT_CHUNK - 1) / RT_CHUNK + 1;
     {   // everything below stays allocated until the call returns: fail with ELIMIT before allocating when it cannot fit
         size_t free_b = 0, total_b = 0;
-        FDR_TRY(cudaMemGetInfo(&free_b, &total_b));
+        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
         // per row: the rows, file ids, sort keys / values / order, the q-value work columns, flags, training list, (peptide, file) keys and
         // values, segment arrays, the five outputs and the sort's temporary storage; the peptide table; per file the maxima and alignments;
         // both models' chunk partials; and the peptide x file matrix, at most one row per referenced peptide
@@ -3060,11 +3028,10 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
                         (unsigned long long)n_files, need, (unsigned long long)free_b);
     }
     const bool fma = host_math_variant() != 1;
-    FdrArena A;
+    DevArena A;
     cudaStream_t st = 0;
-    cudaEvent_t ev[5] = {};
-    struct EvFree { cudaEvent_t* e; ~EvFree() { for (int i = 0; i < 5; i++) if (e[i]) cudaEventDestroy(e[i]); } } ev_free{ev};
-    for (auto& e : ev) FDR_TRY(cudaEventCreate(&e));
+    StageEvents<5> ev;
+    CUDA_TRY(ev.create());
     sage_b200_feature* d_rows = nullptr;
     uint32_t *d_file = nullptr, *d_off = nullptr, *d_idx = nullptr, *d_order = nullptr, *d_isdec = nullptr, *d_dscan = nullptr, *d_train = nullptr,
              *d_val = nullptr, *d_val2 = nullptr, *d_seg = nullptr, *d_prow = nullptr, *d_keep = nullptr, *d_mrow = nullptr, *d_count = nullptr;
@@ -3075,165 +3042,140 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
     unsigned long long* d_passing = nullptr;
     double *d_segmin = nullptr, *d_mat = nullptr, *d_mean = nullptr;
     sage_b200_alignment* d_align = nullptr;
-    FDR_TRY(A.alloc(&d_rows, n));
-    FDR_TRY(A.alloc(&d_file, n));
-    FDR_TRY(A.alloc(&d_off, n_pep + 1));
-    FDR_TRY(A.alloc(&d_seq, nres));
-    FDR_TRY(A.alloc(&d_mono, n_pep));
-    FDR_TRY(A.alloc(&d_key, n));
-    FDR_TRY(A.alloc(&d_key2, n));
-    FDR_TRY(A.alloc(&d_idx, n));
-    FDR_TRY(A.alloc(&d_order, n));
-    FDR_TRY(A.alloc(&d_isdec, n));
-    FDR_TRY(A.alloc(&d_dscan, n));
-    FDR_TRY(A.alloc(&d_q, n));
-    FDR_TRY(A.alloc(&d_rq, n));
-    FDR_TRY(A.alloc(&d_rqmin, n));
-    FDR_TRY(A.alloc(&d_flag, n));
-    FDR_TRY(A.alloc(&d_train, n));
-    FDR_TRY(A.alloc(&d_val, n));
-    FDR_TRY(A.alloc(&d_val2, n));
-    FDR_TRY(A.alloc(&d_seg, n));
-    FDR_TRY(A.alloc(&d_segmin, n));
-    FDR_TRY(A.alloc(&d_prow, n));
-    FDR_TRY(A.alloc(&d_keep, n));
-    FDR_TRY(A.alloc(&d_mrow, n));
-    FDR_TRY(A.alloc(&d_count, 4));
-    FDR_TRY(A.alloc(&d_passing, 1));
-    FDR_TRY(A.alloc(&d_maxrt, n_files));
-    FDR_TRY(A.alloc(&d_align, n_files));
-    for (auto& o : d_out) FDR_TRY(A.alloc(&o, n));
-    FDR_TRY(cudaMemcpyAsync(d_rows, rows, sizeof(sage_b200_feature) * n, cudaMemcpyHostToDevice, st));
-    FDR_TRY(cudaMemcpyAsync(d_file, file_id, 4 * n, cudaMemcpyHostToDevice, st));
-    FDR_TRY(cudaMemcpyAsync(d_off, P->residue_offsets, 4 * (n_pep + 1), cudaMemcpyHostToDevice, st));
-    if (nres) FDR_TRY(cudaMemcpyAsync(d_seq, P->sequence, nres, cudaMemcpyHostToDevice, st));
-    FDR_TRY(cudaMemcpyAsync(d_mono, P->monoisotopic, 4 * n_pep, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(A.alloc(&d_rows, n));
+    CUDA_TRY(A.alloc(&d_file, n));
+    CUDA_TRY(A.alloc(&d_off, n_pep + 1));
+    CUDA_TRY(A.alloc(&d_seq, nres));
+    CUDA_TRY(A.alloc(&d_mono, n_pep));
+    CUDA_TRY(A.alloc(&d_key, n));
+    CUDA_TRY(A.alloc(&d_key2, n));
+    CUDA_TRY(A.alloc(&d_idx, n));
+    CUDA_TRY(A.alloc(&d_order, n));
+    CUDA_TRY(A.alloc(&d_isdec, n));
+    CUDA_TRY(A.alloc(&d_dscan, n));
+    CUDA_TRY(A.alloc(&d_q, n));
+    CUDA_TRY(A.alloc(&d_rq, n));
+    CUDA_TRY(A.alloc(&d_rqmin, n));
+    CUDA_TRY(A.alloc(&d_flag, n));
+    CUDA_TRY(A.alloc(&d_train, n));
+    CUDA_TRY(A.alloc(&d_val, n));
+    CUDA_TRY(A.alloc(&d_val2, n));
+    CUDA_TRY(A.alloc(&d_seg, n));
+    CUDA_TRY(A.alloc(&d_segmin, n));
+    CUDA_TRY(A.alloc(&d_prow, n));
+    CUDA_TRY(A.alloc(&d_keep, n));
+    CUDA_TRY(A.alloc(&d_mrow, n));
+    CUDA_TRY(A.alloc(&d_count, 4));
+    CUDA_TRY(A.alloc(&d_passing, 1));
+    CUDA_TRY(A.alloc(&d_maxrt, n_files));
+    CUDA_TRY(A.alloc(&d_align, n_files));
+    for (auto& o : d_out) CUDA_TRY(A.alloc(&o, n));
+    CUDA_TRY(cudaMemcpyAsync(d_rows, rows, sizeof(sage_b200_feature) * n, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_file, file_id, 4 * n, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_off, P->residue_offsets, 4 * (n_pep + 1), cudaMemcpyHostToDevice, st));
+    if (nres) CUDA_TRY(cudaMemcpyAsync(d_seq, P->sequence, nres, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_mono, P->monoisotopic, 4 * n_pep, cudaMemcpyHostToDevice, st));
     const RtPeptides pk{d_off, d_seq, d_mono};
     const unsigned g = (unsigned)((n + 255) / 256);
     thrust::counting_iterator<uint32_t> count_it(0);
-    char* tmp = nullptr;
-    size_t tmp_bytes = 0;
-    auto ensure_tmp = [&](size_t b) -> int {   // one temporary buffer for every cub call, grown when a call needs more
-        if (b <= tmp_bytes) return 0;
-        FDR_TRY(A.alloc(&tmp, b));
-        tmp_bytes = b;
-        return 0;
-    };
     auto read_count = [&](uint64_t* v) -> int {
         uint32_t c = 0;
-        FDR_TRY(cudaMemcpyAsync(&c, d_count, 4, cudaMemcpyDeviceToHost, st));
-        FDR_TRY(cudaStreamSynchronize(st));
+        CUDA_TRY(cudaMemcpyAsync(&c, d_count, 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
         *v = c;
         return 0;
     };
 
     // 1. par_sort_unstable_by(poisson.total_cmp), ties by input row, then spectrum_q_value (runner.rs:517-520)
-    FDR_TRY(cudaEventRecord(ev[0], st));
+    CUDA_TRY(cudaEventRecord(ev[0], st));
     k_rt_poisson_key<<<g, 256, 0, st>>>(d_rows, n, d_key, d_idx);
-    FDR_TRY(cudaGetLastError());
-    {
-        size_t tb = 0, tb2 = 0, tb3 = 0;
-        FDR_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key2, d_idx, d_order, (int)n, 0, 64, st));
-        FDR_TRY(cub::DeviceScan::InclusiveSum(nullptr, tb2, d_isdec, d_dscan, (int)n, st));
-        FDR_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
-        if (int rc = ensure_tmp(std::max(tb, std::max(tb2, tb3)))) return rc;
-        FDR_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, d_key, d_key2, d_idx, d_order, (int)n, 0, 64, st));
-        k_fdr_sorted_decoy<<<g, 256, 0, st>>>(d_rows, d_order, n, d_isdec);
-        FDR_TRY(cudaGetLastError());
-        FDR_TRY(cub::DeviceScan::InclusiveSum(tmp, tb2, d_isdec, d_dscan, (int)n, st));
-        k_fdr_q_raw<<<g, 256, 0, st>>>(d_dscan, n, d_rq);
-        FDR_TRY(cudaGetLastError());
-        FDR_TRY(cub::DeviceScan::InclusiveScan(tmp, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
-        FDR_TRY(cudaMemsetAsync(d_passing, 0, 8, st));
-        k_fdr_q_out<<<g, 256, 0, st>>>(d_rqmin, d_order, n, d_q, d_passing);
-        FDR_TRY(cudaGetLastError());
-    }
+    CUDA_TRY(cudaGetLastError());
+    if (int rc = spectrum_q_values(st, A, d_rows, n, d_key, d_key2, d_idx, d_isdec, d_dscan, d_rq, d_rqmin, d_order, d_q, d_passing)) return rc;
     // the training rows (label == 1 && spectrum_q <= 0.01) in poisson order
     k_rt_train_flag<<<g, 256, 0, st>>>(d_rows, d_order, d_q, n, d_flag);
-    FDR_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     uint64_t n_train = 0;
     {
         size_t tb = 0;
-        FDR_TRY(cub::DeviceSelect::Flagged(nullptr, tb, d_order, d_flag, d_train, d_count, (int)n, st));
-        if (int rc = ensure_tmp(tb)) return rc;
-        FDR_TRY(cub::DeviceSelect::Flagged(tmp, tb, d_order, d_flag, d_train, d_count, (int)n, st));
+        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, d_order, d_flag, d_train, d_count, (int)n, st));
+        CUDA_TRY(A.reserve_tmp(tb));
+        CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, d_order, d_flag, d_train, d_count, (int)n, st));
         if (int rc = read_count(&n_train)) return rc;
     }
-    FDR_TRY(cudaEventRecord(ev[1], st));
+    CUDA_TRY(cudaEventRecord(ev[1], st));
 
     // 2. global_alignment (retention_alignment.rs:95-173)
-    FDR_TRY(cudaMemsetAsync(d_maxrt, 0, 4 * n_files, st));
+    CUDA_TRY(cudaMemsetAsync(d_maxrt, 0, 4 * n_files, st));
     k_rt_max_rt<<<g, 256, 0, st>>>(d_rows, d_file, n, d_maxrt);
-    FDR_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     uint64_t n_seg = 0, n_pr = 0, n_rows = 0;
     if (n_train) {
         const unsigned gt = (unsigned)((n_train + 255) / 256);
         k_rt_pf_key<<<gt, 256, 0, st>>>(d_rows, d_file, d_train, n_train, d_key);
-        FDR_TRY(cudaGetLastError());
+        CUDA_TRY(cudaGetLastError());
         size_t tb = 0;
-        FDR_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key2, d_train, d_val, (int)n_train, 0, 64, st));
-        if (int rc = ensure_tmp(tb)) return rc;
-        FDR_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, d_key, d_key2, d_train, d_val, (int)n_train, 0, 64, st));   // stable: poisson order kept
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key2, d_train, d_val, (int)n_train, 0, 64, st));
+        CUDA_TRY(A.reserve_tmp(tb));
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, d_key, d_key2, d_train, d_val, (int)n_train, 0, 64, st));   // stable: poisson order kept
         k_rt_heads<<<gt, 256, 0, st>>>(d_key2, n_train, d_flag);
-        FDR_TRY(cudaGetLastError());
-        FDR_TRY(cub::DeviceSelect::Flagged(nullptr, tb, count_it, d_flag, d_seg, d_count, (int)n_train, st));
-        if (int rc = ensure_tmp(tb)) return rc;
-        FDR_TRY(cub::DeviceSelect::Flagged(tmp, tb, count_it, d_flag, d_seg, d_count, (int)n_train, st));
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, count_it, d_flag, d_seg, d_count, (int)n_train, st));
+        CUDA_TRY(A.reserve_tmp(tb));
+        CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, count_it, d_flag, d_seg, d_count, (int)n_train, st));
         if (int rc = read_count(&n_seg)) return rc;
         const unsigned gs = (unsigned)((n_seg + 255) / 256);
         k_rt_seg_min<<<gs, 256, 0, st>>>(d_rows, d_key2, d_val, d_seg, n_seg, n_train, d_segmin, d_flag);
-        FDR_TRY(cudaGetLastError());
-        FDR_TRY(cub::DeviceSelect::Flagged(nullptr, tb, count_it, d_flag, d_prow, d_count, (int)n_seg, st));
-        if (int rc = ensure_tmp(tb)) return rc;
-        FDR_TRY(cub::DeviceSelect::Flagged(tmp, tb, count_it, d_flag, d_prow, d_count, (int)n_seg, st));
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, count_it, d_flag, d_prow, d_count, (int)n_seg, st));
+        CUDA_TRY(A.reserve_tmp(tb));
+        CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, count_it, d_flag, d_prow, d_count, (int)n_seg, st));
         if (int rc = read_count(&n_pr)) return rc;
         const unsigned gp = (unsigned)((n_pr + 255) / 256);
         k_rt_row_mean<<<gp, 256, 0, st>>>(d_key2, d_seg, d_segmin, d_prow, n_pr, n_seg, d_maxrt, d_keep);
-        FDR_TRY(cudaGetLastError());
-        FDR_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_keep, d_mrow, (int)n_pr, st));
-        if (int rc = ensure_tmp(tb)) return rc;
-        FDR_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, d_keep, d_mrow, (int)n_pr, st));
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_keep, d_mrow, (int)n_pr, st));
+        CUDA_TRY(A.reserve_tmp(tb));
+        CUDA_TRY(cub::DeviceScan::ExclusiveSum(A.tmp, tb, d_keep, d_mrow, (int)n_pr, st));
         uint32_t last[2] = {0, 0};
-        FDR_TRY(cudaMemcpyAsync(&last[0], d_mrow + n_pr - 1, 4, cudaMemcpyDeviceToHost, st));
-        FDR_TRY(cudaMemcpyAsync(&last[1], d_keep + n_pr - 1, 4, cudaMemcpyDeviceToHost, st));
-        FDR_TRY(cudaStreamSynchronize(st));
+        CUDA_TRY(cudaMemcpyAsync(&last[0], d_mrow + n_pr - 1, 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(&last[1], d_keep + n_pr - 1, 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
         n_rows = (uint64_t)last[0] + last[1];
-        FDR_TRY(A.alloc(&d_mat, n_rows * n_files));
-        FDR_TRY(A.alloc(&d_mean, n_rows));
-        FDR_TRY(cudaMemsetAsync(d_mat, 0xFF, 8 * n_rows * n_files, st));   // NaN where a peptide was not seen in a file
+        CUDA_TRY(A.alloc(&d_mat, n_rows * n_files));
+        CUDA_TRY(A.alloc(&d_mean, n_rows));
+        CUDA_TRY(cudaMemsetAsync(d_mat, 0xFF, 8 * n_rows * n_files, st));   // NaN where a peptide was not seen in a file
         k_rt_fill<<<gp, 256, 0, st>>>(d_key2, d_seg, d_segmin, d_prow, n_pr, n_seg, d_maxrt, d_keep, d_mrow, n_files, d_mat, d_mean);
-        FDR_TRY(cudaGetLastError());
+        CUDA_TRY(cudaGetLastError());
     }
     k_rt_align<<<(unsigned)((n_files + 127) / 128), 128, 0, st>>>(d_mat, d_mean, n_rows, n_files, d_maxrt, d_align);
-    FDR_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     float* d_aligned = d_out[0];
     k_rt_aligned<<<g, 256, 0, st>>>(d_rows, d_file, n, d_align, d_aligned);
-    FDR_TRY(cudaGetLastError());
-    FDR_TRY(cudaEventRecord(ev[2], st));
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(ev[2], st));
 
     // 3. retention_model::predict, 4. mobility_model::predict
     if (int rc = rt_model<0>(st, A, fma, pk, d_rows, n, d_train, n_train, d_aligned, d_aligned, d_out[1], d_out[2], &out->rt_fitted, &out->rt_r2,
                              &out->rt_eps, out->rt_beta))
         return rc;
-    FDR_TRY(cudaEventRecord(ev[3], st));
+    CUDA_TRY(cudaEventRecord(ev[3], st));
     if (int rc = rt_model<1>(st, A, fma, pk, d_rows, n, d_train, n_train, nullptr, d_aligned, d_out[3], d_out[4], &out->ims_fitted, &out->ims_r2,
                              &out->ims_eps, out->ims_beta))
         return rc;
-    FDR_TRY(cudaEventRecord(ev[4], st));
+    CUDA_TRY(cudaEventRecord(ev[4], st));
 
     float* dst[5] = {out->aligned_rt, out->predicted_rt, out->delta_rt_model, out->predicted_ims, out->delta_ims_model};
-    for (int c = 0; c < 5; c++) FDR_TRY(cudaMemcpyAsync(dst[c], d_out[c], 4 * n, cudaMemcpyDeviceToHost, st));
-    if (out->spectrum_q) FDR_TRY(cudaMemcpyAsync(out->spectrum_q, d_q, 4 * n, cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaMemcpyAsync(out->alignments, d_align, sizeof(sage_b200_alignment) * n_files, cudaMemcpyDeviceToHost, st));
-    FDR_TRY(cudaStreamSynchronize(st));
+    for (int c = 0; c < 5; c++) CUDA_TRY(cudaMemcpyAsync(dst[c], d_out[c], 4 * n, cudaMemcpyDeviceToHost, st));
+    if (out->spectrum_q) CUDA_TRY(cudaMemcpyAsync(out->spectrum_q, d_q, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->alignments, d_align, sizeof(sage_b200_alignment) * n_files, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     out->training_rows = n_train;
     out->aligned_peptides = n_rows;
     float* ms[4] = {&out->ms_sort_q, &out->ms_alignment, &out->ms_rt_model, &out->ms_ims_model};
-    for (int i = 0; i < 4; i++) FDR_TRY(cudaEventElapsedTime(ms[i], ev[i], ev[i + 1]));
-    FDR_TRY(cudaEventElapsedTime(&out->ms_total, ev[0], ev[4]));
+    for (int i = 0; i < 4; i++) CUDA_TRY(cudaEventElapsedTime(ms[i], ev[i], ev[i + 1]));
+    CUDA_TRY(cudaEventElapsedTime(&out->ms_total, ev[0], ev[4]));
     return 0;
 }
-#undef FDR_TRY
 
 #if SAGE_B200_PHASE_CLOCKS
 // variant builds only (not declared in the header): cycles per k_score phase summed over CTAs since the last reset
