@@ -389,6 +389,44 @@ typedef struct {
 int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_peptides* peptides, const sage_b200_feature* rows, const uint32_t* file_id, uint64_t n,
                          uint64_t n_files, sage_b200_rt_out* out);
 
+/* ---------------------------------------------------------------------------------------------------------------------------------------------
+ * Picked FDR (fdr.rs): picked_peptide and picked_protein (runner.rs:534-537, Competition::assign_q_value) and picked_precursor (runner.rs:572).
+ * Every output is reproducible bit for bit under the definitions of DESIGN.md §12; competition entries are ordered by the first row that
+ * reaches them, so call these on the rows in spectrum_fdr's sorted order, as the runner does.
+ */
+typedef struct {
+    const float* cterm;               /* [n_peptides] Peptide::cterm, NaN = None; NULL = None for every peptide */
+    const uint32_t* n_proteins;       /* [n_peptides] Peptide::proteins.len() */
+    const uint32_t* protein;          /* [n_peptides] id of the single protein name (equal ids <=> equal names); read only where n_proteins == 1 */
+    uint8_t generate_decoys;          /* IndexedDatabase::generate_decoys */
+} sage_b200_picked_params;
+typedef struct {
+    float* peptide_q;                 /* [n] indexed like the rows */
+    float* protein_q;                 /* [n]; 1.0 for rows whose peptide has != 1 protein */
+    uint64_t peptide_passing, protein_passing;   /* assign_q_value's return values: target rows at q <= 0.01 */
+    uint64_t peptide_entries, protein_entries;   /* competition entries (the maps' sizes) */
+    float ms_keys, ms_peptide, ms_protein, ms_total;   /* CUDA-event stage times: peptide keys, each competition, the whole call */
+} sage_b200_picked_out;
+/* picked_peptide then picked_protein over the rows. peptides: the table the rows' PeptideIx index (residue_offsets, sequence, modifications,
+ * nterm and decoy are read; the decoy flag is Peptide::decoy). The call takes no db handle: the caller passes the same table the searched db
+ * was built from (sage_b200_db_create / _build), since a PeptideIx means nothing against another table; only its size is checked here, through
+ * the PeptideIx bound. picked_protein's Ix is (protein, side) with generate_decoys and the protein alone without; the reference's Ix is the
+ * string `decoy_tag + name`, so a target protein whose name starts with the decoy tag would share an Ix with a decoy there, and not here. EINVAL for a null required pointer, a peptide_idx outside the table, or two
+ * distinct peptides on one side with one key (the reference panics; the message names both PeptideIx); ELIMIT beyond 2^31 - 1 rows, beyond
+ * 65535 * 4096 rows (the KDE's chunk grid) or when the work buffers do not fit the device's free memory (checked before allocating).
+ * n == 0: no device work. */
+int sage_b200_picked_fdr(int device, const sage_b200_peptides* peptides, const sage_b200_picked_params* p, const sage_b200_feature* rows,
+                         const float* discriminant_score, uint64_t n, sage_b200_picked_out* out);
+/* picked_precursor over quantify's rows in sage_b200_lfq_integrate's order: score = Peak::score, decoy (nonzero = decoy). q_value[n] is
+ * indexed like the rows; *passing counts target rows at q <= 0.05. EINVAL for a null pointer; ELIMIT beyond 2^31 - 1 rows or when the work
+ * buffers do not fit the device's free memory (checked before allocating). n == 0: no device work. */
+int sage_b200_picked_precursor(int device, const double* score, const uint8_t* decoy, uint64_t n, float* q_value, uint64_t* passing);
+/* White-box hook: entry_rank[i] = the rank, in first-appearance order, of row i's picked_peptide entry. hash_bits (3..64) truncates the key
+ * hash so that distinct keys collide and the exact comparison that separates them is exercised; with hash_bits < 64 at most 2^16 rows
+ * (ELIMIT beyond: equal-hash runs are compared pairwise). */
+int sage_b200_competition_keys(int device, const sage_b200_peptides* peptides, const sage_b200_picked_params* p, const uint32_t* peptide_idx, uint64_t n,
+                               uint32_t hash_bits, uint32_t* entry_rank);
+
 /* Page-locked host buffers: spectra/feature arrays placed here are copied by DMA without a staging memcpy. */
 void* sage_b200_host_alloc(size_t bytes);
 /* The same for a batch sage_b200_score_batch_multi cuts into n_devices contiguous blocks: the i-th of n equal parts of the buffer is placed on the

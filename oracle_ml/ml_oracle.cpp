@@ -18,12 +18,19 @@
 //   mobility_model.rs       MobilityModel::embed / fit / predict
 // in the orders DESIGN.md §11 defines: poisson ties by input row, ordered maps (ascending PeptideIx, ascending file), fit chunks of RT_CHUNK
 // training rows merged in order.
+//
+// Also restates fdr.rs:16-287 (Competition::assign_q_value, picked_peptide, picked_protein, picked_precursor) with real key strings:
+// Peptide::reverse and Display (peptide.rs:307-318, 390-406) written out with Rust's shortest round-trip f32 formatting, and
+// insertion-ordered maps, in the definitions of DESIGN.md §12.
 #include <algorithm>
+#include <charconv>
 #include <chrono>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <map>
+#include <string>
+#include <unordered_map>
 #include <thread>
 #include <vector>
 
@@ -676,6 +683,202 @@ double mo_predict_rt(const uint32_t* off, const uint8_t* seq, const float* mono,
         }
     }
     return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ fdr.rs (picked FDR)
+namespace {
+
+std::string fmt_plus(float x) {   // `{:+}` of an f32: shortest round-trip, positional, signed; NaN prints "NaN"
+    if (std::isnan(x)) return "NaN";
+    if (std::isinf(x)) return x > 0 ? "+inf" : "-inf";
+    char buf[128];
+    auto r = std::to_chars(buf, buf + sizeof buf, x, std::chars_format::fixed);
+    std::string s(buf, r.ptr);
+    return std::signbit(x) ? s : "+" + s;
+}
+
+struct PepTable {
+    const uint32_t* off;
+    const uint8_t* seq;
+    const float* mods;
+    const float* nterm;
+    const float* cterm;   // NULL = None everywhere
+    const uint8_t* decoy;
+};
+
+std::string display(const PepTable& T, uint32_t i, bool reversed) {   // impl Display for Peptide, of the peptide or of its reverse()
+    const uint32_t a = T.off[i], L = T.off[i + 1] - a;
+    std::string s(T.seq + a, T.seq + a + L);
+    std::vector<float> m(T.mods + a, T.mods + a + L);
+    const uint32_t n = L == 0 ? 0 : L - 1;
+    if (reversed && n > 1) {
+        std::reverse(s.begin() + 1, s.begin() + n);
+        std::reverse(m.begin() + 1, m.begin() + n);
+    }
+    std::string out;
+    if (!std::isnan(T.nterm[i])) out += "[" + fmt_plus(T.nterm[i]) + "]-";
+    for (uint32_t k = 0; k < L; k++) {
+        out += s[k];
+        if (m[k] != 0.0f) out += "[" + fmt_plus(m[k]) + "]";   // NaN != 0.0 holds
+    }
+    if (T.cterm && !std::isnan(T.cterm[i])) out += "-[" + fmt_plus(T.cterm[i]) + "]";
+    return out;
+}
+
+struct Comp {
+    float forward = -3.40282347e+38f, reverse = -3.40282347e+38f;
+    bool has_f = false, has_r = false;
+    std::string fix, rix;
+};
+
+// An insertion-ordered map: entries in the order their key first appears.
+struct CompMap {
+    std::unordered_map<std::string, size_t> at;
+    std::vector<Comp> entries;
+    Comp& entry(const std::string& key) {
+        auto it = at.find(key);
+        if (it != at.end()) return entries[it->second];
+        at.emplace(key, entries.size());
+        entries.emplace_back();
+        return entries.back();
+    }
+};
+
+float fmax_rust(float acc, float v) { return v > acc ? v : acc; }
+float fmin_q(float a, float b) {   // DESIGN.md §12: NaN ignored, -0.0 below +0.0
+    if (std::isnan(a)) return b;
+    if (std::isnan(b)) return a;
+    if (a < b) return a;
+    if (b < a) return b;
+    return std::signbit(a) ? a : b;
+}
+int64_t total_key(float x) {
+    int32_t b;
+    memcpy(&b, &x, 4);
+    return (int64_t)(b ^ ((b >> 31) & 0x7FFFFFFF));
+}
+
+struct QRow {
+    std::string ix;
+    bool decoy;
+    float score, q;
+};
+
+// fdr.rs:87-111 over rows in pre-sort order; pep_of(row) gives each sorted row's PEP.
+template <class Pep>
+uint64_t q_tail(std::vector<QRow>& rows, Pep pep_of, float threshold) {
+    std::stable_sort(rows.begin(), rows.end(), [](const QRow& a, const QRow& b) { return total_key(b.score) < total_key(a.score); });
+    float decoy = 1.0f, target = 0.0f;
+    for (QRow& r : rows) {
+        decoy += pep_of(r);
+        if (!r.decoy) target += 1.0f;
+        r.q = decoy / target;
+    }
+    float q_min = 1.0f;
+    uint64_t passing = 0;
+    for (size_t k = rows.size(); k-- > 0;) {
+        q_min = fmin_q(q_min, rows[k].q);
+        rows[k].q = q_min;
+        if (q_min <= threshold && !rows[k].decoy) passing++;
+    }
+    return passing;
+}
+
+// Competition::assign_q_value (fdr.rs:59-120)
+uint64_t assign_q_value(const CompMap& map, int threads, std::unordered_map<std::string, float>* out) {
+    const size_t m = map.entries.size();
+    std::vector<double> score(m);
+    std::vector<uint8_t> dec(m);
+    for (size_t e = 0; e < m; e++) {
+        const Comp& c = map.entries[e];
+        score[e] = (double)(c.reverse > c.forward ? c.reverse : c.forward);
+        dec[e] = c.reverse >= c.forward;
+    }
+    std::vector<QRow> rows;
+    for (const Comp& c : map.entries) {
+        if (c.has_f) rows.push_back({c.fix, false, c.forward, 1.0f});
+        if (c.has_r) rows.push_back({c.rix, true, c.reverse, 1.0f});
+    }
+    if (m == 0) return 0;
+    const Estimator est = kde_build(score.data(), dec.data(), m, 1000, true, 1.0, threads);
+    const uint64_t passing = q_tail(rows, [&](const QRow& r) { return (float)est.posterior_error((double)r.score); }, 0.01f);
+    for (const QRow& r : rows) (*out)[r.ix] = r.q;   // later rows overwrite
+    return passing;
+}
+
+}  // namespace
+
+extern "C" {
+
+// picked_peptide then picked_protein. Proteins of peptide i: names [prot_off[i], prot_off[i+1]) of the list whose name k is
+// chars[name_off[k] .. name_off[k+1]). Returns 0, or -1 for two distinct peptides on one side with one key (clash[0..1]).
+int mo_picked_fdr(const uint32_t* off, const uint8_t* seq, const float* mods, const float* nterm, const float* cterm, const uint8_t* decoy,
+                  const uint32_t* prot_off, const uint64_t* name_off, const char* chars, const char* decoy_tag, int generate_decoys,
+                  const uint32_t* pep_idx, const float* disc, uint64_t n, int threads, float* peptide_q, float* protein_q, uint64_t* passing,
+                  uint64_t* entries, uint32_t* clash) {
+    const PepTable T{off, seq, mods, nterm, cterm, decoy};
+    std::unordered_map<uint32_t, std::string> keys;
+    CompMap pm;
+    for (uint64_t i = 0; i < n; i++) {   // fdr.rs:125-144
+        const uint32_t p = pep_idx[i];
+        auto it = keys.find(p);
+        if (it == keys.end()) it = keys.emplace(p, display(T, p, generate_decoys && decoy[p])).first;
+        Comp& e = pm.entry(it->second);
+        const std::string ix = std::to_string(p);
+        std::string& side_ix = decoy[p] ? e.rix : e.fix;
+        bool& has = decoy[p] ? e.has_r : e.has_f;
+        if (has && side_ix != ix) {
+            clash[0] = (uint32_t)std::stoul(side_ix);
+            clash[1] = p;
+            return -1;
+        }
+        float& sc = decoy[p] ? e.reverse : e.forward;
+        sc = fmax_rust(sc, disc[i]);
+        side_ix = ix;
+        has = true;
+    }
+    std::unordered_map<std::string, float> pq;
+    passing[0] = assign_q_value(pm, threads, &pq);
+    entries[0] = pm.entries.size();
+    for (uint64_t i = 0; i < n; i++) peptide_q[i] = pq.at(std::to_string(pep_idx[i]));   // fdr.rs:148-150
+
+    auto name = [&](uint32_t k) { return std::string(chars + name_off[k], chars + name_off[k + 1]); };
+    auto proteins = [&](uint32_t p) {   // Peptide::proteins(decoy_tag, generate_decoys), peptide.rs:81-96
+        std::string s;
+        for (uint32_t k = prot_off[p]; k < prot_off[p + 1]; k++) {
+            if (k > prot_off[p]) s += ";";
+            s += (decoy[p] && generate_decoys) ? std::string(decoy_tag) + name(k) : name(k);
+        }
+        return s;
+    };
+    CompMap rm;
+    for (uint64_t i = 0; i < n; i++) {   // fdr.rs:160-177: the key is the protein list, here of length 1
+        const uint32_t p = pep_idx[i];
+        if (prot_off[p + 1] - prot_off[p] != 1) continue;
+        Comp& e = rm.entry(name(prot_off[p]));
+        if (decoy[p]) { e.reverse = fmax_rust(e.reverse, disc[i]); e.rix = proteins(p); e.has_r = true; }
+        else { e.forward = fmax_rust(e.forward, disc[i]); e.fix = proteins(p); e.has_f = true; }
+    }
+    std::unordered_map<std::string, float> rq;
+    passing[1] = assign_q_value(rm, threads, &rq);
+    entries[1] = rm.entries.size();
+    for (uint64_t i = 0; i < n; i++) {   // fdr.rs:181-187
+        const uint32_t p = pep_idx[i];
+        protein_q[i] = prot_off[p + 1] - prot_off[p] == 1 ? rq.at(proteins(p)) : 1.0f;
+    }
+    return 0;
+}
+
+// picked_precursor (fdr.rs:228-287) over the rows in the given order.
+uint64_t mo_picked_precursor(const double* score, const uint8_t* decoy, uint64_t n, float* q) {
+    std::vector<QRow> rows(n);
+    for (uint64_t i = 0; i < n; i++) rows[i] = {std::to_string(i), decoy[i] != 0, (float)score[i], 1.0f};
+    // `decoy += 1.0` on decoy rows and `target += 1.0` on target rows: the tail's sum with PEP 1 / 0 (+0.0 leaves an f32 as it is)
+    const uint64_t passing = q_tail(rows, [](const QRow& r) { return r.decoy ? 1.0f : 0.0f; }, 0.05f);
+    for (const QRow& r : rows) q[std::stoull(r.ix)] = r.q;
+    return passing;
 }
 
 }  // extern "C"

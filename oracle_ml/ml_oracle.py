@@ -41,6 +41,9 @@ def lib():
         _lib.mo_linreg_fit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.mo_predict_rt.restype = C.c_double
         _lib.mo_predict_rt.argtypes = [C.c_void_p] * 5 + [C.c_uint64, C.c_uint64, C.c_int] + [C.c_void_p] * 13
+        _lib.mo_picked_fdr.argtypes = [C.c_void_p] * 9 + [C.c_char_p, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int] + [C.c_void_p] * 5
+        _lib.mo_picked_precursor.restype = C.c_uint64
+        _lib.mo_picked_precursor.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
     return _lib
 
 
@@ -131,3 +134,44 @@ def predict_rt(peptides, features, file_id, n_files, threads=None) -> dict:
                rt_fitted=bool(fitted[0]), rt_r2=float(r2[0]), rt_eps=float(eps[0]), rt_beta=rt_beta, ims_fitted=bool(fitted[1]), ims_r2=float(r2[1]),
                ims_eps=float(eps[1]), ims_beta=ims_beta, seconds=secs, threads=threads)
     return res
+
+
+class PickedClash(ValueError):
+    """Two distinct peptides on one side with one key: the reference panics at fdr.rs:149."""
+
+
+def picked_fdr(peptides, pep_idx, score, proteins, cterm=None, generate_decoys=True, decoy_tag="rev_", threads=None) -> dict:
+    """picked_peptide then picked_protein (fdr.rs) on the CPU with real key strings. `peptides` has seq_off, seq, mods, nterm and decoy;
+    proteins[p] is Peptide::proteins of peptide p (a list of names). The same keys as sage_b200.picked_fdr (stage times aside), plus `seconds`."""
+    import time
+    off, seq, mods, nterm, dec = (np.ascontiguousarray(a, t) for a, t in ((peptides.seq_off, np.uint32), (peptides.seq, np.uint8), (peptides.mods, np.float32),
+                                                                             (peptides.nterm, np.float32), (peptides.decoy, np.uint8)))
+    ct = None if cterm is None else np.ascontiguousarray(cterm, np.float32)
+    names = [nm.encode() for lst in proteins for nm in lst]
+    prot_off = np.zeros(len(proteins) + 1, np.uint32)
+    prot_off[1:] = np.cumsum([len(lst) for lst in proteins])
+    name_off = np.zeros(len(names) + 1, np.uint64)
+    name_off[1:] = np.cumsum([len(b) for b in names])
+    chars = np.frombuffer(b"".join(names) + b"\0", np.uint8).copy()
+    idx = np.ascontiguousarray(pep_idx, np.uint32)
+    disc = np.ascontiguousarray(score, np.float32)
+    n = len(idx)
+    pq, rq = np.zeros(n, np.float32), np.zeros(n, np.float32)
+    passing, entries, clash = np.zeros(2, np.uint64), np.zeros(2, np.uint64), np.zeros(2, np.uint32)
+    t0 = time.perf_counter()
+    rc = lib().mo_picked_fdr(_p(off), _p(seq), _p(mods), _p(nterm), _p(ct), _p(dec), _p(prot_off), _p(name_off), _p(chars), decoy_tag.encode(),
+                             int(bool(generate_decoys)), _p(idx), _p(disc), n, int(threads or default_threads()), _p(pq), _p(rq), _p(passing), _p(entries),
+                             _p(clash))
+    if rc != 0:
+        raise PickedClash(f"peptides {clash[0]} and {clash[1]} share a key on one side")
+    return dict(peptide_q=pq, protein_q=rq, peptide_passing=int(passing[0]), protein_passing=int(passing[1]), peptide_entries=int(entries[0]),
+                protein_entries=int(entries[1]), seconds=time.perf_counter() - t0)
+
+
+def picked_precursor(score, decoy):
+    """picked_precursor (fdr.rs:228-287) on the CPU over the rows in the given order: (q per row, passing)."""
+    s = np.ascontiguousarray(score, np.float64)
+    d = np.ascontiguousarray(decoy, np.uint8)
+    q = np.zeros(len(s), np.float32)
+    passing = lib().mo_picked_precursor(_p(s), _p(d), len(s), _p(q))
+    return q, int(passing)

@@ -91,6 +91,7 @@ EXPORTED_SYMBOLS = [
     "sage_b200_host_log_variant", "sage_b200_host_log1pf_exact", "sage_b200_device_log", "sage_b200_bind_thread_to_device", "sage_b200_host_alloc_blocks",
     "sage_b200_lfq_create", "sage_b200_lfq_add_ms1", "sage_b200_lfq_integrate", "sage_b200_lfq_get_info", "sage_b200_lfq_export", "sage_b200_lfq_destroy",
     "sage_b200_spectrum_fdr", "sage_b200_kde_build", "sage_b200_device_math", "sage_b200_predict_rt",
+    "sage_b200_picked_fdr", "sage_b200_picked_precursor", "sage_b200_competition_keys",
 ]
 
 _lib = None
@@ -846,3 +847,83 @@ def predict_rt(db: IndexedDatabase, peptides: Peptides, features: np.ndarray, fi
                     f"{m}_eps": float(getattr(out, f"{m}_eps")), f"{m}_beta": np.array(getattr(out, f"{m}_beta")[:d], np.float64)})
     res.update({s: float(getattr(out, s)) for s in RT_STAGES})
     return res
+
+
+# ------------------------------------------------------------------------------------------------ picked FDR (fdr.rs)
+class CPickedParams(C.Structure):
+    _fields_ = [("cterm", C.c_void_p), ("n_proteins", C.c_void_p), ("protein", C.c_void_p), ("generate_decoys", C.c_uint8)]
+
+
+PICKED_STAGES = ["ms_keys", "ms_peptide", "ms_protein", "ms_total"]
+
+
+class CPickedOut(C.Structure):
+    _fields_ = [("peptide_q", C.c_void_p), ("protein_q", C.c_void_p), ("peptide_passing", C.c_uint64), ("protein_passing", C.c_uint64),
+                ("peptide_entries", C.c_uint64), ("protein_entries", C.c_uint64)] + [(s, C.c_float) for s in PICKED_STAGES]
+
+
+def _picked_params(peptides: Peptides, n_proteins, protein, cterm, generate_decoys, keep: list) -> CPickedParams:
+    n = len(peptides)
+    cols = []
+    for name, x, dt in (("cterm", cterm, np.float32), ("n_proteins", n_proteins, np.uint32), ("protein", protein, np.uint32)):
+        if x is None:
+            cols.append(None)
+            continue
+        a = np.ascontiguousarray(x, dt)
+        if len(a) != n:
+            raise ValueError(f"{name} must have one value per peptide")
+        keep.append(a)
+        cols.append(_ptr(a))
+    return CPickedParams(*cols, int(bool(generate_decoys)))
+
+
+def picked_fdr(peptides: Peptides, features: np.ndarray, discriminant_score, n_proteins, protein, cterm=None, generate_decoys: bool = True,
+               device: int = 0) -> dict:
+    """picked_peptide then picked_protein (fdr.rs:123-190, runner.rs:534-537) on the device. `features` are FEATURE_DTYPE rows in the order the
+    runner holds them (spectrum_fdr's sorted order: entries are ordered by the first row that reaches them), `discriminant_score` one f32 per
+    row, `peptides` the table the rows' PeptideIx index. Per peptide: `n_proteins` (Peptide::proteins.len()), `protein` (an id of the single
+    protein name, equal ids for equal names; read where n_proteins == 1) and `cterm` (NaN = None; None = no C-terminal modifications).
+    Returns peptide_q and protein_q (f32, indexed like the rows; protein_q is 1.0 where the peptide has != 1 protein), peptide_passing,
+    protein_passing, peptide_entries, protein_entries and the stage times (ms_*)."""
+    rows = np.ascontiguousarray(features)
+    if rows.dtype != FEATURE_DTYPE:
+        raise TypeError("features must have FEATURE_DTYPE")
+    n = len(rows)
+    score = np.ascontiguousarray(discriminant_score, np.float32)
+    if len(score) != n:
+        raise ValueError("discriminant_score must have one value per row")
+    keep: list = []
+    cp = peptides._c(keep)
+    params = _picked_params(peptides, n_proteins, protein, cterm, generate_decoys, keep)
+    res = dict(peptide_q=np.zeros(n, np.float32), protein_q=np.zeros(n, np.float32))
+    out = CPickedOut(_ptr(res["peptide_q"]), _ptr(res["protein_q"]))
+    _check(load_library().sage_b200_picked_fdr(C.c_int(device), C.byref(cp), C.byref(params), _ptr(rows), _ptr(score), C.c_uint64(n), C.byref(out)))
+    res.update({k: int(getattr(out, k)) for k in ("peptide_passing", "protein_passing", "peptide_entries", "protein_entries")})
+    res.update({s: float(getattr(out, s)) for s in PICKED_STAGES})
+    return res
+
+
+def picked_precursor(score, decoy, device: int = 0):
+    """picked_precursor (fdr.rs:228-287, runner.rs:572) on the device over FeatureMap.quantify()'s rows: `score` (Peak::score, f64) and `decoy`.
+    Returns (q_value f32 indexed like the rows, passing = target rows at q <= 0.05)."""
+    s = np.ascontiguousarray(score, np.float64)
+    d = np.ascontiguousarray(decoy, np.uint8)
+    if len(d) != len(s):
+        raise ValueError("decoy must have one value per row")
+    q = np.zeros(len(s), np.float32)
+    passing = C.c_uint64(0)
+    _check(load_library().sage_b200_picked_precursor(C.c_int(device), _ptr(s), _ptr(d), C.c_uint64(len(s)), _ptr(q), C.byref(passing)))
+    return q, int(passing.value)
+
+
+def competition_keys(peptides: Peptides, peptide_idx, cterm=None, generate_decoys: bool = True, hash_bits: int = 64, device: int = 0) -> np.ndarray:
+    """Test hook: each row's picked_peptide entry rank (first-appearance order). hash_bits < 64 truncates the key hash so that distinct keys
+    collide and the exact comparison that separates them runs."""
+    idx = np.ascontiguousarray(peptide_idx, np.uint32)
+    keep: list = []
+    cp = peptides._c(keep)
+    params = _picked_params(peptides, None, None, cterm, generate_decoys, keep)
+    out = np.zeros(len(idx), np.uint32)
+    _check(load_library().sage_b200_competition_keys(C.c_int(device), C.byref(cp), C.byref(params), _ptr(idx), C.c_uint64(len(idx)),
+                                                     C.c_uint32(int(hash_bits)), _ptr(out)))
+    return out

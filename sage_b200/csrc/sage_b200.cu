@@ -22,6 +22,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <chrono>
 #include <condition_variable>
 #include <memory>
@@ -35,6 +36,7 @@
 #include "lfq.cuh"
 #include "fdr.cuh"
 #include "rt.cuh"
+#include "picked.cuh"
 
 using namespace sb;
 
@@ -3174,6 +3176,421 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
     float* ms[4] = {&out->ms_sort_q, &out->ms_alignment, &out->ms_rt_model, &out->ms_ims_model};
     for (int i = 0; i < 4; i++) CUDA_TRY(cudaEventElapsedTime(ms[i], ev[i], ev[i + 1]));
     CUDA_TRY(cudaEventElapsedTime(&out->ms_total, ev[0], ev[4]));
+    return 0;
+}
+
+// ================================================================================== picked FDR (fdr.rs; kernels in picked.cuh)
+static unsigned grid256(uint64_t n) { return (unsigned)((n + 255) / 256); }
+static constexpr uint32_t PICKED_HOOK_MAX_ROWS = 1u << 16;   // competition_keys with hash_bits < 64
+
+// Checks run before the device is looked at, and the capacity check before anything is allocated. Per competing row: keys, indices, sorted
+// copies, ranks, scores, flags, the q-value tail's columns and the sorts' temporary storage; per row of the call also the key material.
+static int picked_limits(const char* what, uint64_t n) {
+    if (n > (uint64_t)INT32_MAX) return fail(SAGE_B200_ELIMIT, "%s: more than 2^31 - 1 rows", what);
+    if (n > (uint64_t)65535 * KDE_CHUNK) return fail(SAGE_B200_ELIMIT, "%s: more than 65535 KDE chunks of %d rows", what, KDE_CHUNK);
+    return 0;
+}
+static int picked_memory(const char* what, uint64_t n, uint64_t extra) {
+    size_t free_b = 0, total_b = 0;
+    CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+    const uint64_t need = n * 256 + extra + 2 * 8000ull * (n / KDE_CHUNK + 2) + (64ull << 20);
+    if (need > free_b) return fail(SAGE_B200_ELIMIT, "%s: %llu rows need about %llu bytes of device memory, %llu free", what, (unsigned long long)n,
+                                   (unsigned long long)need, (unsigned long long)free_b);
+    return 0;
+}
+
+// The q-value tail shared by assign_q_value (fdr.rs:87-119) and picked_precursor (fdr.rs:255-286), over R rows in their pre-sort order:
+// the stable descending sort, the PEPs (from the KDE's bins, or 1 / 0 by decoy flag when bins == NULL), the sequential running sum, q, the
+// suffix minimum, passing, and the q of each of the n_ix ixs (the latest sorted row that carries it wins).
+static int picked_tail(cudaStream_t st, DevArena& A, uint32_t R, const float* q_score, const uint8_t* q_decoy, const uint32_t* q_ix,
+                       const uint32_t* q_key, const uint32_t* q_idx, const double* bins, const double* moments, float threshold, uint32_t n_ix,
+                       float* q_ix_val, unsigned long long* d_passing) {
+    CUDA_TRY(cudaMemsetAsync(d_passing, 0, 8, st));
+    if (R == 0) return 0;
+    uint32_t *key_s = nullptr, *order = nullptr, *is_t = nullptr, *tinc = nullptr, *win = nullptr;
+    float *pep = nullptr, *sum = nullptr, *rq = nullptr, *rqmin = nullptr, *q = nullptr;
+    CUDA_TRY(A.alloc(&key_s, R));
+    CUDA_TRY(A.alloc(&order, R));
+    CUDA_TRY(A.alloc(&is_t, R));
+    CUDA_TRY(A.alloc(&tinc, R));
+    CUDA_TRY(A.alloc(&win, n_ix));
+    CUDA_TRY(A.alloc(&pep, R));
+    CUDA_TRY(A.alloc(&sum, R));
+    CUDA_TRY(A.alloc(&rq, R));
+    CUDA_TRY(A.alloc(&rqmin, R));
+    CUDA_TRY(A.alloc(&q, R));
+    size_t tb = 0, tb2 = 0, tb3 = 0;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, q_key, key_s, q_idx, order, (int)R, 0, 32, st));
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, tb2, is_t, tinc, (int)R, st));
+    CUDA_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb3, rq, rqmin, PickedMin(), (int)R, st));
+    CUDA_TRY(A.reserve_tmp(std::max(tb, std::max(tb2, tb3))));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, q_key, key_s, q_idx, order, (int)R, 0, 32, st));   // stable: pre-sort order on ties
+    const unsigned g = grid256(R);
+    k_picked_pep<<<g, 256, 0, st>>>(order, q_score, q_decoy, R, bins, moments, pep, is_t);
+    CUDA_TRY(cudaGetLastError());
+    k_picked_running_sum<<<1, 32, 0, st>>>(pep, R, sum);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(A.tmp, tb2, is_t, tinc, (int)R, st));
+    k_picked_q_raw<<<g, 256, 0, st>>>(sum, tinc, R, rq);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceScan::InclusiveScan(A.tmp, tb3, rq, rqmin, PickedMin(), (int)R, st));
+    CUDA_TRY(cudaMemsetAsync(win, 0, 4ull * n_ix, st));
+    k_picked_q_min<<<g, 256, 0, st>>>(rqmin, q_decoy, order, q_ix, R, threshold, q, win, d_passing);
+    CUDA_TRY(cudaGetLastError());
+    k_picked_q_ix<<<g, 256, 0, st>>>(q, order, q_ix, win, R, q_ix_val);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+// Competition::assign_q_value (fdr.rs:59-120) over m competing rows: d_key groups them into entries (equal key = one entry), d_decoy picks the
+// side, d_score is the discriminant. d_pep (peptide level) holds each row's PeptideIx for the same-side check. d_rank[m] receives each row's
+// entry rank (first-appearance order); with d_out == NULL the call stops there. Otherwise d_out[m] receives each row's q.
+static int picked_competition(cudaStream_t st, DevArena& A, bool fma, uint32_t m, const uint32_t* d_key, const uint8_t* d_decoy, const float* d_score,
+                              const uint32_t* d_pep, bool ix_has_side, uint32_t* d_rank, float* d_out, uint64_t* entries, uint64_t* passing) {
+    *entries = *passing = 0;
+    if (m == 0) return 0;
+    thrust::counting_iterator<uint32_t> count_it(0);
+    uint32_t *idx = nullptr, *key_s = nullptr, *row_s = nullptr, *head = nullptr, *ginc = nullptr, *first = nullptr, *first_s = nullptr, *gidx = nullptr,
+             *g_sorted = nullptr, *rank_of_group = nullptr, *cnt = nullptr;
+    CUDA_TRY(A.alloc(&idx, m));
+    CUDA_TRY(A.alloc(&key_s, m));
+    CUDA_TRY(A.alloc(&row_s, m));
+    CUDA_TRY(A.alloc(&head, m));
+    CUDA_TRY(A.alloc(&ginc, m));
+    CUDA_TRY(A.alloc(&cnt, 4));
+    const unsigned g = grid256(m);
+    auto read_u32 = [&](const uint32_t* d, uint32_t* v) -> int {
+        CUDA_TRY(cudaMemcpyAsync(v, d, 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        return 0;
+    };
+    // 1. entries: sort (key, row); a run's head row is the first row that reaches the entry; rank the entries by it
+    size_t tb = 0;
+    k_picked_iota<<<g, 256, 0, st>>>(m, idx);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, key_s, idx, row_s, (int)m, 0, 32, st));
+    CUDA_TRY(A.reserve_tmp(tb));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, d_key, key_s, idx, row_s, (int)m, 0, 32, st));
+    k_picked_heads<<<g, 256, 0, st>>>(key_s, m, head);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, tb, head, ginc, (int)m, st));
+    CUDA_TRY(A.reserve_tmp(tb));
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(A.tmp, tb, head, ginc, (int)m, st));
+    uint32_t G = 0;
+    if (int rc = read_u32(ginc + m - 1, &G)) return rc;
+    CUDA_TRY(A.alloc(&first, G));
+    CUDA_TRY(A.alloc(&first_s, G));
+    CUDA_TRY(A.alloc(&gidx, G));
+    CUDA_TRY(A.alloc(&g_sorted, G));
+    CUDA_TRY(A.alloc(&rank_of_group, G));
+    CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, row_s, head, first, cnt, (int)m, st));
+    CUDA_TRY(A.reserve_tmp(tb));
+    CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, row_s, head, first, cnt, (int)m, st));
+    const unsigned gg = grid256(G);
+    k_picked_iota<<<gg, 256, 0, st>>>(G, gidx);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, first, first_s, gidx, g_sorted, (int)G, 0, 32, st));
+    CUDA_TRY(A.reserve_tmp(tb));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, first, first_s, gidx, g_sorted, (int)G, 0, 32, st));
+    k_picked_scatter_rank<<<gg, 256, 0, st>>>(g_sorted, G, rank_of_group);
+    CUDA_TRY(cudaGetLastError());
+    uint32_t *side_key = nullptr, *sk_s = nullptr, *row2_s = nullptr, *seg = nullptr;
+    CUDA_TRY(A.alloc(&side_key, m));
+    k_picked_row_rank<<<g, 256, 0, st>>>(row_s, ginc, rank_of_group, d_decoy, m, d_rank, side_key, idx);
+    CUDA_TRY(cudaGetLastError());
+    *entries = G;
+    if (!d_out) return 0;
+
+    // 2. fold each (entry, side) in row order (fdr.rs:125-144 / 160-177)
+    CUDA_TRY(A.alloc(&sk_s, m));
+    CUDA_TRY(A.alloc(&row2_s, m));
+    CUDA_TRY(A.alloc(&seg, m));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, side_key, sk_s, idx, row2_s, (int)m, 0, 32, st));
+    CUDA_TRY(A.reserve_tmp(tb));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, side_key, sk_s, idx, row2_s, (int)m, 0, 32, st));   // stable: row order within a side
+    k_picked_heads<<<g, 256, 0, st>>>(sk_s, m, head);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, count_it, head, seg, cnt, (int)m, st));
+    CUDA_TRY(A.reserve_tmp(tb));
+    CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, count_it, head, seg, cnt, (int)m, st));
+    uint32_t S = 0;
+    if (int rc = read_u32(cnt, &S)) return rc;
+    float* side_score = nullptr;
+    uint8_t *side_has = nullptr, *kde_flags = nullptr;
+    uint32_t *clash = nullptr, *n_rows = nullptr, *row_off = nullptr;
+    CUDA_TRY(A.alloc(&side_score, 2ull * G));
+    CUDA_TRY(A.alloc(&side_has, 2ull * G));
+    CUDA_TRY(A.alloc(&clash, 3));
+    CUDA_TRY(cudaMemsetAsync(side_has, 0, 2ull * G, st));
+    CUDA_TRY(cudaMemsetAsync(clash, 0, 12, st));
+    k_picked_fold<<<grid256(S), 256, 0, st>>>(sk_s, row2_s, seg, S, m, d_score, d_pep, side_score, side_has, clash);
+    CUDA_TRY(cudaGetLastError());
+    if (d_pep) {
+        uint32_t c[3];
+        CUDA_TRY(cudaMemcpyAsync(c, clash, 12, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (c[2]) return fail(SAGE_B200_EINVAL, "picked_fdr: peptides %u and %u are distinct on one side with one key (the reference panics)", c[0], c[1]);
+    }
+
+    // 3. the KDE over the entries in rank order (fdr.rs:51-57), the rows (fdr.rs:69-85), the q-value tail
+    double *kde_score = nullptr, *bins = nullptr, *moments = nullptr;
+    CUDA_TRY(A.alloc(&kde_score, G));
+    CUDA_TRY(A.alloc(&kde_flags, 2ull * G));
+    CUDA_TRY(A.alloc(&n_rows, G));
+    CUDA_TRY(A.alloc(&row_off, G));
+    CUDA_TRY(A.alloc(&bins, 1000));
+    CUDA_TRY(A.alloc(&moments, 4));
+    k_picked_entries<<<gg, 256, 0, st>>>(side_score, side_has, G, kde_score, kde_flags, n_rows);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, n_rows, row_off, (int)G, st));
+    CUDA_TRY(A.reserve_tmp(tb));
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(A.tmp, tb, n_rows, row_off, (int)G, st));
+    if (int rc = fdr_kde(st, A, kde_score, kde_flags, kde_flags + G, G, 1000, true, 1.0, fma, bins, moments)) return rc;
+    float *q_score = nullptr, *q_ix_val = nullptr;
+    uint8_t* q_decoy = nullptr;
+    uint32_t *q_ix = nullptr, *q_key = nullptr, *q_idx = nullptr;
+    unsigned long long* d_passing = nullptr;
+    CUDA_TRY(A.alloc(&q_score, S));
+    CUDA_TRY(A.alloc(&q_decoy, S));
+    CUDA_TRY(A.alloc(&q_ix, S));
+    CUDA_TRY(A.alloc(&q_key, S));
+    CUDA_TRY(A.alloc(&q_idx, S));
+    CUDA_TRY(A.alloc(&q_ix_val, 2ull * G));
+    CUDA_TRY(A.alloc(&d_passing, 1));
+    k_picked_rows<<<gg, 256, 0, st>>>(side_score, side_has, row_off, G, ix_has_side, q_score, q_decoy, q_ix, q_key, q_idx);
+    CUDA_TRY(cudaGetLastError());
+    if (int rc = picked_tail(st, A, S, q_score, q_decoy, q_ix, q_key, q_idx, bins, moments, 0.01f, 2 * G, q_ix_val, d_passing)) return rc;
+    k_picked_gather<<<g, 256, 0, st>>>(d_rank, d_decoy, m, ix_has_side, q_ix_val, d_out);
+    CUDA_TRY(cudaGetLastError());
+    unsigned long long pass = 0;
+    CUDA_TRY(cudaMemcpyAsync(&pass, d_passing, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    *passing = pass;
+    return 0;
+}
+
+static int picked_check_peptides(const char* what, const sage_b200_peptides* P, const sage_b200_picked_params* p, bool proteins) {
+    if (!P || !p || (proteins && (!p->n_proteins || !p->protein))) return fail(SAGE_B200_EINVAL, "%s: null argument", what);
+    if (P->n_peptides && (!P->residue_offsets || !P->sequence || !P->modifications || !P->nterm || !P->decoy))
+        return fail(SAGE_B200_EINVAL, "%s: null peptide array", what);
+    if (P->n_peptides >= 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "%s: too many peptides for u32 PeptideIx", what);
+    return 0;
+}
+
+// The peptide keys of the rows (fdr.rs:126-131): the referenced peptides' key material goes to the device compacted, each is hashed and
+// grouped exactly; d_key[i] = the group of row i's peptide. Also each row's decoy flag and PeptideIx.
+static int picked_peptide_keys(cudaStream_t st, DevArena& A, const sage_b200_peptides* P, const sage_b200_picked_params* p, const uint32_t* pep_idx,
+                               uint32_t n, uint32_t hash_bits, uint32_t* d_key, uint8_t* d_decoy, uint32_t* d_pep) {
+    const uint64_t n_pep = P->n_peptides;
+    std::vector<uint32_t> slot_of(n_pep, ~0u), row_slot(n), off(1, 0);
+    std::vector<uint8_t> row_decoy(n), seq, rev;
+    std::vector<float> mods, nterm, cterm;
+    for (uint32_t i = 0; i < n; i++) slot_of[pep_idx[i]] = 0;
+    for (uint64_t q = 0; q < n_pep; q++) {
+        if (slot_of[q]) continue;
+        slot_of[q] = (uint32_t)nterm.size();
+        const uint32_t a = P->residue_offsets[q], b = P->residue_offsets[q + 1];
+        seq.insert(seq.end(), P->sequence + a, P->sequence + b);
+        mods.insert(mods.end(), P->modifications + a, P->modifications + b);
+        off.push_back((uint32_t)seq.size());
+        nterm.push_back(P->nterm[q]);
+        cterm.push_back(p->cterm ? p->cterm[q] : std::numeric_limits<float>::quiet_NaN());
+        rev.push_back(p->generate_decoys && P->decoy[q] ? 1 : 0);
+    }
+    for (uint32_t i = 0; i < n; i++) {
+        row_slot[i] = slot_of[pep_idx[i]];
+        row_decoy[i] = P->decoy[pep_idx[i]] ? 1 : 0;
+    }
+    const uint32_t U = (uint32_t)nterm.size();
+    uint32_t *d_off = nullptr, *d_row_slot = nullptr, *d_u = nullptr, *d_u_s = nullptr, *d_group = nullptr;
+    uint8_t *d_seq = nullptr, *d_rev = nullptr;
+    float *d_mods = nullptr, *d_nterm = nullptr, *d_cterm = nullptr;
+    uint64_t *d_hash = nullptr, *d_hash_s = nullptr;
+    CUDA_TRY(A.alloc(&d_off, U + 1));
+    CUDA_TRY(A.alloc(&d_seq, seq.size()));
+    CUDA_TRY(A.alloc(&d_mods, mods.size()));
+    CUDA_TRY(A.alloc(&d_nterm, U));
+    CUDA_TRY(A.alloc(&d_cterm, U));
+    CUDA_TRY(A.alloc(&d_rev, U));
+    CUDA_TRY(A.alloc(&d_row_slot, n));
+    CUDA_TRY(A.alloc(&d_u, U));
+    CUDA_TRY(A.alloc(&d_u_s, U));
+    CUDA_TRY(A.alloc(&d_group, U));
+    CUDA_TRY(A.alloc(&d_hash, U));
+    CUDA_TRY(A.alloc(&d_hash_s, U));
+    CUDA_TRY(cudaMemcpyAsync(d_off, off.data(), 4ull * (U + 1), cudaMemcpyHostToDevice, st));
+    if (!seq.empty()) {
+        CUDA_TRY(cudaMemcpyAsync(d_seq, seq.data(), seq.size(), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_mods, mods.data(), 4 * mods.size(), cudaMemcpyHostToDevice, st));
+    }
+    CUDA_TRY(cudaMemcpyAsync(d_nterm, nterm.data(), 4ull * U, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_cterm, cterm.data(), 4ull * U, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_rev, rev.data(), U, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_row_slot, row_slot.data(), 4ull * n, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_decoy, row_decoy.data(), n, cudaMemcpyHostToDevice, st));
+    if (d_pep) CUDA_TRY(cudaMemcpyAsync(d_pep, pep_idx, 4ull * n, cudaMemcpyHostToDevice, st));
+    const PickedPeptides pk{d_off, d_seq, d_mods, d_nterm, d_cterm, d_rev};
+    const uint64_t mask = hash_bits >= 64 ? ~0ull : ((1ull << hash_bits) - 1);
+    k_picked_hash<<<grid256(U), 256, 0, st>>>(pk, U, mask, d_hash, d_u);
+    CUDA_TRY(cudaGetLastError());
+    size_t tb = 0;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_hash, d_hash_s, d_u, d_u_s, (int)U, 0, 64, st));
+    CUDA_TRY(A.reserve_tmp(tb));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, d_hash, d_hash_s, d_u, d_u_s, (int)U, 0, 64, st));
+    k_picked_group<<<grid256(U), 256, 0, st>>>(pk, d_hash_s, d_u_s, U, d_group);
+    CUDA_TRY(cudaGetLastError());
+    k_picked_peptide_keys<<<grid256(n), 256, 0, st>>>(d_row_slot, d_group, n, d_key);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int sage_b200_picked_fdr(int device, const sage_b200_peptides* P, const sage_b200_picked_params* p, const sage_b200_feature* rows,
+                                    const float* discriminant_score, uint64_t n, sage_b200_picked_out* out) {
+    if (!out || (n && (!rows || !discriminant_score || !out->peptide_q || !out->protein_q))) return fail(SAGE_B200_EINVAL, "picked_fdr: null argument");
+    if (int rc = picked_check_peptides("picked_fdr", P, p, true)) return rc;
+    if (int rc = picked_limits("picked_fdr", n)) return rc;
+    out->peptide_passing = out->protein_passing = out->peptide_entries = out->protein_entries = 0;
+    out->ms_keys = out->ms_peptide = out->ms_protein = out->ms_total = 0.0f;
+    std::vector<uint32_t> pep_idx(n);
+    for (uint64_t i = 0; i < n; i++) {
+        pep_idx[i] = rows[i].peptide_idx;
+        if (pep_idx[i] >= P->n_peptides)
+            return fail(SAGE_B200_EINVAL, "picked_fdr: row %llu has peptide_idx %u outside the peptide table (%llu peptides)", (unsigned long long)i,
+                        pep_idx[i], (unsigned long long)P->n_peptides);
+    }
+    if (n == 0) return 0;
+    if (int rc = select_device(device)) return rc;
+    const uint64_t nres = P->residue_offsets[P->n_peptides];
+    if (int rc = picked_memory("picked_fdr", 2 * n, 16 * nres + 32 * P->n_peptides)) return rc;
+    // picked_protein's rows: those whose peptide has exactly one protein (fdr.rs:160-162), keyed by that protein's id
+    std::vector<uint32_t> prot_row, prot_key;
+    std::vector<uint8_t> prot_decoy;
+    std::vector<float> prot_score;
+    for (uint64_t i = 0; i < n; i++) {
+        const uint32_t q = pep_idx[i];
+        if (p->n_proteins[q] != 1) continue;
+        prot_row.push_back((uint32_t)i);
+        prot_key.push_back(p->protein[q]);
+        prot_decoy.push_back(P->decoy[q] ? 1 : 0);
+        prot_score.push_back(discriminant_score[i]);
+    }
+    const uint32_t m = (uint32_t)prot_row.size();
+    const bool fma = host_math_variant() != 1;
+    DevArena A;
+    cudaStream_t st = 0;
+    StageEvents<4> ev;
+    CUDA_TRY(ev.create());
+    uint32_t *d_key = nullptr, *d_pep = nullptr, *d_rank = nullptr, *d_pkey = nullptr, *d_prank = nullptr;
+    uint8_t *d_decoy = nullptr, *d_pdecoy = nullptr;
+    float *d_score = nullptr, *d_q = nullptr, *d_pscore = nullptr, *d_pq = nullptr;
+    CUDA_TRY(A.alloc(&d_key, n));
+    CUDA_TRY(A.alloc(&d_pep, n));
+    CUDA_TRY(A.alloc(&d_rank, n));
+    CUDA_TRY(A.alloc(&d_decoy, n));
+    CUDA_TRY(A.alloc(&d_score, n));
+    CUDA_TRY(A.alloc(&d_q, n));
+    CUDA_TRY(A.alloc(&d_pkey, m));
+    CUDA_TRY(A.alloc(&d_prank, m));
+    CUDA_TRY(A.alloc(&d_pdecoy, m));
+    CUDA_TRY(A.alloc(&d_pscore, m));
+    CUDA_TRY(A.alloc(&d_pq, m));
+    CUDA_TRY(cudaMemcpyAsync(d_score, discriminant_score, 4 * n, cudaMemcpyHostToDevice, st));
+    if (m) {
+        CUDA_TRY(cudaMemcpyAsync(d_pkey, prot_key.data(), 4ull * m, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_pdecoy, prot_decoy.data(), m, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_pscore, prot_score.data(), 4ull * m, cudaMemcpyHostToDevice, st));
+    }
+    CUDA_TRY(cudaEventRecord(ev[0], st));
+    if (int rc = picked_peptide_keys(st, A, P, p, pep_idx.data(), (uint32_t)n, 64, d_key, d_decoy, d_pep)) return rc;
+    CUDA_TRY(cudaEventRecord(ev[1], st));
+    if (int rc = picked_competition(st, A, fma, (uint32_t)n, d_key, d_decoy, d_score, d_pep, true, d_rank, d_q, &out->peptide_entries, &out->peptide_passing))
+        return rc;
+    CUDA_TRY(cudaEventRecord(ev[2], st));
+    // Ix of picked_protein is proteins(decoy_tag, generate_decoys): the tagged name per side with generate_decoys, else the name alone
+    if (int rc = picked_competition(st, A, fma, m, d_pkey, d_pdecoy, d_pscore, nullptr, p->generate_decoys != 0, d_prank, d_pq, &out->protein_entries,
+                                    &out->protein_passing))
+        return rc;
+    CUDA_TRY(cudaEventRecord(ev[3], st));
+    std::vector<float> pq(m);
+    CUDA_TRY(cudaMemcpyAsync(out->peptide_q, d_q, 4 * n, cudaMemcpyDeviceToHost, st));
+    if (m) CUDA_TRY(cudaMemcpyAsync(pq.data(), d_pq, 4ull * m, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    for (uint64_t i = 0; i < n; i++) out->protein_q[i] = 1.0f;
+    for (uint32_t c = 0; c < m; c++) out->protein_q[prot_row[c]] = pq[c];
+    CUDA_TRY(cudaEventElapsedTime(&out->ms_keys, ev[0], ev[1]));
+    CUDA_TRY(cudaEventElapsedTime(&out->ms_peptide, ev[1], ev[2]));
+    CUDA_TRY(cudaEventElapsedTime(&out->ms_protein, ev[2], ev[3]));
+    CUDA_TRY(cudaEventElapsedTime(&out->ms_total, ev[0], ev[3]));
+    return 0;
+}
+
+extern "C" int sage_b200_picked_precursor(int device, const double* score, const uint8_t* decoy, uint64_t n, float* q_value, uint64_t* passing) {
+    if (!passing || (n && (!score || !decoy || !q_value))) return fail(SAGE_B200_EINVAL, "picked_precursor: null argument");
+    if (n > (uint64_t)INT32_MAX) return fail(SAGE_B200_ELIMIT, "picked_precursor: more than 2^31 - 1 rows");
+    *passing = 0;
+    if (n == 0) return 0;
+    if (int rc = select_device(device)) return rc;
+    if (int rc = picked_memory("picked_precursor", n, 0)) return rc;
+    DevArena A;
+    cudaStream_t st = 0;
+    const uint32_t R = (uint32_t)n;
+    double* d_in = nullptr;
+    float *d_score = nullptr, *d_q = nullptr;
+    uint8_t* d_decoy = nullptr;
+    uint32_t *d_ix = nullptr, *d_key = nullptr, *d_idx = nullptr;
+    unsigned long long* d_passing = nullptr;
+    CUDA_TRY(A.alloc(&d_in, n));
+    CUDA_TRY(A.alloc(&d_score, n));
+    CUDA_TRY(A.alloc(&d_q, n));
+    CUDA_TRY(A.alloc(&d_decoy, n));
+    CUDA_TRY(A.alloc(&d_ix, n));
+    CUDA_TRY(A.alloc(&d_key, n));
+    CUDA_TRY(A.alloc(&d_idx, n));
+    CUDA_TRY(A.alloc(&d_passing, 1));
+    std::vector<uint8_t> flags(n);
+    for (uint64_t i = 0; i < n; i++) flags[i] = decoy[i] ? 1 : 0;
+    CUDA_TRY(cudaMemcpyAsync(d_in, score, 8 * n, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_decoy, flags.data(), n, cudaMemcpyHostToDevice, st));
+    k_picked_precursor_rows<<<grid256(n), 256, 0, st>>>(d_in, R, d_score, d_ix, d_key, d_idx);
+    CUDA_TRY(cudaGetLastError());
+    if (int rc = picked_tail(st, A, R, d_score, d_decoy, d_ix, d_key, d_idx, nullptr, nullptr, 0.05f, R, d_q, d_passing)) return rc;
+    unsigned long long pass = 0;
+    CUDA_TRY(cudaMemcpyAsync(q_value, d_q, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&pass, d_passing, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    *passing = pass;
+    return 0;
+}
+
+extern "C" int sage_b200_competition_keys(int device, const sage_b200_peptides* P, const sage_b200_picked_params* p, const uint32_t* peptide_idx, uint64_t n,
+                                          uint32_t hash_bits, uint32_t* entry_rank) {
+    if (n && (!peptide_idx || !entry_rank)) return fail(SAGE_B200_EINVAL, "competition_keys: null argument");
+    if (hash_bits < 3 || hash_bits > 64) return fail(SAGE_B200_EINVAL, "competition_keys: hash_bits %u outside 3..64", hash_bits);
+    // a truncated hash makes equal-hash runs of about n / 2^hash_bits peptides, compared pairwise: bound that work
+    if (hash_bits < 64 && n > PICKED_HOOK_MAX_ROWS)
+        return fail(SAGE_B200_ELIMIT, "competition_keys: more than %u rows with a truncated hash", PICKED_HOOK_MAX_ROWS);
+    if (int rc = picked_check_peptides("competition_keys", P, p, false)) return rc;
+    if (int rc = picked_limits("competition_keys", n)) return rc;
+    for (uint64_t i = 0; i < n; i++)
+        if (peptide_idx[i] >= P->n_peptides)
+            return fail(SAGE_B200_EINVAL, "competition_keys: row %llu has peptide_idx %u outside the peptide table (%llu peptides)", (unsigned long long)i,
+                        peptide_idx[i], (unsigned long long)P->n_peptides);
+    if (n == 0) return 0;
+    if (int rc = select_device(device)) return rc;
+    const uint64_t nres = P->residue_offsets[P->n_peptides];
+    if (int rc = picked_memory("competition_keys", n, 16 * nres + 32 * P->n_peptides)) return rc;
+    DevArena A;
+    cudaStream_t st = 0;
+    uint32_t *d_key = nullptr, *d_rank = nullptr;
+    uint8_t* d_decoy = nullptr;
+    CUDA_TRY(A.alloc(&d_key, n));
+    CUDA_TRY(A.alloc(&d_rank, n));
+    CUDA_TRY(A.alloc(&d_decoy, n));
+    if (int rc = picked_peptide_keys(st, A, P, p, peptide_idx, (uint32_t)n, hash_bits, d_key, d_decoy, nullptr)) return rc;
+    uint64_t entries = 0, passing = 0;
+    if (int rc = picked_competition(st, A, true, (uint32_t)n, d_key, d_decoy, nullptr, nullptr, true, d_rank, nullptr, &entries, &passing)) return rc;
+    CUDA_TRY(cudaMemcpyAsync(entry_rank, d_rank, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
