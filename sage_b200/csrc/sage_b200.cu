@@ -95,6 +95,14 @@ struct DevBuf {
         cap = want;
         return 0;
     }
+    // cub's two-phase call f(tmp, bytes) with this buffer as its temporary storage: f(nullptr, bytes) sizes it, then f runs.
+    template <class F>
+    cudaError_t two_phase(F f) {
+        size_t b = 0;
+        if (cudaError_t e = f(nullptr, b)) return e;
+        if (reserve(b)) return cudaErrorMemoryAllocation;
+        return f(p, b);
+    }
     template <class T>
     T* as() const { return reinterpret_cast<T*>(p); }
 };
@@ -144,22 +152,34 @@ struct DevArena {
         if (e == cudaSuccess) tmp_bytes = b;
         return e;
     }
+    // cub's two-phase call f(tmp, bytes) on the growable buffer: f(nullptr, bytes) sizes it (plus `pad` bytes reserved), then f runs.
+    template <class F>
+    cudaError_t two_phase(F f, size_t pad = 0) {
+        size_t b = 0;
+        if (cudaError_t e = f(nullptr, b)) return e;
+        if (cudaError_t e = reserve_tmp(b + pad)) return e;
+        return f(tmp, b);
+    }
 };
 
-// The events that time the stages of one call.
-template <int N>
-struct StageEvents {
-    cudaEvent_t ev[N] = {};
-    StageEvents() = default;
-    StageEvents(const StageEvents&) = delete;
-    StageEvents& operator=(const StageEvents&) = delete;
-    ~StageEvents() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
-    cudaError_t create() {
-        for (cudaEvent_t& e : ev)
-            if (cudaError_t r = cudaEventCreate(&e)) return r;
-        return cudaSuccess;
-    }
-    cudaEvent_t operator[](int i) const { return ev[i]; }
+// A non-blocking stream and an event, each destroyed with its owner (with the owner's device current) and created by create().
+struct Stream {
+    cudaStream_t s = nullptr;
+    Stream() = default;
+    Stream(const Stream&) = delete;
+    Stream& operator=(const Stream&) = delete;
+    ~Stream() { if (s) cudaStreamDestroy(s); }
+    cudaError_t create() { return cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking); }
+    operator cudaStream_t() const { return s; }
+};
+struct Event {
+    cudaEvent_t e = nullptr;
+    Event() = default;
+    Event(const Event&) = delete;
+    Event& operator=(const Event&) = delete;
+    ~Event() { if (e) cudaEventDestroy(e); }
+    cudaError_t create() { return cudaEventCreate(&e); }
+    operator cudaEvent_t() const { return e; }
 };
 
 // Host -> device copy of a PAGEABLE array (a Rust Vec<f32>, a numpy array) through a pinned staging buffer: a few pool threads copy 2 MB pieces
@@ -395,10 +415,11 @@ static int db_upload_peptides(sage_b200_db* db, const sage_b200_peptides* P, con
     return 0;
 }
 
-// A db under construction: destroyed unless released to the caller.
-using DbGuard = std::unique_ptr<sage_b200_db, void (*)(sage_b200_db*)>;
+// A handle under construction: destroyed (by its C destroy function) unless released to the caller.
+template <class T>
+using Guard = std::unique_ptr<T, void (*)(T*)>;
 
-static int db_new(int device, DbGuard& out) {
+static int db_new(int device, Guard<sage_b200_db>& out) {
     if (int rc = select_device(device)) return rc;
     out.reset(new sage_b200_db());
     out->device = device;
@@ -495,7 +516,7 @@ extern "C" int sage_b200_db_create(const sage_b200_peptides* peptides, const sag
     if (index->n_fragments && (!index->fragment_peptide || !index->fragment_mz || !index->bucket_min)) return fail(SAGE_B200_EINVAL, "index: null array");
     const uint64_t nb_expect = (index->n_fragments + index->bucket_size - 1) / index->bucket_size;
     if (index->n_buckets != nb_expect) return fail(SAGE_B200_EINVAL, "n_buckets %llu != ceil(n_fragments/bucket_size) %llu", (unsigned long long)index->n_buckets, (unsigned long long)nb_expect);
-    DbGuard guard(nullptr, sage_b200_db_destroy);
+    Guard<sage_b200_db> guard(nullptr, sage_b200_db_destroy);
     if (int rc = db_new(device, guard)) return rc;
     sage_b200_db* db = guard.get();
     if (int rc = db_upload_peptides(db, peptides, index->ion_kinds, index->n_ion_kinds)) return rc;
@@ -563,7 +584,7 @@ extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t b
     if (!out || !peptides || !ion_kinds) return fail(SAGE_B200_EINVAL, "db_build: null argument");
     if (bucket_size == 0 || (bucket_size & (bucket_size - 1)) || bucket_size > (1ull << 30))
         return fail(SAGE_B200_EINVAL, "bucket_size must be a power of two (Builder::make_parameters rounds up, database.rs:97)");
-    DbGuard guard(nullptr, sage_b200_db_destroy);
+    Guard<sage_b200_db> guard(nullptr, sage_b200_db_destroy);
     if (int rc = db_new(device, guard)) return rc;
     sage_b200_db* db = guard.get();
     if (int rc = db_upload_peptides(db, peptides, ion_kinds, n_ion_kinds)) return rc;
@@ -608,10 +629,8 @@ extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t b
                                                                   nullptr, d_off, k32a, pa);
             CUDA_TRY(cudaGetLastError());
             if (nf > 0x7FFFFFFFull) return fail(SAGE_B200_ELIMIT, "more than 2^31 fragments: sort in slabs not implemented");
-            size_t tb = 0;
-            CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint32_t*)k32a, k32b, (const uint32_t*)pa, pb, (int)nf));
-            CUDA_TRY(S.reserve_tmp(tb + 16));
-            CUDA_TRY(cub::DeviceRadixSort::SortPairs(S.tmp, tb, (const uint32_t*)k32a, k32b, (const uint32_t*)pa, pb, (int)nf));
+            CUDA_TRY(S.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint32_t*)k32a, k32b, (const uint32_t*)pa, pb, (int)nf); },
+                                 16));
         }
         // (2) bucket minima + (bucket, PeptideIx) keys, then a stable sort inside buckets (database.rs:337-346)
         uint64_t *k64a = nullptr, *k64b = nullptr;
@@ -621,10 +640,8 @@ extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t b
         k_bucket_keys<<<(unsigned)((nf + 255) / 256), 256>>>(nf, shift, k32b, pb, k64a, mza, (float*)db->d_bucket_min);
         CUDA_TRY(cudaGetLastError());
         const int end_bit = std::min<int>(64, 32 + (int)ceil_log2_u64(nb + 1) + 1);
-        size_t tb = 0;
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)k64a, k64b, (const uint32_t*)mza, mzb, (int)nf, 0, end_bit));
-        CUDA_TRY(A.reserve_tmp(tb + 16));
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, (const uint64_t*)k64a, k64b, (const uint32_t*)mza, mzb, (int)nf, 0, end_bit));
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)k64a, k64b, (const uint32_t*)mza, mzb, (int)nf, 0, end_bit); },
+                             16));
         k_pack_fragments<<<(unsigned)((nf + 255) / 256), 256>>>(nf, k64b, mzb, (uint2*)db->d_frag);
         CUDA_TRY(cudaGetLastError());
         CUDA_TRY(cudaDeviceSynchronize());
@@ -678,10 +695,8 @@ static bool sort_block_major(const sage_b200_db* db, DevArena& A, uint32_t block
     k_wide_keys<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, block, k_a, p_a);
     int nb_bits = 1;
     while (nb_bits < 32 && (n_block >> nb_bits)) nb_bits++;
-    size_t tb = 0;
-    if (cub::DeviceRadixSort::SortPairs(nullptr, tb, (const uint64_t*)k_a, *keys, (const uint32_t*)p_a, *peps, (int)nf, 0, 32 + nb_bits) != cudaSuccess ||
-        A.reserve_tmp(tb + 16) != cudaSuccess ||
-        cub::DeviceRadixSort::SortPairs(A.tmp, tb, (const uint64_t*)k_a, *keys, (const uint32_t*)p_a, *peps, (int)nf, 0, 32 + nb_bits) != cudaSuccess)
+    if (A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)k_a, *keys, (const uint32_t*)p_a, *peps, (int)nf, 0, 32 + nb_bits); },
+                    16) != cudaSuccess)
         return false;
     k_wide_block_offsets<<<(n_block + 1 + 255) / 256, 256>>>(nf, *keys, n_block, blk_off);
     // m/z range of the index (positive floats order like their bit patterns)
@@ -895,12 +910,16 @@ struct ChunkState {
 // One in-flight chunk: its own stream, device buffers, pinned staging and pending-download bookkeeping. score_batch alternates
 // between two lanes so that the H2D copy of chunk i+1 and the D2H of chunk i-1 overlap the kernels of chunk i.
 struct Lane {
-    cudaStream_t stream = nullptr;   // kernels + D2H
-    cudaStream_t copy = nullptr;     // H2D: masses first (all the counting kernels need), intensities behind them, overlapping setup + preliminary scoring
-    cudaEvent_t ev[9] = {};   // 0/1 H2D, 6 run start, 2 setup end, 8 counting kernels end, 3 replay end, 4 k_score end, 7/5 D2H
-    cudaStream_t copy2 = nullptr;    // (unused: a second H2D stream did not overtake the queued bulk copies, see chunk_upload)
-    cudaEvent_t ev_masses = nullptr, ev_intens = nullptr, ev_small = nullptr;
-    cudaEvent_t ev_part[MASS_PARTS] = {};   // masses of the spectra [part_lo[p], part_lo[p+1]) are on the device
+    Stream stream;   // kernels + D2H
+    Stream copy;     // H2D: masses first (all the counting kernels need), intensities behind them, overlapping setup + preliminary scoring
+    // No work is ever queued on `spare`, but creating it keeps the lane streams' creation order: without it the second lane's streams come
+    // one position earlier, and cfg4's score_batch (open search, several chunks over both lanes) measured about 2 % slower end to end on an
+    // H100 80GB HBM3 at 700 W, kernels unchanged. The driver hands out hardware work queues to streams in creation order.
+    Stream spare;
+    // stage boundaries of the chunk in flight: its timings (counters, SAGE_B200_TRACE) and the wait on the other lane's k_score
+    Event ev_h2d_begin, ev_h2d_end, ev_run, ev_setup_end, ev_count_end, ev_replay_end, ev_score_end, ev_d2h_begin, ev_d2h_end;
+    Event ev_masses, ev_intens, ev_small;
+    Event ev_part[MASS_PARTS];   // masses of the spectra [part_lo[p], part_lo[p+1]) are on the device
     DevBuf d_small, d_masses, d_intens, d_queries, d_hits, d_keys, d_features, d_counts, d_counters, d_dbgk, d_dbgm, d_sort, d_sorttmp, d_wlist, d_wslots,
         d_witems, d_citems, d_nlist, d_nslots;
     PinBuf h_small, h_masses, h_intens, h_features, h_counts, h_counters;
@@ -918,17 +937,17 @@ struct Lane {
     std::unique_ptr<StagePool> pool{new StagePool};   // copy threads of staged_h2d (started by the first pageable chunk)
     int stager_rc = 0;
     char stager_msg[256] = {0};
-    void release() {
-        if (stager.joinable()) stager.join();
-        for (auto& e : ev) if (e) cudaEventDestroy(e);
-        if (ev_masses) cudaEventDestroy(ev_masses);
-        if (ev_intens) cudaEventDestroy(ev_intens);
-        if (ev_small) cudaEventDestroy(ev_small);
-        for (auto& e : ev_part) if (e) cudaEventDestroy(e);
-        if (copy2) cudaStreamDestroy(copy2);
-        if (stream) cudaStreamDestroy(stream);
-        if (copy) cudaStreamDestroy(copy);
+    cudaError_t create() {
+        for (Stream* s : {&stream, &copy, &spare})
+            if (cudaError_t e = s->create()) return e;
+        for (Event* ev : {&ev_h2d_begin, &ev_h2d_end, &ev_run, &ev_setup_end, &ev_count_end, &ev_replay_end, &ev_score_end, &ev_d2h_begin, &ev_d2h_end, &ev_masses,
+                          &ev_intens, &ev_small})
+            if (cudaError_t e = ev->create()) return e;
+        for (Event& ev : ev_part)
+            if (cudaError_t e = ev.create()) return e;
+        return cudaSuccess;
     }
+    ~Lane() { if (stager.joinable()) stager.join(); }   // the staging thread uses the stream, the pinned buffers and the pool
 };
 
 struct sage_b200_scorer {
@@ -960,7 +979,7 @@ struct sage_b200_scorer {
     int first_chunk_pct = 0;   // chosen by A/B on cfg2 (e2e) against 10..35 %
     // SAGE_B200_TRACE=1: per-chunk device timeline (ms since the start of the call) on stderr
     bool trace = false;
-    cudaEvent_t ev_base = nullptr;
+    Event ev_base;
     std::chrono::steady_clock::time_point t_base;
     sage_b200_counters last{};
 };
@@ -973,7 +992,8 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
     if (p->score_type > 1) return fail(SAGE_B200_EINVAL, "bad score_type");
     CUDA_TRY(cudaSetDevice(db->device));
     if (int rc = ensure_kernel_attributes(db->device)) return rc;
-    sage_b200_scorer* s = new sage_b200_scorer();
+    Guard<sage_b200_scorer> guard(new sage_b200_scorer(), sage_b200_scorer_destroy);
+    sage_b200_scorer* s = guard.get();
     s->db = db;
     s->device = db->device;
     s->params = *p;
@@ -990,7 +1010,7 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
     v.n_iso = (v.min_iso != v.max_iso) ? (uint32_t)std::max(0, v.max_iso - v.min_iso + 1) : 1;
     v.n_ch_max = v.max_charge >= v.min_charge ? v.max_charge - v.min_charge + 1 : 0;
     if (v.n_ch_max < 1) v.n_ch_max = 1;  // known-charge spectra still need one slot
-    if (v.n_iso > 32 || v.n_ch_max > 16) { delete s; return fail(SAGE_B200_ELIMIT, "isotope range > 32 or charge range > 16 not supported"); }
+    if (v.n_iso > 32 || v.n_ch_max > 16) return fail(SAGE_B200_ELIMIT, "isotope range > 32 or charge range > 16 not supported");
     v.qmax = std::max<uint32_t>(1, v.n_iso) * v.n_ch_max;
     v.lcap = std::max<uint32_t>(std::max<uint32_t>(v.n_iso, v.n_ch_max), 1) * v.kparam;
     v.wide_tile = WIDE_TILE;
@@ -1007,7 +1027,7 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
             const double x = (double)n;
             tab[n] = x * std::log(x) - x + 0.5 * std::log(x) + 0.5 * std::log(3.14159265358979323846 * 2.0 * x);
         }
-        if (int rc = s->d_lnfact.reserve(8 * N)) { delete s; return rc; }
+        if (int rc = s->d_lnfact.reserve(8 * N)) return rc;
         CUDA_TRY(cudaMemcpy(s->d_lnfact.p, tab.data(), 8 * N, cudaMemcpyHostToDevice));
         v.lnfact_tab = s->d_lnfact.as<double>();
         v.lnfact_n = N;
@@ -1016,16 +1036,7 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
     v.score_fast = 1;
     if (const char* e = getenv("SAGE_B200_SCORE_FAST")) v.score_fast = atoi(e) != 0;
     if (const char* e = getenv("SAGE_B200_SORT")) s->sort_spectra = atoi(e);
-    for (Lane& L : s->lanes) {
-        CUDA_TRY(cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking));
-        CUDA_TRY(cudaStreamCreateWithFlags(&L.copy, cudaStreamNonBlocking));
-        for (auto& e : L.ev) CUDA_TRY(cudaEventCreate(&e));
-        CUDA_TRY(cudaEventCreate(&L.ev_masses));
-        CUDA_TRY(cudaEventCreate(&L.ev_intens));
-        CUDA_TRY(cudaEventCreate(&L.ev_small));
-        for (auto& e : L.ev_part) CUDA_TRY(cudaEventCreate(&e));
-        CUDA_TRY(cudaStreamCreateWithFlags(&L.copy2, cudaStreamNonBlocking));
-    }
+    for (Lane& L : s->lanes) CUDA_TRY(L.create());
     if (const char* e = getenv("SAGE_B200_PIPELINE_CHUNKS")) s->pipeline_chunks = std::max(1, atoi(e));
     if (const char* e = getenv("SAGE_B200_TRACE")) s->trace = e[0] == '1';
     if (const char* e = getenv("SAGE_B200_SCORE_SPLIT")) s->score_split = atoi(e) != 0;
@@ -1035,8 +1046,8 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
     if (s->narrow_block != 0 && s->narrow_block < 64) s->narrow_block = 64;
     if (const char* e = getenv("SAGE_B200_MASS_PARTS")) s->mass_parts = std::min(MASS_PARTS, std::max(1, atoi(e)));
     if (const char* e = getenv("SAGE_B200_FIRST_CHUNK_PCT")) s->first_chunk_pct = std::min(50, std::max(0, atoi(e)));
-    CUDA_TRY(cudaEventCreate(&s->ev_base));
-    *out = s;
+    CUDA_TRY(s->ev_base.create());
+    *out = guard.release();
     return 0;
 }
 
@@ -1094,8 +1105,6 @@ extern "C" int sage_b200_scorer_set_option(sage_b200_scorer* s, const char* name
 extern "C" void sage_b200_scorer_destroy(sage_b200_scorer* s) {
     if (!s) return;
     cudaSetDevice(s->device);
-    for (Lane& L : s->lanes) L.release();
-    if (s->ev_base) cudaEventDestroy(s->ev_base);
     delete s;
 }
 
@@ -1166,7 +1175,7 @@ static int chunk_upload(sage_b200_scorer* S, Lane& L, const sage_b200_spectra* s
     //                           thread already queues the kernels (chunk_run joins it before k_score is queued).
     cudaStream_t cp = L.copy;
     if ((rc = lane_join_stager(L))) return rc;
-    CUDA_TRY(cudaEventRecord(L.ev[0], cp));
+    CUDA_TRY(cudaEventRecord(L.ev_h2d_begin, cp));
     const float* src_m = sp->masses + pk0;
     const float* src_i = sp->intensities + pk0;
     const bool pin_m = npk == 0 || is_pinned(src_m), pin_i = npk == 0 || is_pinned(src_i);
@@ -1254,14 +1263,14 @@ static int chunk_upload(sage_b200_scorer* S, Lane& L, const sage_b200_spectra* s
         L.stager = std::thread([lane, device, dst, src_i, npk, cp]() {
             cudaSetDevice(device);
             int r = staged_h2d(dst, src_i, 4 * npk, lane->h_intens, *lane->pool, cp);
-            if (r == 0 && (cudaEventRecord(lane->ev_intens, cp) != cudaSuccess || cudaEventRecord(lane->ev[1], cp) != cudaSuccess)) r = fail(SAGE_B200_ECUDA, "event record failed after the staged copy");
+            if (r == 0 && (cudaEventRecord(lane->ev_intens, cp) != cudaSuccess || cudaEventRecord(lane->ev_h2d_end, cp) != cudaSuccess)) r = fail(SAGE_B200_ECUDA, "event record failed after the staged copy");
             if (r) snprintf(lane->stager_msg, sizeof lane->stager_msg, "%s", g_last_error.c_str());
             lane->stager_rc = r;
         });
     } else {
         if (npk) CUDA_TRY(cudaMemcpyAsync(L.d_intens.p, src_i, 4 * npk, cudaMemcpyHostToDevice, cp));
         CUDA_TRY(cudaEventRecord(L.ev_intens, cp));
-        CUDA_TRY(cudaEventRecord(L.ev[1], cp));
+        CUDA_TRY(cudaEventRecord(L.ev_h2d_end, cp));
     }
     S->last.h2d_bytes += C.small_bytes + 8 * npk;
     C.loaded = true;
@@ -1306,10 +1315,10 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
     bv.counters = L.d_counters.as<unsigned long long>();
 
     // kernels of the two lanes never overlap (measured: k_score of one chunk next to k_prelim_narrow of the other slows both); only
-    // copies overlap kernels. ev[4] = end of the other lane's k_score (a never-recorded event counts as complete).
-    CUDA_TRY(cudaStreamWaitEvent(st, S->lanes[(&L - S->lanes) ^ 1].ev[4], 0));
+    // copies overlap kernels. Wait for the end of the other lane's k_score (a never-recorded event counts as complete).
+    CUDA_TRY(cudaStreamWaitEvent(st, S->lanes[(&L - S->lanes) ^ 1].ev_score_end, 0));
     CUDA_TRY(cudaStreamWaitEvent(st, L.ev_small, 0));
-    CUDA_TRY(cudaEventRecord(L.ev[6], st));
+    CUDA_TRY(cudaEventRecord(L.ev_run, st));
     CUDA_TRY(cudaMemsetAsync(L.d_counters.p, 0, 8 * (C_COUNT + (size_t)sv.qmax), st));
     const bool annotate = sv.annotate && S->frag_dst != nullptr;
     if (annotate) {   // fragment offsets are global across the chunks of one call: start this chunk's counter at what was used so far
@@ -1362,7 +1371,7 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(L.d_sorttmp.p, sort_tmp, sk_in, sk_out, sv_in, sv_out, (int)n, sort_lo, sort_bits, st));
         bv.order = sv_out;
     }
-    CUDA_TRY(cudaEventRecord(L.ev[2], st));
+    CUDA_TRY(cudaEventRecord(L.ev_setup_end, st));
     if (C.nparts <= 1) CUDA_TRY(cudaStreamWaitEvent(st, L.ev_masses, 0));   // the counting kernels read the peak masses
     uint64_t launches = 1;
 
@@ -1389,7 +1398,7 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
     k_prelim_narrow<<<(unsigned)std::min<uint64_t>(C.nitems, (uint64_t)db->sm_count * PRELIM_CTAS), PRELIM_THREADS, pep_smem, st>>>(db->v, svq, bv, C.pmax, L.d_nlist.as<uint64_t>(),
                                                                                                                          S->narrow_cta ? nv : NarrowIndexView{});
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaEventRecord(L.ev[8], st));   // narrow counting kernels done (the open-search kernel, when present, is timed with the replays)
+    CUDA_TRY(cudaEventRecord(L.ev_count_end, st));   // narrow counting kernels done (the open-search kernel, when present, is timed with the replays)
     // narrow windows (<= NARROW_CAP peptides): 32-bit heap keys, half the shared memory
     k_replay<true><<<(unsigned)((C.nitems + REPLAY_THREADS - 1) / REPLAY_THREADS), REPLAY_THREADS, rsm / 2, st>>>(sv, bv, L.d_nlist.as<uint64_t>(), L.d_nslots.as<ReplaySlot>(),
                                                                                                                  (uint32_t)C.nitems, nullptr, n);
@@ -1410,7 +1419,7 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
         CUDA_TRY(cudaGetLastError());
         launches += 2;
     }
-    CUDA_TRY(cudaEventRecord(L.ev[3], st));
+    CUDA_TRY(cudaEventRecord(L.ev_replay_end, st));
 
     // ---- candidate scoring + feature assembly (first reader of the intensities)
     if ((rc = lane_join_stager(L))) return rc;   // ev_intens is recorded by the staging thread of a pageable chunk
@@ -1453,7 +1462,7 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
         CUDA_TRY(cudaGetLastError());
         launches++;
     }
-    CUDA_TRY(cudaEventRecord(L.ev[4], st));
+    CUDA_TRY(cudaEventRecord(L.ev_score_end, st));
     CUDA_TRY(cudaMemcpyAsync(L.h_counters.p, L.d_counters.p, 8 * C_COUNT, cudaMemcpyDeviceToHost, st));
     L.launches = launches;
     L.dbg = dbg;
@@ -1472,10 +1481,10 @@ static int chunk_download(sage_b200_scorer* S, Lane& L, sage_b200_feature* fdst,
     const bool f_pinned = is_pinned(fdst), c_pinned = is_pinned(cdst);
     if (!f_pinned && (rc = L.h_features.reserve(fbytes))) return rc;
     if (!c_pinned && (rc = L.h_counts.reserve(4 * (size_t)n))) return rc;
-    CUDA_TRY(cudaEventRecord(L.ev[7], st));
+    CUDA_TRY(cudaEventRecord(L.ev_d2h_begin, st));
     CUDA_TRY(cudaMemcpyAsync(f_pinned ? (void*)fdst : L.h_features.p, L.d_features.p, fbytes, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(c_pinned ? (void*)cdst : L.h_counts.p, L.d_counts.p, 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaEventRecord(L.ev[5], st));
+    CUDA_TRY(cudaEventRecord(L.ev_d2h_end, st));
     L.fdst = fdst; L.cdst = cdst; L.f_pinned = f_pinned; L.c_pinned = c_pinned;
     L.downloading = true;
     S->last.d2h_bytes += fbytes + 4 * (size_t)n;
@@ -1502,7 +1511,6 @@ static int lane_finish(sage_b200_scorer* S, Lane& L) {
     if (!C.loaded) return 0;
     { const int jrc = lane_join_stager(L); if (jrc) return jrc; }
     CUDA_TRY(cudaStreamSynchronize(L.copy));
-    CUDA_TRY(cudaStreamSynchronize(L.copy2));
     for (int attempt = 0;; attempt++) {
         CUDA_TRY(cudaStreamSynchronize(L.stream));
         if (!L.ran) break;
@@ -1533,8 +1541,8 @@ static int lane_finish(sage_b200_scorer* S, Lane& L) {
     }
     if (S->trace && L.ran && L.downloading) {
         float t[8];
-        const int order[8] = {0, 1, 6, 2, 3, 4, 7, 5};
-        for (int i = 0; i < 8; i++) cudaEventElapsedTime(&t[i], S->ev_base, L.ev[order[i]]);
+        const cudaEvent_t marks[8] = {L.ev_h2d_begin, L.ev_h2d_end, L.ev_run, L.ev_setup_end, L.ev_replay_end, L.ev_score_end, L.ev_d2h_begin, L.ev_d2h_end};
+        for (int i = 0; i < 8; i++) cudaEventElapsedTime(&t[i], S->ev_base, marks[i]);
         const double now = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - S->t_base).count();
         float tm = 0;
         cudaEventElapsedTime(&tm, S->ev_base, L.ev_masses);
@@ -1543,14 +1551,14 @@ static int lane_finish(sage_b200_scorer* S, Lane& L) {
     }
     sage_b200_counters& T = S->last;
     float ms;
-    if (C.timed_upload) { cudaEventElapsedTime(&ms, L.ev[0], L.ev[1]); T.ms_h2d += ms; T.ms_total += ms; C.timed_upload = false; }
+    if (C.timed_upload) { cudaEventElapsedTime(&ms, L.ev_h2d_begin, L.ev_h2d_end); T.ms_h2d += ms; T.ms_total += ms; C.timed_upload = false; }
     if (L.ran) {
         const unsigned long long* hc = (const unsigned long long*)L.h_counters.p;
-        cudaEventElapsedTime(&ms, L.ev[6], L.ev[2]); T.ms_setup += ms;
-        cudaEventElapsedTime(&ms, L.ev[2], L.ev[3]); T.ms_prelim += ms;
-        cudaEventElapsedTime(&ms, L.ev[2], L.ev[8]); T.ms_prelim_count += ms;
-        cudaEventElapsedTime(&ms, L.ev[3], L.ev[4]); T.ms_score += ms;
-        cudaEventElapsedTime(&ms, L.ev[6], L.ev[4]); T.ms_total += ms;
+        cudaEventElapsedTime(&ms, L.ev_run, L.ev_setup_end); T.ms_setup += ms;
+        cudaEventElapsedTime(&ms, L.ev_setup_end, L.ev_replay_end); T.ms_prelim += ms;
+        cudaEventElapsedTime(&ms, L.ev_setup_end, L.ev_count_end); T.ms_prelim_count += ms;
+        cudaEventElapsedTime(&ms, L.ev_replay_end, L.ev_score_end); T.ms_score += ms;
+        cudaEventElapsedTime(&ms, L.ev_run, L.ev_score_end); T.ms_total += ms;
         T.spectra += C.n; T.peaks += C.npk; T.queries += hc[C_QUERIES]; T.tasks += hc[C_TASKS]; T.pages += hc[C_PAGES]; T.entries_scanned += hc[C_ENTRIES];
         T.matched_fragments += hc[C_MATCHED]; T.candidates_scored += hc[C_CANDS]; T.peptide_record_floats += hc[C_PEPFLOATS]; T.psms += hc[C_PSMS];
         T.wide_queries += hc[C_WIDE]; T.pep_queries += hc[C_PEPQ]; T.pep_fallbacks += hc[C_PEPFALLBACK]; T.wide_overflows += hc[C_WOVERFLOW];
@@ -1571,7 +1579,7 @@ static int lane_finish(sage_b200_scorer* S, Lane& L) {
         const size_t fbytes = (size_t)C.n * S->sv.report_psms * sizeof(sage_b200_feature);
         if (!L.f_pinned) memcpy(L.fdst, L.h_features.p, fbytes);
         if (!L.c_pinned) memcpy(L.cdst, L.h_counts.p, 4 * (size_t)C.n);
-        cudaEventElapsedTime(&ms, L.ev[7], L.ev[5]); T.ms_d2h += ms; T.ms_total += ms;
+        cudaEventElapsedTime(&ms, L.ev_d2h_begin, L.ev_d2h_end); T.ms_d2h += ms; T.ms_total += ms;
         L.downloading = false;
     }
     return 0;
@@ -1595,17 +1603,24 @@ static int check_spectra(const sage_b200_spectra* sp) {
     return 0;
 }
 
+// Waits for everything queued on both lanes and marks them empty. Returns the first synchronisation error.
+static cudaError_t idle_lanes(sage_b200_scorer* S) {
+    cudaError_t first = cudaSuccess;
+    for (Lane& L : S->lanes) {
+        const cudaError_t a = cudaStreamSynchronize(L.copy), b = cudaStreamSynchronize(L.stream);
+        if (first == cudaSuccess) first = a != cudaSuccess ? a : b;
+        L.chunk.loaded = false; L.ran = false; L.downloading = false;
+    }
+    return first;
+}
+
 // Error exit of a batch call: the other lane may still have an H2D reading the caller's arrays or a D2H writing into them. Drain both lanes
 // before the error is returned, so the caller may free or reuse its buffers at once; the error message of the failure is preserved.
 static int drain_lanes(sage_b200_scorer* S, int rc) {
     const std::string msg = g_last_error;
-    for (Lane& L : S->lanes) {
+    for (Lane& L : S->lanes)
         if (L.stager.joinable()) L.stager.join();   // it reads the caller's arrays
-        if (L.copy) cudaStreamSynchronize(L.copy);
-        if (L.copy2) cudaStreamSynchronize(L.copy2);
-        if (L.stream) cudaStreamSynchronize(L.stream);
-        L.chunk.loaded = false; L.ran = false; L.downloading = false;
-    }
+    idle_lanes(S);
     cudaGetLastError();
     S->frag_dst = nullptr;
     g_last_error = msg;
@@ -1630,12 +1645,7 @@ extern "C" int sage_b200_score_batch(sage_b200_scorer* S, const sage_b200_spectr
     S->frag_dst = annotate ? fragments : nullptr;
     S->frag_cap = annotate ? fragment_capacity : 0;
     S->frag_used = 0;
-    for (Lane& L : S->lanes) {   // a previous call may have failed half-way: make sure nothing is still queued on the lanes
-        CUDA_TRY(cudaStreamSynchronize(L.copy));
-        CUDA_TRY(cudaStreamSynchronize(L.copy2));
-        CUDA_TRY(cudaStreamSynchronize(L.stream));
-        L.chunk.loaded = false; L.ran = false; L.downloading = false;
-    }
+    CUDA_TRY(idle_lanes(S));   // a previous call may have failed half-way: make sure nothing is still queued on the lanes
     if (S->trace) { S->t_base = std::chrono::steady_clock::now(); CUDA_TRY(cudaEventRecord(S->ev_base, S->lanes[0].stream)); }
     for (int restart = 0;; restart++) {
         rc = score_batch_chunks(S, sp, features, counts, annotate);
@@ -1661,10 +1671,17 @@ extern "C" int sage_b200_score_batch(sage_b200_scorer* S, const sage_b200_spectr
     return 0;
 }
 
+// The end of the chunk of at most `len` spectra that starts at c0: halved until its peaks fit the lane's staging bound (one spectrum always fits).
+static uint64_t chunk_end(const sage_b200_spectra* sp, uint64_t c0, uint64_t len) {
+    const uint64_t max_peaks = 1ull << 25;
+    uint64_t c1 = std::min<uint64_t>(sp->n, c0 + len);
+    while (c1 > c0 + 1 && sp->peak_offsets[c1] - sp->peak_offsets[c0] > max_peaks) c1 = c0 + (c1 - c0) / 2;
+    return c1;
+}
+
 // The chunk loop of score_batch (two pipelined lanes). Returns SAGE_B200_ERECHUNK when an open-search chunk must be cut smaller.
 static int score_batch_chunks(sage_b200_scorer* S, const sage_b200_spectra* sp, sage_b200_feature* features, uint32_t* counts, bool annotate) {
     int rc = 0;
-    const uint64_t max_peaks = 1ull << 25;
     // Chunks are as large as the staging bounds allow: on cfg2 one 50k chunk computes faster than two 25k chunks (the kernels process
     // spectra in precursor order, so a denser chunk shares more index lines). Inside a chunk the intensities copy overlaps setup + preliminary
     // scoring; across chunks (two lanes) the whole H2D of chunk i+1 and the D2H of chunk i-1 overlap the kernels of chunk i.
@@ -1678,8 +1695,7 @@ static int score_batch_chunks(sage_b200_scorer* S, const sage_b200_spectra* sp, 
     uint64_t c0 = 0;
     int li = 0;
     while (c0 < sp->n) {
-        uint64_t c1 = std::min<uint64_t>(sp->n, c0 + (c0 == 0 && first ? first : target));
-        while (c1 > c0 + 1 && sp->peak_offsets[c1] - sp->peak_offsets[c0] > max_peaks) c1 = c0 + (c1 - c0) / 2;
+        const uint64_t c1 = chunk_end(sp, c0, c0 == 0 && first ? first : target);
         Lane& L = S->lanes[li];
         if ((rc = lane_finish(S, L))) return rc;   // the chunk that used this lane two iterations ago
         const double ti0 = S->trace ? std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - S->t_base).count() : 0.0;
@@ -1823,17 +1839,15 @@ extern "C" int sage_b200_quick_score(sage_b200_scorer* S, const sage_b200_spectr
     CUDA_TRY(cudaMemset(S->d_keep.p, 0, npep + 16));
     S->last = sage_b200_counters{};
     S->frag_dst = nullptr;
-    for (Lane& L : S->lanes) { L.chunk.loaded = false; L.ran = false; L.downloading = false; }
+    CUDA_TRY(idle_lanes(S));
     S->quick_mode = prefilter_low_memory ? 2u : 1u;
-    const uint64_t max_peaks = 1ull << 25;
     Lane& L = S->lanes[0];
     for (int restart = 0; restart < 4; restart++) {
         uint64_t c0 = 0;
         rc = 0;
         const uint64_t max_chunk = wide_max_chunk(S->wide_per_spectrum, 32768);
         while (c0 < sp->n && rc == 0) {
-            uint64_t c1 = std::min<uint64_t>(sp->n, c0 + max_chunk);
-            while (c1 > c0 + 1 && sp->peak_offsets[c1] - sp->peak_offsets[c0] > max_peaks) c1 = c0 + (c1 - c0) / 2;
+            const uint64_t c1 = chunk_end(sp, c0, max_chunk);
             if ((rc = chunk_upload(S, L, sp, c0, c1)) == 0 && (rc = chunk_run(S, L, false)) == 0) rc = lane_finish(S, L);
             c0 = c1;
         }
@@ -1905,7 +1919,7 @@ extern "C" int64_t sage_b200_initial_hits(sage_b200_scorer* S, const sage_b200_s
     if (rc) return rc;
     if (sp->n != 1) return fail(SAGE_B200_EINVAL, "initial_hits takes exactly one spectrum");
     std::lock_guard<std::mutex> lock(S->mu);
-    if (cudaSetDevice(S->db->device) != cudaSuccess) return fail(SAGE_B200_ECUDA, "cudaSetDevice failed");
+    CUDA_TRY(cudaSetDevice(S->db->device));
     S->last = sage_b200_counters{};
     std::vector<sage_b200_feature> f(S->sv.report_psms);
     uint32_t cnt = 0;
@@ -1917,9 +1931,8 @@ extern "C" int64_t sage_b200_initial_hits(sage_b200_scorer* S, const sage_b200_s
     L.chunk.loaded = false;
     std::vector<uint64_t> keys(S->sv.kparam);
     uint32_t meta[4] = {0, 0, 0, 0};
-    if (cudaMemcpy(keys.data(), L.d_dbgk.p, 8 * (size_t)S->sv.kparam, cudaMemcpyDeviceToHost) != cudaSuccess ||
-        cudaMemcpy(meta, L.d_dbgm.p, 16, cudaMemcpyDeviceToHost) != cudaSuccess)
-        return fail(SAGE_B200_ECUDA, "initial_hits: readback failed");
+    CUDA_TRY(cudaMemcpy(keys.data(), L.d_dbgk.p, 8 * (size_t)S->sv.kparam, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(meta, L.d_dbgm.p, 16, cudaMemcpyDeviceToHost));
     const uint32_t nk = meta[0];
     for (uint32_t i = 0; i < nk && i < cap; i++) {
         const uint64_t k = keys[i];
@@ -2120,8 +2133,8 @@ struct sage_b200_lfq {
     sage_b200_alignment* d_align = nullptr;
     std::vector<uint32_t> slot_pep;   // slot -> PeptideIx, ascending
     DevBuf sp_off, sp_mass, sp_int, sp_mob, sp_file, sp_sst, counts, offsets, cell[2], value[2], tmp, ids, o_present, o_rt, o_sa, o_score, o_areas;
-    cudaStream_t st = nullptr;
-    cudaEvent_t ev[2] = {nullptr, nullptr};
+    Stream st;
+    Event ev[2];
     sage_b200_lfq_info info{};
     uint64_t scratch_bytes() const {
         uint64_t b = 0;
@@ -2155,9 +2168,6 @@ static int lfq_elapsed(sage_b200_lfq* L, float& ms) {
 extern "C" void sage_b200_lfq_destroy(sage_b200_lfq* L) {
     if (!L) return;
     cudaSetDevice(L->device);
-    for (cudaEvent_t e : L->ev)
-        if (e) cudaEventDestroy(e);
-    if (L->st) cudaStreamDestroy(L->st);
     delete L;
 }
 
@@ -2184,13 +2194,8 @@ static int lfq_build(sage_b200_lfq* L, const sage_b200_db* db, const sage_b200_p
                                                                        d_first);
     if (n_pep) k_lfq_flag<<<(unsigned)((n_pep + 255) / 256), 256, 0, st>>>(n_pep, d_first, d_flag);
     CUDA_TRY(cudaGetLastError());
-    {
-        size_t tb = 0;
-        thrust::counting_iterator<uint32_t> it(0);
-        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, it, d_flag, d_slots, d_nsel, (int)n_pep, st));
-        if (int rc = L->tmp.reserve(tb)) return rc;
-        CUDA_TRY(cub::DeviceSelect::Flagged(L->tmp.p, tb, it, d_flag, d_slots, d_nsel, (int)n_pep, st));
-    }
+    thrust::counting_iterator<uint32_t> it(0);
+    CUDA_TRY(L->tmp.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, d_flag, d_slots, d_nsel, (int)n_pep, st); }));
     uint32_t n_slots = 0;
     CUDA_TRY(cudaMemcpyAsync(&n_slots, d_nsel, 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -2335,26 +2340,21 @@ extern "C" int sage_b200_lfq_create(const sage_b200_db* db, const sage_b200_pept
         if (F->file_id[i] >= n_files)
             return fail(SAGE_B200_EINVAL, "lfq_create: feature %llu has file_id %u >= n_files %llu", (unsigned long long)i, F->file_id[i], (unsigned long long)n_files);
     }
-    sage_b200_lfq* L = new sage_b200_lfq();
+    Guard<sage_b200_lfq> guard(new sage_b200_lfq(), sage_b200_lfq_destroy);
+    sage_b200_lfq* L = guard.get();
     L->device = db->device;
     L->p = *params;
     L->n_files = (uint32_t)n_files;
     L->n_charges = (uint32_t)params->max_precursor_charge - params->min_precursor_charge + 1;
-    if (cudaStreamCreateWithFlags(&L->st, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreate(&L->ev[0]) != cudaSuccess ||
-        cudaEventCreate(&L->ev[1]) != cudaSuccess) {
-        sage_b200_lfq_destroy(L);
-        return fail(SAGE_B200_ECUDA, "lfq_create: stream / event creation failed");
-    }
-    if (int rc = lfq_build(L, db, peptides, F, alignments)) {
-        sage_b200_lfq_destroy(L);
-        return rc;
-    }
+    CUDA_TRY(L->st.create());
+    for (Event& e : L->ev) CUDA_TRY(e.create());
+    if (int rc = lfq_build(L, db, peptides, F, alignments)) return rc;
     L->info.n_peptides = L->n_slots;
     L->info.n_ranges = L->n_ranges;
     L->info.n_pages = L->n_pages;
     L->info.n_grids = L->n_grids;
     L->info.n_files = L->n_files;
-    *out = L;
+    *out = guard.release();
     return 0;
 }
 
@@ -2398,10 +2398,7 @@ static int lfq_trace_chunk(sage_b200_lfq* L, const sage_b200_ms1* m, uint64_t a,
     const unsigned blocks = (unsigned)((ns * 32 + LFQ_THREADS - 1) / LFQ_THREADS);
     k_lfq_trace<false><<<blocks, LFQ_THREADS, 0, st>>>(t);
     CUDA_TRY(cudaGetLastError());
-    size_t tb = 0;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, L->counts.as<uint64_t>(), L->offsets.as<uint64_t>(), (int)np, st));
-    if ((rc = L->tmp.reserve(tb))) return rc;
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(L->tmp.p, tb, L->counts.as<uint64_t>(), L->offsets.as<uint64_t>(), (int)np, st));
+    CUDA_TRY(L->tmp.two_phase([&](void* tmp, size_t& b) { return cub::DeviceScan::ExclusiveSum(tmp, b, L->counts.as<uint64_t>(), L->offsets.as<uint64_t>(), (int)np, st); }));
     uint64_t last[2] = {0, 0};
     CUDA_TRY(cudaMemcpyAsync(&last[0], L->offsets.as<uint64_t>() + np - 1, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(&last[1], L->counts.as<uint64_t>() + np - 1, 8, cudaMemcpyDeviceToHost, st));
@@ -2418,11 +2415,10 @@ static int lfq_trace_chunk(sage_b200_lfq* L, const sage_b200_ms1* m, uint64_t a,
     CUDA_TRY(cudaGetLastError());
     const uint64_t cells = L->n_grids * L->n_files * LFQ_ISO * LFQ_GRID;
     const int end_bit = std::max(1, (int)ceil_log2_u64(cells));
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, L->cell[0].as<uint64_t>(), L->cell[1].as<uint64_t>(), L->value[0].as<double>(), L->value[1].as<double>(),
-                                             (int)nc, 0, end_bit, st));
-    if ((rc = L->tmp.reserve(tb))) return rc;
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(L->tmp.p, tb, L->cell[0].as<uint64_t>(), L->cell[1].as<uint64_t>(), L->value[0].as<double>(),
-                                             L->value[1].as<double>(), (int)nc, 0, end_bit, st));
+    CUDA_TRY(L->tmp.two_phase([&](void* tmp, size_t& b) {
+        return cub::DeviceRadixSort::SortPairs(tmp, b, L->cell[0].as<uint64_t>(), L->cell[1].as<uint64_t>(), L->value[0].as<double>(), L->value[1].as<double>(),
+                                               (int)nc, 0, end_bit, st);
+    }));
     k_lfq_fold<<<(unsigned)((nc + 255) / 256), 256, 0, st>>>(nc, L->cell[1].as<uint64_t>(), L->value[1].as<double>(), (double*)L->d_grids,
                                                             (uint8_t*)L->d_touched, (uint64_t)L->n_files * LFQ_ISO * LFQ_GRID);
     CUDA_TRY(cudaGetLastError());
@@ -2466,12 +2462,11 @@ extern "C" int sage_b200_lfq_integrate(sage_b200_lfq* L, sage_b200_lfq_row* rows
     int rc;
     CUDA_TRY(cudaEventRecord(L->ev[0], st));
     if ((rc = L->ids.reserve(4 * L->n_grids + 16)) || (rc = L->o_present.reserve(4 * L->n_grids + 16))) return rc;
-    size_t tb = 0;
     thrust::counting_iterator<uint32_t> it(0);
     uint32_t* d_n = L->o_present.as<uint32_t>() + L->n_grids;   // the selected count lives behind the present flags' room
-    CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, it, (const uint8_t*)L->d_touched, L->ids.as<uint32_t>(), d_n, (int)L->n_grids, st));
-    if ((rc = L->tmp.reserve(tb))) return rc;
-    CUDA_TRY(cub::DeviceSelect::Flagged(L->tmp.p, tb, it, (const uint8_t*)L->d_touched, L->ids.as<uint32_t>(), d_n, (int)L->n_grids, st));
+    CUDA_TRY(L->tmp.two_phase([&](void* t, size_t& b) {
+        return cub::DeviceSelect::Flagged(t, b, it, (const uint8_t*)L->d_touched, L->ids.as<uint32_t>(), d_n, (int)L->n_grids, st);
+    }));
     uint32_t nt = 0;
     CUDA_TRY(cudaMemcpyAsync(&nt, d_n, 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -2648,13 +2643,10 @@ static int fdr_kde(cudaStream_t st, DevArena& A, const double* d_scores, const u
                    bool monotonic, double bw_factor, bool fma, double* d_out_bins, double* d_moments) {
     double *d_sel = nullptr, *part[2] = {nullptr, nullptr};
     uint64_t* d_nsel = nullptr;
-    size_t tb = 0;
     CUDA_TRY(A.alloc(&d_sel, 2 * n));
     CUDA_TRY(A.alloc(&d_nsel, 2));
-    CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, d_scores, d_decoy, d_sel, d_nsel, (int64_t)n, st));
-    CUDA_TRY(A.reserve_tmp(tb));
-    CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, d_scores, d_decoy, d_sel, d_nsel, (int64_t)n, st));           // decoys in row order
-    CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, d_scores, d_target, d_sel + n, d_nsel + 1, (int64_t)n, st));  // targets in row order
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_scores, d_decoy, d_sel, d_nsel, (int64_t)n, st); }));   // decoys in row order
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_scores, d_target, d_sel + n, d_nsel + 1, (int64_t)n, st); }));   // targets in row order
     uint64_t m[2];
     CUDA_TRY(cudaMemcpyAsync(m, d_nsel, 16, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -2800,8 +2792,8 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
 
     DevArena A;
     cudaStream_t st = 0;
-    StageEvents<6> ev;
-    CUDA_TRY(ev.create());
+    Event ev[6];
+    for (Event& e : ev) CUDA_TRY(e.create());
     sage_b200_feature* d_rows = nullptr;
     double *d_mass = nullptr, *d_mbins = nullptr, *d_mmom = nullptr, *d_X = nullptr, *d_means = nullptr, *d_scatter = nullptr, *d_coef = nullptr,
            *d_disc = nullptr, *d_dbins = nullptr, *d_dmom = nullptr;
@@ -3032,8 +3024,8 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
     const bool fma = host_math_variant() != 1;
     DevArena A;
     cudaStream_t st = 0;
-    StageEvents<5> ev;
-    CUDA_TRY(ev.create());
+    Event ev[5];
+    for (Event& e : ev) CUDA_TRY(e.create());
     sage_b200_feature* d_rows = nullptr;
     uint32_t *d_file = nullptr, *d_off = nullptr, *d_idx = nullptr, *d_order = nullptr, *d_isdec = nullptr, *d_dscan = nullptr, *d_train = nullptr,
              *d_val = nullptr, *d_val2 = nullptr, *d_seg = nullptr, *d_prow = nullptr, *d_keep = nullptr, *d_mrow = nullptr, *d_count = nullptr;
@@ -3097,13 +3089,8 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
     k_rt_train_flag<<<g, 256, 0, st>>>(d_rows, d_order, d_q, n, d_flag);
     CUDA_TRY(cudaGetLastError());
     uint64_t n_train = 0;
-    {
-        size_t tb = 0;
-        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, d_order, d_flag, d_train, d_count, (int)n, st));
-        CUDA_TRY(A.reserve_tmp(tb));
-        CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, d_order, d_flag, d_train, d_count, (int)n, st));
-        if (int rc = read_count(&n_train)) return rc;
-    }
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_order, d_flag, d_train, d_count, (int)n, st); }));
+    if (int rc = read_count(&n_train)) return rc;
     CUDA_TRY(cudaEventRecord(ev[1], st));
 
     // 2. global_alignment (retention_alignment.rs:95-173)
@@ -3115,29 +3102,22 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
         const unsigned gt = (unsigned)((n_train + 255) / 256);
         k_rt_pf_key<<<gt, 256, 0, st>>>(d_rows, d_file, d_train, n_train, d_key);
         CUDA_TRY(cudaGetLastError());
-        size_t tb = 0;
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key2, d_train, d_val, (int)n_train, 0, 64, st));
-        CUDA_TRY(A.reserve_tmp(tb));
-        CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, d_key, d_key2, d_train, d_val, (int)n_train, 0, 64, st));   // stable: poisson order kept
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) {   // stable: poisson order kept
+            return cub::DeviceRadixSort::SortPairs(t, b, d_key, d_key2, d_train, d_val, (int)n_train, 0, 64, st);
+        }));
         k_rt_heads<<<gt, 256, 0, st>>>(d_key2, n_train, d_flag);
         CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, count_it, d_flag, d_seg, d_count, (int)n_train, st));
-        CUDA_TRY(A.reserve_tmp(tb));
-        CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, count_it, d_flag, d_seg, d_count, (int)n_train, st));
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_flag, d_seg, d_count, (int)n_train, st); }));
         if (int rc = read_count(&n_seg)) return rc;
         const unsigned gs = (unsigned)((n_seg + 255) / 256);
         k_rt_seg_min<<<gs, 256, 0, st>>>(d_rows, d_key2, d_val, d_seg, n_seg, n_train, d_segmin, d_flag);
         CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, count_it, d_flag, d_prow, d_count, (int)n_seg, st));
-        CUDA_TRY(A.reserve_tmp(tb));
-        CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, count_it, d_flag, d_prow, d_count, (int)n_seg, st));
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_flag, d_prow, d_count, (int)n_seg, st); }));
         if (int rc = read_count(&n_pr)) return rc;
         const unsigned gp = (unsigned)((n_pr + 255) / 256);
         k_rt_row_mean<<<gp, 256, 0, st>>>(d_key2, d_seg, d_segmin, d_prow, n_pr, n_seg, d_maxrt, d_keep);
         CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, d_keep, d_mrow, (int)n_pr, st));
-        CUDA_TRY(A.reserve_tmp(tb));
-        CUDA_TRY(cub::DeviceScan::ExclusiveSum(A.tmp, tb, d_keep, d_mrow, (int)n_pr, st));
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_keep, d_mrow, (int)n_pr, st); }));
         uint32_t last[2] = {0, 0};
         CUDA_TRY(cudaMemcpyAsync(&last[0], d_mrow + n_pr - 1, 4, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(&last[1], d_keep + n_pr - 1, 4, cudaMemcpyDeviceToHost, st));
@@ -3265,17 +3245,12 @@ static int picked_competition(cudaStream_t st, DevArena& A, bool fma, uint32_t m
         return 0;
     };
     // 1. entries: sort (key, row); a run's head row is the first row that reaches the entry; rank the entries by it
-    size_t tb = 0;
     k_picked_iota<<<g, 256, 0, st>>>(m, idx);
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, key_s, idx, row_s, (int)m, 0, 32, st));
-    CUDA_TRY(A.reserve_tmp(tb));
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, d_key, key_s, idx, row_s, (int)m, 0, 32, st));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_key, key_s, idx, row_s, (int)m, 0, 32, st); }));
     k_picked_heads<<<g, 256, 0, st>>>(key_s, m, head);
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, tb, head, ginc, (int)m, st));
-    CUDA_TRY(A.reserve_tmp(tb));
-    CUDA_TRY(cub::DeviceScan::InclusiveSum(A.tmp, tb, head, ginc, (int)m, st));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, head, ginc, (int)m, st); }));
     uint32_t G = 0;
     if (int rc = read_u32(ginc + m - 1, &G)) return rc;
     CUDA_TRY(A.alloc(&first, G));
@@ -3283,15 +3258,11 @@ static int picked_competition(cudaStream_t st, DevArena& A, bool fma, uint32_t m
     CUDA_TRY(A.alloc(&gidx, G));
     CUDA_TRY(A.alloc(&g_sorted, G));
     CUDA_TRY(A.alloc(&rank_of_group, G));
-    CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, row_s, head, first, cnt, (int)m, st));
-    CUDA_TRY(A.reserve_tmp(tb));
-    CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, row_s, head, first, cnt, (int)m, st));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, row_s, head, first, cnt, (int)m, st); }));
     const unsigned gg = grid256(G);
     k_picked_iota<<<gg, 256, 0, st>>>(G, gidx);
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, first, first_s, gidx, g_sorted, (int)G, 0, 32, st));
-    CUDA_TRY(A.reserve_tmp(tb));
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, first, first_s, gidx, g_sorted, (int)G, 0, 32, st));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, first, first_s, gidx, g_sorted, (int)G, 0, 32, st); }));
     k_picked_scatter_rank<<<gg, 256, 0, st>>>(g_sorted, G, rank_of_group);
     CUDA_TRY(cudaGetLastError());
     uint32_t *side_key = nullptr, *sk_s = nullptr, *row2_s = nullptr, *seg = nullptr;
@@ -3305,14 +3276,12 @@ static int picked_competition(cudaStream_t st, DevArena& A, bool fma, uint32_t m
     CUDA_TRY(A.alloc(&sk_s, m));
     CUDA_TRY(A.alloc(&row2_s, m));
     CUDA_TRY(A.alloc(&seg, m));
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, side_key, sk_s, idx, row2_s, (int)m, 0, 32, st));
-    CUDA_TRY(A.reserve_tmp(tb));
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, side_key, sk_s, idx, row2_s, (int)m, 0, 32, st));   // stable: row order within a side
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) {   // stable: row order within a side
+        return cub::DeviceRadixSort::SortPairs(t, b, side_key, sk_s, idx, row2_s, (int)m, 0, 32, st);
+    }));
     k_picked_heads<<<g, 256, 0, st>>>(sk_s, m, head);
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cub::DeviceSelect::Flagged(nullptr, tb, count_it, head, seg, cnt, (int)m, st));
-    CUDA_TRY(A.reserve_tmp(tb));
-    CUDA_TRY(cub::DeviceSelect::Flagged(A.tmp, tb, count_it, head, seg, cnt, (int)m, st));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, head, seg, cnt, (int)m, st); }));
     uint32_t S = 0;
     if (int rc = read_u32(cnt, &S)) return rc;
     float* side_score = nullptr;
@@ -3342,9 +3311,7 @@ static int picked_competition(cudaStream_t st, DevArena& A, bool fma, uint32_t m
     CUDA_TRY(A.alloc(&moments, 4));
     k_picked_entries<<<gg, 256, 0, st>>>(side_score, side_has, G, kde_score, kde_flags, n_rows);
     CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, n_rows, row_off, (int)G, st));
-    CUDA_TRY(A.reserve_tmp(tb));
-    CUDA_TRY(cub::DeviceScan::ExclusiveSum(A.tmp, tb, n_rows, row_off, (int)G, st));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, n_rows, row_off, (int)G, st); }));
     if (int rc = fdr_kde(st, A, kde_score, kde_flags, kde_flags + G, G, 1000, true, 1.0, fma, bins, moments)) return rc;
     float *q_score = nullptr, *q_ix_val = nullptr;
     uint8_t* q_decoy = nullptr;
@@ -3433,10 +3400,7 @@ static int picked_peptide_keys(cudaStream_t st, DevArena& A, const sage_b200_pep
     const uint64_t mask = hash_bits >= 64 ? ~0ull : ((1ull << hash_bits) - 1);
     k_picked_hash<<<grid256(U), 256, 0, st>>>(pk, U, mask, d_hash, d_u);
     CUDA_TRY(cudaGetLastError());
-    size_t tb = 0;
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_hash, d_hash_s, d_u, d_u_s, (int)U, 0, 64, st));
-    CUDA_TRY(A.reserve_tmp(tb));
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, d_hash, d_hash_s, d_u, d_u_s, (int)U, 0, 64, st));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_hash, d_hash_s, d_u, d_u_s, (int)U, 0, 64, st); }));
     k_picked_group<<<grid256(U), 256, 0, st>>>(pk, d_hash_s, d_u_s, U, d_group);
     CUDA_TRY(cudaGetLastError());
     k_picked_peptide_keys<<<grid256(n), 256, 0, st>>>(d_row_slot, d_group, n, d_key);
@@ -3478,8 +3442,8 @@ extern "C" int sage_b200_picked_fdr(int device, const sage_b200_peptides* P, con
     const bool fma = host_math_variant() != 1;
     DevArena A;
     cudaStream_t st = 0;
-    StageEvents<4> ev;
-    CUDA_TRY(ev.create());
+    Event ev[4];
+    for (Event& e : ev) CUDA_TRY(e.create());
     uint32_t *d_key = nullptr, *d_pep = nullptr, *d_rank = nullptr, *d_pkey = nullptr, *d_prank = nullptr;
     uint8_t *d_decoy = nullptr, *d_pdecoy = nullptr;
     float *d_score = nullptr, *d_q = nullptr, *d_pscore = nullptr, *d_pq = nullptr;
