@@ -427,6 +427,68 @@ int sage_b200_picked_precursor(int device, const double* score, const uint8_t* d
 int sage_b200_competition_keys(int device, const sage_b200_peptides* peptides, const sage_b200_picked_params* p, const uint32_t* peptide_idx, uint64_t n,
                                uint32_t hash_bits, uint32_t* entry_rank);
 
+/* ---------------------------------------------------------------------------------------------------------------------------------------------
+ * Protein grouping and picked protein-group FDR (protein_grouping.rs generate_protein_groups, fdr.rs picked_protein_group; runner.rs:513-572).
+ * Every output is reproducible exactly under the definitions of DESIGN.md §13:
+ *   - a protein name is an id (equal ids <=> equal names). Names containing '/' or ';', and a target name that starts with the decoy tag,
+ *     are not modelled: the first change the reference's strings and group counts, the second makes a target and a tagged decoy share a key;
+ *   - pass 1 uses threshold.clamp(0, 1) (NaN stays NaN and selects nothing), pass 2 uses 1.0; a pass annotates only rows still unannotated;
+ *   - competition entries are ordered by the first row that reaches them: call this on the rows in spectrum_fdr's sorted order.
+ * Strings are not built here. The caller builds the reference's `protein_groups` string of row i from the outputs:
+ *   - pass[i] > 0: for each group g in row_groups[row_group_offsets[i] .. row_group_offsets[i+1]), the member names of g, each written
+ *     decoy_tag + name when group_decoy[g] && generate_decoys, sorted and joined with '/'; these group strings sorted and joined with ';';
+ *   - pass[i] == 0 (fallback): Peptide::proteins(decoy_tag, generate_decoys), the peptide's names in stored order joined with ';', each
+ *     written decoy_tag + name when the peptide is a decoy and generate_decoys is set.
+ */
+typedef struct {
+    const uint32_t* protein_offsets;  /* [n_peptides + 1] peptide p's proteins are protein_ids[protein_offsets[p] .. protein_offsets[p+1]) */
+    const uint32_t* protein_ids;      /* Peptide::proteins as name ids, in stored order (a repeated name stays repeated); each < n_names */
+    uint64_t n_names;
+    uint8_t protein_grouping;         /* 0: no grouping, every row takes the fallback */
+    uint8_t has_threshold;            /* 1: Some(threshold), two passes; 0: None, pass 2 only */
+    uint8_t generate_decoys;          /* IndexedDatabase::generate_decoys */
+    float threshold;                  /* the confident peptide q-value threshold of pass 1 */
+} sage_b200_protein_group_params;
+typedef struct {
+    uint32_t* num_protein_groups;     /* [n] Feature::num_protein_groups */
+    float* protein_group_q;           /* [n] Feature::protein_group_q: 1.0 for rows with num_protein_groups != 1 */
+    uint8_t* pass;                    /* [n] the pass that annotated the row: 1 or 2, 0 = fallback */
+    uint64_t* row_group_offsets;      /* [n + 1] */
+    uint32_t* row_groups;             /* [row capacity] each annotated row's covered groups, ascending; fallback rows have none.
+                                         row capacity = the sum over rows of their peptide's protein count */
+    uint64_t* group_offsets;          /* [group capacity + 1] the group tables of pass 1 then pass 2, concatenated; group g of pass 2 is
+                                         groups[0] + g. group capacity = 2 * min(protein_offsets[n_peptides], 2 * n_names) */
+    uint32_t* group_members;          /* [group capacity] name ids of each group, ascending */
+    uint8_t* group_covered;           /* [group capacity] 1: the group is in the cover */
+    uint8_t* group_decoy;             /* [group capacity] the decoy flag of the group's (name, decoy) keys */
+    uint64_t peptides[2];             /* per pass: distinct PeptideIx in the pass's peptide set */
+    uint64_t proteins[2];             /* per pass: distinct (name, decoy) keys (ProteinIx) */
+    uint64_t meta_peptides[2], groups[2], edges[2];
+    uint64_t covered[2];              /* groups in the cover */
+    uint64_t forced[2];               /* groups forced in by a peptide of degree 1 */
+    uint64_t greedy_picks[2];         /* add_largest_to_cover picks */
+    uint64_t components[2];           /* connected components left after the forced picks */
+    uint64_t largest_component[2];    /* groups in the largest of them */
+    uint64_t annotated[2];            /* rows annotated by the pass */
+    uint64_t passing;                 /* picked_protein_group's return: target rows at q <= 0.01 */
+    uint64_t entries;                 /* picked_protein_group's competition entries */
+    float ms_build[2], ms_cover[2], ms_lookup[2], ms_picked, ms_total;   /* CUDA-event stage times of the call */
+} sage_b200_protein_group_out;
+/* generate_protein_groups(db, rows, protein_grouping, has_threshold ? Some(threshold) : None) then picked_protein_group. rows: the Feature
+ * rows (peptide_idx and label are read); peptide_q and discriminant_score: [n] each, indexed like the rows; peptides: the table the rows'
+ * PeptideIx index (only n_peptides and decoy are read). The group set of a pass reads the label (label != -1); the lookup and the
+ * competition side read Peptide::decoy, as the reference does. EINVAL for a null required pointer, a peptide_idx outside the table,
+ * protein_offsets not starting at 0 or decreasing, or a protein id >= n_names; ELIMIT beyond 2^31 - 1 rows, 65535 * 4096 rows (the KDE's chunk
+ * grid), 2^30 names or 2^31 - 1 protein entries, or when the work buffers do not fit the device's free memory (checked before allocating).
+ * The argument checks run before the device is looked at. n == 0: no device work. */
+int sage_b200_protein_groups(int device, const sage_b200_peptides* peptides, const sage_b200_protein_group_params* p, const sage_b200_feature* rows,
+                             const float* peptide_q, const float* discriminant_score, uint64_t n, sage_b200_protein_group_out* out);
+/* Test hook: BipartiteGraph::new(edges, n_left, n_right).into_cover() (protein_grouping.rs) on the device, edge k = (left[k], right[k]);
+ * parallel edges allowed. cover[n_left] receives 1 for each left node in the cover. EINVAL for a null pointer or an endpoint out of range;
+ * ELIMIT beyond 2^31 - 1 edges or nodes. */
+int sage_b200_bipartite_cover(int device, const uint32_t* left, const uint32_t* right, uint64_t n_edges, uint64_t n_left, uint64_t n_right,
+                              uint8_t* cover);
+
 /* Page-locked host buffers: spectra/feature arrays placed here are copied by DMA without a staging memcpy. */
 void* sage_b200_host_alloc(size_t bytes);
 /* The same for a batch sage_b200_score_batch_multi cuts into n_devices contiguous blocks: the i-th of n equal parts of the buffer is placed on the

@@ -22,6 +22,9 @@
 // Also restates fdr.rs:16-287 (Competition::assign_q_value, picked_peptide, picked_protein, picked_precursor) with real key strings:
 // Peptide::reverse and Display (peptide.rs:307-318, 390-406) written out with Rust's shortest round-trip f32 formatting, and
 // insertion-ordered maps, in the definitions of DESIGN.md §12.
+//
+// Also restates protein_grouping.rs (generate_protein_groups, the literal BipartiteGraph loop) and fdr.rs:192-226 (picked_protein_group)
+// with real name strings, in the definitions of DESIGN.md §13.
 #include <algorithm>
 #include <charconv>
 #include <chrono>
@@ -29,6 +32,7 @@
 #include <cstdint>
 #include <cstring>
 #include <map>
+#include <set>
 #include <string>
 #include <unordered_map>
 #include <thread>
@@ -879,6 +883,248 @@ uint64_t mo_picked_precursor(const double* score, const uint8_t* decoy, uint64_t
     const uint64_t passing = q_tail(rows, [](const QRow& r) { return r.decoy ? 1.0f : 0.0f; }, 0.05f);
     for (const QRow& r : rows) q[std::stoull(r.ix)] = r.q;
     return passing;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ protein_grouping.rs, fdr.rs:192-226
+// generate_protein_groups and picked_protein_group with real name strings and the reference's order of steps: ordered maps where the reference
+// sorts, the literal BipartiteGraph loop (trim to a fixpoint, add the largest, repeat), Peptide::proteins for the fallback.
+namespace {
+
+using ProteinKey = std::pair<std::string, bool>;
+
+// BipartiteGraph (protein_grouping.rs), literally.
+struct Bipartite {
+    std::vector<std::pair<uint32_t, uint32_t>> edges;
+    std::vector<uint32_t> original, left_degree, right_degree;
+    std::vector<uint8_t> left_cover, right_cover;
+    uint64_t picks = 0;
+    Bipartite(std::vector<std::pair<uint32_t, uint32_t>> e, size_t n_left, size_t n_right)
+        : edges(std::move(e)), left_degree(n_left, 0), right_degree(n_right, 0), left_cover(n_left, 0), right_cover(n_right, 0) {
+        for (auto [l, r] : edges) {
+            left_degree[l]++;
+            right_degree[r]++;
+        }
+        original = left_degree;
+    }
+    void trim() {
+        size_t prev = 0;
+        while (prev != edges.size()) {
+            prev = edges.size();
+            for (auto [l, r] : edges)
+                if (right_degree[r] == 1) left_cover[l] = 1;
+            std::vector<std::pair<uint32_t, uint32_t>> kept;
+            for (auto [l, r] : edges) {
+                if (left_cover[l]) {
+                    right_cover[r] = 1;
+                    left_degree[l]--;
+                    right_degree[r]--;
+                } else {
+                    kept.push_back({l, r});
+                }
+            }
+            edges.swap(kept);
+            kept.clear();
+            for (auto [l, r] : edges) {
+                if (right_cover[r]) {
+                    left_degree[l]--;
+                    right_degree[r]--;
+                } else {
+                    kept.push_back({l, r});
+                }
+            }
+            edges.swap(kept);
+        }
+    }
+    void add_largest() {   // max_by_key over (remaining, original): the last of equal maxima
+        size_t best = 0;
+        for (size_t i = 1; i < left_degree.size(); i++)
+            if (std::make_pair(left_degree[i], original[i]) >= std::make_pair(left_degree[best], original[best])) best = i;
+        left_cover[best] = 1;
+        picks++;
+    }
+    std::vector<uint8_t> into_cover() {
+        while (!edges.empty()) {
+            trim();
+            if (!edges.empty()) add_largest();
+        }
+        return left_cover;
+    }
+};
+
+struct GroupingInput {
+    const uint32_t* prot_off;
+    const uint64_t* name_off;
+    const char* chars;
+    const uint8_t* decoy;
+    std::string name(uint32_t k) const { return std::string(chars + name_off[k], chars + name_off[k + 1]); }
+};
+
+std::string format_name(const ProteinKey& k, const std::string& tag, bool generate_decoys) {
+    return k.second && generate_decoys ? tag + k.first : k.first;
+}
+
+// annotate_features at one threshold: rows with an empty string are unannotated. Appends the pass's group table lines
+// ("<covered> <decoy> <sorted names joined by />") and writes [peptides, meta peptides, groups, covered, greedy picks, annotated] to stats.
+void annotate(const GroupingInput& in, const uint32_t* pep_idx, const int32_t* label, const float* peptide_q, uint64_t n, float threshold,
+              const std::string& tag, bool generate_decoys, std::vector<std::string>& groups_of_row, std::vector<uint32_t>& num,
+              std::vector<uint8_t>& pass, uint8_t pass_no, std::string& table, uint64_t* stats) {
+    std::set<uint32_t> peptides;
+    for (uint64_t i = 0; i < n; i++)
+        if (label[i] != -1 && peptide_q[i] < threshold) peptides.insert(pep_idx[i]);
+    // ProteinGrouper::build
+    std::map<ProteinKey, uint32_t> protein_index;
+    std::vector<ProteinKey> proteins;
+    std::set<std::vector<uint32_t>> meta_peptides;
+    for (uint32_t p : peptides) {
+        std::vector<uint32_t> list;
+        for (uint32_t k = in.prot_off[p]; k < in.prot_off[p + 1]; k++) {
+            ProteinKey key{in.name(k), in.decoy[p] != 0};
+            auto it = protein_index.find(key);
+            if (it == protein_index.end()) {
+                it = protein_index.emplace(key, (uint32_t)proteins.size()).first;
+                proteins.push_back(key);
+            }
+            list.push_back(it->second);
+        }
+        std::sort(list.begin(), list.end());
+        meta_peptides.insert(list);
+    }
+    std::map<uint32_t, std::vector<size_t>> prot_to_metapeps;
+    size_t i_meta = 0;
+    for (const auto& mp : meta_peptides) {
+        for (uint32_t prot : mp) prot_to_metapeps[prot].push_back(i_meta);
+        i_meta++;
+    }
+    std::map<std::vector<size_t>, std::vector<uint32_t>> evidence_to_group;
+    for (const auto& [prot, metas] : prot_to_metapeps) evidence_to_group[metas].push_back(prot);
+    std::vector<std::vector<uint32_t>> groups;
+    std::vector<std::pair<uint32_t, uint32_t>> edges;
+    for (const auto& [metas, group] : evidence_to_group) {
+        for (size_t m : metas) edges.push_back({(uint32_t)groups.size(), (uint32_t)m});
+        groups.push_back(group);
+    }
+    // into_group_map
+    Bipartite graph(edges, groups.size(), meta_peptides.size());
+    const std::vector<uint8_t> cover = graph.into_cover();
+    std::map<ProteinKey, std::vector<uint32_t>> protein_to_groups;
+    std::vector<std::string> group_str(groups.size());
+    uint64_t covered = 0;
+    for (size_t g = 0; g < groups.size(); g++) {
+        std::vector<std::string> fmt, raw;
+        for (uint32_t ix : groups[g]) {
+            fmt.push_back(format_name(proteins[ix], tag, generate_decoys));
+            raw.push_back(proteins[ix].first);
+        }
+        std::sort(fmt.begin(), fmt.end());
+        std::sort(raw.begin(), raw.end());
+        for (size_t k = 0; k < fmt.size(); k++) group_str[g] += (k ? "/" : "") + fmt[k];
+        table += std::to_string((int)cover[g]) + " " + std::to_string((int)proteins[groups[g][0]].second) + " ";
+        for (size_t k = 0; k < raw.size(); k++) table += (k ? "/" : "") + raw[k];
+        table += "\n";
+        if (!cover[g]) continue;
+        covered++;
+        for (uint32_t ix : groups[g]) protein_to_groups[proteins[ix]].push_back((uint32_t)g);
+    }
+    // the lookup of every row still unannotated
+    uint64_t annotated = 0;
+    for (uint64_t i = 0; i < n; i++) {
+        if (pass[i]) continue;
+        const uint32_t p = pep_idx[i];
+        std::set<uint32_t> group_set;
+        for (uint32_t k = in.prot_off[p]; k < in.prot_off[p + 1]; k++) {
+            auto it = protein_to_groups.find({in.name(k), in.decoy[p] != 0});
+            if (it != protein_to_groups.end()) group_set.insert(it->second.begin(), it->second.end());
+        }
+        if (group_set.empty()) continue;
+        std::vector<std::string> strs;
+        for (uint32_t g : group_set) strs.push_back(group_str[g]);
+        std::sort(strs.begin(), strs.end());
+        std::string s;
+        for (size_t k = 0; k < strs.size(); k++) s += (k ? ";" : "") + strs[k];
+        num[i] = (uint32_t)std::count(s.begin(), s.end(), ';') + 1;
+        groups_of_row[i] = s;
+        pass[i] = pass_no;
+        annotated++;
+    }
+    stats[0] = peptides.size();
+    stats[1] = meta_peptides.size();
+    stats[2] = groups.size();
+    stats[3] = covered;
+    stats[4] = graph.picks;
+    stats[5] = annotated;
+}
+
+std::string g_grouping_text;
+
+}  // namespace
+
+extern "C" {
+
+// generate_protein_groups then picked_protein_group. Names as for mo_picked_fdr. Writes num / pass / q per row, and to stats: pass 1's then
+// pass 2's [peptides, meta peptides, groups, covered, greedy picks, annotated], passing, entries. Returns the length of the text kept for
+// mo_grouping_text: each row's protein_groups string, then pass 1's and pass 2's group table lines, each line ended by '\n'.
+uint64_t mo_protein_groups(const uint32_t* prot_off, const uint64_t* name_off, const char* chars, const uint8_t* decoy, const uint32_t* pep_idx,
+                           const int32_t* label, const float* peptide_q, const float* disc, uint64_t n, int protein_grouping, int has_threshold,
+                           float threshold, int generate_decoys, const char* decoy_tag, int threads, uint32_t* num, uint8_t* pass, float* q,
+                           uint64_t* stats) {
+    const GroupingInput in{prot_off, name_off, chars, decoy};
+    const std::string tag(decoy_tag);
+    std::vector<std::string> strs(n);
+    std::vector<uint32_t> count(n, 0);
+    std::vector<uint8_t> row_pass(n, 0);
+    std::string tables[2];
+    std::fill(stats, stats + 14, 0);
+    if (protein_grouping) {
+        if (has_threshold) {
+            float t = threshold;   // f32::clamp(0.0, 1.0): NaN stays NaN
+            if (t < 0.0f) t = 0.0f;
+            if (t > 1.0f) t = 1.0f;
+            annotate(in, pep_idx, label, peptide_q, n, t, tag, generate_decoys, strs, count, row_pass, 1, tables[0], stats);
+        }
+        annotate(in, pep_idx, label, peptide_q, n, 1.0f, tag, generate_decoys, strs, count, row_pass, 2, tables[1], stats + 6);
+    }
+    for (uint64_t i = 0; i < n; i++) {   // the fallback: Peptide::proteins(decoy_tag, generate_decoys)
+        if (row_pass[i]) continue;
+        const uint32_t p = pep_idx[i];
+        std::string s;
+        for (uint32_t k = prot_off[p]; k < prot_off[p + 1]; k++) s += (k > prot_off[p] ? ";" : "") + format_name({in.name(k), decoy[p] != 0}, tag, generate_decoys);
+        strs[i] = s;
+        count[i] = prot_off[p + 1] - prot_off[p];
+    }
+    // picked_protein_group: key and Ix are the string
+    CompMap map;
+    for (uint64_t i = 0; i < n; i++) {
+        if (count[i] != 1) continue;
+        Comp& e = map.entry(strs[i]);
+        if (decoy[pep_idx[i]]) { e.reverse = fmax_rust(e.reverse, disc[i]); e.rix = strs[i]; e.has_r = true; }
+        else { e.forward = fmax_rust(e.forward, disc[i]); e.fix = strs[i]; e.has_f = true; }
+    }
+    std::unordered_map<std::string, float> scores;
+    stats[12] = assign_q_value(map, threads, &scores);
+    stats[13] = map.entries.size();
+    g_grouping_text.clear();
+    for (uint64_t i = 0; i < n; i++) {
+        num[i] = count[i];
+        pass[i] = row_pass[i];
+        q[i] = count[i] == 1 ? scores.at(strs[i]) : 1.0f;
+        g_grouping_text += strs[i] + "\n";
+    }
+    g_grouping_text += tables[0] + tables[1];
+    return g_grouping_text.size();
+}
+
+void mo_grouping_text(char* dst) { memcpy(dst, g_grouping_text.data(), g_grouping_text.size()); }
+
+// BipartiteGraph::new(edges, n_left, n_right).into_cover(), literally. Returns the number of add_largest picks.
+uint64_t mo_bipartite_cover(const uint32_t* left, const uint32_t* right, uint64_t n_edges, uint64_t n_left, uint64_t n_right, uint8_t* cover) {
+    std::vector<std::pair<uint32_t, uint32_t>> edges(n_edges);
+    for (uint64_t k = 0; k < n_edges; k++) edges[k] = {left[k], right[k]};
+    Bipartite graph(std::move(edges), n_left, n_right);
+    const std::vector<uint8_t> c = graph.into_cover();
+    std::copy(c.begin(), c.end(), cover);
+    return graph.picks;
 }
 
 }  // extern "C"

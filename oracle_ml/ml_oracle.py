@@ -44,6 +44,11 @@ def lib():
         _lib.mo_picked_fdr.argtypes = [C.c_void_p] * 9 + [C.c_char_p, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int] + [C.c_void_p] * 5
         _lib.mo_picked_precursor.restype = C.c_uint64
         _lib.mo_picked_precursor.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+        _lib.mo_protein_groups.restype = C.c_uint64
+        _lib.mo_protein_groups.argtypes = [C.c_void_p] * 8 + [C.c_uint64, C.c_int, C.c_int, C.c_float, C.c_int, C.c_char_p, C.c_int] + [C.c_void_p] * 4
+        _lib.mo_grouping_text.argtypes = [C.c_void_p]
+        _lib.mo_bipartite_cover.restype = C.c_uint64
+        _lib.mo_bipartite_cover.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p]
     return _lib
 
 
@@ -140,6 +145,16 @@ class PickedClash(ValueError):
     """Two distinct peptides on one side with one key: the reference panics at fdr.rs:149."""
 
 
+def _name_table(proteins):
+    names = [nm.encode() for lst in proteins for nm in lst]
+    prot_off = np.zeros(len(proteins) + 1, np.uint32)
+    prot_off[1:] = np.cumsum([len(lst) for lst in proteins])
+    name_off = np.zeros(len(names) + 1, np.uint64)
+    name_off[1:] = np.cumsum([len(b) for b in names])
+    chars = np.frombuffer(b"".join(names) + b"\0", np.uint8).copy()
+    return prot_off, name_off, chars
+
+
 def picked_fdr(peptides, pep_idx, score, proteins, cterm=None, generate_decoys=True, decoy_tag="rev_", threads=None) -> dict:
     """picked_peptide then picked_protein (fdr.rs) on the CPU with real key strings. `peptides` has seq_off, seq, mods, nterm and decoy;
     proteins[p] is Peptide::proteins of peptide p (a list of names). The same keys as sage_b200.picked_fdr (stage times aside), plus `seconds`."""
@@ -175,3 +190,52 @@ def picked_precursor(score, decoy):
     q = np.zeros(len(s), np.float32)
     passing = lib().mo_picked_precursor(_p(s), _p(d), len(s), _p(q))
     return q, int(passing)
+
+
+GROUPING_STATS = ("peptides", "meta_peptides", "groups", "covered", "greedy_picks", "annotated")
+
+
+def protein_groups(decoy, proteins, pep_idx, label, peptide_q, score, protein_grouping=True, threshold=0.01, generate_decoys=True, decoy_tag="rev_",
+                   threads=None) -> dict:
+    """generate_protein_groups then picked_protein_group (protein_grouping.rs, fdr.rs:192-226) on the CPU with real name strings. decoy[p] is
+    Peptide::decoy and proteins[p] Peptide::proteins (a list of names) of peptide p; threshold None is the reference's None. Returns
+    protein_groups (the strings), num_protein_groups, pass, protein_group_q per row; tables (per pass, a list of (covered, decoy, raw names
+    sorted and joined with '/') in group order); per-pass counts as 2-element lists (GROUPING_STATS); passing, entries, seconds, threads."""
+    import time
+    prot_off, name_off, chars = _name_table(proteins)
+    dec = np.ascontiguousarray(decoy, np.uint8)
+    idx = np.ascontiguousarray(pep_idx, np.uint32)
+    lab = np.ascontiguousarray(label, np.int32)
+    pq = np.ascontiguousarray(peptide_q, np.float32)
+    disc = np.ascontiguousarray(score, np.float32)
+    n = len(idx)
+    num, passes, q, stats = np.zeros(n, np.uint32), np.zeros(n, np.uint8), np.zeros(n, np.float32), np.zeros(14, np.uint64)
+    threads = int(threads or default_threads())
+    t0 = time.perf_counter()
+    size = lib().mo_protein_groups(_p(prot_off), _p(name_off), _p(chars), _p(dec), _p(idx), _p(lab), _p(pq), _p(disc), n, int(bool(protein_grouping)),
+                                   int(threshold is not None), float("nan") if threshold is None else float(threshold), int(bool(generate_decoys)),
+                                   decoy_tag.encode(), threads, _p(num), _p(passes), _p(q), _p(stats))
+    secs = time.perf_counter() - t0
+    buf = np.zeros(size, np.uint8)
+    lib().mo_grouping_text(_p(buf))
+    lines = buf.tobytes().decode().split("\n")[:-1] if size else []
+    st = stats.reshape(-1)
+    res = dict(protein_groups=lines[:n], num_protein_groups=num, **{"pass": passes}, protein_group_q=q, passing=int(st[12]), entries=int(st[13]),
+               seconds=secs, threads=threads)
+    res.update({k: [int(st[j]), int(st[6 + j])] for j, k in enumerate(GROUPING_STATS)})
+    tables, at = [], n
+    for k in range(2):
+        g = res["groups"][k]
+        tables.append([(int(c), int(d), names) for c, d, names in (ln.split(" ", 2) for ln in lines[at:at + g])])
+        at += g
+    res["tables"] = tables
+    return res
+
+
+def bipartite_cover(left, right, n_left, n_right):
+    """BipartiteGraph::new(edges, n_left, n_right).into_cover(), the literal loop: (cover as bools, add_largest picks)."""
+    lft = np.ascontiguousarray(left, np.uint32)
+    rgt = np.ascontiguousarray(right, np.uint32)
+    cover = np.zeros(int(n_left), np.uint8)
+    picks = lib().mo_bipartite_cover(_p(lft), _p(rgt), len(lft), int(n_left), int(n_right), _p(cover))
+    return cover.astype(bool), int(picks)

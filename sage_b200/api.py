@@ -91,7 +91,7 @@ EXPORTED_SYMBOLS = [
     "sage_b200_host_log_variant", "sage_b200_host_log1pf_exact", "sage_b200_device_log", "sage_b200_bind_thread_to_device", "sage_b200_host_alloc_blocks",
     "sage_b200_lfq_create", "sage_b200_lfq_add_ms1", "sage_b200_lfq_integrate", "sage_b200_lfq_get_info", "sage_b200_lfq_export", "sage_b200_lfq_destroy",
     "sage_b200_spectrum_fdr", "sage_b200_kde_build", "sage_b200_device_math", "sage_b200_predict_rt",
-    "sage_b200_picked_fdr", "sage_b200_picked_precursor", "sage_b200_competition_keys",
+    "sage_b200_picked_fdr", "sage_b200_picked_precursor", "sage_b200_competition_keys", "sage_b200_protein_groups", "sage_b200_bipartite_cover",
 ]
 
 _lib = None
@@ -927,3 +927,111 @@ def competition_keys(peptides: Peptides, peptide_idx, cterm=None, generate_decoy
     _check(load_library().sage_b200_competition_keys(C.c_int(device), C.byref(cp), C.byref(params), _ptr(idx), C.c_uint64(len(idx)),
                                                      C.c_uint32(int(hash_bits)), _ptr(out)))
     return out
+
+
+# ------------------------------------------------------------------------------------------------ protein grouping (protein_grouping.rs)
+class CProteinGroupParams(C.Structure):
+    _fields_ = [("protein_offsets", C.c_void_p), ("protein_ids", C.c_void_p), ("n_names", C.c_uint64), ("protein_grouping", C.c_uint8),
+                ("has_threshold", C.c_uint8), ("generate_decoys", C.c_uint8), ("threshold", C.c_float)]
+
+
+PROTEIN_GROUP_COUNTS = ["peptides", "proteins", "meta_peptides", "groups", "edges", "covered", "forced", "greedy_picks", "components",
+                        "largest_component", "annotated"]
+PROTEIN_GROUP_STAGES = ["ms_build", "ms_cover", "ms_lookup"]
+
+
+class CProteinGroupOut(C.Structure):
+    _fields_ = ([(c, C.c_void_p) for c in ("num_protein_groups", "protein_group_q", "pass", "row_group_offsets", "row_groups", "group_offsets",
+                                            "group_members", "group_covered", "group_decoy")]
+                + [(c, C.c_uint64 * 2) for c in PROTEIN_GROUP_COUNTS] + [("passing", C.c_uint64), ("entries", C.c_uint64)]
+                + [(s, C.c_float * 2) for s in PROTEIN_GROUP_STAGES] + [("ms_picked", C.c_float), ("ms_total", C.c_float)])
+
+
+def protein_groups(peptides: Peptides, features: np.ndarray, peptide_q, discriminant_score, protein_offsets, protein_ids, n_names: int,
+                   protein_grouping: bool = True, threshold: float | None = 0.01, generate_decoys: bool = True, device: int = 0) -> dict:
+    """generate_protein_groups then picked_protein_group (protein_grouping.rs, fdr.rs:192-226, runner.rs:540-545) on the device.
+    `features` are FEATURE_DTYPE rows in spectrum_fdr's sorted order (peptide_idx and label are read), `peptide_q` and `discriminant_score` one
+    f32 per row. Peptide p's proteins are the name ids protein_ids[protein_offsets[p]:protein_offsets[p + 1]] in stored order (equal ids for
+    equal names, each < n_names). threshold None is the reference's None: pass 2 only.
+    Returns num_protein_groups, protein_group_q, pass (1 or 2, 0 = fallback) per row; each row's covered groups as row_group_offsets /
+    row_groups; the group table of both passes (group_offsets, group_members as ascending ids, group_covered, group_decoy; pass 2's groups
+    follow pass 1's); per-pass counts as 2-element lists (PROTEIN_GROUP_COUNTS); passing, entries and the stage times. protein_group_strings
+    builds the reference's strings from it."""
+    rows = np.ascontiguousarray(features)
+    if rows.dtype != FEATURE_DTYPE:
+        raise TypeError("features must have FEATURE_DTYPE")
+    n = len(rows)
+    pq = np.ascontiguousarray(peptide_q, np.float32)
+    score = np.ascontiguousarray(discriminant_score, np.float32)
+    if len(pq) != n or len(score) != n:
+        raise ValueError("peptide_q and discriminant_score must have one value per row")
+    off = np.ascontiguousarray(protein_offsets, np.uint32)
+    ids = np.ascontiguousarray(protein_ids, np.uint32)
+    if len(off) != len(peptides) + 1:
+        raise ValueError("protein_offsets must have one value per peptide, plus one")
+    pep_idx = rows["peptide_idx"].astype(np.int64)
+    row_cap = int((off[1:].astype(np.int64) - off[:-1])[pep_idx[pep_idx < len(peptides)]].sum()) if n else 0
+    group_cap = 2 * min(int(off[-1]), 2 * int(n_names))
+    res = dict(num_protein_groups=np.zeros(n, np.uint32), protein_group_q=np.zeros(n, np.float32), row_pass=np.zeros(n, np.uint8),
+               row_group_offsets=np.zeros(n + 1, np.uint64), row_groups=np.zeros(row_cap, np.uint32), group_offsets=np.zeros(group_cap + 1, np.uint64),
+               group_members=np.zeros(group_cap, np.uint32), group_covered=np.zeros(group_cap, np.uint8), group_decoy=np.zeros(group_cap, np.uint8))
+    out = CProteinGroupOut(*[_ptr(res[k]) for k in ("num_protein_groups", "protein_group_q", "row_pass", "row_group_offsets", "row_groups",
+                                                    "group_offsets", "group_members", "group_covered", "group_decoy")])
+    params = CProteinGroupParams(_ptr(off), _ptr(ids), int(n_names), int(bool(protein_grouping)), int(threshold is not None), int(bool(generate_decoys)),
+                                 float("nan") if threshold is None else float(threshold))
+    keep: list = []
+    cp = peptides._c(keep)
+    _check(load_library().sage_b200_protein_groups(C.c_int(device), C.byref(cp), C.byref(params), _ptr(rows), _ptr(pq), _ptr(score), C.c_uint64(n),
+                                                   C.byref(out)))
+    res["pass"] = res.pop("row_pass")
+    res.update({c: [int(v) for v in getattr(out, c)] for c in PROTEIN_GROUP_COUNTS})
+    n_groups = sum(res["groups"])
+    res["row_groups"] = res["row_groups"][:int(res["row_group_offsets"][-1])]
+    res["group_offsets"] = res["group_offsets"][:n_groups + 1]
+    res["group_members"] = res["group_members"][:int(res["group_offsets"][-1])]
+    res["group_covered"] = res["group_covered"][:n_groups]
+    res["group_decoy"] = res["group_decoy"][:n_groups]
+    res.update(passing=int(out.passing), entries=int(out.entries), ms_picked=float(out.ms_picked), ms_total=float(out.ms_total))
+    res.update({s: [float(v) for v in getattr(out, s)] for s in PROTEIN_GROUP_STAGES})
+    return res
+
+
+def _format_name(name: str, decoy: bool, decoy_tag: str, generate_decoys: bool) -> str:
+    return decoy_tag + name if decoy and generate_decoys else name
+
+
+def group_string(result: dict, g: int, names, decoy_tag: str = "rev_", generate_decoys: bool = True) -> str:
+    """ProteinGroup::format of group g of protein_groups' table: its member names, tagged when the group is a decoy, sorted, joined with '/'."""
+    a, b = int(result["group_offsets"][g]), int(result["group_offsets"][g + 1])
+    dec = bool(result["group_decoy"][g])
+    return "/".join(sorted(_format_name(names[i], dec, decoy_tag, generate_decoys) for i in result["group_members"][a:b].tolist()))
+
+
+def protein_group_strings(result: dict, rows: np.ndarray, peptides: Peptides, protein_offsets, protein_ids, names, decoy_tag: str = "rev_",
+                          generate_decoys: bool = True) -> list:
+    """The reference's Feature::protein_groups of each row from protein_groups' result (the rule of include/sage_b200.h): a grouped row joins
+    its groups' strings, sorted, with ';'; a fallback row is Peptide::proteins(decoy_tag, generate_decoys). names[id] is the name of an id."""
+    off = np.asarray(protein_offsets)
+    ids = np.asarray(protein_ids)
+    roff = result["row_group_offsets"]
+    out = []
+    for i, p in enumerate(np.asarray(rows["peptide_idx"]).tolist()):
+        if result["pass"][i]:
+            gs = result["row_groups"][int(roff[i]):int(roff[i + 1])].tolist()
+            out.append(";".join(sorted(group_string(result, g, names, decoy_tag, generate_decoys) for g in gs)))
+        else:
+            dec = bool(peptides.decoy[p])
+            out.append(";".join(_format_name(names[k], dec, decoy_tag, generate_decoys) for k in ids[off[p]:off[p + 1]].tolist()))
+    return out
+
+
+def bipartite_cover(left, right, n_left: int, n_right: int, device: int = 0) -> np.ndarray:
+    """Test hook: BipartiteGraph::new(edges, n_left, n_right).into_cover() (protein_grouping.rs) on the device: a bool per left node."""
+    lft = np.ascontiguousarray(left, np.uint32)
+    rgt = np.ascontiguousarray(right, np.uint32)
+    if len(lft) != len(rgt):
+        raise ValueError("left and right must have one value per edge")
+    cover = np.zeros(int(n_left), np.uint8)
+    _check(load_library().sage_b200_bipartite_cover(C.c_int(device), _ptr(lft), _ptr(rgt), C.c_uint64(len(lft)), C.c_uint64(int(n_left)),
+                                                    C.c_uint64(int(n_right)), _ptr(cover)))
+    return cover.astype(bool)

@@ -8,6 +8,9 @@
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 #include <cub/device/device_reduce.cuh>
+#include <cub/device/device_merge_sort.cuh>
+#include <cub/device/device_run_length_encode.cuh>
+#include <cub/device/device_segmented_sort.cuh>
 #include <cuda_runtime.h>
 #include <thrust/iterator/counting_iterator.h>
 
@@ -37,6 +40,7 @@
 #include "fdr.cuh"
 #include "rt.cuh"
 #include "picked.cuh"
+#include "protein_groups.cuh"
 
 using namespace sb;
 
@@ -3554,6 +3558,510 @@ extern "C" int sage_b200_competition_keys(int device, const sage_b200_peptides* 
     uint64_t entries = 0, passing = 0;
     if (int rc = picked_competition(st, A, true, (uint32_t)n, d_key, d_decoy, nullptr, nullptr, true, d_rank, nullptr, &entries, &passing)) return rc;
     CUDA_TRY(cudaMemcpyAsync(entry_rank, d_rank, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// ================================================================================== protein grouping (protein_grouping.rs; kernels in protein_groups.cuh)
+// Kernel launches over n items; n == 0 launches nothing.
+#define PG_LAUNCH(kernel, n, ...)                                                        \
+    do {                                                                                 \
+        if ((n) > 0) {                                                                   \
+            kernel<<<grid256(n), 256, 0, st>>>(__VA_ARGS__);                             \
+            CUDA_TRY(cudaGetLastError());                                                \
+        }                                                                                \
+    } while (0)
+
+static int pg_read(cudaStream_t st, const void* d, void* h, size_t bytes) {
+    CUDA_TRY(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// out[0..n] = exclusive prefix sum of in[0..n) (in[n] must be 0); returns out[n] in *total.
+static int pg_offsets(cudaStream_t st, DevArena& A, const uint32_t* in, uint32_t* out, uint32_t n, uint32_t* total) {
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, in, out, (int)n + 1, st); }));
+    return pg_read(st, out + n, total, 4);
+}
+
+struct PgCoverStats {
+    uint64_t forced = 0, greedy = 0, components = 0, largest = 0, covered = 0;
+};
+
+// BipartiteGraph::into_cover (protein_grouping.rs) over E edges (el[k], er[k]) between G left and M right nodes; lcov[G] receives the cover.
+// Phase 1 is the first trim's forced picks; phase 2 the greedy of each connected component of what remains (DESIGN.md §13).
+static int pg_cover(cudaStream_t st, DevArena& A, uint32_t E, uint32_t G, uint32_t M, const uint32_t* el, const uint32_t* er, uint8_t* lcov,
+                    PgCoverStats* s) {
+    *s = {};
+    if (G) CUDA_TRY(cudaMemsetAsync(lcov, 0, G, st));
+    if (E == 0) return 0;
+    uint32_t *ldeg, *rdeg, *loff, *roff, *key_s, *ladj, *radj, *rcov, *rem, *parent, tot = 0;
+    uint8_t* active;
+    unsigned long long* cnt;
+    CUDA_TRY(A.alloc(&ldeg, G + 1));
+    CUDA_TRY(A.alloc(&rdeg, M + 1));
+    CUDA_TRY(A.alloc(&loff, G + 1));
+    CUDA_TRY(A.alloc(&roff, M + 1));
+    CUDA_TRY(A.alloc(&key_s, E));
+    CUDA_TRY(A.alloc(&ladj, E));
+    CUDA_TRY(A.alloc(&radj, E));
+    CUDA_TRY(A.alloc(&rcov, M));
+    CUDA_TRY(A.alloc(&rem, G));
+    CUDA_TRY(A.alloc(&parent, G + M));
+    CUDA_TRY(A.alloc(&active, G));
+    CUDA_TRY(A.alloc(&cnt, 3));   // forced, greedy picks, covered
+    CUDA_TRY(cudaMemsetAsync(ldeg, 0, 4ull * (G + 1), st));
+    CUDA_TRY(cudaMemsetAsync(rdeg, 0, 4ull * (M + 1), st));
+    CUDA_TRY(cudaMemsetAsync(rcov, 0, 4ull * M, st));
+    CUDA_TRY(cudaMemsetAsync(cnt, 0, 24, st));
+    PG_LAUNCH(k_pg_degrees, E, el, er, E, ldeg, rdeg);
+    if (int rc = pg_offsets(st, A, ldeg, loff, G, &tot)) return rc;
+    if (int rc = pg_offsets(st, A, rdeg, roff, M, &tot)) return rc;
+    // adjacency of each left node (by a sort on the left end) and of each right node
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, el, key_s, er, ladj, (int)E, 0, 32, st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, er, key_s, el, radj, (int)E, 0, 32, st); }));
+    PG_LAUNCH(k_pg_forced, E, el, er, rdeg, E, lcov);
+    PG_LAUNCH(k_pg_count, G, lcov, G, cnt);
+    PG_LAUNCH(k_pg_cover_rights, E, el, er, lcov, E, rcov);
+    PG_LAUNCH(k_pg_remaining, G, ladj, loff, lcov, rcov, G, rem, active);
+    PG_LAUNCH(k_picked_iota, G + M, G + M, parent);
+    PG_LAUNCH(k_pg_union, E, el, er, lcov, rcov, E, G, parent);
+    // the groups left with edges, by component (ascending group index within one)
+    thrust::counting_iterator<uint32_t> it(0);
+    uint32_t *act, *comp, *lefts, *uniq, *clen, *coff, *large, *nsel, n_act = 0, n_comp = 0, n_large = 0;
+    uint8_t* lflag;
+    CUDA_TRY(A.alloc(&act, G));
+    CUDA_TRY(A.alloc(&nsel, 1));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, active, act, nsel, (int)G, st); }));
+    if (int rc = pg_read(st, nsel, &n_act, 4)) return rc;
+    if (n_act) {
+        CUDA_TRY(A.alloc(&comp, n_act));
+        CUDA_TRY(A.alloc(&lefts, n_act));
+        CUDA_TRY(A.alloc(&uniq, n_act));
+        CUDA_TRY(A.alloc(&clen, n_act + 1));
+        CUDA_TRY(A.alloc(&coff, n_act + 1));
+        PG_LAUNCH(k_pg_comp_of, n_act, parent, act, n_act, comp);
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, comp, key_s, act, lefts, (int)n_act, 0, 32, st); }));
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRunLengthEncode::Encode(t, b, key_s, uniq, clen, nsel, (int)n_act, st); }));
+        if (int rc = pg_read(st, nsel, &n_comp, 4)) return rc;
+        CUDA_TRY(cudaMemsetAsync(clen + n_comp, 0, 4, st));
+        if (int rc = pg_offsets(st, A, clen, coff, n_comp, &tot)) return rc;
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceReduce::Max(t, b, clen, uniq, (int)n_comp, st); }));
+        uint32_t largest = 0;
+        if (int rc = pg_read(st, uniq, &largest, 4)) return rc;
+        CUDA_TRY(A.alloc(&lflag, n_comp));
+        CUDA_TRY(A.alloc(&large, n_comp));
+        PG_LAUNCH(k_pg_large_flag, n_comp, clen, n_comp, lflag);
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, lflag, large, nsel, (int)n_comp, st); }));
+        if (int rc = pg_read(st, nsel, &n_large, 4)) return rc;
+        k_pg_greedy_warp<<<(unsigned)((32ull * n_comp + 255) / 256), 256, 0, st>>>(coff, clen, n_comp, lefts, ldeg, ladj, loff, radj, roff, rem, rcov, lcov,
+                                                                                  cnt + 1);
+        CUDA_TRY(cudaGetLastError());
+        if (n_large) {
+            k_pg_greedy_cta<<<n_large, PG_CTA, 0, st>>>(large, coff, clen, lefts, ldeg, ladj, loff, radj, roff, rem, rcov, lcov, cnt + 1);
+            CUDA_TRY(cudaGetLastError());
+        }
+        s->components = n_comp;
+        s->largest = largest;
+    }
+    PG_LAUNCH(k_pg_count, G, lcov, G, cnt + 2);
+    unsigned long long c[3];
+    if (int rc = pg_read(st, cnt, c, 24)) return rc;
+    s->forced = c[0];
+    s->greedy = c[1];
+    s->covered = c[2];
+    return 0;
+}
+
+// The inputs of the call on the device.
+struct PgInputs {
+    uint32_t n, n_pep, n_names;
+    const uint32_t *pep, *poff, *pids;
+    const uint8_t *label_ok, *pdecoy;
+    const float* q;
+    const uint64_t* cap_off;
+};
+
+// One pass's group table on the device: group g has members[goff[g] .. goff[g+1]) (name ids, ascending), gdecoy[g], lcov[g].
+struct PgTable {
+    uint32_t G = 0, P = 0;
+    uint32_t *goff = nullptr, *members = nullptr;
+    uint8_t *gdecoy = nullptr, *lcov = nullptr;
+};
+
+// annotate_features (protein_grouping.rs) at one threshold: ProteinGrouper::build, into_group_map's cover, and the lookup of every row still
+// unannotated (pass[i] == 0), whose distinct covered groups (numbered from `base`) go to the row's slot of `scratch`.
+static int pg_pass(cudaStream_t st, DevArena& A, const PgInputs& in, float threshold, uint8_t pass_no, uint32_t base, uint8_t* pass, uint32_t* count,
+                   uint32_t* scratch, PgTable* T, sage_b200_protein_group_out* out, cudaEvent_t ev_built, cudaEvent_t ev_covered) {
+    const int k = pass_no - 1;
+    const uint32_t NK = 2 * in.n_names;
+    thrust::counting_iterator<uint32_t> it(0);
+    uint32_t *nsel, U = 0;
+    uint8_t* mark;
+    CUDA_TRY(A.alloc(&nsel, 1));
+    CUDA_TRY(A.alloc(&mark, in.n_pep));
+    // 1. the peptide set, ascending PeptideIx
+    CUDA_TRY(cudaMemsetAsync(mark, 0, in.n_pep, st));
+    PG_LAUNCH(k_pg_mark, in.n, in.pep, in.label_ok, in.q, in.n, threshold, mark);
+    uint32_t* set;
+    CUDA_TRY(A.alloc(&set, in.n_pep));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, mark, set, nsel, (int)in.n_pep, st); }));
+    if (int rc = pg_read(st, nsel, &U, 4)) return rc;
+    out->peptides[k] = U;
+    uint32_t M = 0, P = 0, G = 0, E = 0, T_pairs = 0, tot = 0;
+    uint32_t *pix_of_key = nullptr, *group_of = nullptr, *el = nullptr, *er = nullptr;
+    CUDA_TRY(A.alloc(&pix_of_key, NK));
+    CUDA_TRY(cudaMemsetAsync(pix_of_key, 0xFF, 4ull * NK, st));
+    if (U) {
+        // 2. the (peptide, protein) pairs; ProteinIx by first encounter
+        uint32_t *len, *soff, *pair_key, *first, *present, *first_p, *first_s, *key_by_pix;
+        uint8_t* flag;
+        CUDA_TRY(A.alloc(&len, U + 1));
+        CUDA_TRY(A.alloc(&soff, U + 1));
+        CUDA_TRY(cudaMemsetAsync(len + U, 0, 4, st));
+        PG_LAUNCH(k_pg_set_len, U, set, in.poff, U, len);
+        if (int rc = pg_offsets(st, A, len, soff, U, &T_pairs)) return rc;
+        CUDA_TRY(A.alloc(&pair_key, T_pairs));
+        CUDA_TRY(A.alloc(&first, NK));
+        CUDA_TRY(A.alloc(&flag, NK));
+        CUDA_TRY(cudaMemsetAsync(first, 0xFF, 4ull * NK, st));
+        PG_LAUNCH(k_pg_flatten, U, set, soff, in.poff, in.pids, in.pdecoy, U, pair_key, first);
+        PG_LAUNCH(k_pg_key_present, NK, first, NK, flag);
+        CUDA_TRY(A.alloc(&present, NK));
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, flag, present, nsel, (int)NK, st); }));
+        if (int rc = pg_read(st, nsel, &P, 4)) return rc;
+        CUDA_TRY(A.alloc(&first_p, P));
+        CUDA_TRY(A.alloc(&first_s, P));
+        CUDA_TRY(A.alloc(&key_by_pix, P));
+        PG_LAUNCH(k_pg_gather_u32, P, first, present, P, first_p);
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, first_p, first_s, present, key_by_pix, (int)P, 0, 32, st); }));
+        PG_LAUNCH(k_pg_scatter_rank, P, key_by_pix, P, pix_of_key);
+        // 3. each peptide's sorted ProteinIx list; meta-peptides = the distinct lists, ranked lexicographically
+        uint32_t *pix, *pix_s, *idx, *head, *incl, *mrep;
+        CUDA_TRY(A.alloc(&pix, T_pairs));
+        CUDA_TRY(A.alloc(&pix_s, T_pairs));
+        CUDA_TRY(A.alloc(&idx, U));
+        CUDA_TRY(A.alloc(&head, U));
+        CUDA_TRY(A.alloc(&incl, U));
+        CUDA_TRY(A.alloc(&mrep, U));
+        PG_LAUNCH(k_pg_pair_pix, T_pairs, pair_key, pix_of_key, T_pairs, pix);
+        if (T_pairs)
+            CUDA_TRY(A.two_phase([&](void* t, size_t& b) {
+                return cub::DeviceSegmentedSort::SortKeys(t, b, pix, pix_s, (int)T_pairs, (int)U, soff, soff + 1, st);
+            }));
+        PG_LAUNCH(k_picked_iota, U, U, idx);
+        const PgLexLess meta_less{pix_s, soff};
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceMergeSort::StableSortKeys(t, b, idx, (int)U, meta_less, st); }));
+        PG_LAUNCH(k_pg_lex_heads, U, idx, pix_s, soff, U, head);
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, head, incl, (int)U, st); }));
+        if (int rc = pg_read(st, incl + U - 1, &M, 4)) return rc;
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, idx, head, mrep, nsel, (int)U, st); }));
+        if (P) {
+            // 4. each protein's evidence: the meta-peptides that hold it, ascending, with multiplicity
+            uint32_t *mlen, *moff, *pdeg, *ev, *ev_off, TM = 0;
+            uint64_t *pairs, *pairs_s;
+            CUDA_TRY(A.alloc(&mlen, M + 1));
+            CUDA_TRY(A.alloc(&moff, M + 1));
+            CUDA_TRY(cudaMemsetAsync(mlen + M, 0, 4, st));
+            PG_LAUNCH(k_pg_csr_len, M, mrep, soff, M, mlen);
+            if (int rc = pg_offsets(st, A, mlen, moff, M, &TM)) return rc;
+            CUDA_TRY(A.alloc(&pdeg, P + 1));
+            CUDA_TRY(A.alloc(&ev_off, P + 1));
+            CUDA_TRY(A.alloc(&pairs, TM));
+            CUDA_TRY(A.alloc(&pairs_s, TM));
+            CUDA_TRY(A.alloc(&ev, TM));
+            CUDA_TRY(cudaMemsetAsync(pdeg, 0, 4ull * (P + 1), st));
+            PG_LAUNCH(k_pg_meta_pairs, M, mrep, pix_s, soff, moff, M, pairs, pdeg);
+            CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, pairs, pairs_s, (int)TM, 0, 64, st); }));
+            PG_LAUNCH(k_pg_low32, TM, pairs_s, TM, ev);
+            if (int rc = pg_offsets(st, A, pdeg, ev_off, P, &tot)) return rc;
+            // 5. groups: proteins of equal evidence, ranked by it; members in ascending id; edges (group, each evidence entry)
+            uint32_t *pidx, *phead, *pincl, *grep, *gsize, *elen, *eoff;
+            uint64_t *mem, *mem_s;
+            CUDA_TRY(A.alloc(&pidx, P));
+            CUDA_TRY(A.alloc(&phead, P));
+            CUDA_TRY(A.alloc(&pincl, P));
+            CUDA_TRY(A.alloc(&grep, P));
+            CUDA_TRY(A.alloc(&group_of, P));
+            PG_LAUNCH(k_picked_iota, P, P, pidx);
+            const PgLexLess group_less{ev, ev_off};
+            CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceMergeSort::StableSortKeys(t, b, pidx, (int)P, group_less, st); }));
+            PG_LAUNCH(k_pg_lex_heads, P, pidx, ev, ev_off, P, phead);
+            CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, phead, pincl, (int)P, st); }));
+            if (int rc = pg_read(st, pincl + P - 1, &G, 4)) return rc;
+            PG_LAUNCH(k_pg_rank_of, P, pidx, pincl, P, group_of);
+            CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, pidx, phead, grep, nsel, (int)P, st); }));
+            CUDA_TRY(A.alloc(&gsize, G + 1));
+            CUDA_TRY(A.alloc(&T->goff, G + 1));
+            CUDA_TRY(A.alloc(&T->members, P));
+            CUDA_TRY(A.alloc(&T->gdecoy, G));
+            CUDA_TRY(A.alloc(&mem, P));
+            CUDA_TRY(A.alloc(&mem_s, P));
+            CUDA_TRY(cudaMemsetAsync(gsize, 0, 4ull * (G + 1), st));
+            PG_LAUNCH(k_pg_members, P, group_of, key_by_pix, P, mem, gsize, T->gdecoy);
+            CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, mem, mem_s, (int)P, 0, 64, st); }));
+            PG_LAUNCH(k_pg_low32, P, mem_s, P, T->members);
+            if (int rc = pg_offsets(st, A, gsize, T->goff, G, &tot)) return rc;
+            CUDA_TRY(A.alloc(&elen, G + 1));
+            CUDA_TRY(A.alloc(&eoff, G + 1));
+            CUDA_TRY(cudaMemsetAsync(elen + G, 0, 4, st));
+            PG_LAUNCH(k_pg_csr_len, G, grep, ev_off, G, elen);
+            if (int rc = pg_offsets(st, A, elen, eoff, G, &E)) return rc;
+            CUDA_TRY(A.alloc(&el, E));
+            CUDA_TRY(A.alloc(&er, E));
+            PG_LAUNCH(k_pg_edges, G, grep, ev, ev_off, eoff, G, el, er);
+        }
+    }
+    T->G = G;
+    T->P = P;
+    out->proteins[k] = P;
+    out->meta_peptides[k] = M;
+    out->groups[k] = G;
+    out->edges[k] = E;
+    CUDA_TRY(cudaEventRecord(ev_built, st));
+    // 6. the cover
+    CUDA_TRY(A.alloc(&T->lcov, G));
+    PgCoverStats cs;
+    if (int rc = pg_cover(st, A, E, G, M, el, er, T->lcov, &cs)) return rc;
+    out->covered[k] = cs.covered;
+    out->forced[k] = cs.forced;
+    out->greedy_picks[k] = cs.greedy;
+    out->components[k] = cs.components;
+    out->largest_component[k] = cs.largest;
+    CUDA_TRY(cudaEventRecord(ev_covered, st));
+    // 7. the rows still unannotated
+    if (G) {
+        unsigned long long* d_ann;
+        CUDA_TRY(A.alloc(&d_ann, 1));
+        CUDA_TRY(cudaMemsetAsync(d_ann, 0, 8, st));
+        PG_LAUNCH(k_pg_lookup, in.n, in.pep, in.n, in.poff, in.pids, in.pdecoy, in.cap_off, pix_of_key, group_of, T->lcov, base, pass_no, pass, count,
+                  scratch, d_ann);
+        unsigned long long ann = 0;
+        if (int rc = pg_read(st, d_ann, &ann, 8)) return rc;
+        out->annotated[k] = ann;
+    }
+    return 0;
+}
+
+extern "C" int sage_b200_protein_groups(int device, const sage_b200_peptides* P, const sage_b200_protein_group_params* p, const sage_b200_feature* rows,
+                                        const float* peptide_q, const float* discriminant_score, uint64_t n, sage_b200_protein_group_out* out) {
+    if (!out || !P || !p) return fail(SAGE_B200_EINVAL, "protein_groups: null argument");
+    if (n && (!rows || !peptide_q || !discriminant_score || !out->num_protein_groups || !out->protein_group_q || !out->pass || !out->row_group_offsets ||
+              !out->row_groups || !out->group_offsets || !out->group_members || !out->group_covered || !out->group_decoy))
+        return fail(SAGE_B200_EINVAL, "protein_groups: null argument");
+    if (!p->protein_offsets || (P->n_peptides && !P->decoy)) return fail(SAGE_B200_EINVAL, "protein_groups: null peptide array");
+    if (P->n_peptides >= 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "protein_groups: too many peptides for u32 PeptideIx");
+    if (int rc = picked_limits("protein_groups", n)) return rc;
+    if (p->n_names >= (1ull << 30)) return fail(SAGE_B200_ELIMIT, "protein_groups: 2^30 or more protein names");
+    const uint64_t n_pep = P->n_peptides;
+    if (p->protein_offsets[0] != 0) return fail(SAGE_B200_EINVAL, "protein_groups: protein_offsets[0] is %u, not 0", p->protein_offsets[0]);
+    for (uint64_t q = 0; q < n_pep; q++)
+        if (p->protein_offsets[q + 1] < p->protein_offsets[q])
+            return fail(SAGE_B200_EINVAL, "protein_groups: protein_offsets decreases at peptide %llu", (unsigned long long)q);
+    const uint64_t NP = p->protein_offsets[n_pep];
+    if (NP >= (uint64_t)INT32_MAX) return fail(SAGE_B200_ELIMIT, "protein_groups: 2^31 - 1 or more protein entries");
+    if (NP && !p->protein_ids) return fail(SAGE_B200_EINVAL, "protein_groups: null protein_ids");
+    for (uint64_t j = 0; j < NP; j++)
+        if (p->protein_ids[j] >= p->n_names)
+            return fail(SAGE_B200_EINVAL, "protein_groups: protein id %u at entry %llu is not below n_names (%llu)", p->protein_ids[j], (unsigned long long)j,
+                        (unsigned long long)p->n_names);
+    std::vector<uint32_t> pep_idx(n);
+    std::vector<uint8_t> label_ok(n);
+    std::vector<uint64_t> cap_off(n + 1, 0);
+    for (uint64_t i = 0; i < n; i++) {
+        pep_idx[i] = rows[i].peptide_idx;
+        if (pep_idx[i] >= n_pep)
+            return fail(SAGE_B200_EINVAL, "protein_groups: row %llu has peptide_idx %u outside the peptide table (%llu peptides)", (unsigned long long)i,
+                        pep_idx[i], (unsigned long long)n_pep);
+        label_ok[i] = rows[i].label != -1;
+        cap_off[i + 1] = cap_off[i] + (p->protein_offsets[pep_idx[i] + 1] - p->protein_offsets[pep_idx[i]]);
+    }
+    for (int k = 0; k < 2; k++)
+        out->peptides[k] = out->proteins[k] = out->meta_peptides[k] = out->groups[k] = out->edges[k] = out->covered[k] = out->forced[k] =
+            out->greedy_picks[k] = out->components[k] = out->largest_component[k] = out->annotated[k] = 0;
+    out->passing = out->entries = 0;
+    out->ms_build[0] = out->ms_build[1] = out->ms_cover[0] = out->ms_cover[1] = out->ms_lookup[0] = out->ms_lookup[1] = out->ms_picked = out->ms_total = 0.0f;
+    if (n == 0) {
+        out->row_group_offsets[0] = 0;
+        return 0;
+    }
+    if (int rc = select_device(device)) return rc;
+    const uint64_t cap = cap_off[n];
+    if (int rc = picked_memory("protein_groups", n, 96 * NP + 48 * p->n_names + 8 * cap + 16 * n_pep)) return rc;
+    const uint32_t N = (uint32_t)n;
+    const bool gen = p->generate_decoys != 0, fma = host_math_variant() != 1;
+    DevArena A;
+    cudaStream_t st = 0;
+    Event ev[9];
+    for (Event& e : ev) CUDA_TRY(e.create());
+    uint32_t *d_pep, *d_poff, *d_pids, *d_count, *d_scratch, *d_csr_len, *d_rows_out;
+    uint8_t *d_label, *d_pdecoy, *d_pass;
+    float *d_q, *d_score;
+    uint64_t *d_cap, *d_out_off;
+    CUDA_TRY(A.alloc(&d_pep, N));
+    CUDA_TRY(A.alloc(&d_poff, n_pep + 1));
+    CUDA_TRY(A.alloc(&d_pids, NP));
+    CUDA_TRY(A.alloc(&d_label, N));
+    CUDA_TRY(A.alloc(&d_pdecoy, n_pep));
+    CUDA_TRY(A.alloc(&d_q, N));
+    CUDA_TRY(A.alloc(&d_score, N));
+    CUDA_TRY(A.alloc(&d_cap, N + 1));
+    CUDA_TRY(A.alloc(&d_pass, N));
+    CUDA_TRY(A.alloc(&d_count, N));
+    CUDA_TRY(A.alloc(&d_scratch, cap));
+    std::vector<uint8_t> pdecoy(n_pep);
+    for (uint64_t q = 0; q < n_pep; q++) pdecoy[q] = P->decoy[q] ? 1 : 0;
+    CUDA_TRY(cudaMemcpyAsync(d_pep, pep_idx.data(), 4ull * N, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_poff, p->protein_offsets, 4 * (n_pep + 1), cudaMemcpyHostToDevice, st));
+    if (NP) CUDA_TRY(cudaMemcpyAsync(d_pids, p->protein_ids, 4 * NP, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_label, label_ok.data(), N, cudaMemcpyHostToDevice, st));
+    if (n_pep) CUDA_TRY(cudaMemcpyAsync(d_pdecoy, pdecoy.data(), n_pep, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_q, peptide_q, 4ull * N, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_score, discriminant_score, 4ull * N, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_cap, cap_off.data(), 8ull * (N + 1), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemsetAsync(d_pass, 0, N, st));
+    CUDA_TRY(cudaMemsetAsync(d_count, 0, 4ull * N, st));
+    CUDA_TRY(cudaEventRecord(ev[0], st));
+    const PgInputs in{N, (uint32_t)n_pep, (uint32_t)p->n_names, d_pep, d_poff, d_pids, d_label, d_pdecoy, d_q, d_cap};
+
+    // generate_protein_groups: pass 1 at threshold.clamp(0, 1) (NaN stays NaN), pass 2 at 1.0; then the fallback
+    PgTable T[2];
+    for (int k = 0; k < 2; k++) {
+        cudaEvent_t e0 = ev[3 * k], e1 = ev[3 * k + 1], e2 = ev[3 * k + 2], e3 = ev[3 * k + 3];
+        if (k == 0) CUDA_TRY(cudaEventRecord(e0, st));
+        const bool run = p->protein_grouping && (k == 1 || p->has_threshold);
+        if (run) {
+            float t = 1.0f;
+            if (k == 0) {
+                t = p->threshold;
+                if (t < 0.0f) t = 0.0f;
+                if (t > 1.0f) t = 1.0f;
+            }
+            if (int rc = pg_pass(st, A, in, t, (uint8_t)(k + 1), T[0].G, d_pass, d_count, d_scratch, &T[k], out, e1, e2)) return rc;
+        } else {
+            CUDA_TRY(cudaEventRecord(e1, st));
+            CUDA_TRY(cudaEventRecord(e2, st));
+        }
+        CUDA_TRY(cudaEventRecord(e3, st));
+    }
+    CUDA_TRY(A.alloc(&d_csr_len, N + 1));
+    CUDA_TRY(A.alloc(&d_out_off, N + 1));
+    CUDA_TRY(cudaMemsetAsync(d_csr_len + N, 0, 4, st));
+    PG_LAUNCH(k_pg_fallback, N, d_pep, N, d_poff, d_pass, d_count, d_csr_len);
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) {
+        return cub::DeviceScan::ExclusiveSum(t, b, d_csr_len, d_out_off, (int)N + 1, st);
+    }));
+    uint64_t n_out = 0;
+    if (int rc = pg_read(st, d_out_off + N, &n_out, 8)) return rc;
+    CUDA_TRY(A.alloc(&d_rows_out, n_out));
+    PG_LAUNCH(k_pg_compact_rows, N, d_cap, d_out_off, d_scratch, d_csr_len, N, d_rows_out);
+
+    // the group tables of both passes, concatenated
+    const uint32_t Gt = T[0].G + T[1].G, Pt = T[0].P + T[1].P;
+    if (2ull * p->n_names + Gt >= 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "protein_groups: 2 * n_names + groups reach 2^32");
+    uint32_t *goff, *members;
+    uint8_t *gdecoy, *gcov;
+    CUDA_TRY(A.alloc(&goff, Gt + 1));
+    CUDA_TRY(A.alloc(&members, Pt));
+    CUDA_TRY(A.alloc(&gdecoy, Gt));
+    CUDA_TRY(A.alloc(&gcov, Gt));
+    CUDA_TRY(cudaMemsetAsync(goff, 0, 4, st));
+    for (int k = 0, g0 = 0, p0 = 0; k < 2; g0 += T[k].G, p0 += T[k].P, k++) {
+        if (!T[k].G) continue;
+        CUDA_TRY(cudaMemcpyAsync(goff + g0 + 1, T[k].goff + 1, 4ull * T[k].G, cudaMemcpyDeviceToDevice, st));
+        PG_LAUNCH(k_pg_add, T[k].G, goff + g0 + 1, T[k].G, (uint32_t)p0);
+        CUDA_TRY(cudaMemcpyAsync(members + p0, T[k].members, 4ull * T[k].P, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(gdecoy + g0, T[k].gdecoy, T[k].G, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(gcov + g0, T[k].lcov, T[k].G, cudaMemcpyDeviceToDevice, st));
+    }
+
+    // picked_protein_group (fdr.rs:192-226): rows with one group string, keyed by it, side Peptide::decoy, Ix = the key
+    uint32_t *rep, *gidx, *gidx_s, *key, *crow, *ckey, *crank, *nsel, m = 0;
+    uint64_t *hash, *hash_s;
+    uint8_t *side, *competes, *cside;
+    float *cscore, *cq, *d_pgq;
+    CUDA_TRY(A.alloc(&rep, Gt));
+    CUDA_TRY(A.alloc(&gidx, Gt));
+    CUDA_TRY(A.alloc(&gidx_s, Gt));
+    CUDA_TRY(A.alloc(&hash, Gt));
+    CUDA_TRY(A.alloc(&hash_s, Gt));
+    PG_LAUNCH(k_pg_group_hash, Gt, goff, members, gdecoy, Gt, gen, hash, gidx);
+    if (Gt) CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, hash, hash_s, gidx, gidx_s, (int)Gt, 0, 64, st); }));
+    PG_LAUNCH(k_pg_group_rep, Gt, goff, members, gdecoy, gen, hash_s, gidx_s, Gt, rep);
+    CUDA_TRY(A.alloc(&key, N));
+    CUDA_TRY(A.alloc(&side, N));
+    CUDA_TRY(A.alloc(&competes, N));
+    CUDA_TRY(A.alloc(&crow, N));
+    CUDA_TRY(A.alloc(&ckey, N));
+    CUDA_TRY(A.alloc(&cside, N));
+    CUDA_TRY(A.alloc(&cscore, N));
+    CUDA_TRY(A.alloc(&crank, N));
+    CUDA_TRY(A.alloc(&cq, N));
+    CUDA_TRY(A.alloc(&d_pgq, N));
+    CUDA_TRY(A.alloc(&nsel, 1));
+    PG_LAUNCH(k_pg_row_keys, N, d_pep, N, d_pass, d_count, d_out_off, d_rows_out, goff, members, gdecoy, rep, d_poff, d_pids, d_pdecoy, gen,
+              (uint32_t)p->n_names, key, side, competes);
+    thrust::counting_iterator<uint32_t> it(0);
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, competes, crow, nsel, (int)N, st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, key, competes, ckey, nsel, (int)N, st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, side, competes, cside, nsel, (int)N, st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_score, competes, cscore, nsel, (int)N, st); }));
+    if (int rc = pg_read(st, nsel, &m, 4)) return rc;
+    if (int rc = picked_competition(st, A, fma, m, ckey, cside, cscore, nullptr, false, crank, cq, &out->entries, &out->passing)) return rc;
+    PG_LAUNCH(k_pg_fill, N, d_pgq, N, 1.0f);
+    PG_LAUNCH(k_pg_scatter_q, m, crow, cq, m, d_pgq);
+    CUDA_TRY(cudaEventRecord(ev[7], st));
+
+    // outputs
+    std::vector<uint32_t> h_goff(Gt + 1);
+    CUDA_TRY(cudaMemcpyAsync(out->num_protein_groups, d_count, 4ull * N, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->protein_group_q, d_pgq, 4ull * N, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->pass, d_pass, N, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out->row_group_offsets, d_out_off, 8ull * (N + 1), cudaMemcpyDeviceToHost, st));
+    if (n_out) CUDA_TRY(cudaMemcpyAsync(out->row_groups, d_rows_out, 4 * n_out, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(h_goff.data(), goff, 4ull * (Gt + 1), cudaMemcpyDeviceToHost, st));
+    if (Pt) CUDA_TRY(cudaMemcpyAsync(out->group_members, members, 4ull * Pt, cudaMemcpyDeviceToHost, st));
+    if (Gt) {
+        CUDA_TRY(cudaMemcpyAsync(out->group_covered, gcov, Gt, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(out->group_decoy, gdecoy, Gt, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA_TRY(cudaStreamSynchronize(st));
+    for (uint32_t g = 0; g <= Gt; g++) out->group_offsets[g] = h_goff[g];
+    for (int k = 0; k < 2; k++) {
+        CUDA_TRY(cudaEventElapsedTime(&out->ms_build[k], ev[3 * k], ev[3 * k + 1]));
+        CUDA_TRY(cudaEventElapsedTime(&out->ms_cover[k], ev[3 * k + 1], ev[3 * k + 2]));
+        CUDA_TRY(cudaEventElapsedTime(&out->ms_lookup[k], ev[3 * k + 2], ev[3 * k + 3]));
+    }
+    CUDA_TRY(cudaEventElapsedTime(&out->ms_picked, ev[6], ev[7]));
+    CUDA_TRY(cudaEventElapsedTime(&out->ms_total, ev[0], ev[7]));
+    return 0;
+}
+
+extern "C" int sage_b200_bipartite_cover(int device, const uint32_t* left, const uint32_t* right, uint64_t n_edges, uint64_t n_left, uint64_t n_right,
+                                         uint8_t* cover) {
+    if ((n_edges && (!left || !right)) || (n_left && !cover)) return fail(SAGE_B200_EINVAL, "bipartite_cover: null argument");
+    if (n_edges > (uint64_t)INT32_MAX || n_left + n_right > (uint64_t)INT32_MAX) return fail(SAGE_B200_ELIMIT, "bipartite_cover: 2^31 - 1 or more edges or nodes");
+    for (uint64_t k = 0; k < n_edges; k++)
+        if (left[k] >= n_left || right[k] >= n_right)
+            return fail(SAGE_B200_EINVAL, "bipartite_cover: edge %llu (%u, %u) is out of range", (unsigned long long)k, left[k], right[k]);
+    if (n_left == 0) return 0;
+    if (int rc = select_device(device)) return rc;
+    if (int rc = picked_memory("bipartite_cover", n_edges, 64 * (n_left + n_right))) return rc;
+    DevArena A;
+    cudaStream_t st = 0;
+    const uint32_t E = (uint32_t)n_edges, G = (uint32_t)n_left, M = (uint32_t)n_right;
+    uint32_t *el, *er;
+    uint8_t* lcov;
+    CUDA_TRY(A.alloc(&el, E));
+    CUDA_TRY(A.alloc(&er, E));
+    CUDA_TRY(A.alloc(&lcov, G));
+    if (E) {
+        CUDA_TRY(cudaMemcpyAsync(el, left, 4ull * E, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(er, right, 4ull * E, cudaMemcpyHostToDevice, st));
+    }
+    PgCoverStats cs;
+    if (int rc = pg_cover(st, A, E, G, M, el, er, lcov, &cs)) return rc;
+    CUDA_TRY(cudaMemcpyAsync(cover, lcov, G, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     return 0;
 }
