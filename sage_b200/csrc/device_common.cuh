@@ -25,7 +25,7 @@ constexpr int SCORE_MIN_CTAS = SAGE_B200_SCORE_MIN_CTAS;   // k_score CTAs per S
 #define SAGE_B200_SCORE_UNROLL 1
 #endif
 #ifndef SAGE_B200_SCORE_MIN_CTAS_SPLIT
-#define SAGE_B200_SCORE_MIN_CTAS_SPLIT 11   /* 40 registers, 30 bytes of spills; measured on cfg2, H100 SXM at 700 W (score phase, ms): 10 -> 1.176, 11 -> 1.141 (12 compiles to the same 40 registers) */
+#define SAGE_B200_SCORE_MIN_CTAS_SPLIT 11   /* 40 registers, no spills; measured on cfg2, H100 SXM at 700 W on the kernel of that time (score phase, ms): 10 -> 1.176, 11 -> 1.141 (12 compiles to the same 40 registers) */
 #endif
 constexpr int SCORE_MIN_CTAS_SPLIT = SAGE_B200_SCORE_MIN_CTAS_SPLIT;   // k_score<true> keeps no records / order / marks in shared memory
 constexpr uint32_t SCORE_UNROLL = SAGE_B200_SCORE_UNROLL;   // tasks per lane and iteration of k_score's phase B (1 or 2; chosen by A/B on cfg2)

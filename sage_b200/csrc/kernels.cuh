@@ -203,25 +203,27 @@ __device__ __forceinline__ void lut_build(const float* arr, uint32_t n, const Lu
 }
 // Same table for an ASCENDING array that carries a +inf sentinel at arr[n]: every thread owns a run of consecutive cells, finds the first
 // one's count by binary search and walks forward for the others (start[c] is non-decreasing in c). O(cells / threads * log n + n) per thread
-// with uniform trip counts; the values are those of lut_build by construction (same edge expression, same `<`).
-__device__ __forceinline__ void lut_build_walk(const float* arr, uint32_t n, const LutParams& L, uint16_t* start, uint32_t t0, uint32_t stride,
-                                               uint32_t cells) {
-    const uint32_t per = (cells + stride - 1) / stride;
+// with uniform trip counts; the values are those of lut_build by construction (same edge expression, same `<`). STRIDE = threads of the block.
+template <uint32_t STRIDE>
+__device__ __forceinline__ void lut_build_walk(const float* arr, uint32_t n, const LutParams& L, uint16_t* start, uint32_t t0, uint32_t cells) {
+    const uint32_t per = (cells + STRIDE - 1) / STRIDE;
     const uint32_t c0 = t0 * per, c1 = min(cells, c0 + per);
     if (!(L.inv_w > 0.0f)) {
         for (uint32_t c = c0; c < c1; c++) start[c] = 0;
         return;
     }
     if (c0 >= c1) return;
+    // lut_edge's cell width, divided once: the compiler keeps the IEEE division (reciprocal, refinement, slow-path test) inside the walk
+    const float w = 1.0f / L.inv_w;
     uint32_t i = 0;
     if (c0 > 0) {
-        const float e = lut_edge(L, c0);
+        const float e = L.base + (float)c0 * w;
         uint32_t hi = n;
         while (i < hi) { const uint32_t m = (i + hi) >> 1; if (arr[m] < e) i = m + 1; else hi = m; }
     }
     start[c0] = (uint16_t)i;
     for (uint32_t c = c0 + 1; c < c1; c++) {
-        const float e = lut_edge(L, c);
+        const float e = L.base + (float)c * w;
         while (arr[i] < e) i++;   // arr[n] = +inf stops the walk
         start[c] = (uint16_t)i;
     }
@@ -1755,7 +1757,10 @@ __shared__ long long s_ph_prev;
 // Shared-memory tile of score_candidates_flat. Static (compile-time addresses: no base-pointer arithmetic in the task loop).
 struct ScoreTile {
     CandHdr hdr[K_MAX + 1];        // candidate headers + sentinel
-    double hkey[K_MAX];            // sort keys of build_features (hyperscore, -inf when below min_matched_peaks)
+    union {
+        double hkey[K_MAX];        // fused: sort keys of build_features (hyperscore, -inf when below min_matched_peaks)
+        uint8_t cand[SCORE_TILE];  // SPLIT: candidate of each task slot of the tile (phase B writes it, the emit reads it for the hits)
+    };
     float term[SCORE_TILE];        // phase B: m/z of a hit; phase B': its ppm term
     float inten[SCORE_TILE];       // phase B: index of the first in-window peak; phase B': matched intensity
     uint32_t mask[SCORE_TILE / 32];
@@ -1765,6 +1770,7 @@ struct ScoreTile {
     unsigned long long hit_base;   // SPLIT: this spectrum's slice of the hit arena
     uint32_t hit_room;             // SPLIT: 0 when the arena is too small (the host re-runs the chunk with the exact size)
 };
+static_assert(SCORE_TILE <= sizeof(double) * K_MAX && K_MAX <= 255, "the slot -> candidate bytes fit in hkey's bytes and hold a candidate index");
 
 // (kind, ion index) of entry ki of a candidate's ion table (kinds concatenated, `nions` ions each): kind << 13 | index (<= 6 kinds, < 255 ions)
 __device__ __forceinline__ uint32_t kind_index(uint32_t ki, uint32_t nions) {
@@ -1876,14 +1882,15 @@ __device__ __forceinline__ void score_candidates_flat(const DbView& db, const Sc
         const uint32_t chunk = (((tn + nwarps - 1) / nwarps) + STEP - 1) & ~(STEP - 1);
         const uint32_t w_lo = min(tn, warp * chunk), w_hi = min(tn, w_lo + chunk);
         uint32_t c = 0, wcount = 0;
-        CandHdr h = S.hdr[0];
-        if (w_lo < w_hi) {   // cursor start: largest c with base[c] <= first task of this lane (binary search over the <= 128 headers)
-            const uint32_t t_first = t0 + min(w_lo + lane, w_hi - 1);
-            uint32_t lo = 0, hi = ncand;   // invariant: base[lo] <= t_first (base[0] = 0), answer in [lo, hi)
-            while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (S.hdr[mid].base <= t_first) lo = mid; else hi = mid; }
-            c = lo;
-            h = S.hdr[c];
+        if (w_lo < w_hi) {   // cursor start, once per warp: the last candidate whose tasks start at or before the warp's first task (bases ascend)
+            const uint32_t t_first = t0 + w_lo;
+            uint32_t n_le = 0;
+#pragma unroll
+            for (uint32_t k = 0; k < (uint32_t)K_MAX; k += 32)
+                n_le += (uint32_t)__popc(__ballot_sync(0xffffffffu, k + lane < ncand && S.hdr[k + lane].base <= t_first));
+            c = n_le - 1;   // base[0] = 0 <= t_first; no lane's first task lies before t_first
         }
+        CandHdr h = S.hdr[c];
         for (uint32_t s0 = w_lo; s0 < w_hi; s0 += STEP) {
             const uint32_t slotA = s0 + lane, slotB = slotA + 32;
             const bool inA = slotA < w_hi, inB = SCORE_UNROLL == 2 && slotB < w_hi;
@@ -1895,11 +1902,13 @@ __device__ __forceinline__ void score_candidates_flat(const DbView& db, const Sc
                 const uint32_t t = t0 + slotA;
                 while (t >= h.next) { c++; h = S.hdr[c]; }   // skips zero-length candidates; the sentinel's next = 2^32 - 1 > t
                 hA = h; fA = t - h.base;
+                if (SPLIT) S.cand[slotA] = (uint8_t)c;   // the candidate of a hit, for the emit (written for every task: one store either way)
             }
             if (inB) {
                 const uint32_t t = t0 + slotB;
                 while (t >= h.next) { c++; h = S.hdr[c]; }
                 hB = h; fB = t - h.base;
+                if (SPLIT) S.cand[slotB] = (uint8_t)c;
             }
             if (FAST) {
                 // f = (kind*nions + idx)*nfc + fc-1, nfc in 1..3: branch-free decode; both loads in flight before the first use
@@ -1985,12 +1994,9 @@ __device__ __forceinline__ void score_candidates_flat(const DbView& db, const Sc
             while (m8) {
                 const uint32_t bit = q8 + (uint32_t)__ffs(m8) - 1;
                 m8 &= m8 - 1;
-                const uint32_t slot = (word << 5) + bit, t = t0 + slot;
-                uint32_t lo = 0, hi = ncand;   // candidate of the task: largest c with base[c] <= t, skipping zero-length ones
-                while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (S.hdr[mid].base <= t) lo = mid; else hi = mid; }
-                while (t >= S.hdr[lo].next) lo++;
-                const CandHdr hh = S.hdr[lo];
-                const uint32_t f = t - hh.base;
+                const uint32_t slot = (word << 5) + bit;
+                const CandHdr hh = S.hdr[S.cand[slot]];
+                const uint32_t f = t0 + slot - hh.base;
                 const uint32_t ki = hh.nfc == 1 ? f : (hh.nfc == 2 ? f >> 1 : f / hh.nfc);
                 if (room) {
                     const unsigned long long g = S.hit_base + hits_before + p + (uint32_t)__popc(wm & ((1u << bit) - 1u));
@@ -2059,9 +2065,10 @@ __device__ __forceinline__ void score_candidates_flat(const DbView& db, const Sc
         uint32_t h0 = inc2 - hcnt;
 #pragma unroll
         for (uint32_t w = 0; w < nwarps; w++) if (w < warp) h0 += S.scan[w];
-        if (tid < ncand) {
+        if (tid < ncand) {   // the candidate's fields are read back from shared memory: kept in registers, they spilled across the tile loop
+            const CandHdr h = S.hdr[tid];
             CandOut co;
-            co.key = key; co.h0 = h0; co.hcnt = hcnt; co.nions = (uint16_t)nions; co.nfc = (uint8_t)nfc; co.plen = (uint8_t)L; co.pad = 0;
+            co.key = cur[tid]; co.h0 = h0; co.hcnt = hcnt; co.nions = h.nions; co.nfc = h.nfc; co.plen = (uint8_t)(h.nions + 1); co.pad = 0;
             so.cand[(size_t)spec * sc.kparam + tid] = co;
         }
         return;
@@ -2128,13 +2135,13 @@ __device__ SB_RARE void annotate_candidate_warp(const DbView& db, const ScorerVi
 // exact binary-search emulation is used for this spectrum.
 __device__ __forceinline__ bool spectrum_lut_setup(const float* masses /*masses[np] == +inf*/, uint32_t np, uint16_t* lut, LutParams& lp) {
     bool bad = np == 0 || np >= 65536;
-    for (uint32_t i = threadIdx.x; i < np; i += blockDim.x) {
+    for (uint32_t i = threadIdx.x; i < np; i += SCORE_THREADS) {
         const float m = masses[i];
         bad |= !(m > 0.0f) || (i > 0 && !(m >= masses[i - 1]));
     }
     if (__syncthreads_or(bad)) return false;
     lp = lut_params(masses[0], masses[np - 1], SPEC_LUT_CELLS);
-    lut_build_walk(masses, np, lp, lut, threadIdx.x, blockDim.x, SPEC_LUT_CELLS);   // masses verified ascending above; masses[np] == +inf (k_score)
+    lut_build_walk<SCORE_THREADS>(masses, np, lp, lut, threadIdx.x, SPEC_LUT_CELLS);   // masses verified ascending above; masses[np] == +inf (k_score)
     __syncthreads();
     return true;
 }
