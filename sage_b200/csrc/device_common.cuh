@@ -189,7 +189,8 @@ struct ReplaySlot { unsigned long long off; uint32_t item, n_list, state /*0 = r
 // Device counters (u64 slots)
 enum { C_TASKS = 0, C_PAGES, C_ENTRIES, C_MATCHED, C_CANDS, C_PEPFLOATS, C_PSMS, C_QUERIES, C_WIDE, C_MAXPOT, C_WORK, C_ERR, C_PEPQ, C_PEPFALLBACK, C_WSLOT, C_WOVERFLOW, C_FRAGS,
        C_NLIST /* bump cursor of the narrow key-list arena */, C_NCTA /* queries listed in cta_items */, C_NLIST_NEED /* arena entries this chunk needs (exact upper bound) */,
-       C_HITS /* bump cursor of the split scorer's hit arena (entries reserved = tasks of the spectrum) */, C_COUNT };
+       C_HITS /* bump cursor of the split scorer's hit arena (entries reserved = tasks of the spectrum) */,
+       C_EXACT /* narrow queries listed in exact_items (>= 2^16 matches: recounted exactly by k_prelim_exact) */, C_COUNT };
 
 struct DbView {
     const uint2* frag;        // {peptide_index, fragment_mz bits}, reference bucket layout
@@ -290,6 +291,7 @@ struct BatchView {
     // small the affected queries produce no hits, the host sees need > capacity in the counters and re-runs the chunk with exact sizes.
     uint32_t* wide_items;             // compacted item ids of the open-search (mode 2) queries, wide_cap entries
     uint32_t* cta_items;              // compacted item ids of the narrow queries counted by a whole CTA (modes 1 and 3), n * qmax entries
+    uint32_t* exact_items;            // item ids of the narrow queries with >= 2^16 matches (k_prelim_exact), n * qmax entries
     ReplaySlot* nslots;               // one per item (narrow kernels); k_setup_queries resets them to "nothing to replay"
     uint32_t wide_cap;
     unsigned long long nlist_cap;     // entries in the narrow key-list arena

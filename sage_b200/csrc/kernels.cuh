@@ -300,8 +300,25 @@ __device__ __forceinline__ uint32_t page_lower_bound_dir(const DbView& db, uint3
 // One (peak, fragment charge) probe of matched_peaks_with_isotope (scoring.rs:358-374) against the fragment index: pages from the
 // bucket minima, per page the PeptideIx window (grid cell + short binary search, then the forward walk that ends exactly at
 // inner_right, database.rs:506-511), exact filter (database.rs:514-534), shared-memory count increment (u16 pairs in cnt32).
+// PreScore::matched is a u16 and the reference's release build does not check overflow: a slot's count wraps, and every match that finds
+// it at 0 (the first, and the first after each wrap) counts the candidate again in scored_candidates (scoring.rs:363-372). The counting
+// kernels keep two u16 counts per 32-bit word, where an even slot's overflow would carry into its neighbour. No slot can pass 2^16 unless
+// the query has >= 2^16 matches in all, a sum the kernels count anyway: such queries are listed for k_prelim_exact, which counts their
+// window again with one u32 per slot and rewrites their keys, so the common path keeps its registers.
+constexpr uint32_t EXACT_TRIGGER = 0x10000u;
+constexpr uint32_t EXACT_SEG = NARROW_CAP / 2;   // window slots k_prelim_exact counts per pass
+// One match of window slot idx: a u16 half of a packed word, or (EXACT) a u32 per slot of the segment [s0, s0 + EXACT_SEG).
+template <bool EXACT>
+__device__ __forceinline__ void count_match(uint32_t* cnt32, uint32_t idx, uint32_t s0) {
+    if (EXACT) {
+        if (idx - s0 < EXACT_SEG) atomicAdd(&cnt32[idx - s0], 1u);
+    } else {
+        atomicAdd(&cnt32[idx >> 1], 1u << ((idx & 1) * 16));
+    }
+}
+template <bool EXACT = false>
 __device__ __forceinline__ void index_probe(const DbView& db, const QueryDesc& q, float flo, float fhi, uint32_t* cnt32, uint32_t& matched, uint32_t& pages,
-                                            uint32_t& entries) {
+                                            uint32_t& entries, uint32_t s0 = 0) {
     uint32_t bl, br;
     bucket_range(db, flo, fhi, bl, br);
     for (uint32_t page = bl; page < br; page++) {
@@ -319,8 +336,7 @@ __device__ __forceinline__ void index_probe(const DbView& db, const QueryDesc& q
             if (f.x > q.pre_hi) break;
             const float fmz = __uint_as_float(f.y);
             if (f.x >= q.eff_lo && f.x <= q.eff_hi && fmz >= flo && fmz <= fhi) {
-                const uint32_t idx = f.x - q.pre_lo;
-                atomicAdd(&cnt32[idx >> 1], 1u << ((idx & 1) * 16));
+                count_match<EXACT>(cnt32, f.x - q.pre_lo, s0);
                 matched++;
             }
         }
@@ -356,8 +372,9 @@ __device__ __forceinline__ uint32_t narrow_start_cell(const NarrowIndexView& nv,
     const float tt = (flo - nv.base) * nv.inv_w;
     return tt > 1.0f ? (uint32_t)((int)fminf(tt, (float)(nv.cells - 1)) - 1) : 0u;
 }
+template <bool EXACT = false>
 __device__ __forceinline__ void block_probe_warp(const NarrowIndexView& nv, const QueryDesc& q, uint32_t b0, uint32_t b1, bool act, float flo, float fhi,
-                                                 uint32_t* cnt32, uint32_t& matched) {
+                                                 uint32_t* cnt32, uint32_t& matched, uint32_t s0 = 0) {
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t c = narrow_start_cell(nv, flo);
     for (uint32_t blk = b0; blk <= b1; blk++) {   // warp-uniform: b0, b1 belong to the query
@@ -386,8 +403,7 @@ __device__ __forceinline__ void block_probe_warp(const NarrowIndexView& nv, cons
                     stop |= m[j] > fhi;
                     const uint32_t pid = pep0 + o[j];
                     if (!stop && m[j] >= flo && pid >= q.eff_lo && pid <= q.eff_hi) {
-                        const uint32_t idx = pid - q.pre_lo;
-                        atomicAdd(&cnt32[idx >> 1], 1u << ((idx & 1) * 16));
+                        count_match<EXACT>(cnt32, pid - q.pre_lo, s0);
                         matched++;
                     }
                 }
@@ -409,8 +425,7 @@ __device__ __forceinline__ void block_probe_warp(const NarrowIndexView& nv, cons
                     stop = fmz > hi_s;
                     if (!stop && fmz >= lo_s) {
                         if (pid >= q.eff_lo && pid <= q.eff_hi) {
-                            const uint32_t idx = pid - q.pre_lo;
-                            atomicAdd(&cnt32[idx >> 1], 1u << ((idx & 1) * 16));
+                            count_match<EXACT>(cnt32, pid - q.pre_lo, s0);
                             matched++;   // counted on the lane that saw the entry: the warp sums `matched` afterwards
                         }
                     }
@@ -597,6 +612,7 @@ __device__ __forceinline__ void narrow_cta_query(const DbView& db, const ScorerV
         if (tid == 0) {
             h->n = n; h->default_run = 0; h->matched_peaks = matched_total; h->scored_candidates = nzt;
             slot->off = 0; slot->item = item; slot->n_list = 0; slot->state = 1; slot->k = k;
+            if (matched_total >= EXACT_TRIGGER) b.exact_items[atomicAdd(b.counters + C_EXACT, 1ull)] = item;
         }
         return;
     }
@@ -636,6 +652,7 @@ __device__ __forceinline__ void narrow_cta_query(const DbView& db, const ScorerV
     if (tid == 0) {
         h->n = k; h->default_run = 0; h->matched_peaks = matched_total; h->scored_candidates = nzt;
         slot->off = loff; slot->item = item; slot->n_list = wbase; slot->state = 0; slot->k = k;
+        if (matched_total >= EXACT_TRIGGER) b.exact_items[atomicAdd(b.counters + C_EXACT, 1ull)] = item;
     }
 }
 
@@ -739,6 +756,82 @@ __global__ void __launch_bounds__(WARPQ_WARPS * 32, WARPQ_MIN_CTAS) k_prelim_nar
     if (lane == 0) {
         h->n = k; h->default_run = 0; h->matched_peaks = matched; h->scored_candidates = nzc;
         if (n > k) { slot->off = loff; slot->n_list = wbase; slot->state = 0; slot->k = k; }
+        if (matched >= EXACT_TRIGGER) b.exact_items[atomicAdd(b.counters + C_EXACT, 1ull)] = item;
+    }
+}
+
+// The narrow queries with >= 2^16 matches (EXACT_TRIGGER), one CTA each: the window again in segments of EXACT_SEG slots with one u32 count
+// per slot, then the keys the counting kernel wrote are rewritten with the reference's wrapped u16 counts, in the same dense order (the
+// literal first k slots, then every later slot the query touched), and scored_candidates becomes the sum of ceil(count / 2^16). A slot whose
+// count wrapped to exactly 0 keeps its PeptideIx: the reference set it when the count was 0, so it is scored, not PreScore::default().
+__global__ void __launch_bounds__(PRELIM_THREADS) k_prelim_exact(DbView db, ScorerView sc, BatchView b, uint64_t* nlist, NarrowIndexView nv) {
+    __shared__ uint32_t cnt32[EXACT_SEG];
+    __shared__ uint32_t s_warp[PRELIM_THREADS / 32];
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = PRELIM_THREADS / 32;
+    const uint32_t total = (uint32_t)min(b.counters[C_EXACT], (unsigned long long)b.n * sc.qmax);
+    for (uint32_t it = blockIdx.x; it < total; it += gridDim.x) {
+        const uint32_t item = b.exact_items[it];
+        const uint32_t s = item / sc.qmax;
+        const QueryDesc q = b.queries[item];
+        const uint32_t p0 = b.peak_off[s], np = b.peak_off[s + 1] - p0;
+        const uint32_t nfc = q.nfc, ntask = np * nfc;
+        const uint32_t n = q.potential, k = min(n, sc.kparam);
+        ReplaySlot* const slot = b.nslots + item;
+        uint64_t* const dst = n <= k ? b.hit_keys + (size_t)item * sc.kparam : nlist + slot->off;
+        uint32_t nzc = 0, wbase = k;
+        for (uint32_t s0 = 0; s0 < n; s0 += EXACT_SEG) {
+            for (uint32_t i = tid; i < EXACT_SEG; i += PRELIM_THREADS) cnt32[i] = 0;
+            __syncthreads();
+            uint32_t dm = 0, dp = 0, de = 0;
+            if (nv.mz != nullptr) {
+                const uint32_t blk0 = q.pre_lo / nv.block, blk1 = min(q.pre_hi, db.n_pep - 1) / nv.block;
+                for (uint32_t t0 = warp * 32; t0 < ntask; t0 += PRELIM_THREADS) {
+                    const uint32_t t = t0 + lane;
+                    const bool act = t < ntask;
+                    float flo = 0.0f, fhi = 0.0f;
+                    if (act) {
+                        const uint32_t p = t / nfc, fc = t - p * nfc + 1;
+                        tol_bounds(sc.fragment_tol, __fmul_rn(__ldg(b.masses + p0 + p), (float)fc), flo, fhi);   // scoring.rs:360
+                    }
+                    block_probe_warp<true>(nv, q, blk0, blk1, act, flo, fhi, cnt32, dm, s0);
+                }
+            } else {
+                for (uint32_t t = tid; t < ntask; t += PRELIM_THREADS) {
+                    const uint32_t p = t / nfc, fc = t - p * nfc + 1;
+                    float flo, fhi;
+                    tol_bounds(sc.fragment_tol, __fmul_rn(__ldg(b.masses + p0 + p), (float)fc), flo, fhi);   // scoring.rs:360
+                    index_probe<true>(db, q, flo, fhi, cnt32, dm, dp, de, s0);
+                }
+            }
+            __syncthreads();
+            const uint32_t s1 = min(n, s0 + EXACT_SEG);
+            for (uint32_t base = s0; base < s1; base += PRELIM_THREADS) {   // uniform trip count: every thread reaches the barriers
+                const uint32_t i = base + tid;
+                const uint32_t c = i < s1 ? cnt32[i - s0] : 0u;
+                nzc += (c >> 16) + ((c & 0xFFFFu) != 0u);   // ceil(c / 2^16)
+                const uint64_t key = c ? prescore_key(c & 0xFFFFu, q.pre_lo + i, q.charge, q.iso) : PRESCORE_DEFAULT;
+                if (i < k) dst[i] = key;   // k <= EXACT_SEG: the literal slots lie in the first segment
+                const bool emit = i >= k && c != 0;
+                const uint32_t ball = __ballot_sync(0xffffffffu, emit);
+                if (lane == 0) s_warp[warp] = __popc(ball);
+                __syncthreads();
+                uint32_t off = 0, tot = 0;
+                for (uint32_t w = 0; w < nwarps; w++) {
+                    const uint32_t x = s_warp[w];
+                    if (w < warp) off += x;
+                    tot += x;
+                }
+                if (emit) dst[wbase + off + __popc(ball & ((1u << lane) - 1))] = key;
+                wbase += tot;
+                __syncthreads();
+            }
+        }
+        const uint32_t nzt = block_sum_u32(nzc, s_warp);
+        if (tid == 0) {
+            b.hits[item].scored_candidates = nzt;
+            if (n > k) slot->n_list = wbase;
+        }
+        __syncthreads();
     }
 }
 
@@ -926,10 +1019,13 @@ __global__ void __launch_bounds__(WIDE_THREADS, WIDE_CTAS) k_prelim_wide(DbView 
                     const float flo = S.u.blk.flo[j];
                     uint32_t lo = blen, hi = blen;   // NaN bounds: empty run
                     if (flo == flo && S.u.blk.fhi[j] == S.u.blk.fhi[j]) {
-                        const float tt = (flo - wv.base) * wv.inv_w;
-                        const int c = tt > 1.0f ? (int)fminf(tt, (float)(wv.cells - 1)) - 1 : 0;
-                        lo = __ldg(lutb + c);
-                        hi = __ldg(lutb + min((uint32_t)c + 3u, wv.cells));
+                        lo = 0;
+                        if (wv.inv_w > 0.0f) {
+                            const float tt = (flo - wv.base) * wv.inv_w;
+                            const int c = tt > 1.0f ? (int)fminf(tt, (float)(wv.cells - 1)) - 1 : 0;
+                            lo = __ldg(lutb + c);
+                            hi = __ldg(lutb + min((uint32_t)c + 3u, wv.cells));
+                        }   // else no LUT (an index with m/z <= 0 or a degenerate range): the bisection runs over the whole block
                         while (lo < hi) {
                             const uint32_t mid = lo + ((hi - lo) >> 1);
                             if (__uint_as_float(__ldg(&ent[mid].y)) < flo) lo = mid + 1; else hi = mid;
@@ -2894,7 +2990,8 @@ __global__ void k_window_sample(DbView db, Tol ptol, uint32_t samples, unsigned 
     const uint32_t a = pep_partition(db, lo, false), b = pep_partition(db, hi, true);
     atomicAdd(sum, (unsigned long long)(b > a ? b - a : 0u));
 }
-// rng[0] = min, rng[1] = max of the m/z bit patterns (fragment m/z are positive floats: bit order == value order)
+// rng[0] = min, rng[1] = max of the m/z bit patterns. Bit order is value order only for positive floats: an index holding m/z <= 0 yields a
+// range the host treats as degenerate (set_mz_cells: no LUT, every search covers the whole block).
 __global__ void k_frag_mz_range(uint64_t n_frag, const uint2* frag, uint32_t* rng) {
     uint32_t lo = 0xFFFFFFFFu, hi = 0u;
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_frag; i += (uint64_t)gridDim.x * blockDim.x) {

@@ -1363,8 +1363,9 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
         if ((rc = L.d_wlist.reserve((size_t)C.wide_cap * WIDE_LMAX * 8))) return rc;
         if ((rc = L.d_wslots.reserve((size_t)C.wide_cap * sizeof(WideSlot)))) return rc;
     }
-    if ((rc = L.d_citems.reserve(4 * C.nitems))) return rc;
+    if ((rc = L.d_citems.reserve(8 * C.nitems))) return rc;
     bv.cta_items = L.d_citems.as<uint32_t>();
+    bv.exact_items = bv.cta_items + C.nitems;
     bv.nslots = L.d_nslots.as<ReplaySlot>();
     bv.wide_items = L.d_witems.as<uint32_t>();
     bv.wide_cap = C.wide_cap;
@@ -1402,12 +1403,16 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
     k_prelim_narrow<<<(unsigned)std::min<uint64_t>(C.nitems, (uint64_t)db->sm_count * PRELIM_CTAS), PRELIM_THREADS, pep_smem, st>>>(db->v, svq, bv, C.pmax, L.d_nlist.as<uint64_t>(),
                                                                                                                          S->narrow_cta ? nv : NarrowIndexView{});
     CUDA_TRY(cudaGetLastError());
+    // the rare queries with >= 2^16 matches, listed by both counting kernels: exact wrapped u16 counts (kernels.cuh: EXACT_TRIGGER). Usually
+    // there are none, so the grid is small: the launch costs one short kernel, and a listed query is a whole pass over its window anyway
+    k_prelim_exact<<<(unsigned)std::min<uint64_t>(C.nitems, 8), PRELIM_THREADS, 0, st>>>(db->v, svq, bv, L.d_nlist.as<uint64_t>(), nv);
+    CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(L.ev_count_end, st));   // narrow counting kernels done (the open-search kernel, when present, is timed with the replays)
     // narrow windows (<= NARROW_CAP peptides): 32-bit heap keys, half the shared memory
     k_replay<true><<<(unsigned)((C.nitems + REPLAY_THREADS - 1) / REPLAY_THREADS), REPLAY_THREADS, rsm / 2, st>>>(sv, bv, L.d_nlist.as<uint64_t>(), L.d_nslots.as<ReplaySlot>(),
                                                                                                                  (uint32_t)C.nitems, nullptr, n);
     CUDA_TRY(cudaGetLastError());
-    launches += 3;
+    launches += 4;
     if (C.wide_cap) {
         const int ctas = (int)std::min<uint64_t>((uint64_t)db->sm_count * WIDE_CTAS, C.wide_cap);
         const WideIndexView wv = db_wide_index(db, sv.wide_tile);   // built on first use (the first open-search chunk of a scorer is a re-run anyway)
