@@ -489,6 +489,61 @@ int sage_b200_protein_groups(int device, const sage_b200_peptides* peptides, con
 int sage_b200_bipartite_cover(int device, const uint32_t* left, const uint32_t* right, uint64_t n_edges, uint64_t n_left, uint64_t n_right,
                               uint8_t* cover);
 
+/* ---------------------------------------------------------------------------------------------------------------------------------------------
+ * Digest (Parameters::digest, database.rs:162-258): FASTA text -> the sorted, merged peptide table with its protein lists, in PeptideIx order.
+ * The FASTA is parsed on the host (fasta.rs:14-56, one pass); cleavage, windows, per-protein de-duplication, grouping, modification
+ * enumeration, the sort and the merge run on the device. The table is the reference's bit for bit under the definitions of DESIGN.md §14;
+ * the parameters are normalised as Builder does: max_variable_mods is raised to 1, invalid mod specs are skipped, static specs are ordered
+ * by spec (a repeated spec: the last mass wins), variable (spec, mass) pairs are stable-sorted by spec.
+ * create -> get_info (the sizes) -> export (caller-allocated arrays) -> destroy.
+ */
+typedef struct sage_b200_digest sage_b200_digest;
+
+/* Builder (database.rs:17-41) without the index fields. */
+typedef struct {
+    uint8_t missed_cleavages;
+    uint64_t min_len, max_len;                /* max_len <= 255 (the library's peptide-length limit) */
+    const char* cleave_at;                    /* "" = non-specific (missed cleavages taken as 0), "$" = no cleavage; NULL = "" */
+    const char* restrict_;                    /* NULL = "" */
+    uint8_t c_terminal, semi_enzymatic;
+    float peptide_min_mass, peptide_max_mass; /* inclusive */
+    const char* const* static_specs;          /* "C", "^", "[", "$", "]", "^Q", ...; n_static entries */
+    const float* static_masses;
+    uint64_t n_static;
+    const char* const* variable_specs;        /* one entry per (spec, mass) */
+    const float* variable_masses;
+    uint64_t n_variable;
+    uint64_t max_variable_mods;               /* <= 8 */
+    const char* decoy_tag;                    /* NULL = "rev_" */
+    uint8_t generate_decoys;
+} sage_b200_digest_params;
+
+typedef struct {
+    uint64_t n_peptides, n_residues, n_protein_refs, n_names, name_bytes;   /* the export's array sizes */
+    uint64_t n_proteins;              /* proteins kept by the FASTA parser */
+    uint64_t n_windows, n_groups, n_candidates, n_rows;   /* length-filtered windows, group_digests groups, (group, combination) candidates, rows before the merge */
+    uint64_t device_bytes;            /* HBM the handle holds (the output table) */
+    uint64_t peak_device_bytes;       /* HBM the call held at its peak (temporaries and output) */
+    float ms_parse;                   /* host wall clock of the FASTA parse and the parameter normalisation */
+    float ms_upload, ms_sites, ms_windows, ms_group, ms_expand, ms_sort, ms_merge, ms_total;   /* CUDA-event stage times */
+    float ms_wall;                    /* host wall clock of the create call */
+} sage_b200_digest_info;
+
+/* EINVAL for a null fasta (with fasta_len > 0), params or out, a null spec array with a nonzero count, or a non-finite mod mass; ELIMIT for
+ * max_len > 255, max_variable_mods > 8, 2^32 or more residues, 2^32 - 2 or more windows, candidates or output rows, more than 65535
+ * variable sites on one peptide, or when the work buffers do not fit the device's free memory (checked before each stage allocates; the
+ * message names the byte count). An empty FASTA, or one whose every peptide is filtered, gives an empty table. */
+int sage_b200_digest_create(int device, const char* fasta, uint64_t fasta_len, const sage_b200_digest_params* params, sage_b200_digest** out);
+int sage_b200_digest_get_info(const sage_b200_digest* d, sage_b200_digest_info* info);
+/* Any pointer may be NULL. residue_offsets / protein_offsets: [n_peptides + 1]; sequence / modifications: [n_residues]; nterm, cterm (NaN =
+ * None), monoisotopic, decoy, missed_cleavages, semi_enzymatic: [n_peptides]; protein_ids: [n_protein_refs], ascending within a peptide, each
+ * the rank of the accession in the names table (a repeated accession stays repeated); name_offsets: [n_names + 1] into name_bytes
+ * [name_bytes]: the distinct accessions in byte order. */
+int sage_b200_digest_export(const sage_b200_digest* d, uint32_t* residue_offsets, uint8_t* sequence, float* modifications, float* nterm, float* cterm,
+                            float* monoisotopic, uint8_t* decoy, uint8_t* missed_cleavages, uint8_t* semi_enzymatic, uint32_t* protein_offsets,
+                            uint32_t* protein_ids, uint64_t* name_offsets, char* name_bytes);
+void sage_b200_digest_destroy(sage_b200_digest* d);
+
 /* Page-locked host buffers: spectra/feature arrays placed here are copied by DMA without a staging memcpy. */
 void* sage_b200_host_alloc(size_t bytes);
 /* The same for a batch sage_b200_score_batch_multi cuts into n_devices contiguous blocks: the i-th of n equal parts of the buffer is placed on the

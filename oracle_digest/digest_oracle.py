@@ -1,0 +1,106 @@
+"""ctypes binding of the CPU oracle's digest with bulk accessors (oracle_digest/digest_oracle.cpp, which compiles oracle/sage_oracle.cpp).
+
+TEST INFRASTRUCTURE ONLY: imported by tests/, __graft_entry__ and tools/bench_digest.py. Never imported by the sage_b200 package.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import os
+import subprocess
+
+import numpy as np
+
+_HERE = os.path.dirname(os.path.abspath(__file__))
+_SRC = os.path.join(_HERE, "digest_oracle.cpp")
+_DEP = os.path.join(os.path.dirname(_HERE), "oracle", "sage_oracle.cpp")
+_SO = os.path.join(_HERE, "_build", "libdigest_oracle.so")
+# the oracle's own flags (oracle/Makefile): no FMA contraction, no fast-math
+CXXFLAGS = ["-O3", "-march=x86-64-v3", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-fopenmp", "-fPIC", "-shared", "-Wall",
+            "-Wno-unused-function"]
+
+_lib = None
+
+
+def build(force: bool = False) -> str:
+    if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < max(os.path.getmtime(_SRC), os.path.getmtime(_DEP)):
+        os.makedirs(os.path.dirname(_SO), exist_ok=True)
+        env = dict(os.environ)
+        env.pop("CXX", None)
+        subprocess.check_call(["/usr/bin/g++"] + CXXFLAGS + ["-o", _SO, _SRC], env=env)
+    return _SO
+
+
+def lib():
+    global _lib
+    if _lib is None:
+        build()
+        _lib = C.CDLL(_SO)
+        _lib.sod_digest.restype = C.c_void_p
+        for f in ("sod_free", "sod_sizes", "sod_export", "sod_db_sizes", "sod_db_export"):
+            getattr(_lib, f).restype = None
+    return _lib
+
+
+def _build_params(kw: dict, keep: list):
+    from oracle.oracle import KIND, BuildParams
+    bp = BuildParams()
+    bp.bucket_size = kw.get("bucket_size", 8192)
+    bp.missed_cleavages = kw.get("missed_cleavages", 0)
+    bp.min_len, bp.max_len = kw.get("min_len", 5), kw.get("max_len", 50)
+    bp.cleave_at, bp.restrict_ = kw.get("cleave_at", "KR").encode(), kw.get("restrict", "P").encode()
+    bp.c_terminal, bp.semi_enzymatic = int(kw.get("c_terminal", True)), int(kw.get("semi_enzymatic", False))
+    bp.peptide_min_mass, bp.peptide_max_mass = kw.get("peptide_min_mass", 500.0), kw.get("peptide_max_mass", 5000.0)
+    kinds = (C.c_uint8 * 2)(KIND["b"], KIND["y"])
+    bp.ion_kinds, bp.n_kinds, bp.min_ion_index = kinds, 2, 2
+    sm = list((kw.get("static_mods") or {}).items())
+    sspec = (C.c_char_p * max(1, len(sm)))(*[k.encode() for k, _ in sm])
+    smass = (C.c_float * max(1, len(sm)))(*[v for _, v in sm])
+    bp.static_mod_specs, bp.static_mod_masses, bp.n_static = sspec, smass, len(sm)
+    vm = [(k, m) for k, ms in (kw.get("variable_mods") or {}).items() for m in ms]
+    vspec = (C.c_char_p * max(1, len(vm)))(*[k.encode() for k, _ in vm])
+    vmass = (C.c_float * max(1, len(vm)))(*[v for _, v in vm])
+    bp.var_mod_specs, bp.var_mod_masses, bp.n_var = vspec, vmass, len(vm)
+    bp.max_variable_mods = kw.get("max_variable_mods", 2)
+    bp.decoy_tag = kw.get("decoy_tag", "rev_").encode()
+    bp.generate_decoys = int(kw.get("generate_decoys", True))
+    keep += [kinds, sspec, smass, vspec, vmass]
+    return bp
+
+
+def _table(sizes_fn, export_fn, h) -> dict:
+    sz = np.zeros(4, np.uint64)
+    sizes_fn(h, sz.ctypes.data_as(C.c_void_p))
+    n, nres, nref, nb = (int(x) for x in sz)
+    t = dict(seq_off=np.empty(n + 1, np.uint32), seq=np.empty(nres, np.uint8), mods=np.empty(nres, np.float32), nterm=np.empty(n, np.float32),
+             cterm=np.empty(n, np.float32), mono=np.empty(n, np.float32), decoy=np.empty(n, np.uint8), missed=np.empty(n, np.uint8),
+             semi=np.empty(n, np.uint8), prot_off=np.empty(n + 1, np.uint64), name_off=np.empty(nref + 1, np.uint64), names=np.empty(max(nb, 1), np.uint8))
+    export_fn(h, *[t[k].ctypes.data_as(C.c_void_p) for k in ("seq_off", "seq", "mods", "nterm", "cterm", "mono", "decoy", "missed", "semi", "prot_off",
+                                                             "name_off", "names")])
+    return t
+
+
+def digest(fasta, **kw) -> dict:
+    """The oracle's digest() of FASTA text (str or bytes) with OracleDB.from_fasta's keywords: the peptide table in PeptideIx order with
+    semi_enzymatic, and every peptide's proteins as a CSR of name strings (prot_off into name_off into names)."""
+    text = fasta.encode() if isinstance(fasta, str) else bytes(fasta)
+    keep: list = []
+    bp = _build_params(kw, keep)
+    L = lib()
+    h = C.c_void_p(L.sod_digest(C.c_char_p(text), C.byref(bp)))
+    try:
+        return _table(L.sod_sizes, L.sod_export, h)
+    finally:
+        L.sod_free(h)
+
+
+def db_table(db) -> dict:
+    """The same table of a database the oracle built from FASTA (OracleDB.from_fasta)."""
+    L = lib()
+    return _table(L.sod_db_sizes, L.sod_db_export, db.h)
+
+
+def protein_lists(t: dict) -> list:
+    """Each peptide's proteins as a list of bytes, in stored order."""
+    raw = t["names"].tobytes()
+    no, po = t["name_off"], t["prot_off"]
+    return [[raw[no[j]:no[j + 1]] for j in range(po[i], po[i + 1])] for i in range(len(po) - 1)]

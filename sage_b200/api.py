@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import time
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -92,6 +93,7 @@ EXPORTED_SYMBOLS = [
     "sage_b200_lfq_create", "sage_b200_lfq_add_ms1", "sage_b200_lfq_integrate", "sage_b200_lfq_get_info", "sage_b200_lfq_export", "sage_b200_lfq_destroy",
     "sage_b200_spectrum_fdr", "sage_b200_kde_build", "sage_b200_device_math", "sage_b200_predict_rt",
     "sage_b200_picked_fdr", "sage_b200_picked_precursor", "sage_b200_competition_keys", "sage_b200_protein_groups", "sage_b200_bipartite_cover",
+    "sage_b200_digest_create", "sage_b200_digest_get_info", "sage_b200_digest_export", "sage_b200_digest_destroy",
 ]
 
 _lib = None
@@ -120,6 +122,7 @@ def load_library(build: bool = True):
     lib.sage_b200_db_destroy.argtypes = [C.c_void_p]
     lib.sage_b200_scorer_destroy.argtypes = [C.c_void_p]
     lib.sage_b200_lfq_destroy.argtypes = [C.c_void_p]
+    lib.sage_b200_digest_destroy.argtypes = [C.c_void_p]
     _lib = lib
     return lib
 
@@ -415,6 +418,19 @@ class IndexedDatabase:
         _check(load_library().sage_b200_db_build(C.byref(cp), C.c_uint64(int(bucket_size)), _ptr(kinds), C.c_uint64(len(kinds)),
                                                  C.c_uint64(int(min_ion_index)), C.c_int(device), C.byref(h)))
         return IndexedDatabase(h.value, peptides)
+
+    @staticmethod
+    def from_fasta(fasta, *, bucket_size=8192, ion_kinds=("b", "y"), min_ion_index=2, device=0, **digest_args) -> "IndexedDatabase":
+        """Builder::make_parameters + Parameters::build (database.rs:96-115, 260) from FASTA text: digest_fasta, then build_from_peptides on
+        the digested table. `bucket_size` is rounded up to a power of two. The digest result stays on the db as `.digest` (protein lists,
+        cterm, semi_enzymatic for picked_fdr, protein_groups and the writers)."""
+        if isinstance(bucket_size, bool) or not isinstance(bucket_size, (int, np.integer)) or not 1 <= int(bucket_size) <= 1 << 30:
+            raise ValueError(f"bucket_size must be an integer in 1..2^30, got {bucket_size!r}")
+        bs = 1 << (int(bucket_size) - 1).bit_length()
+        d = digest_fasta(fasta, device=device, **digest_args)
+        db = IndexedDatabase.build_from_peptides(d.peptides, bucket_size=bs, ion_kinds=ion_kinds, min_ion_index=min_ion_index, device=device)
+        db.digest = d
+        return db
 
     def export_index(self):
         nf, nb = self.info["n_fragments"], self.info["n_buckets"]
@@ -1035,3 +1051,98 @@ def bipartite_cover(left, right, n_left: int, n_right: int, device: int = 0) -> 
     _check(load_library().sage_b200_bipartite_cover(C.c_int(device), _ptr(lft), _ptr(rgt), C.c_uint64(len(lft)), C.c_uint64(int(n_left)),
                                                     C.c_uint64(int(n_right)), _ptr(cover)))
     return cover.astype(bool)
+
+
+# ------------------------------------------------------------------------------------------------ digest (database.rs:162-258)
+class CDigestParams(C.Structure):
+    _fields_ = [("missed_cleavages", C.c_uint8), ("min_len", C.c_uint64), ("max_len", C.c_uint64), ("cleave_at", C.c_char_p), ("restrict_", C.c_char_p),
+                ("c_terminal", C.c_uint8), ("semi_enzymatic", C.c_uint8), ("peptide_min_mass", C.c_float), ("peptide_max_mass", C.c_float),
+                ("static_specs", C.c_void_p), ("static_masses", C.c_void_p), ("n_static", C.c_uint64),
+                ("variable_specs", C.c_void_p), ("variable_masses", C.c_void_p), ("n_variable", C.c_uint64),
+                ("max_variable_mods", C.c_uint64), ("decoy_tag", C.c_char_p), ("generate_decoys", C.c_uint8)]
+
+
+DIGEST_COUNTS = ("n_peptides", "n_residues", "n_protein_refs", "n_names", "name_bytes", "n_proteins", "n_windows", "n_groups", "n_candidates", "n_rows",
+                 "device_bytes", "peak_device_bytes")
+DIGEST_TIMES = ("ms_parse", "ms_upload", "ms_sites", "ms_windows", "ms_group", "ms_expand", "ms_sort", "ms_merge", "ms_total", "ms_wall")
+
+
+class CDigestInfo(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in DIGEST_COUNTS] + [(n, C.c_float) for n in DIGEST_TIMES]
+
+
+@dataclass
+class DigestResult:
+    """The digested peptide table (one row per PeptideIx) and what only the digest knows: cterm (NaN = None), semi_enzymatic, and each
+    peptide's proteins as a CSR of ids (protein_offsets, protein_ids) into `names`, the distinct accessions in byte order (id = rank).
+    Ids are ascending within a peptide and a repeated accession stays repeated, as Peptide::proteins after its sort."""
+    peptides: Peptides
+    cterm: np.ndarray
+    semi_enzymatic: np.ndarray
+    protein_offsets: np.ndarray
+    protein_ids: np.ndarray
+    names: list
+    info: dict
+
+    @property
+    def n_proteins(self) -> np.ndarray:
+        """Peptide::proteins.len() per peptide, as picked_fdr takes it."""
+        return np.diff(self.protein_offsets).astype(np.uint32)
+
+    @property
+    def protein(self) -> np.ndarray:
+        """The id of each peptide's first protein (0 for a peptide without proteins): picked_fdr reads it where n_proteins == 1."""
+        ids = np.append(self.protein_ids, np.uint32(0))
+        return np.where(self.n_proteins > 0, ids[self.protein_offsets[:-1]], 0).astype(np.uint32)
+
+    def proteins(self, i: int) -> list:
+        """Peptide::proteins of peptide i as accessions (target names; the decoy tag is added when output is formatted)."""
+        return [self.names[j] for j in self.protein_ids[self.protein_offsets[i]:self.protein_offsets[i + 1]]]
+
+
+def _spec_arrays(mods: dict | None, keep: list, variable: bool):
+    items = [(k, m) for k, ms in (mods or {}).items() for m in (ms if variable else [ms])]
+    specs = (C.c_char_p * max(1, len(items)))(*[k.encode() for k, _ in items])
+    masses = np.array([m for _, m in items] or [0.0], np.float32)
+    keep += [specs, masses]
+    return C.cast(specs, C.c_void_p), _ptr(masses), len(items)
+
+
+def digest_fasta(fasta, *, missed_cleavages=0, min_len=5, max_len=50, cleave_at="KR", restrict="P", c_terminal=True, semi_enzymatic=False,
+                 peptide_min_mass=500.0, peptide_max_mass=5000.0, static_mods=None, variable_mods=None, max_variable_mods=2, decoy_tag="rev_",
+                 generate_decoys=True, device=0) -> DigestResult:
+    """Parameters::digest (database.rs:162-258) on the device: FASTA text (str or bytes) to the sorted, merged peptide table. Keywords and
+    defaults are Builder::default()'s. static_mods maps a spec ("C", "^", "[Q", ...) to a mass, variable_mods a spec to a list of masses."""
+    text = fasta.encode() if isinstance(fasta, str) else bytes(fasta)
+    keep: list = []
+    p = CDigestParams()
+    p.missed_cleavages, p.min_len, p.max_len = int(missed_cleavages), int(min_len), int(max_len)
+    p.cleave_at, p.restrict_ = cleave_at.encode(), restrict.encode()
+    p.c_terminal, p.semi_enzymatic = int(bool(c_terminal)), int(bool(semi_enzymatic))
+    p.peptide_min_mass, p.peptide_max_mass = float(peptide_min_mass), float(peptide_max_mass)
+    p.static_specs, p.static_masses, p.n_static = _spec_arrays(static_mods, keep, False)
+    p.variable_specs, p.variable_masses, p.n_variable = _spec_arrays(variable_mods, keep, True)
+    p.max_variable_mods, p.decoy_tag, p.generate_decoys = int(max_variable_mods), decoy_tag.encode(), int(bool(generate_decoys))
+    lib = load_library()
+    h = C.c_void_p()
+    _check(lib.sage_b200_digest_create(C.c_int(device), C.c_char_p(text), C.c_uint64(len(text)), C.byref(p), C.byref(h)))
+    try:
+        ci = CDigestInfo()
+        _check(lib.sage_b200_digest_get_info(h, C.byref(ci)))
+        info = {k: getattr(ci, k) for k, _ in CDigestInfo._fields_}
+        n, nres, nref = info["n_peptides"], info["n_residues"], info["n_protein_refs"]
+        a = dict(seq_off=np.empty(n + 1, np.uint32), seq=np.empty(nres, np.uint8), mods=np.empty(nres, np.float32), nterm=np.empty(n, np.float32),
+                 cterm=np.empty(n, np.float32), mono=np.empty(n, np.float32), decoy=np.empty(n, np.uint8), missed=np.empty(n, np.uint8),
+                 semi=np.empty(n, np.uint8), prot_off=np.empty(n + 1, np.uint32), ids=np.empty(nref, np.uint32),
+                 name_off=np.empty(info["n_names"] + 1, np.uint64), names=np.empty(max(1, info["name_bytes"]), np.uint8))
+        t = time.perf_counter()
+        _check(lib.sage_b200_digest_export(h, *[_ptr(a[k]) for k in ("seq_off", "seq", "mods", "nterm", "cterm", "mono", "decoy", "missed", "semi",
+                                                                     "prot_off", "ids", "name_off", "names")]))
+        info["ms_export"] = (time.perf_counter() - t) * 1e3
+    finally:
+        lib.sage_b200_digest_destroy(h)
+    raw = a["names"].tobytes()
+    no = a["name_off"]
+    names = [raw[no[i]:no[i + 1]].decode("utf-8", errors="surrogateescape") for i in range(len(no) - 1)]
+    pep = Peptides(a["seq_off"], a["seq"], a["mods"], a["nterm"], a["mono"], a["decoy"], a["missed"])
+    return DigestResult(pep, a["cterm"], a["semi"].astype(bool), a["prot_off"], a["ids"], names, info)

@@ -41,6 +41,7 @@
 #include "rt.cuh"
 #include "picked.cuh"
 #include "protein_groups.cuh"
+#include "digest.cuh"
 
 using namespace sb;
 
@@ -4079,3 +4080,521 @@ extern "C" int sage_b200_debug_phase_cycles(unsigned long long* out16, int reset
     return 0;
 }
 #endif
+
+// ================================================================================== digest (database.rs:162-258; kernels in digest.cuh)
+struct sage_b200_digest {
+    int device = 0;
+    DevArena out;   // the output table, exact-size
+    uint32_t *d_res_off = nullptr, *d_ref_off = nullptr, *d_ids = nullptr;
+    uint8_t *d_seq = nullptr, *d_decoy = nullptr, *d_missed = nullptr, *d_semi = nullptr;
+    float *d_mods = nullptr, *d_nterm = nullptr, *d_cterm = nullptr, *d_mono = nullptr;
+    std::vector<uint64_t> name_off;
+    std::string names;
+    sage_b200_digest_info info{};
+};
+
+extern "C" void sage_b200_digest_destroy(sage_b200_digest* d) {
+    if (!d) return;
+    cudaSetDevice(d->device);
+    delete d;
+}
+
+// ModificationSpecificity::from_str (modification.rs:63-100): "^", "$", "[", "]" with an optional residue, or one residue of mass.rs's
+// VALID_AA (a second character after a residue is ignored); anything else is invalid and skipped by the Builder.
+static bool dg_parse_spec(const char* s, DgSpec& out) {
+    const size_t n = strlen(s);
+    if (n == 0 || n > 2) return false;
+    const int rest = n > 1 ? (int)(uint8_t)s[1] : -1;
+    switch (s[0]) {
+        case '^': out.kind = DG_SPEC_PEP_N; out.residue = rest; return true;
+        case '$': out.kind = DG_SPEC_PEP_C; out.residue = rest; return true;
+        case '[': out.kind = DG_SPEC_PROT_N; out.residue = rest; return true;
+        case ']': out.kind = DG_SPEC_PROT_C; out.residue = rest; return true;
+        default:
+            if (!strchr("ACDEFGHIKLMNPQRSTVWYUO", s[0])) return false;
+            out.kind = DG_SPEC_RESIDUE;
+            out.residue = (uint8_t)s[0];
+            return true;
+    }
+}
+
+struct DgFasta {
+    std::vector<uint8_t> res;
+    std::vector<uint32_t> off{0};
+    std::vector<std::string> acc;
+    std::vector<uint8_t> decoy;
+};
+
+static bool dg_space(uint8_t c) { return c == ' ' || c == '\t' || c == '\n' || c == '\v' || c == '\f' || c == '\r'; }
+
+// Fasta::parse (fasta.rs:14-56): lines split on '\n' with a trailing '\r' dropped, empty lines skipped, then trimmed; '>' starts a header
+// whose first whitespace-separated token is the accession. A protein is kept when it has residues, and with generate_decoys only when its
+// accession does not contain the decoy tag; without generate_decoys a tagged protein is kept as a decoy.
+static int dg_parse_fasta(const char* text, uint64_t len, const std::string& tag, bool generate_decoys, DgFasta& F) {
+    std::string last_id;
+    auto flush = [&]() -> int {
+        size_t a = 0;
+        while (a < last_id.size() && dg_space((uint8_t)last_id[a])) a++;
+        size_t b = a;
+        while (b < last_id.size() && !dg_space((uint8_t)last_id[b])) b++;
+        std::string acc = last_id.substr(a, b - a);
+        const bool tagged = acc.find(tag) != std::string::npos;
+        if (tagged && generate_decoys) {
+            F.res.resize(F.off.back());
+            return 0;
+        }
+        if (F.res.size() >= 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "digest: 2^32 or more residues");
+        F.off.push_back((uint32_t)F.res.size());
+        F.acc.push_back(std::move(acc));
+        F.decoy.push_back(tagged ? 1 : 0);
+        return 0;
+    };
+    uint64_t pos = 0;
+    while (pos <= len) {
+        const char* nl = pos < len ? (const char*)memchr(text + pos, '\n', len - pos) : nullptr;
+        uint64_t a = pos, b = nl ? (uint64_t)(nl - text) : len;
+        pos = nl ? b + 1 : len + 1;
+        if (b > a && text[b - 1] == '\r') b--;
+        if (b == a) continue;
+        while (a < b && dg_space((uint8_t)text[a])) a++;
+        while (b > a && dg_space((uint8_t)text[b - 1])) b--;
+        if (b > a && text[a] == '>') {
+            if (F.res.size() > F.off.back())
+                if (int rc = flush()) return rc;
+            last_id.assign(text + a + 1, b - a - 1);
+        } else {
+            F.res.insert(F.res.end(), (const uint8_t*)text + a, (const uint8_t*)text + b);
+        }
+    }
+    if (F.res.size() > F.off.back())
+        if (int rc = flush()) return rc;
+    if (F.res.size() >= 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "digest: 2^32 or more residues");
+    return 0;
+}
+
+struct DgMax {
+    __device__ uint32_t operator()(uint32_t a, uint32_t b) const { return a > b ? a : b; }
+};
+__global__ void k_dg_u64_to_u32(const uint64_t* __restrict__ a, uint64_t n, uint32_t* __restrict__ b) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) b[i] = (uint32_t)a[i];
+}
+
+static int dg_memory(const char* stage, uint64_t bytes) {
+    size_t free_b = 0, total_b = 0;
+    CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+    if (bytes + (64ull << 20) > free_b)
+        return fail(SAGE_B200_ELIMIT, "digest: the %s stage needs about %llu bytes of device memory, %llu free", stage, (unsigned long long)bytes,
+                    (unsigned long long)free_b);
+    return 0;
+}
+
+static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, const std::vector<DgSpec>& statics, const std::vector<DgSpec>& vars,
+                  const std::vector<uint32_t>& prot_name) {
+    sage_b200_digest_info& I = D->info;
+    const uint32_t P = (uint32_t)F.acc.size();
+    const uint64_t R = F.res.size();
+    Stream st;
+    CUDA_TRY(st.create());
+    Event ev[8];
+    for (Event& e : ev) CUDA_TRY(e.create());
+    DevArena A;
+    auto done = [&]() { I.peak_device_bytes = A.bytes + D->out.bytes; I.device_bytes = D->out.bytes; };
+    auto read = [&](void* h, const void* d, size_t b) -> int {
+        CUDA_TRY(cudaMemcpyAsync(h, d, b, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        return 0;
+    };
+    thrust::counting_iterator<uint32_t> count_it(0);
+    uint32_t* d_cnt = nullptr;
+    CUDA_TRY(A.alloc(&d_cnt, 1));
+
+    // upload
+    if (int rc = dg_memory("upload", R + 16ull * P + 64)) return rc;
+    CUDA_TRY(cudaEventRecord(ev[0], st));
+    uint8_t *d_res = nullptr, *d_pdecoy = nullptr;
+    uint32_t *d_poff = nullptr, *d_pname = nullptr;
+    DgSpec *d_statics = nullptr, *d_vars = nullptr;
+    CUDA_TRY(A.alloc(&d_res, R));
+    CUDA_TRY(A.alloc(&d_poff, P + 1));
+    CUDA_TRY(A.alloc(&d_pdecoy, P));
+    CUDA_TRY(A.alloc(&d_pname, P));
+    CUDA_TRY(A.alloc(&d_statics, statics.size()));
+    CUDA_TRY(A.alloc(&d_vars, vars.size()));
+    CUDA_TRY(cudaMemcpyAsync(d_res, F.res.data(), R, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_poff, F.off.data(), 4ull * (P + 1), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_pdecoy, F.decoy.data(), P, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_pname, prot_name.data(), 4ull * P, cudaMemcpyHostToDevice, st));
+    if (!statics.empty()) CUDA_TRY(cudaMemcpyAsync(d_statics, statics.data(), sizeof(DgSpec) * statics.size(), cudaMemcpyHostToDevice, st));
+    if (!vars.empty()) CUDA_TRY(cudaMemcpyAsync(d_vars, vars.data(), sizeof(DgSpec) * vars.size(), cudaMemcpyHostToDevice, st));
+    DgParams p = hp;
+    p.statics = d_statics;
+    p.vars = d_vars;
+    CUDA_TRY(cudaEventRecord(ev[1], st));
+
+    // 1. cleavage sites: count, scan, write
+    uint32_t *d_ncut = nullptr, *d_cut_off = nullptr, *d_cuts = nullptr;
+    CUDA_TRY(A.alloc(&d_ncut, P + 1));
+    CUDA_TRY(A.alloc(&d_cut_off, P + 1));
+    CUDA_TRY(cudaMemsetAsync(d_ncut, 0, 4ull * (P + 1), st));
+    const unsigned gw = (unsigned)((32ull * P + 255) / 256);
+    k_dg_sites<<<gw, 256, 0, st>>>(d_res, d_poff, P, p, d_ncut, nullptr, nullptr);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_ncut, d_cut_off, (int)(P + 1), st); }));
+    uint32_t n_cuts = 0;
+    if (int rc = read(&n_cuts, d_cut_off + P, 4)) return rc;
+    CUDA_TRY(A.alloc(&d_cuts, n_cuts));
+    k_dg_sites<<<gw, 256, 0, st>>>(d_res, d_poff, P, p, nullptr, d_cut_off, d_cuts);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(ev[2], st));
+
+    // 2. windows: count, scan, write
+    uint64_t *d_nwin = nullptr, *d_win_off = nullptr;
+    CUDA_TRY(A.alloc(&d_nwin, P + 1));
+    CUDA_TRY(A.alloc(&d_win_off, P + 1));
+    CUDA_TRY(cudaMemsetAsync(d_nwin, 0, 8ull * (P + 1), st));
+    k_dg_windows<<<grid256(P), 256, 0, st>>>(d_poff, d_cut_off, d_cuts, P, p, d_nwin, nullptr, nullptr);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nwin, d_win_off, (int)(P + 1), st); }));
+    uint64_t W64 = 0;
+    if (int rc = read(&W64, d_win_off + P, 8)) return rc;
+    if (W64 >= 0xFFFFFFFEull) return fail(SAGE_B200_ELIMIT, "digest: %llu windows (2^32 - 2 or more)", (unsigned long long)W64);
+    const uint32_t W = (uint32_t)W64;
+    I.n_windows = W;
+    if (W == 0) return done(), 0;
+    // windows, hashes and indices twice each, classes, keys twice, flags and the sorts' temporary storage
+    if (int rc = dg_memory("window", 100ull * W)) return rc;
+    DgWin* d_win = nullptr;
+    CUDA_TRY(A.alloc(&d_win, W));
+    k_dg_windows<<<grid256(P), 256, 0, st>>>(d_poff, d_cut_off, d_cuts, P, p, nullptr, d_win_off, d_win);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(ev[3], st));
+
+    // 3. per-protein `seen` and group_digests: sort by hash, exact classes, stable sort by class, keep each protein's first window of a class,
+    // stable sort by (class, Position, decoy): a group is a run, its first window the lowest protein's
+    uint64_t *d_hash = nullptr, *d_hash_s = nullptr, *d_key = nullptr, *d_key_k = nullptr, *d_key3 = nullptr;
+    uint32_t *d_idx = nullptr, *d_idx_s = nullptr, *d_rs = nullptr, *d_cls = nullptr, *d_cls_s = nullptr, *d_idx2 = nullptr, *d_idx_k = nullptr, *d_idx3 = nullptr,
+             *d_head = nullptr;
+    uint8_t* d_keep = nullptr;
+    CUDA_TRY(A.alloc(&d_hash, W));
+    CUDA_TRY(A.alloc(&d_hash_s, W));
+    CUDA_TRY(A.alloc(&d_idx, W));
+    CUDA_TRY(A.alloc(&d_idx_s, W));
+    CUDA_TRY(A.alloc(&d_rs, W));
+    CUDA_TRY(A.alloc(&d_cls, W));
+    const unsigned gW = grid256(W);
+    k_dg_hash<<<gW, 256, 0, st>>>(d_res, d_win, W, d_hash, d_idx);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_hash, d_hash_s, d_idx, d_idx_s, (int)W, 0, 64, st); }));
+    k_dg_run_start<<<gW, 256, 0, st>>>(d_hash_s, W, d_rs);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveScan(t, b, d_rs, d_rs, DgMax(), (int)W, st); }));
+    k_dg_class<<<gW, 256, 0, st>>>(d_res, d_win, d_idx_s, d_rs, W, d_cls);
+    CUDA_TRY(cudaGetLastError());
+    const int cbits = (int)std::max<uint32_t>(1, ceil_log2_u64(W));
+    CUDA_TRY(A.alloc(&d_cls_s, W));
+    CUDA_TRY(A.alloc(&d_idx2, W));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_cls, d_cls_s, d_idx_s, d_idx2, (int)W, 0, cbits, st); }));
+    CUDA_TRY(A.alloc(&d_keep, W));
+    CUDA_TRY(A.alloc(&d_key, W));
+    k_dg_seen<<<gW, 256, 0, st>>>(d_win, d_cls_s, d_idx2, d_pdecoy, W, d_keep, d_key);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.alloc(&d_key_k, W));
+    CUDA_TRY(A.alloc(&d_idx_k, W));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_key, d_keep, d_key_k, d_cnt, (int)W, st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_idx2, d_keep, d_idx_k, d_cnt, (int)W, st); }));
+    uint32_t Kc = 0;
+    if (int rc = read(&Kc, d_cnt, 4)) return rc;
+    CUDA_TRY(A.alloc(&d_key3, Kc));
+    CUDA_TRY(A.alloc(&d_idx3, Kc));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_key_k, d_key3, d_idx_k, d_idx3, (int)Kc, 0, cbits + 3, st); }));
+    CUDA_TRY(A.alloc(&d_head, Kc));
+    k_dg_heads64<<<grid256(Kc), 256, 0, st>>>(d_key3, Kc, d_head);
+    CUDA_TRY(cudaGetLastError());
+    uint32_t* d_gstart = nullptr;
+    CUDA_TRY(A.alloc(&d_gstart, Kc + 1));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_head, d_gstart, d_cnt, (int)Kc, st); }));
+    uint32_t G = 0;
+    if (int rc = read(&G, d_cnt, 4)) return rc;
+    I.n_groups = G;
+    CUDA_TRY(cudaMemcpyAsync(d_gstart + G, &Kc, 4, cudaMemcpyHostToDevice, st));
+    uint32_t *d_gwin = nullptr, *d_gcls = nullptr;
+    uint8_t *d_gmeta = nullptr, *d_cls_target = nullptr;
+    CUDA_TRY(A.alloc(&d_gwin, G));
+    CUDA_TRY(A.alloc(&d_gcls, G));
+    CUDA_TRY(A.alloc(&d_gmeta, G));
+    CUDA_TRY(A.alloc(&d_cls_target, W));
+    CUDA_TRY(cudaMemsetAsync(d_cls_target, 0, W, st));
+    const unsigned gG = grid256(G);
+    k_dg_groups<<<gG, 256, 0, st>>>(d_key3, d_idx3, d_gstart, G, d_gwin, d_gmeta, d_gcls, d_cls_target);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaEventRecord(ev[4], st));
+
+    // 4. Peptide::try_from, the variable-mod sites, the forms (apply, the mass filter, reverse and the targets filter)
+    float* d_gbase = nullptr;
+    uint32_t *d_nsite = nullptr, *d_site_off = nullptr, *d_overflow = nullptr;
+    uint64_t *d_nform = nullptr, *d_form_off = nullptr;
+    uint8_t* d_revt = nullptr;
+    CUDA_TRY(A.alloc(&d_gbase, G));
+    CUDA_TRY(A.alloc(&d_nsite, G + 1));
+    CUDA_TRY(A.alloc(&d_site_off, G + 1));
+    CUDA_TRY(A.alloc(&d_nform, G + 1));
+    CUDA_TRY(A.alloc(&d_form_off, G + 1));
+    CUDA_TRY(A.alloc(&d_revt, G));
+    CUDA_TRY(A.alloc(&d_overflow, 1));
+    CUDA_TRY(cudaMemsetAsync(d_nsite + G, 0, 4, st));
+    CUDA_TRY(cudaMemsetAsync(d_nform + G, 0, 8, st));
+    CUDA_TRY(cudaMemsetAsync(d_overflow, 0, 4, st));
+    k_dg_group_info<<<gG, 256, 0, st>>>(d_res, d_win, d_gwin, d_gmeta, G, p, d_hash_s, d_idx_s, W, d_gbase, d_nsite, d_nform, d_revt, d_overflow);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nsite, d_site_off, (int)(G + 1), st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nform, d_form_off, (int)(G + 1), st); }));
+    uint32_t n_sites = 0, overflow = 0;
+    uint64_t T64 = 0;
+    if (int rc = read(&n_sites, d_site_off + G, 4)) return rc;
+    if (int rc = read(&T64, d_form_off + G, 8)) return rc;
+    if (int rc = read(&overflow, d_overflow, 4)) return rc;
+    if (overflow) return fail(SAGE_B200_ELIMIT, "digest: a peptide has more than 65535 variable-modification sites");
+    if (T64 >= (1ull << 31)) return fail(SAGE_B200_ELIMIT, "digest: %llu (peptide, modification combination) candidates (2^31 or more)", (unsigned long long)T64);
+    const uint32_t T = (uint32_t)T64;
+    I.n_candidates = T;
+    if (T == 0) return done(), 0;
+    if (int rc = dg_memory("expansion", 8ull * n_sites + 12ull * T)) return rc;
+    uint32_t *d_site_code = nullptr, *d_rows = nullptr, *d_row_off = nullptr;
+    float* d_site_mass = nullptr;
+    CUDA_TRY(A.alloc(&d_site_code, n_sites));
+    CUDA_TRY(A.alloc(&d_site_mass, n_sites));
+    k_dg_site_fill<<<gG, 256, 0, st>>>(d_res, d_win, d_gwin, d_gmeta, d_site_off, G, p, d_site_code, d_site_mass);
+    CUDA_TRY(cudaGetLastError());
+    DgView V{d_res, d_poff, d_win, d_gwin, d_gmeta, d_site_off, d_site_code, d_site_mass, nullptr, nullptr, p};
+    CUDA_TRY(A.alloc(&d_rows, T + 1));
+    CUDA_TRY(A.alloc(&d_row_off, T + 1));
+    CUDA_TRY(cudaMemsetAsync(d_rows + T, 0, 4, st));
+    k_dg_expand<<<grid256(T), 256, 0, st>>>(V, d_form_off, G, T, d_gbase, d_gcls, d_cls_target, d_revt, d_rows, nullptr, nullptr, nullptr);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_rows, d_row_off, (int)(T + 1), st); }));
+    uint32_t N = 0;
+    if (int rc = read(&N, d_row_off + T, 4)) return rc;
+    if (N >= 0xFFFFFFFEu) return fail(SAGE_B200_ELIMIT, "digest: 2^32 - 2 or more peptide rows");
+    I.n_rows = N;
+    if (N == 0) return done(), 0;
+    // forms and masses, keys and indices twice, run flags and positions, merge heads, and the merge sort's buffers
+    if (int rc = dg_memory("sort", 64ull * N)) return rc;
+    DgForm* d_forms = nullptr;
+    float* d_fmono = nullptr;
+    CUDA_TRY(A.alloc(&d_forms, N));
+    CUDA_TRY(A.alloc(&d_fmono, N));
+    k_dg_expand<<<grid256(T), 256, 0, st>>>(V, d_form_off, G, T, d_gbase, d_gcls, d_cls_target, d_revt, d_rows, d_row_off, d_forms, d_fmono);
+    CUDA_TRY(cudaGetLastError());
+    V.forms = d_forms;
+    V.form_mono = d_fmono;
+    CUDA_TRY(cudaEventRecord(ev[5], st));
+
+    // 5. reorder_peptides' sort: stable radix sort by total_cmp(mono), then a stable merge sort of the equal-mono runs by initial_sort
+    uint32_t *d_mkey = nullptr, *d_mkey_s = nullptr, *d_fidx = nullptr, *d_order = nullptr, *d_rpos = nullptr, *d_rval = nullptr;
+    uint8_t* d_inrun = nullptr;
+    CUDA_TRY(A.alloc(&d_mkey, N));
+    CUDA_TRY(A.alloc(&d_mkey_s, N));
+    CUDA_TRY(A.alloc(&d_fidx, N));
+    CUDA_TRY(A.alloc(&d_order, N));
+    CUDA_TRY(A.alloc(&d_inrun, N));
+    const unsigned gN = grid256(N);
+    k_dg_mono_key<<<gN, 256, 0, st>>>(d_fmono, N, d_mkey, d_fidx);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_mkey, d_mkey_s, d_fidx, d_order, (int)N, 0, 32, st); }));
+    k_dg_in_run<<<gN, 256, 0, st>>>(d_mkey_s, N, d_inrun);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.alloc(&d_rpos, N));
+    CUDA_TRY(A.alloc(&d_rval, N));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_inrun, d_rpos, d_cnt, (int)N, st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_order, d_inrun, d_rval, d_cnt, (int)N, st); }));
+    uint32_t M = 0;
+    if (int rc = read(&M, d_cnt, 4)) return rc;
+    if (M) {
+        const DgRowLess less{V};
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceMergeSort::StableSortKeys(t, b, d_rval, (int)M, less, st); }));
+        k_dg_scatter<<<grid256(M), 256, 0, st>>>(d_rpos, d_rval, M, d_order);
+        CUDA_TRY(cudaGetLastError());
+    }
+    CUDA_TRY(cudaEventRecord(ev[6], st));
+
+    // 6. reorder_peptides' merge and the output table
+    uint32_t *d_mhead = nullptr, *d_first = nullptr;
+    CUDA_TRY(A.alloc(&d_mhead, N));
+    CUDA_TRY(A.alloc(&d_first, N + 1));
+    k_dg_merge_heads<<<gN, 256, 0, st>>>(V, d_order, N, d_mhead);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_mhead, d_first, d_cnt, (int)N, st); }));
+    uint32_t n_pep = 0;
+    if (int rc = read(&n_pep, d_cnt, 4)) return rc;
+    CUDA_TRY(cudaMemcpyAsync(d_first + n_pep, &N, 4, cudaMemcpyHostToDevice, st));
+    // offsets in 64 bits, so that a table of 2^32 residues or protein references or more is reported rather than wrapped
+    uint64_t *d_nres = nullptr, *d_nref = nullptr, *d_res_off64 = nullptr, *d_ref_off64 = nullptr;
+    CUDA_TRY(A.alloc(&d_nres, n_pep + 1));
+    CUDA_TRY(A.alloc(&d_nref, n_pep + 1));
+    CUDA_TRY(A.alloc(&d_res_off64, n_pep + 1));
+    CUDA_TRY(A.alloc(&d_ref_off64, n_pep + 1));
+    CUDA_TRY(cudaMemsetAsync(d_nres + n_pep, 0, 8, st));
+    CUDA_TRY(cudaMemsetAsync(d_nref + n_pep, 0, 8, st));
+    k_dg_pep_counts<<<grid256(n_pep), 256, 0, st>>>(V, d_order, d_first, n_pep, d_gstart, d_nres, d_nref);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nres, d_res_off64, (int)(n_pep + 1), st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nref, d_ref_off64, (int)(n_pep + 1), st); }));
+    uint64_t n_res = 0, n_ref = 0;
+    if (int rc = read(&n_res, d_res_off64 + n_pep, 8)) return rc;
+    if (int rc = read(&n_ref, d_ref_off64 + n_pep, 8)) return rc;
+    if (n_res > 0xFFFFFFFFull || n_ref >= 0x7FFFFFFFull)
+        return fail(SAGE_B200_ELIMIT, "digest: %llu residues / %llu protein references in the table (u32 offsets)", (unsigned long long)n_res,
+                    (unsigned long long)n_ref);
+    if (int rc = dg_memory("output", 5ull * n_res + 30ull * n_pep + 8ull * n_ref)) return rc;
+    DevArena& O = D->out;
+    uint32_t* d_ids_raw = nullptr;
+    CUDA_TRY(O.alloc(&D->d_res_off, n_pep + 1));
+    CUDA_TRY(O.alloc(&D->d_ref_off, n_pep + 1));
+    CUDA_TRY(O.alloc(&D->d_ids, n_ref));
+    CUDA_TRY(O.alloc(&D->d_seq, n_res));
+    CUDA_TRY(O.alloc(&D->d_mods, n_res));
+    CUDA_TRY(O.alloc(&D->d_nterm, n_pep));
+    CUDA_TRY(O.alloc(&D->d_cterm, n_pep));
+    CUDA_TRY(O.alloc(&D->d_mono, n_pep));
+    CUDA_TRY(O.alloc(&D->d_decoy, n_pep));
+    CUDA_TRY(O.alloc(&D->d_missed, n_pep));
+    CUDA_TRY(O.alloc(&D->d_semi, n_pep));
+    CUDA_TRY(A.alloc(&d_ids_raw, n_ref));
+    k_dg_u64_to_u32<<<grid256(n_pep + 1), 256, 0, st>>>(d_res_off64, n_pep + 1, D->d_res_off);
+    CUDA_TRY(cudaGetLastError());
+    k_dg_u64_to_u32<<<grid256(n_pep + 1), 256, 0, st>>>(d_ref_off64, n_pep + 1, D->d_ref_off);
+    CUDA_TRY(cudaGetLastError());
+    k_dg_export<<<grid256(n_pep), 256, 0, st>>>(V, d_order, d_first, n_pep, d_gstart, d_idx3, d_pname, D->d_res_off, D->d_ref_off, D->d_seq, D->d_mods,
+                                                D->d_nterm, D->d_cterm, D->d_mono, D->d_decoy, D->d_missed, D->d_semi, d_ids_raw);
+    CUDA_TRY(cudaGetLastError());
+    // proteins.sort_unstable() (database.rs:250): ids are name ranks, so an ascending sort of the ids is the sort of the names
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) {
+        return cub::DeviceSegmentedSort::SortKeys(t, b, d_ids_raw, D->d_ids, (int)n_ref, (int)n_pep, D->d_ref_off, D->d_ref_off + 1, st);
+    }));
+    CUDA_TRY(cudaEventRecord(ev[7], st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    I.n_peptides = n_pep;
+    I.n_residues = n_res;
+    I.n_protein_refs = n_ref;
+    float* ms[7] = {&I.ms_upload, &I.ms_sites, &I.ms_windows, &I.ms_group, &I.ms_expand, &I.ms_sort, &I.ms_merge};
+    for (int i = 0; i < 7; i++) CUDA_TRY(cudaEventElapsedTime(ms[i], ev[i], ev[i + 1]));
+    CUDA_TRY(cudaEventElapsedTime(&I.ms_total, ev[0], ev[7]));
+    done();
+    return 0;
+}
+
+extern "C" int sage_b200_digest_create(int device, const char* fasta, uint64_t fasta_len, const sage_b200_digest_params* p, sage_b200_digest** out) {
+    const auto t0 = std::chrono::steady_clock::now();
+    if (!out || !p || (fasta_len && !fasta)) return fail(SAGE_B200_EINVAL, "digest_create: null argument");
+    *out = nullptr;
+    if ((p->n_static && (!p->static_specs || !p->static_masses)) || (p->n_variable && (!p->variable_specs || !p->variable_masses)))
+        return fail(SAGE_B200_EINVAL, "digest_create: null modification array");
+    if (p->max_len > 255) return fail(SAGE_B200_ELIMIT, "digest: max_len %llu > 255 (the library's peptide-length limit)", (unsigned long long)p->max_len);
+    if (p->max_variable_mods > DG_KMAX) return fail(SAGE_B200_ELIMIT, "digest: max_variable_mods %llu > %u", (unsigned long long)p->max_variable_mods, DG_KMAX);
+    for (uint64_t i = 0; i < p->n_static; i++)
+        if (!p->static_specs[i] || !std::isfinite(p->static_masses[i])) return fail(SAGE_B200_EINVAL, "digest: static mod %llu: null spec or non-finite mass", (unsigned long long)i);
+    for (uint64_t i = 0; i < p->n_variable; i++)
+        if (!p->variable_specs[i] || !std::isfinite(p->variable_masses[i]))
+            return fail(SAGE_B200_EINVAL, "digest: variable mod %llu: null spec or non-finite mass", (unsigned long long)i);
+    // Builder::make_parameters and Enzyme::new (database.rs:96-115, enzyme.rs:145-184)
+    DgParams hp{};
+    const std::string cleave_at = p->cleave_at ? p->cleave_at : "", restrict_ = p->restrict_ ? p->restrict_ : "";
+    hp.min_len = (uint32_t)std::min<uint64_t>(p->min_len, 256);
+    hp.max_len = (uint32_t)p->max_len;
+    hp.missed = p->missed_cleavages;
+    hp.c_terminal = p->c_terminal ? 1 : 0;
+    hp.has_enzyme = !cleave_at.empty();
+    if (!hp.has_enzyme) {
+        hp.missed = 0;
+    } else if (cleave_at == "$") {
+        hp.dollar = 1;
+        hp.c_terminal = 1;
+    } else {
+        for (char c : cleave_at) if (c >= 'A' && c <= 'Z') hp.cleave |= 1u << (c - 'A');
+        for (char c : restrict_) if (c >= 'A' && c <= 'Z') hp.restrict_ |= 1u << (c - 'A');
+        hp.semi = p->semi_enzymatic ? 1 : 0;
+    }
+    hp.generate_decoys = p->generate_decoys ? 1 : 0;
+    hp.kmax = (uint32_t)std::max<uint64_t>(p->max_variable_mods, 1);
+    hp.min_mass = p->peptide_min_mass;
+    hp.max_mass = p->peptide_max_mass;
+    auto spec_less = [](const DgSpec& a, const DgSpec& b) { return a.kind != b.kind ? a.kind < b.kind : a.residue < b.residue; };
+    std::vector<DgSpec> statics, vars;
+    for (uint64_t i = 0; i < p->n_static; i++) {   // a map keyed by spec: ordered, the last mass of a repeated spec wins
+        DgSpec s{};
+        if (!dg_parse_spec(p->static_specs[i], s)) continue;
+        s.mass = p->static_masses[i];
+        auto it = std::lower_bound(statics.begin(), statics.end(), s, spec_less);
+        if (it != statics.end() && !spec_less(s, *it)) it->mass = s.mass;
+        else statics.insert(it, s);
+    }
+    for (uint64_t i = 0; i < p->n_variable; i++) {
+        DgSpec s{};
+        if (!dg_parse_spec(p->variable_specs[i], s)) continue;
+        s.mass = p->variable_masses[i];
+        vars.push_back(s);
+    }
+    std::stable_sort(vars.begin(), vars.end(), spec_less);
+    hp.n_static = (uint32_t)statics.size();
+    hp.n_var = (uint32_t)vars.size();
+
+    Guard<sage_b200_digest> guard(new sage_b200_digest(), sage_b200_digest_destroy);
+    sage_b200_digest* D = guard.get();
+    D->device = device;
+    DgFasta F;
+    if (int rc = dg_parse_fasta(fasta, fasta_len, p->decoy_tag ? p->decoy_tag : "rev_", p->generate_decoys != 0, F)) return rc;
+    // the names table: distinct accessions in byte order, a protein's id is its accession's rank
+    std::vector<uint32_t> order(F.acc.size()), prot_name(F.acc.size());
+    for (uint32_t i = 0; i < order.size(); i++) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return F.acc[a] < F.acc[b]; });
+    D->name_off.push_back(0);
+    for (size_t k = 0; k < order.size(); k++) {
+        if (k == 0 || F.acc[order[k]] != F.acc[order[k - 1]]) {
+            D->names += F.acc[order[k]];
+            D->name_off.push_back(D->names.size());
+        }
+        prot_name[order[k]] = (uint32_t)(D->name_off.size() - 2);
+    }
+    sage_b200_digest_info& I = D->info;
+    I.n_proteins = F.acc.size();
+    I.n_names = D->name_off.size() - 1;
+    I.name_bytes = D->names.size();
+    I.ms_parse = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (int rc = select_device(device)) return rc;
+    if (!F.acc.empty())
+        if (int rc = dg_run(D, F, hp, statics, vars, prot_name)) return rc;
+    I.ms_wall = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    *out = guard.release();
+    return 0;
+}
+
+extern "C" int sage_b200_digest_get_info(const sage_b200_digest* D, sage_b200_digest_info* info) {
+    if (!D || !info) return fail(SAGE_B200_EINVAL, "digest_get_info: null argument");
+    *info = D->info;
+    return 0;
+}
+
+extern "C" int sage_b200_digest_export(const sage_b200_digest* D, uint32_t* residue_offsets, uint8_t* sequence, float* modifications, float* nterm,
+                                       float* cterm, float* monoisotopic, uint8_t* decoy, uint8_t* missed_cleavages, uint8_t* semi_enzymatic,
+                                       uint32_t* protein_offsets, uint32_t* protein_ids, uint64_t* name_offsets, char* name_bytes) {
+    if (!D) return fail(SAGE_B200_EINVAL, "digest_export: null handle");
+    const sage_b200_digest_info& I = D->info;
+    if (name_offsets) memcpy(name_offsets, D->name_off.data(), 8 * D->name_off.size());
+    if (name_bytes && !D->names.empty()) memcpy(name_bytes, D->names.data(), D->names.size());
+    const uint64_t n = I.n_peptides;
+    if (n == 0) {
+        if (residue_offsets) residue_offsets[0] = 0;
+        if (protein_offsets) protein_offsets[0] = 0;
+        return 0;
+    }
+    CUDA_TRY(cudaSetDevice(D->device));
+    struct Copy { void* dst; const void* src; uint64_t bytes; };
+    const Copy copies[] = {{residue_offsets, D->d_res_off, 4 * (n + 1)}, {sequence, D->d_seq, I.n_residues}, {modifications, D->d_mods, 4 * I.n_residues},
+                           {nterm, D->d_nterm, 4 * n}, {cterm, D->d_cterm, 4 * n}, {monoisotopic, D->d_mono, 4 * n}, {decoy, D->d_decoy, n},
+                           {missed_cleavages, D->d_missed, n}, {semi_enzymatic, D->d_semi, n}, {protein_offsets, D->d_ref_off, 4 * (n + 1)},
+                           {protein_ids, D->d_ids, 4 * I.n_protein_refs}};
+    for (const Copy& c : copies)
+        if (c.dst && c.bytes) CUDA_TRY(cudaMemcpy(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost));
+    return 0;
+}
