@@ -150,6 +150,20 @@ struct DevArena {
         if (e == cudaSuccess) { ps.push_back(p); bytes += b; *out = (T*)p; }
         return e;
     }
+    // alloc(out, count + pad), then the copy of `count` items from `host` queued on st.
+    template <class T>
+    cudaError_t upload(T** out, const T* host, size_t count, cudaStream_t st, size_t pad = 0) {
+        cudaError_t e = alloc(out, count + pad);
+        if (e == cudaSuccess && count) e = cudaMemcpyAsync(*out, host, count * sizeof(T), cudaMemcpyHostToDevice, st);
+        return e;
+    }
+    // alloc(out, count), then zeroed on st.
+    template <class T>
+    cudaError_t zeros(T** out, size_t count, cudaStream_t st) {
+        cudaError_t e = alloc(out, count);
+        if (e == cudaSuccess && count) e = cudaMemsetAsync(*out, 0, count * sizeof(T), st);
+        return e;
+    }
     // A larger request allocates a new buffer; the old one stays until the arena goes (work queued on a stream may still use it).
     cudaError_t reserve_tmp(size_t b) {
         if (tmp && b <= tmp_bytes) return cudaSuccess;
@@ -167,13 +181,18 @@ struct DevArena {
     }
 };
 
-// A non-blocking stream and an event, each destroyed with its owner (with the owner's device current) and created by create().
+// A non-blocking stream and an event, each destroyed with its owner (with the owner's device current) and created by create(). The stream
+// waits for its queued work before it goes: declared after the DevArena and host buffers that work uses, it keeps them alive until it ends.
 struct Stream {
     cudaStream_t s = nullptr;
     Stream() = default;
     Stream(const Stream&) = delete;
     Stream& operator=(const Stream&) = delete;
-    ~Stream() { if (s) cudaStreamDestroy(s); }
+    ~Stream() {
+        if (!s) return;
+        cudaStreamSynchronize(s);
+        cudaStreamDestroy(s);
+    }
     cudaError_t create() { return cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking); }
     operator cudaStream_t() const { return s; }
 };
@@ -186,6 +205,28 @@ struct Event {
     cudaError_t create() { return cudaEventCreate(&e); }
     operator cudaEvent_t() const { return e; }
 };
+
+// Blocks of 256 threads that cover n items.
+static unsigned grid256(uint64_t n) { return (unsigned)((n + 255) / 256); }
+
+// A kernel launch and its check: LAUNCH(k<<<grid, block, smem, st>>>(args)).
+#define LAUNCH(...)                         \
+    do {                                    \
+        __VA_ARGS__;                        \
+        CUDA_TRY(cudaGetLastError());       \
+    } while (0)
+// `kernel` over n items in blocks of 256 on stream st, checked; n == 0 launches nothing.
+#define LAUNCH_N(kernel, n, st, ...)                                                  \
+    do {                                                                              \
+        if ((n) > 0) LAUNCH(kernel<<<grid256(n), 256, 0, st>>>(__VA_ARGS__));         \
+    } while (0)
+
+// Copies `bytes` from the device to the host on st and waits for the stream.
+static int read_back(cudaStream_t st, void* host, const void* dev, size_t bytes) {
+    CUDA_TRY(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
 
 // Host -> device copy of a PAGEABLE array (a Rust Vec<f32>, a numpy array) through a pinned staging buffer: a few pool threads copy 2 MB pieces
 // into the staging buffer while the calling thread submits each piece's DMA as soon as it is staged, so the memcpy (one core copies
@@ -844,55 +885,60 @@ static int ensure_kernel_attributes(int device) {
     return 0;
 }
 
+// One step of the xorshift64 generator that draws the inputs of the host libm probes below.
+static uint64_t xorshift64(uint64_t& s) {
+    s ^= s << 13;
+    s ^= s >> 7;
+    s ^= s << 17;
+    return s;
+}
+
 // Which build of glibc's log() is the host libm (glibc_log.cuh)? Both variants are evaluated on the CPU and compared with std::log bit for bit
 // on a few thousand inputs of the kinds the path feeds it: hyperscore products, lambda, arguments near 1 (the only region where the two
 // variants differ). Returns 0 (FMA-contracted), 1 (plain), or -1 when neither matches (non-glibc libm: the device then uses variant 0 and
 // hyperscore / poisson agree with the host to <= 1 ulp instead of bit for bit).
 extern "C" int sage_b200_host_log_variant(void) {
-    static int cached = -2;
-    if (cached != -2) return cached;
-    uint64_t st = 0x9E3779B97F4A7C15ull;
-    auto next = [&]() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return st; };
-    bool ok[2] = {true, true};
-    for (int i = 0; i < 6000; i++) {
-        const uint64_t u = next();
-        double x;
-        switch (i % 3) {
-            case 0: x = (double)((float)(u & 0xffffff) * 0.37f + 1.0f) * (double)((float)((u >> 24) & 0xffffff) * 1.91f + 1.0f); break;
-            case 1: x = 0.93 + (double)(u >> 11) * 0x1p-53 * 0.15; break;
-            default: x = (double)(u >> 11) * 0x1p-53 * 64.0; break;
+    static const int variant = []() {   // initialised once, thread-safe
+        uint64_t st = 0x9E3779B97F4A7C15ull;
+        bool ok[2] = {true, true};
+        for (int i = 0; i < 6000; i++) {
+            const uint64_t u = xorshift64(st);
+            double x;
+            switch (i % 3) {
+                case 0: x = (double)((float)(u & 0xffffff) * 0.37f + 1.0f) * (double)((float)((u >> 24) & 0xffffff) * 1.91f + 1.0f); break;
+                case 1: x = 0.93 + (double)(u >> 11) * 0x1p-53 * 0.15; break;
+                default: x = (double)(u >> 11) * 0x1p-53 * 64.0; break;
+            }
+            volatile double vx = x;   // keep the compiler from folding std::log
+            const double ref = std::log(vx);
+            const double a = glog::glibc_log<true>(x), b = glog::glibc_log<false>(x);
+            if (memcmp(&a, &ref, 8)) ok[0] = false;
+            if (memcmp(&b, &ref, 8)) ok[1] = false;
         }
-        volatile double vx = x;   // keep the compiler from folding std::log
-        const double ref = std::log(vx);
-        const double a = glog::glibc_log<true>(x), b = glog::glibc_log<false>(x);
-        if (memcmp(&a, &ref, 8)) ok[0] = false;
-        if (memcmp(&b, &ref, 8)) ok[1] = false;
-    }
-    cached = ok[0] ? 0 : (ok[1] ? 1 : -1);
-    return cached;
+        return ok[0] ? 0 : (ok[1] ? 1 : -1);
+    }();
+    return variant;
 }
 
 // 1 when the host libm's log1pf (Rust's f32::ln_1p, OpenMS hyperscore) is the fdlibm/glibc function the kernels reproduce (glibc_log.cuh).
 extern "C" int sage_b200_host_log1pf_exact(void) {
-    static int cached = -1;
-    if (cached >= 0) return cached;
-    uint64_t st = 0x2545F4914F6CDD1Dull;
-    auto next = [&]() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return st; };
-    int ok = 1;
-    for (int i = 0; i < 20000 && ok; i++) {
-        const uint64_t u = next();
-        float x;
-        switch (i % 3) {
-            case 0: x = (float)(u & 0xffffff) * 3.7f; break;                                  // summed intensities
-            case 1: x = (float)((double)(u >> 11) * 0x1p-53 * 2.0 - 0.9); break;            // around the branch points
-            default: { uint32_t b = (uint32_t)(u >> 33); memcpy(&x, &b, 4); break; }          // any non-negative float
+    static const int exact = []() {   // initialised once, thread-safe
+        uint64_t st = 0x2545F4914F6CDD1Dull;
+        for (int i = 0; i < 20000; i++) {
+            const uint64_t u = xorshift64(st);
+            float x;
+            switch (i % 3) {
+                case 0: x = (float)(u & 0xffffff) * 3.7f; break;                                  // summed intensities
+                case 1: x = (float)((double)(u >> 11) * 0x1p-53 * 2.0 - 0.9); break;            // around the branch points
+                default: { uint32_t b = (uint32_t)(u >> 33); memcpy(&x, &b, 4); break; }          // any non-negative float
+            }
+            volatile float vx = x;
+            const float ref = log1pf(vx), got = glog::glibc_log1pf(x);
+            if (memcmp(&ref, &got, 4) && !(ref != ref && got != got)) return 0;
         }
-        volatile float vx = x;
-        const float ref = log1pf(vx), got = glog::glibc_log1pf(x);
-        if (memcmp(&ref, &got, 4) && !(ref != ref && got != got)) ok = 0;
-    }
-    cached = ok;
-    return cached;
+        return 1;
+    }();
+    return exact;
 }
 
 // ------------------------------------------------------------------------------------------------ scorer
@@ -1981,23 +2027,31 @@ extern "C" int sage_b200_process_spectra(int device, const sage_b200_processor_p
     const size_t smem = (size_t)p2 * 12 + (size_t)pmax * (5 * 4 + 2) + 32;
     if (smem > 200 * 1024) return fail(SAGE_B200_ELIMIT, "spectrum with %u raw peaks exceeds the shared-memory budget of the preprocessing kernel", pmax);
     DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
     uint32_t *d_off = nullptr, *d_cnt = nullptr;
     float *d_mz = nullptr, *d_int = nullptr, *d_om = nullptr, *d_oi = nullptr, *d_tic = nullptr;
     uint8_t* d_chg = nullptr;
-    CUDA_TRY(A.alloc(&d_off, n + 1)); CUDA_TRY(A.alloc(&d_mz, npk + 4)); CUDA_TRY(A.alloc(&d_int, npk + 4)); CUDA_TRY(A.alloc(&d_chg, n));
-    CUDA_TRY(A.alloc(&d_om, npk + 4)); CUDA_TRY(A.alloc(&d_oi, npk + 4)); CUDA_TRY(A.alloc(&d_cnt, n)); CUDA_TRY(A.alloc(&d_tic, n));
-    CUDA_TRY(cudaMemcpy(d_off, off.data(), 4 * (n + 1), cudaMemcpyHostToDevice));
-    if (npk) { CUDA_TRY(cudaMemcpy(d_mz, raw->mz + pk0, 4 * npk, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(d_int, raw->intensity + pk0, 4 * npk, cudaMemcpyHostToDevice)); }
-    CUDA_TRY(cudaMemcpy(d_chg, raw->precursor_charge, n, cudaMemcpyHostToDevice));
+    CUDA_TRY(A.upload(&d_off, off.data(), n + 1, st));
+    CUDA_TRY(A.upload(&d_mz, raw->mz + pk0, npk, st, 4));
+    CUDA_TRY(A.upload(&d_int, raw->intensity + pk0, npk, st, 4));
+    CUDA_TRY(A.upload(&d_chg, raw->precursor_charge, n, st));
+    CUDA_TRY(A.alloc(&d_om, npk + 4));
+    CUDA_TRY(A.alloc(&d_oi, npk + 4));
+    CUDA_TRY(A.alloc(&d_cnt, n));
+    CUDA_TRY(A.alloc(&d_tic, n));
     ProcParams pp{(uint32_t)std::min<uint64_t>(pr->take_top_n, 0xFFFFFFFFull), pr->deisotope ? 1u : 0u, pr->min_deisotope_mz};
     if (int rc = ensure_kernel_attributes(device)) return rc;
-    k_process_ms2<<<(unsigned)n, 32, smem>>>(pp, (uint32_t)n, d_off, d_mz, d_int, d_chg, pmax, p2, d_om, d_oi, d_cnt, d_tic);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_process_ms2<<<(unsigned)n, 32, smem, st>>>(pp, (uint32_t)n, d_off, d_mz, d_int, d_chg, pmax, p2, d_om, d_oi, d_cnt, d_tic));
     std::vector<uint32_t> cnt(n);
     std::vector<float> om(npk), oi(npk);
-    CUDA_TRY(cudaMemcpy(cnt.data(), d_cnt, 4 * n, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(out_tic, d_tic, 4 * n, cudaMemcpyDeviceToHost));
-    if (npk) { CUDA_TRY(cudaMemcpy(om.data(), d_om, 4 * npk, cudaMemcpyDeviceToHost)); CUDA_TRY(cudaMemcpy(oi.data(), d_oi, 4 * npk, cudaMemcpyDeviceToHost)); }
+    CUDA_TRY(cudaMemcpyAsync(cnt.data(), d_cnt, 4 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out_tic, d_tic, 4 * n, cudaMemcpyDeviceToHost, st));
+    if (npk) {
+        CUDA_TRY(cudaMemcpyAsync(om.data(), d_om, 4 * npk, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(oi.data(), d_oi, 4 * npk, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA_TRY(cudaStreamSynchronize(st));
     uint64_t w = 0;   // compact: spectrum i keeps cnt[i] <= raw count peaks
     for (uint64_t i = 0; i < n; i++) {
         memcpy(out_masses + w, om.data() + off[i], 4 * (size_t)cnt[i]);
@@ -2021,19 +2075,19 @@ extern "C" int sage_b200_find_reporter_ions(int device, uint64_t n, const uint64
     std::vector<uint32_t> off(n + 1);
     for (uint64_t i = 0; i <= n; i++) off[i] = (uint32_t)(peak_offsets[i] - pk0);
     DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
     uint32_t* d_off = nullptr;
     float *d_m = nullptr, *d_i = nullptr, *d_l = nullptr, *d_o = nullptr;
-    CUDA_TRY(A.alloc(&d_off, n + 1)); CUDA_TRY(A.alloc(&d_m, npk + 4)); CUDA_TRY(A.alloc(&d_i, npk + 4));
-    CUDA_TRY(A.alloc(&d_l, n_labels)); CUDA_TRY(A.alloc(&d_o, n * n_labels));
-    CUDA_TRY(cudaMemcpy(d_off, off.data(), 4 * (n + 1), cudaMemcpyHostToDevice));
-    if (npk) { CUDA_TRY(cudaMemcpy(d_m, masses + pk0, 4 * npk, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(d_i, intensities + pk0, 4 * npk, cudaMemcpyHostToDevice)); }
-    CUDA_TRY(cudaMemcpy(d_l, labels, 4 * n_labels, cudaMemcpyHostToDevice));
     const uint64_t total = n * n_labels;
-    k_find_reporter_ions<<<(unsigned)((total + 255) / 256), 256>>>((uint32_t)n, (uint32_t)n_labels, d_off, d_m, d_i, d_l,
-                                                                  Tol{label_tolerance.kind, label_tolerance.lo, label_tolerance.hi}, d_o);
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaMemcpy(out, d_o, 4 * total, cudaMemcpyDeviceToHost));
-    return 0;
+    CUDA_TRY(A.upload(&d_off, off.data(), n + 1, st));
+    CUDA_TRY(A.upload(&d_m, masses + pk0, npk, st, 4));
+    CUDA_TRY(A.upload(&d_i, intensities + pk0, npk, st, 4));
+    CUDA_TRY(A.upload(&d_l, labels, n_labels, st));
+    CUDA_TRY(A.alloc(&d_o, total));
+    LAUNCH_N(k_find_reporter_ions, total, st, (uint32_t)n, (uint32_t)n_labels, d_off, d_m, d_i, d_l,
+             Tol{label_tolerance.kind, label_tolerance.lo, label_tolerance.hi}, d_o);
+    return read_back(st, out, d_o, 4 * total);
 }
 
 __global__ void k_device_log(int variant, const double* x, uint64_t n, double* out) {
@@ -2045,13 +2099,13 @@ extern "C" int sage_b200_device_log(int device, int variant, const double* x, ui
     if (!x || !out || variant < 0 || variant > 2) return fail(SAGE_B200_EINVAL, "device_log: bad argument");
     if (int rc = select_device(device)) return rc;
     DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
     double *dx = nullptr, *dy = nullptr;
-    CUDA_TRY(A.alloc(&dx, n));
+    CUDA_TRY(A.upload(&dx, x, n, st));
     CUDA_TRY(A.alloc(&dy, n));
-    CUDA_TRY(cudaMemcpy(dx, x, 8 * n, cudaMemcpyHostToDevice));
-    k_device_log<<<(unsigned)((n + 255) / 256), 256>>>(variant, dx, n, dy);
-    CUDA_TRY(cudaMemcpy(out, dy, 8 * n, cudaMemcpyDeviceToHost));
-    return 0;
+    LAUNCH_N(k_device_log, n, st, variant, dx, n, dy);
+    return read_back(st, out, dy, 8 * n);
 }
 
 extern "C" int sage_b200_counters_get(const sage_b200_scorer* S, sage_b200_counters* out) {
@@ -2190,28 +2244,21 @@ static int lfq_build(sage_b200_lfq* L, const sage_b200_db* db, const sage_b200_p
     uint32_t *d_rows[7] = {}, *d_first = nullptr, *d_slots = nullptr, *d_nsel = nullptr;   // d_rows: the feature columns, 4 bytes per row each
     uint8_t* d_flag = nullptr;
     const void* src[7] = {F->peptide_idx, F->peptide_q, F->label, F->aligned_rt, F->calcmass, F->file_id, F->ims};
-    for (int k = 0; k < 7; k++) {
-        CUDA_TRY(A.alloc(&d_rows[k], n + 4));
-        if (n) CUDA_TRY(cudaMemcpyAsync(d_rows[k], src[k], 4 * n, cudaMemcpyHostToDevice, st));
-    }
+    for (int k = 0; k < 7; k++) CUDA_TRY(A.upload(&d_rows[k], (const uint32_t*)src[k], n, st, 4));
     CUDA_TRY(A.alloc(&d_first, n_pep + 4));
     CUDA_TRY(A.alloc(&d_flag, n_pep + 16));
     CUDA_TRY(A.alloc(&d_slots, n_pep + 4));
     CUDA_TRY(A.alloc(&d_nsel, 4));
     CUDA_TRY(cudaMemsetAsync(d_first, 0xFF, 4 * n_pep, st));
-    if (n)
-        k_lfq_first_row<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, d_rows[0], (const float*)d_rows[1], (const int32_t*)d_rows[2], L->p.peptide_q_value,
-                                                                       d_first);
-    if (n_pep) k_lfq_flag<<<(unsigned)((n_pep + 255) / 256), 256, 0, st>>>(n_pep, d_first, d_flag);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_lfq_first_row, n, st, n, d_rows[0], (const float*)d_rows[1], (const int32_t*)d_rows[2], L->p.peptide_q_value, d_first);
+    LAUNCH_N(k_lfq_flag, n_pep, st, n_pep, d_first, d_flag);
     thrust::counting_iterator<uint32_t> it(0);
     CUDA_TRY(L->tmp.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, d_flag, d_slots, d_nsel, (int)n_pep, st); }));
     uint32_t n_slots = 0;
-    CUDA_TRY(cudaMemcpyAsync(&n_slots, d_nsel, 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    if (int rc = read_back(st, &n_slots, d_nsel, 4)) return rc;
     std::vector<uint32_t> slot_pep(n_slots);
-    if (n_slots) CUDA_TRY(cudaMemcpyAsync(slot_pep.data(), d_slots, 4ull * n_slots, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    if (n_slots)
+        if (int rc = read_back(st, slot_pep.data(), d_slots, 4ull * n_slots)) return rc;
 
     L->n_slots = n_slots;
     L->slot_pep = slot_pep;
@@ -2275,24 +2322,17 @@ static int lfq_build(sage_b200_lfq* L, const sage_b200_db* db, const sage_b200_p
     CUDA_TRY(L->fixed.alloc(&L->d_min_rts, L->n_pages));
     CUDA_TRY(L->fixed.alloc(&L->d_slot_dist, 3ull * n_slots));
     CUDA_TRY(L->fixed.alloc(&L->d_slot_file, n_slots));
-    CUDA_TRY(L->fixed.alloc(&L->d_touched, L->n_grids));
-    CUDA_TRY(L->fixed.alloc(&L->d_align, L->n_files));
-    CUDA_TRY(L->fixed.alloc(&L->d_consts, LFQ_K_WIDTH + LFQ_GRID));
-    CUDA_TRY(L->fixed.alloc(&L->d_grids, cells));
-    CUDA_TRY(cudaMemsetAsync(L->d_grids, 0, grid_bytes, st));
-    CUDA_TRY(cudaMemsetAsync(L->d_touched, 0, L->n_grids, st));
-    CUDA_TRY(cudaMemcpyAsync(L->d_align, align, sizeof(sage_b200_alignment) * L->n_files, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(L->d_consts, consts, sizeof consts, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(L->fixed.zeros(&L->d_touched, L->n_grids, st));
+    CUDA_TRY(L->fixed.upload(&L->d_align, align, L->n_files, st));
+    CUDA_TRY(L->fixed.upload(&L->d_consts, consts, LFQ_K_WIDTH + LFQ_GRID, st));
+    CUDA_TRY(L->fixed.zeros(&L->d_grids, cells, st));
     if (n_slots) {
-        uint16_t* d_cs = nullptr;
+        uint16_t *d_c = nullptr, *d_s = nullptr;
         float* d_exp = nullptr;
-        CUDA_TRY(A.alloc(&d_cs, 2ull * n_slots));
-        CUDA_TRY(A.alloc(&d_exp, expt.size()));
-        CUDA_TRY(cudaMemcpyAsync(d_cs, carbon.data(), 2ull * n_slots, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(d_cs + n_slots, sulfur.data(), 2ull * n_slots, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(d_exp, expt.data(), 4 * expt.size(), cudaMemcpyHostToDevice, st));
-        k_lfq_isotopes<<<(n_slots + 255) / 256, 256, 0, st>>>(n_slots, d_cs, d_cs + n_slots, d_exp, d_exp + max_c + 1, d_exp + max_c + 1 + max_s + 1, L->d_slot_dist);
-        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(A.upload(&d_c, carbon.data(), n_slots, st));
+        CUDA_TRY(A.upload(&d_s, sulfur.data(), n_slots, st));
+        CUDA_TRY(A.upload(&d_exp, expt.data(), expt.size(), st));
+        LAUNCH_N(k_lfq_isotopes, n_slots, st, n_slots, d_c, d_s, d_exp, d_exp + max_c + 1, d_exp + max_c + 1 + max_s + 1, L->d_slot_dist);
 
         // expansion, stable RT sort, stable per-page mass_lo sort (lfq.rs:134-184)
         const uint32_t nr = (uint32_t)L->n_ranges, nt = (uint32_t)(n_slots * L->n_charges * LFQ_ISO);
@@ -2306,22 +2346,18 @@ static int lfq_build(sage_b200_lfq* L, const sage_b200_db* db, const sage_b200_p
             CUDA_TRY(B.alloc(&v32[k], nr));
         }
         CUDA_TRY(B.alloc(&k64, nr));
-        k_lfq_expand<<<(nt + 255) / 256, 256, 0, st>>>(n_slots, L->n_charges, L->p.min_precursor_charge, L->p.ppm_tolerance, L->p.mobility_pct_tolerance,
-                                                      d_slots, d_first, (const float*)d_rows[3], (const float*)d_rows[4], d_rows[5], (const float*)d_rows[6], pre,
-                                                      k32[0], v32[0], L->d_slot_file);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH_N(k_lfq_expand, nt, st, n_slots, L->n_charges, L->p.min_precursor_charge, L->p.ppm_tolerance, L->p.mobility_pct_tolerance, d_slots, d_first,
+                 (const float*)d_rows[3], (const float*)d_rows[4], d_rows[5], (const float*)d_rows[6], pre, k32[0], v32[0], L->d_slot_file);
         size_t tb = 0, tb2 = 0;
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, k32[0], k32[1], v32[0], v32[1], (int)nr, 0, 32, st));
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb2, k64, k64, v32[1], v32[0], (int)nr, 0, 64, st));
         if (int rc = L->tmp.reserve(std::max(tb, tb2))) return rc;
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(L->tmp.p, tb, k32[0], k32[1], v32[0], v32[1], (int)nr, 0, 32, st));
-        k_lfq_page_keys<<<(nr + 255) / 256, 256, 0, st>>>(nr, v32[1], pre, k64, L->d_min_rts);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH_N(k_lfq_page_keys, nr, st, nr, v32[1], pre, k64, L->d_min_rts);
         CUDA_TRY(B.alloc(&k64o, nr));
         const int end_bit = 32 + (int)ceil_log2_u64(L->n_pages + 1);
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(L->tmp.p, tb2, k64, k64o, v32[1], v32[0], (int)nr, 0, end_bit, st));
-        k_lfq_gather<<<(nr + 255) / 256, 256, 0, st>>>(nr, L->n_charges, L->p.combine_charge_states, v32[0], pre, L->d_ranges, L->d_grid_of);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH_N(k_lfq_gather, nr, st, nr, L->n_charges, L->p.combine_charge_states, v32[0], pre, L->d_ranges, L->d_grid_of);
         CUDA_TRY(cudaStreamSynchronize(st));
     }
     return lfq_elapsed(L, L->info.ms_build);
@@ -2406,8 +2442,7 @@ static int lfq_trace_chunk(sage_b200_lfq* L, const sage_b200_ms1* m, uint64_t a,
     t.min_rts = (const float*)L->d_min_rts;
     t.counts = L->counts.as<uint64_t>();
     const unsigned blocks = (unsigned)((ns * 32 + LFQ_THREADS - 1) / LFQ_THREADS);
-    k_lfq_trace<false><<<blocks, LFQ_THREADS, 0, st>>>(t);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_lfq_trace<false><<<blocks, LFQ_THREADS, 0, st>>>(t));
     CUDA_TRY(L->tmp.two_phase([&](void* tmp, size_t& b) { return cub::DeviceScan::ExclusiveSum(tmp, b, L->counts.as<uint64_t>(), L->offsets.as<uint64_t>(), (int)np, st); }));
     uint64_t last[2] = {0, 0};
     CUDA_TRY(cudaMemcpyAsync(&last[0], L->offsets.as<uint64_t>() + np - 1, 8, cudaMemcpyDeviceToHost, st));
@@ -2421,17 +2456,15 @@ static int lfq_trace_chunk(sage_b200_lfq* L, const sage_b200_ms1* m, uint64_t a,
     t.offsets = L->offsets.as<uint64_t>();
     t.cell = L->cell[0].as<uint64_t>();
     t.value = L->value[0].as<double>();
-    k_lfq_trace<true><<<blocks, LFQ_THREADS, 0, st>>>(t);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_lfq_trace<true><<<blocks, LFQ_THREADS, 0, st>>>(t));
     const uint64_t cells = L->n_grids * L->n_files * LFQ_ISO * LFQ_GRID;
     const int end_bit = std::max(1, (int)ceil_log2_u64(cells));
     CUDA_TRY(L->tmp.two_phase([&](void* tmp, size_t& b) {
         return cub::DeviceRadixSort::SortPairs(tmp, b, L->cell[0].as<uint64_t>(), L->cell[1].as<uint64_t>(), L->value[0].as<double>(), L->value[1].as<double>(),
                                                (int)nc, 0, end_bit, st);
     }));
-    k_lfq_fold<<<(unsigned)((nc + 255) / 256), 256, 0, st>>>(nc, L->cell[1].as<uint64_t>(), L->value[1].as<double>(), (double*)L->d_grids,
-                                                            (uint8_t*)L->d_touched, (uint64_t)L->n_files * LFQ_ISO * LFQ_GRID);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_lfq_fold, nc, st, nc, L->cell[1].as<uint64_t>(), L->value[1].as<double>(), (double*)L->d_grids, (uint8_t*)L->d_touched,
+             (uint64_t)L->n_files * LFQ_ISO * LFQ_GRID);
     L->info.contributions += nc;
     return 0;
 }
@@ -2478,8 +2511,7 @@ extern "C" int sage_b200_lfq_integrate(sage_b200_lfq* L, sage_b200_lfq_row* rows
         return cub::DeviceSelect::Flagged(t, b, it, (const uint8_t*)L->d_touched, L->ids.as<uint32_t>(), d_n, (int)L->n_grids, st);
     }));
     uint32_t nt = 0;
-    CUDA_TRY(cudaMemcpyAsync(&nt, d_n, 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    if ((rc = read_back(st, &nt, d_n, 4))) return rc;
     L->info.grids_touched = nt;
     if (nt == 0) { L->info.ms_integrate = 0.0f; return lfq_elapsed(L, L->info.ms_integrate); }
     if ((rc = L->o_rt.reserve(4ull * nt)) || (rc = L->o_sa.reserve(8ull * nt)) || (rc = L->o_score.reserve(8ull * nt)) || (rc = L->o_areas.reserve(8ull * nt * F)))
@@ -2504,8 +2536,7 @@ extern "C" int sage_b200_lfq_integrate(sage_b200_lfq* L, sage_b200_lfq_row* rows
     a.sa = L->o_sa.as<double>();
     a.score = L->o_score.as<double>();
     a.areas = L->o_areas.as<double>();
-    k_lfq_integrate<<<nt, LFQ_THREADS, smem, st>>>(a);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_lfq_integrate<<<nt, LFQ_THREADS, smem, st>>>(a));
     L->info.ms_integrate = 0.0f;
     if ((rc = lfq_elapsed(L, L->info.ms_integrate))) return rc;
 
@@ -2555,11 +2586,12 @@ extern "C" int sage_b200_lfq_export(sage_b200_lfq* L, sage_b200_lfq_range* range
     if (!L) return fail(SAGE_B200_EINVAL, "lfq_export: null handle");
     std::lock_guard<std::mutex> lock(L->mu);
     CUDA_TRY(cudaSetDevice(L->device));
-    CUDA_TRY(cudaStreamSynchronize(L->st));
-    if (ranges && L->n_ranges) CUDA_TRY(cudaMemcpy(ranges, L->d_ranges, sizeof(sage_b200_lfq_range) * L->n_ranges, cudaMemcpyDeviceToHost));
-    if (min_rts && L->n_pages) CUDA_TRY(cudaMemcpy(min_rts, L->d_min_rts, 4 * L->n_pages, cudaMemcpyDeviceToHost));
-    if (grids && L->n_grids) CUDA_TRY(cudaMemcpy(grids, L->d_grids, 8 * L->n_grids * L->n_files * LFQ_ISO * LFQ_GRID, cudaMemcpyDeviceToHost));
-    if (touched && L->n_grids) CUDA_TRY(cudaMemcpy(touched, L->d_touched, L->n_grids, cudaMemcpyDeviceToHost));
+    cudaStream_t st = L->st;
+    if (ranges && L->n_ranges) CUDA_TRY(cudaMemcpyAsync(ranges, L->d_ranges, sizeof(sage_b200_lfq_range) * L->n_ranges, cudaMemcpyDeviceToHost, st));
+    if (min_rts && L->n_pages) CUDA_TRY(cudaMemcpyAsync(min_rts, L->d_min_rts, 4 * L->n_pages, cudaMemcpyDeviceToHost, st));
+    if (grids && L->n_grids) CUDA_TRY(cudaMemcpyAsync(grids, L->d_grids, 8 * L->n_grids * L->n_files * LFQ_ISO * LFQ_GRID, cudaMemcpyDeviceToHost, st));
+    if (touched && L->n_grids) CUDA_TRY(cudaMemcpyAsync(touched, L->d_touched, L->n_grids, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
@@ -2570,10 +2602,9 @@ extern "C" int sage_b200_lfq_export(sage_b200_lfq* L, sage_b200_lfq_range* range
 static int host_math_variant() {
     static const int variant = []() {   // initialised once, thread-safe
         uint64_t st = 0x853C49E6748FEA9Bull;
-        auto next = [&]() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return st; };
         bool ok[2] = {true, true};
         for (int i = 0; i < 9000; i++) {
-            const uint64_t u = next();
+            const uint64_t u = xorshift64(st);
             const double unit = (double)(u >> 11) * 0x1p-53;
             const int f = i % 3;
             const double x = f == 0 ? -0.5 * (unit * 40.0) * (unit * 40.0) : f == 1 ? unit * 200.0 - 0.5 : unit * (1.0 + (double)(u & 7));
@@ -2658,13 +2689,10 @@ static int fdr_kde(cudaStream_t st, DevArena& A, const double* d_scores, const u
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_scores, d_decoy, d_sel, d_nsel, (int64_t)n, st); }));   // decoys in row order
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_scores, d_target, d_sel + n, d_nsel + 1, (int64_t)n, st); }));   // targets in row order
     uint64_t m[2];
-    CUDA_TRY(cudaMemcpyAsync(m, d_nsel, 16, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    k_fdr_kde_moments<<<1, 256, 0, st>>>(d_sel, m[0], d_sel + n, m[1], d_scores, n, d_moments);
-    CUDA_TRY(cudaGetLastError());
+    if (int rc = read_back(st, m, d_nsel, 16)) return rc;
+    LAUNCH(k_fdr_kde_moments<<<1, 256, 0, st>>>(d_sel, m[0], d_sel + n, m[1], d_scores, n, d_moments));
     double mom[2];
-    CUDA_TRY(cudaMemcpyAsync(mom, d_moments, 16, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    if (int rc = read_back(st, mom, d_moments, 16)) return rc;
     double cst[2];
     uint32_t chunks[2];
     for (int c = 0; c < 2; c++) {   // Kde::new (kde.rs:21-32): the bandwidth and normalising constant, host libm pow / sqrt
@@ -2675,16 +2703,13 @@ static int fdr_kde(cudaStream_t st, DevArena& A, const double* d_scores, const u
         CUDA_TRY(A.alloc(&part[c], (size_t)bins * chunks[c]));
         if (chunks[c]) {
             const dim3 grid((bins + 127) / 128, chunks[c]);
-            if (fma) k_fdr_kde_bins<true><<<grid, 128, 0, st>>>(d_sel + c * n, m[c], bins, chunks[c], d_moments, bw, part[c]);
-            else k_fdr_kde_bins<false><<<grid, 128, 0, st>>>(d_sel + c * n, m[c], bins, chunks[c], d_moments, bw, part[c]);
-            CUDA_TRY(cudaGetLastError());
+            if (fma) LAUNCH(k_fdr_kde_bins<true><<<grid, 128, 0, st>>>(d_sel + c * n, m[c], bins, chunks[c], d_moments, bw, part[c]));
+            else LAUNCH(k_fdr_kde_bins<false><<<grid, 128, 0, st>>>(d_sel + c * n, m[c], bins, chunks[c], d_moments, bw, part[c]));
         }
     }
     const double pi = (double)m[0] / (double)n;
-    k_fdr_kde_pep<<<(bins + 127) / 128, 128, 0, st>>>(part[0], chunks[0], part[1], chunks[1], bins, cst[0], cst[1], pi, monotonic, d_out_bins);
-    CUDA_TRY(cudaGetLastError());
-    if (monotonic) k_fdr_kde_monotone<<<1, 1, 0, st>>>(d_out_bins, bins);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_fdr_kde_pep<<<(bins + 127) / 128, 128, 0, st>>>(part[0], chunks[0], part[1], chunks[1], bins, cst[0], cst[1], pi, monotonic, d_out_bins));
+    if (monotonic) LAUNCH(k_fdr_kde_monotone<<<1, 1, 0, st>>>(d_out_bins, bins));
     return 0;
 }
 
@@ -2693,22 +2718,23 @@ extern "C" int sage_b200_kde_build(int device, const double* scores, const uint8
     if (n == 0 || !scores || !decoy || !out_bins || !min_score || !score_step || bins < 2) return fail(SAGE_B200_EINVAL, "kde_build: bad argument");
     if (n > (uint64_t)INT32_MAX || bins > (1u << 24)) return fail(SAGE_B200_ELIMIT, "kde_build: n or bins too large");
     if (int rc = select_device(device)) return rc;
-    DevArena A;
-    double *d_s = nullptr, *d_bins = nullptr, *d_mom = nullptr;
-    uint8_t* d_flags = nullptr;
-    CUDA_TRY(A.alloc(&d_s, n));
-    CUDA_TRY(A.alloc(&d_flags, 2 * n));
-    CUDA_TRY(A.alloc(&d_bins, bins));
-    CUDA_TRY(A.alloc(&d_mom, 4));
     std::vector<uint8_t> flags(2 * n);
     for (uint64_t i = 0; i < n; i++) { flags[i] = decoy[i] != 0; flags[n + i] = decoy[i] == 0; }
-    CUDA_TRY(cudaMemcpy(d_s, scores, 8 * n, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(d_flags, flags.data(), 2 * n, cudaMemcpyHostToDevice));
+    DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
+    double *d_s = nullptr, *d_bins = nullptr, *d_mom = nullptr;
+    uint8_t* d_flags = nullptr;
+    CUDA_TRY(A.upload(&d_s, scores, n, st));
+    CUDA_TRY(A.upload(&d_flags, flags.data(), 2 * n, st));
+    CUDA_TRY(A.alloc(&d_bins, bins));
+    CUDA_TRY(A.alloc(&d_mom, 4));
     const int v = host_math_variant();
-    if (int rc = fdr_kde(0, A, d_s, d_flags, d_flags + n, n, (uint32_t)bins, monotonic != 0, bw_factor, v != 1, d_bins, d_mom)) return rc;
+    if (int rc = fdr_kde(st, A, d_s, d_flags, d_flags + n, n, (uint32_t)bins, monotonic != 0, bw_factor, v != 1, d_bins, d_mom)) return rc;
     double mom[4];
-    CUDA_TRY(cudaMemcpy(out_bins, d_bins, 8 * bins, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(mom, d_mom, 32, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpyAsync(out_bins, d_bins, 8 * bins, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(mom, d_mom, 32, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     *min_score = mom[2];
     *score_step = (mom[3] - mom[2]) / (double)(bins - 1);
     return 0;
@@ -2720,16 +2746,14 @@ extern "C" int sage_b200_device_math(int device, int function, int variant, cons
     if (int rc = select_device(device)) return rc;
     if (variant == -1) variant = host_math_variant() == 1 ? 1 : 0;
     DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
     double *dx = nullptr, *dy = nullptr;
-    CUDA_TRY(A.alloc(&dx, n));
+    CUDA_TRY(A.upload(&dx, x, n, st));
     CUDA_TRY(A.alloc(&dy, n));
-    CUDA_TRY(cudaMemcpy(dx, x, 8 * n, cudaMemcpyHostToDevice));
-    const unsigned g = (unsigned)((n + 255) / 256);
-    if (variant == 0) k_device_math<true><<<g, 256>>>(function, dx, n, dy);
-    else k_device_math<false><<<g, 256>>>(function, dx, n, dy);
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaMemcpy(out, dy, 8 * n, cudaMemcpyDeviceToHost));
-    return 0;
+    if (variant == 0) LAUNCH_N(k_device_math<true>, n, st, function, dx, n, dy);
+    else LAUNCH_N(k_device_math<false>, n, st, function, dx, n, dy);
+    return read_back(st, out, dy, 8 * n);
 }
 
 struct MinF {
@@ -2743,22 +2767,18 @@ template <class Key>
 static int spectrum_q_values(cudaStream_t st, DevArena& A, const sage_b200_feature* d_rows, uint64_t n, const Key* d_key, Key* d_key_sorted,
                              const uint32_t* d_idx, uint32_t* d_isdec, uint32_t* d_dscan, float* d_rq, float* d_rqmin, uint32_t* d_order, float* d_q,
                              unsigned long long* d_passing) {
-    const unsigned g = (unsigned)((n + 255) / 256);
     size_t tb = 0, tb2 = 0, tb3 = 0;
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, d_key, d_key_sorted, d_idx, d_order, (int)n, 0, 8 * (int)sizeof(Key), st));
     CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, tb2, d_isdec, d_dscan, (int)n, st));
     CUDA_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
     CUDA_TRY(A.reserve_tmp(std::max(tb, std::max(tb2, tb3))));
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, d_key, d_key_sorted, d_idx, d_order, (int)n, 0, 8 * (int)sizeof(Key), st));
-    k_fdr_sorted_decoy<<<g, 256, 0, st>>>(d_rows, d_order, n, d_isdec);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_fdr_sorted_decoy, n, st, d_rows, d_order, n, d_isdec);
     CUDA_TRY(cub::DeviceScan::InclusiveSum(A.tmp, tb2, d_isdec, d_dscan, (int)n, st));
-    k_fdr_q_raw<<<g, 256, 0, st>>>(d_dscan, n, d_rq);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_fdr_q_raw, n, st, d_dscan, n, d_rq);
     CUDA_TRY(cub::DeviceScan::InclusiveScan(A.tmp, tb3, d_rq, d_rqmin, MinF(), (int)n, st));
     CUDA_TRY(cudaMemsetAsync(d_passing, 0, 8, st));
-    k_fdr_q_out<<<g, 256, 0, st>>>(d_rqmin, d_order, n, d_q, d_passing);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_fdr_q_out, n, st, d_rqmin, d_order, n, d_q, d_passing);
     return 0;
 }
 
@@ -2801,7 +2821,8 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
     }
 
     DevArena A;
-    cudaStream_t st = 0;
+    Stream st;
+    CUDA_TRY(st.create());
     Event ev[6];
     for (Event& e : ev) CUDA_TRY(e.create());
     sage_b200_feature* d_rows = nullptr;
@@ -2812,7 +2833,7 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
     float *d_disc32 = nullptr, *d_pep = nullptr, *d_q = nullptr, *d_rq = nullptr, *d_rqmin = nullptr, *d_cols[3] = {nullptr, nullptr, nullptr};
     uint32_t *d_key = nullptr, *d_key2 = nullptr, *d_idx = nullptr, *d_order = nullptr, *d_isdec = nullptr, *d_dscan = nullptr;
     unsigned long long* d_passing = nullptr;
-    CUDA_TRY(A.alloc(&d_rows, n));
+    CUDA_TRY(A.upload(&d_rows, rows, n, st));
     CUDA_TRY(A.alloc(&d_mass, n));
     CUDA_TRY(A.alloc(&d_flags, 2 * n));
     CUDA_TRY(A.alloc(&d_mbins, mbins));
@@ -2839,28 +2860,20 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
     CUDA_TRY(A.alloc(&d_passing, 1));
     const float* cols_h[3] = {aligned_rt, delta_rt_model, delta_ims_model};
     for (int c = 0; c < 3; c++)
-        if (cols_h[c]) {
-            CUDA_TRY(A.alloc(&d_cols[c], n));
-            CUDA_TRY(cudaMemcpy(d_cols[c], cols_h[c], 4 * n, cudaMemcpyHostToDevice));
-        }
-    CUDA_TRY(cudaMemcpy(d_rows, rows, sizeof(sage_b200_feature) * n, cudaMemcpyHostToDevice));
-    const unsigned g = (unsigned)((n + 255) / 256);
+        if (cols_h[c]) CUDA_TRY(A.upload(&d_cols[c], cols_h[c], n, st));
 
     // 1. mass-error KDE (linear_discriminant.rs:140-158)
     CUDA_TRY(cudaEventRecord(ev[0], st));
-    k_fdr_mass<<<g, 256, 0, st>>>(d_rows, n, kind, d_mass, d_flags, d_flags + n);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_fdr_mass, n, st, d_rows, n, kind, d_mass, d_flags, d_flags + n);
     if (int rc = fdr_kde(st, A, d_mass, d_flags, d_flags + n, n, mbins, false, bw_factor, fma, d_mbins, d_mmom)) return rc;
     CUDA_TRY(cudaEventRecord(ev[1], st));
     // 2. feature rows (linear_discriminant.rs:162-193)
     const FdrColumns cols{d_cols[0], d_cols[1], d_cols[2]};
-    if (fma) k_fdr_features<true><<<g, 256, 0, st>>>(d_rows, n, cols, d_mass, d_mbins, mbins, d_mmom, d_X);
-    else k_fdr_features<false><<<g, 256, 0, st>>>(d_rows, n, cols, d_mass, d_mbins, mbins, d_mmom, d_X);
-    CUDA_TRY(cudaGetLastError());
+    if (fma) LAUNCH_N(k_fdr_features<true>, n, st, d_rows, n, cols, d_mass, d_mbins, mbins, d_mmom, d_X);
+    else LAUNCH_N(k_fdr_features<false>, n, st, d_rows, n, cols, d_mass, d_mbins, mbins, d_mmom, d_X);
     CUDA_TRY(cudaEventRecord(ev[2], st));
     // 3. LDA class sums and scatter on the device, Gauss::solve on the host (linear_discriminant.rs:63-124, 195-208)
-    k_fdr_lda<<<2, 256, 0, st>>>(d_X, d_flags, n, d_means, d_scatter, d_counts);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_fdr_lda<<<2, 256, 0, st>>>(d_X, d_flags, n, d_means, d_scatter, d_counts));
     std::vector<double> means(2 * FDR_FEATURES), scatter(2 * FDR_FEATURES * FDR_FEATURES);
     uint64_t counts[2];
     CUDA_TRY(cudaMemcpyAsync(means.data(), d_means, 8 * means.size(), cudaMemcpyDeviceToHost, st));
@@ -2886,19 +2899,16 @@ extern "C" int sage_b200_spectrum_fdr(int device, const sage_b200_fdr_params* p,
     // 4. projection, discriminant KDE and posterior errors (linear_discriminant.rs:209-228), or the fallback (runner.rs:284-287)
     if (fitted) {
         CUDA_TRY(cudaMemcpyAsync(d_coef, out->coef, 8 * FDR_FEATURES, cudaMemcpyHostToDevice, st));
-        k_fdr_project<<<g, 256, 0, st>>>(d_X, n, d_coef, d_disc, d_disc32);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH_N(k_fdr_project, n, st, d_X, n, d_coef, d_disc, d_disc32);
         if (int rc = fdr_kde(st, A, d_disc, d_flags, d_flags + n, n, 1000, true, 1.0, fma, d_dbins, d_dmom)) return rc;
-        if (fma) k_fdr_pep<true><<<g, 256, 0, st>>>(d_disc, n, d_dbins, 1000, d_dmom, d_pep);
-        else k_fdr_pep<false><<<g, 256, 0, st>>>(d_disc, n, d_dbins, 1000, d_dmom, d_pep);
+        if (fma) LAUNCH_N(k_fdr_pep<true>, n, st, d_disc, n, d_dbins, 1000, d_dmom, d_pep);
+        else LAUNCH_N(k_fdr_pep<false>, n, st, d_disc, n, d_dbins, 1000, d_dmom, d_pep);
     } else {
-        k_fdr_fallback<<<g, 256, 0, st>>>(d_rows, n, d_disc32, d_pep);
+        LAUNCH_N(k_fdr_fallback, n, st, d_rows, n, d_disc32, d_pep);
     }
-    CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(ev[4], st));
     // 5. stable descending sort (ties by input row) and spectrum_q_value (qvalue.rs)
-    k_fdr_sort_key<<<g, 256, 0, st>>>(d_disc32, n, d_key, d_idx);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_fdr_sort_key, n, st, d_disc32, n, d_key, d_idx);
     if (int rc = spectrum_q_values(st, A, d_rows, n, d_key, d_key2, d_idx, d_isdec, d_dscan, d_rq, d_rqmin, d_order, d_q, d_passing)) return rc;
     CUDA_TRY(cudaEventRecord(ev[5], st));
     unsigned long long passing = 0;
@@ -2935,15 +2945,12 @@ static int rt_model(cudaStream_t st, DevArena& A, bool fma, const RtPeptides& P,
         double *d_part = nullptr, *d_acc = nullptr, *d_sse = nullptr, *d_beta = nullptr;
         CUDA_TRY(A.alloc(&d_part, n_chunks * Dm::NACC));
         CUDA_TRY(A.alloc(&d_acc, Dm::NACC));
-        const dim3 grid((unsigned)n_chunks, (Dm::NACC + 255) / 256);
-        if (fma) k_rt_accumulate<MODEL, true><<<grid, 256, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_part);
-        else k_rt_accumulate<MODEL, false><<<grid, 256, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_part);
-        CUDA_TRY(cudaGetLastError());
-        k_rt_merge<<<(Dm::NACC + 255) / 256, 256, 0, st>>>(d_part, n_chunks, Dm::NACC, d_acc);
-        CUDA_TRY(cudaGetLastError());
+        const dim3 grid((unsigned)n_chunks, grid256(Dm::NACC));
+        if (fma) LAUNCH(k_rt_accumulate<MODEL, true><<<grid, 256, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_part));
+        else LAUNCH(k_rt_accumulate<MODEL, false><<<grid, 256, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_part));
+        LAUNCH_N(k_rt_merge, Dm::NACC, st, d_part, n_chunks, Dm::NACC, d_acc);
         std::vector<double> acc(Dm::NACC);
-        CUDA_TRY(cudaMemcpyAsync(acc.data(), d_acc, 8 * Dm::NACC, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
+        if (int rc = read_back(st, acc.data(), d_acc, 8 * Dm::NACC)) return rc;
         HostMat cov(D, D), b(D, 1);
         for (int j = 0, a = 0; j < D; j++)
             for (int k = j; k < D; k++, a++) cov(j, k) = cov(k, j) = acc[a];
@@ -2951,30 +2958,25 @@ static int rt_model(cudaStream_t st, DevArena& A, bool fma, const RtPeptides& P,
         const double sum_y = acc[Dm::NCOV + D], sum_y2 = acc[Dm::NCOV + D + 1];
         const double nf = (double)n_train, y_mean = sum_y / nf, y_var = sum_y2 - nf * y_mean * y_mean;
         if (gauss_solve(cov, b, &beta, eps)) {
-            CUDA_TRY(A.alloc(&d_beta, D));
+            CUDA_TRY(A.upload(&d_beta, beta.data(), D, st));
             CUDA_TRY(A.alloc(&d_sse, n_chunks));
-            CUDA_TRY(cudaMemcpyAsync(d_beta, beta.data(), 8 * D, cudaMemcpyHostToDevice, st));
-            if (fma) k_rt_sse<MODEL, true><<<(unsigned)n_chunks, 32, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_beta, d_sse);
-            else k_rt_sse<MODEL, false><<<(unsigned)n_chunks, 32, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_beta, d_sse);
-            CUDA_TRY(cudaGetLastError());
+            if (fma) LAUNCH(k_rt_sse<MODEL, true><<<(unsigned)n_chunks, 32, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_beta, d_sse));
+            else LAUNCH(k_rt_sse<MODEL, false><<<(unsigned)n_chunks, 32, 0, st>>>(P, d_rows, d_train, n_train, d_ycol, d_beta, d_sse));
             std::vector<double> chunk_sse(n_chunks);
-            CUDA_TRY(cudaMemcpyAsync(chunk_sse.data(), d_sse, 8 * n_chunks, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaStreamSynchronize(st));
+            if (int rc = read_back(st, chunk_sse.data(), d_sse, 8 * n_chunks)) return rc;
             double sse = -0.0;   // f64 Sum of the chunk sums, in chunk order
             for (double s : chunk_sse) sse = sse + s;
             *r2 = 1.0 - sse / y_var;
             *fitted = 1;
             std::copy(beta.begin(), beta.end(), beta_out);
             const unsigned g = (unsigned)((n + RT_TILE - 1) / RT_TILE);
-            if (fma) k_rt_predict<MODEL, true><<<g, 32, 0, st>>>(P, d_rows, n, d_beta, d_aligned, d_pred, d_delta);
-            else k_rt_predict<MODEL, false><<<g, 32, 0, st>>>(P, d_rows, n, d_beta, d_aligned, d_pred, d_delta);
-            CUDA_TRY(cudaGetLastError());
+            if (fma) LAUNCH(k_rt_predict<MODEL, true><<<g, 32, 0, st>>>(P, d_rows, n, d_beta, d_aligned, d_pred, d_delta));
+            else LAUNCH(k_rt_predict<MODEL, false><<<g, 32, 0, st>>>(P, d_rows, n, d_beta, d_aligned, d_pred, d_delta));
             return 0;
         }
         *eps = 0.0;
     }
-    k_rt_defaults<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, d_pred, d_delta);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_rt_defaults, n, st, n, d_pred, d_delta);
     return 0;
 }
 
@@ -3033,7 +3035,8 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
     }
     const bool fma = host_math_variant() != 1;
     DevArena A;
-    cudaStream_t st = 0;
+    Stream st;
+    CUDA_TRY(st.create());
     Event ev[5];
     for (Event& e : ev) CUDA_TRY(e.create());
     sage_b200_feature* d_rows = nullptr;
@@ -3046,11 +3049,11 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
     unsigned long long* d_passing = nullptr;
     double *d_segmin = nullptr, *d_mat = nullptr, *d_mean = nullptr;
     sage_b200_alignment* d_align = nullptr;
-    CUDA_TRY(A.alloc(&d_rows, n));
-    CUDA_TRY(A.alloc(&d_file, n));
-    CUDA_TRY(A.alloc(&d_off, n_pep + 1));
-    CUDA_TRY(A.alloc(&d_seq, nres));
-    CUDA_TRY(A.alloc(&d_mono, n_pep));
+    CUDA_TRY(A.upload(&d_rows, rows, n, st));
+    CUDA_TRY(A.upload(&d_file, file_id, n, st));
+    CUDA_TRY(A.upload(&d_off, P->residue_offsets, n_pep + 1, st));
+    CUDA_TRY(A.upload(&d_seq, P->sequence, nres, st));
+    CUDA_TRY(A.upload(&d_mono, P->monoisotopic, n_pep, st));
     CUDA_TRY(A.alloc(&d_key, n));
     CUDA_TRY(A.alloc(&d_key2, n));
     CUDA_TRY(A.alloc(&d_idx, n));
@@ -3074,59 +3077,37 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
     CUDA_TRY(A.alloc(&d_maxrt, n_files));
     CUDA_TRY(A.alloc(&d_align, n_files));
     for (auto& o : d_out) CUDA_TRY(A.alloc(&o, n));
-    CUDA_TRY(cudaMemcpyAsync(d_rows, rows, sizeof(sage_b200_feature) * n, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_file, file_id, 4 * n, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_off, P->residue_offsets, 4 * (n_pep + 1), cudaMemcpyHostToDevice, st));
-    if (nres) CUDA_TRY(cudaMemcpyAsync(d_seq, P->sequence, nres, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_mono, P->monoisotopic, 4 * n_pep, cudaMemcpyHostToDevice, st));
     const RtPeptides pk{d_off, d_seq, d_mono};
-    const unsigned g = (unsigned)((n + 255) / 256);
     thrust::counting_iterator<uint32_t> count_it(0);
-    auto read_count = [&](uint64_t* v) -> int {
-        uint32_t c = 0;
-        CUDA_TRY(cudaMemcpyAsync(&c, d_count, 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        *v = c;
-        return 0;
-    };
 
     // 1. par_sort_unstable_by(poisson.total_cmp), ties by input row, then spectrum_q_value (runner.rs:517-520)
     CUDA_TRY(cudaEventRecord(ev[0], st));
-    k_rt_poisson_key<<<g, 256, 0, st>>>(d_rows, n, d_key, d_idx);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_rt_poisson_key, n, st, d_rows, n, d_key, d_idx);
     if (int rc = spectrum_q_values(st, A, d_rows, n, d_key, d_key2, d_idx, d_isdec, d_dscan, d_rq, d_rqmin, d_order, d_q, d_passing)) return rc;
     // the training rows (label == 1 && spectrum_q <= 0.01) in poisson order
-    k_rt_train_flag<<<g, 256, 0, st>>>(d_rows, d_order, d_q, n, d_flag);
-    CUDA_TRY(cudaGetLastError());
-    uint64_t n_train = 0;
+    LAUNCH_N(k_rt_train_flag, n, st, d_rows, d_order, d_q, n, d_flag);
+    uint32_t n_train = 0;
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_order, d_flag, d_train, d_count, (int)n, st); }));
-    if (int rc = read_count(&n_train)) return rc;
+    if (int rc = read_back(st, &n_train, d_count, 4)) return rc;
     CUDA_TRY(cudaEventRecord(ev[1], st));
 
     // 2. global_alignment (retention_alignment.rs:95-173)
     CUDA_TRY(cudaMemsetAsync(d_maxrt, 0, 4 * n_files, st));
-    k_rt_max_rt<<<g, 256, 0, st>>>(d_rows, d_file, n, d_maxrt);
-    CUDA_TRY(cudaGetLastError());
-    uint64_t n_seg = 0, n_pr = 0, n_rows = 0;
+    LAUNCH_N(k_rt_max_rt, n, st, d_rows, d_file, n, d_maxrt);
+    uint32_t n_seg = 0, n_pr = 0;
+    uint64_t n_rows = 0;
     if (n_train) {
-        const unsigned gt = (unsigned)((n_train + 255) / 256);
-        k_rt_pf_key<<<gt, 256, 0, st>>>(d_rows, d_file, d_train, n_train, d_key);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH_N(k_rt_pf_key, n_train, st, d_rows, d_file, d_train, n_train, d_key);
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) {   // stable: poisson order kept
             return cub::DeviceRadixSort::SortPairs(t, b, d_key, d_key2, d_train, d_val, (int)n_train, 0, 64, st);
         }));
-        k_rt_heads<<<gt, 256, 0, st>>>(d_key2, n_train, d_flag);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH_N(k_rt_heads, n_train, st, d_key2, n_train, d_flag);
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_flag, d_seg, d_count, (int)n_train, st); }));
-        if (int rc = read_count(&n_seg)) return rc;
-        const unsigned gs = (unsigned)((n_seg + 255) / 256);
-        k_rt_seg_min<<<gs, 256, 0, st>>>(d_rows, d_key2, d_val, d_seg, n_seg, n_train, d_segmin, d_flag);
-        CUDA_TRY(cudaGetLastError());
+        if (int rc = read_back(st, &n_seg, d_count, 4)) return rc;
+        LAUNCH_N(k_rt_seg_min, n_seg, st, d_rows, d_key2, d_val, d_seg, n_seg, n_train, d_segmin, d_flag);
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_flag, d_prow, d_count, (int)n_seg, st); }));
-        if (int rc = read_count(&n_pr)) return rc;
-        const unsigned gp = (unsigned)((n_pr + 255) / 256);
-        k_rt_row_mean<<<gp, 256, 0, st>>>(d_key2, d_seg, d_segmin, d_prow, n_pr, n_seg, d_maxrt, d_keep);
-        CUDA_TRY(cudaGetLastError());
+        if (int rc = read_back(st, &n_pr, d_count, 4)) return rc;
+        LAUNCH_N(k_rt_row_mean, n_pr, st, d_key2, d_seg, d_segmin, d_prow, n_pr, n_seg, d_maxrt, d_keep);
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_keep, d_mrow, (int)n_pr, st); }));
         uint32_t last[2] = {0, 0};
         CUDA_TRY(cudaMemcpyAsync(&last[0], d_mrow + n_pr - 1, 4, cudaMemcpyDeviceToHost, st));
@@ -3136,14 +3117,11 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
         CUDA_TRY(A.alloc(&d_mat, n_rows * n_files));
         CUDA_TRY(A.alloc(&d_mean, n_rows));
         CUDA_TRY(cudaMemsetAsync(d_mat, 0xFF, 8 * n_rows * n_files, st));   // NaN where a peptide was not seen in a file
-        k_rt_fill<<<gp, 256, 0, st>>>(d_key2, d_seg, d_segmin, d_prow, n_pr, n_seg, d_maxrt, d_keep, d_mrow, n_files, d_mat, d_mean);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH_N(k_rt_fill, n_pr, st, d_key2, d_seg, d_segmin, d_prow, n_pr, n_seg, d_maxrt, d_keep, d_mrow, n_files, d_mat, d_mean);
     }
-    k_rt_align<<<(unsigned)((n_files + 127) / 128), 128, 0, st>>>(d_mat, d_mean, n_rows, n_files, d_maxrt, d_align);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_rt_align<<<(unsigned)((n_files + 127) / 128), 128, 0, st>>>(d_mat, d_mean, n_rows, n_files, d_maxrt, d_align));
     float* d_aligned = d_out[0];
-    k_rt_aligned<<<g, 256, 0, st>>>(d_rows, d_file, n, d_align, d_aligned);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_rt_aligned, n, st, d_rows, d_file, n, d_align, d_aligned);
     CUDA_TRY(cudaEventRecord(ev[2], st));
 
     // 3. retention_model::predict, 4. mobility_model::predict
@@ -3170,7 +3148,6 @@ extern "C" int sage_b200_predict_rt(const sage_b200_db* db, const sage_b200_pept
 }
 
 // ================================================================================== picked FDR (fdr.rs; kernels in picked.cuh)
-static unsigned grid256(uint64_t n) { return (unsigned)((n + 255) / 256); }
 static constexpr uint32_t PICKED_HOOK_MAX_ROWS = 1u << 16;   // competition_keys with hash_bits < 64
 
 // Checks run before the device is looked at, and the capacity check before anything is allocated. Per competing row: keys, indices, sorted
@@ -3215,20 +3192,14 @@ static int picked_tail(cudaStream_t st, DevArena& A, uint32_t R, const float* q_
     CUDA_TRY(cub::DeviceScan::InclusiveScan(nullptr, tb3, rq, rqmin, PickedMin(), (int)R, st));
     CUDA_TRY(A.reserve_tmp(std::max(tb, std::max(tb2, tb3))));
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(A.tmp, tb, q_key, key_s, q_idx, order, (int)R, 0, 32, st));   // stable: pre-sort order on ties
-    const unsigned g = grid256(R);
-    k_picked_pep<<<g, 256, 0, st>>>(order, q_score, q_decoy, R, bins, moments, pep, is_t);
-    CUDA_TRY(cudaGetLastError());
-    k_picked_running_sum<<<1, 32, 0, st>>>(pep, R, sum);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_pep, R, st, order, q_score, q_decoy, R, bins, moments, pep, is_t);
+    LAUNCH(k_picked_running_sum<<<1, 32, 0, st>>>(pep, R, sum));
     CUDA_TRY(cub::DeviceScan::InclusiveSum(A.tmp, tb2, is_t, tinc, (int)R, st));
-    k_picked_q_raw<<<g, 256, 0, st>>>(sum, tinc, R, rq);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_q_raw, R, st, sum, tinc, R, rq);
     CUDA_TRY(cub::DeviceScan::InclusiveScan(A.tmp, tb3, rq, rqmin, PickedMin(), (int)R, st));
     CUDA_TRY(cudaMemsetAsync(win, 0, 4ull * n_ix, st));
-    k_picked_q_min<<<g, 256, 0, st>>>(rqmin, q_decoy, order, q_ix, R, threshold, q, win, d_passing);
-    CUDA_TRY(cudaGetLastError());
-    k_picked_q_ix<<<g, 256, 0, st>>>(q, order, q_ix, win, R, q_ix_val);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_q_min, R, st, rqmin, q_decoy, order, q_ix, R, threshold, q, win, d_passing);
+    LAUNCH_N(k_picked_q_ix, R, st, q, order, q_ix, win, R, q_ix_val);
     return 0;
 }
 
@@ -3248,37 +3219,25 @@ static int picked_competition(cudaStream_t st, DevArena& A, bool fma, uint32_t m
     CUDA_TRY(A.alloc(&head, m));
     CUDA_TRY(A.alloc(&ginc, m));
     CUDA_TRY(A.alloc(&cnt, 4));
-    const unsigned g = grid256(m);
-    auto read_u32 = [&](const uint32_t* d, uint32_t* v) -> int {
-        CUDA_TRY(cudaMemcpyAsync(v, d, 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        return 0;
-    };
     // 1. entries: sort (key, row); a run's head row is the first row that reaches the entry; rank the entries by it
-    k_picked_iota<<<g, 256, 0, st>>>(m, idx);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_iota, m, st, m, idx);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_key, key_s, idx, row_s, (int)m, 0, 32, st); }));
-    k_picked_heads<<<g, 256, 0, st>>>(key_s, m, head);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_heads, m, st, key_s, m, head);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, head, ginc, (int)m, st); }));
     uint32_t G = 0;
-    if (int rc = read_u32(ginc + m - 1, &G)) return rc;
+    if (int rc = read_back(st, &G, ginc + m - 1, 4)) return rc;
     CUDA_TRY(A.alloc(&first, G));
     CUDA_TRY(A.alloc(&first_s, G));
     CUDA_TRY(A.alloc(&gidx, G));
     CUDA_TRY(A.alloc(&g_sorted, G));
     CUDA_TRY(A.alloc(&rank_of_group, G));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, row_s, head, first, cnt, (int)m, st); }));
-    const unsigned gg = grid256(G);
-    k_picked_iota<<<gg, 256, 0, st>>>(G, gidx);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_iota, G, st, G, gidx);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, first, first_s, gidx, g_sorted, (int)G, 0, 32, st); }));
-    k_picked_scatter_rank<<<gg, 256, 0, st>>>(g_sorted, G, rank_of_group);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_scatter_rank, G, st, g_sorted, G, rank_of_group);
     uint32_t *side_key = nullptr, *sk_s = nullptr, *row2_s = nullptr, *seg = nullptr;
     CUDA_TRY(A.alloc(&side_key, m));
-    k_picked_row_rank<<<g, 256, 0, st>>>(row_s, ginc, rank_of_group, d_decoy, m, d_rank, side_key, idx);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_row_rank, m, st, row_s, ginc, rank_of_group, d_decoy, m, d_rank, side_key, idx);
     *entries = G;
     if (!d_out) return 0;
 
@@ -3289,25 +3248,20 @@ static int picked_competition(cudaStream_t st, DevArena& A, bool fma, uint32_t m
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) {   // stable: row order within a side
         return cub::DeviceRadixSort::SortPairs(t, b, side_key, sk_s, idx, row2_s, (int)m, 0, 32, st);
     }));
-    k_picked_heads<<<g, 256, 0, st>>>(sk_s, m, head);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_heads, m, st, sk_s, m, head);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, head, seg, cnt, (int)m, st); }));
     uint32_t S = 0;
-    if (int rc = read_u32(cnt, &S)) return rc;
+    if (int rc = read_back(st, &S, cnt, 4)) return rc;
     float* side_score = nullptr;
     uint8_t *side_has = nullptr, *kde_flags = nullptr;
     uint32_t *clash = nullptr, *n_rows = nullptr, *row_off = nullptr;
     CUDA_TRY(A.alloc(&side_score, 2ull * G));
-    CUDA_TRY(A.alloc(&side_has, 2ull * G));
-    CUDA_TRY(A.alloc(&clash, 3));
-    CUDA_TRY(cudaMemsetAsync(side_has, 0, 2ull * G, st));
-    CUDA_TRY(cudaMemsetAsync(clash, 0, 12, st));
-    k_picked_fold<<<grid256(S), 256, 0, st>>>(sk_s, row2_s, seg, S, m, d_score, d_pep, side_score, side_has, clash);
-    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.zeros(&side_has, 2ull * G, st));
+    CUDA_TRY(A.zeros(&clash, 3, st));
+    LAUNCH_N(k_picked_fold, S, st, sk_s, row2_s, seg, S, m, d_score, d_pep, side_score, side_has, clash);
     if (d_pep) {
         uint32_t c[3];
-        CUDA_TRY(cudaMemcpyAsync(c, clash, 12, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
+        if (int rc = read_back(st, c, clash, 12)) return rc;
         if (c[2]) return fail(SAGE_B200_EINVAL, "picked_fdr: peptides %u and %u are distinct on one side with one key (the reference panics)", c[0], c[1]);
     }
 
@@ -3319,8 +3273,7 @@ static int picked_competition(cudaStream_t st, DevArena& A, bool fma, uint32_t m
     CUDA_TRY(A.alloc(&row_off, G));
     CUDA_TRY(A.alloc(&bins, 1000));
     CUDA_TRY(A.alloc(&moments, 4));
-    k_picked_entries<<<gg, 256, 0, st>>>(side_score, side_has, G, kde_score, kde_flags, n_rows);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_entries, G, st, side_score, side_has, G, kde_score, kde_flags, n_rows);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, n_rows, row_off, (int)G, st); }));
     if (int rc = fdr_kde(st, A, kde_score, kde_flags, kde_flags + G, G, 1000, true, 1.0, fma, bins, moments)) return rc;
     float *q_score = nullptr, *q_ix_val = nullptr;
@@ -3334,14 +3287,11 @@ static int picked_competition(cudaStream_t st, DevArena& A, bool fma, uint32_t m
     CUDA_TRY(A.alloc(&q_idx, S));
     CUDA_TRY(A.alloc(&q_ix_val, 2ull * G));
     CUDA_TRY(A.alloc(&d_passing, 1));
-    k_picked_rows<<<gg, 256, 0, st>>>(side_score, side_has, row_off, G, ix_has_side, q_score, q_decoy, q_ix, q_key, q_idx);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_rows, G, st, side_score, side_has, row_off, G, ix_has_side, q_score, q_decoy, q_ix, q_key, q_idx);
     if (int rc = picked_tail(st, A, S, q_score, q_decoy, q_ix, q_key, q_idx, bins, moments, 0.01f, 2 * G, q_ix_val, d_passing)) return rc;
-    k_picked_gather<<<g, 256, 0, st>>>(d_rank, d_decoy, m, ix_has_side, q_ix_val, d_out);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_gather, m, st, d_rank, d_decoy, m, ix_has_side, q_ix_val, d_out);
     unsigned long long pass = 0;
-    CUDA_TRY(cudaMemcpyAsync(&pass, d_passing, 8, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    if (int rc = read_back(st, &pass, d_passing, 8)) return rc;
     *passing = pass;
     return 0;
 }
@@ -3383,38 +3333,26 @@ static int picked_peptide_keys(cudaStream_t st, DevArena& A, const sage_b200_pep
     uint8_t *d_seq = nullptr, *d_rev = nullptr;
     float *d_mods = nullptr, *d_nterm = nullptr, *d_cterm = nullptr;
     uint64_t *d_hash = nullptr, *d_hash_s = nullptr;
-    CUDA_TRY(A.alloc(&d_off, U + 1));
-    CUDA_TRY(A.alloc(&d_seq, seq.size()));
-    CUDA_TRY(A.alloc(&d_mods, mods.size()));
-    CUDA_TRY(A.alloc(&d_nterm, U));
-    CUDA_TRY(A.alloc(&d_cterm, U));
-    CUDA_TRY(A.alloc(&d_rev, U));
-    CUDA_TRY(A.alloc(&d_row_slot, n));
+    CUDA_TRY(A.upload(&d_off, off.data(), U + 1, st));
+    CUDA_TRY(A.upload(&d_seq, seq.data(), seq.size(), st));
+    CUDA_TRY(A.upload(&d_mods, mods.data(), mods.size(), st));
+    CUDA_TRY(A.upload(&d_nterm, nterm.data(), U, st));
+    CUDA_TRY(A.upload(&d_cterm, cterm.data(), U, st));
+    CUDA_TRY(A.upload(&d_rev, rev.data(), U, st));
+    CUDA_TRY(A.upload(&d_row_slot, row_slot.data(), n, st));
     CUDA_TRY(A.alloc(&d_u, U));
     CUDA_TRY(A.alloc(&d_u_s, U));
     CUDA_TRY(A.alloc(&d_group, U));
     CUDA_TRY(A.alloc(&d_hash, U));
     CUDA_TRY(A.alloc(&d_hash_s, U));
-    CUDA_TRY(cudaMemcpyAsync(d_off, off.data(), 4ull * (U + 1), cudaMemcpyHostToDevice, st));
-    if (!seq.empty()) {
-        CUDA_TRY(cudaMemcpyAsync(d_seq, seq.data(), seq.size(), cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(d_mods, mods.data(), 4 * mods.size(), cudaMemcpyHostToDevice, st));
-    }
-    CUDA_TRY(cudaMemcpyAsync(d_nterm, nterm.data(), 4ull * U, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_cterm, cterm.data(), 4ull * U, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_rev, rev.data(), U, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_row_slot, row_slot.data(), 4ull * n, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(d_decoy, row_decoy.data(), n, cudaMemcpyHostToDevice, st));
     if (d_pep) CUDA_TRY(cudaMemcpyAsync(d_pep, pep_idx, 4ull * n, cudaMemcpyHostToDevice, st));
     const PickedPeptides pk{d_off, d_seq, d_mods, d_nterm, d_cterm, d_rev};
     const uint64_t mask = hash_bits >= 64 ? ~0ull : ((1ull << hash_bits) - 1);
-    k_picked_hash<<<grid256(U), 256, 0, st>>>(pk, U, mask, d_hash, d_u);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_hash, U, st, pk, U, mask, d_hash, d_u);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_hash, d_hash_s, d_u, d_u_s, (int)U, 0, 64, st); }));
-    k_picked_group<<<grid256(U), 256, 0, st>>>(pk, d_hash_s, d_u_s, U, d_group);
-    CUDA_TRY(cudaGetLastError());
-    k_picked_peptide_keys<<<grid256(n), 256, 0, st>>>(d_row_slot, d_group, n, d_key);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_group, U, st, pk, d_hash_s, d_u_s, U, d_group);
+    LAUNCH_N(k_picked_peptide_keys, n, st, d_row_slot, d_group, n, d_key);
     return 0;
 }
 
@@ -3451,7 +3389,8 @@ extern "C" int sage_b200_picked_fdr(int device, const sage_b200_peptides* P, con
     const uint32_t m = (uint32_t)prot_row.size();
     const bool fma = host_math_variant() != 1;
     DevArena A;
-    cudaStream_t st = 0;
+    Stream st;
+    CUDA_TRY(st.create());
     Event ev[4];
     for (Event& e : ev) CUDA_TRY(e.create());
     uint32_t *d_key = nullptr, *d_pep = nullptr, *d_rank = nullptr, *d_pkey = nullptr, *d_prank = nullptr;
@@ -3461,19 +3400,13 @@ extern "C" int sage_b200_picked_fdr(int device, const sage_b200_peptides* P, con
     CUDA_TRY(A.alloc(&d_pep, n));
     CUDA_TRY(A.alloc(&d_rank, n));
     CUDA_TRY(A.alloc(&d_decoy, n));
-    CUDA_TRY(A.alloc(&d_score, n));
+    CUDA_TRY(A.upload(&d_score, discriminant_score, n, st));
     CUDA_TRY(A.alloc(&d_q, n));
-    CUDA_TRY(A.alloc(&d_pkey, m));
+    CUDA_TRY(A.upload(&d_pkey, prot_key.data(), m, st));
     CUDA_TRY(A.alloc(&d_prank, m));
-    CUDA_TRY(A.alloc(&d_pdecoy, m));
-    CUDA_TRY(A.alloc(&d_pscore, m));
+    CUDA_TRY(A.upload(&d_pdecoy, prot_decoy.data(), m, st));
+    CUDA_TRY(A.upload(&d_pscore, prot_score.data(), m, st));
     CUDA_TRY(A.alloc(&d_pq, m));
-    CUDA_TRY(cudaMemcpyAsync(d_score, discriminant_score, 4 * n, cudaMemcpyHostToDevice, st));
-    if (m) {
-        CUDA_TRY(cudaMemcpyAsync(d_pkey, prot_key.data(), 4ull * m, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(d_pdecoy, prot_decoy.data(), m, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(d_pscore, prot_score.data(), 4ull * m, cudaMemcpyHostToDevice, st));
-    }
     CUDA_TRY(cudaEventRecord(ev[0], st));
     if (int rc = picked_peptide_keys(st, A, P, p, pep_idx.data(), (uint32_t)n, 64, d_key, d_decoy, d_pep)) return rc;
     CUDA_TRY(cudaEventRecord(ev[1], st));
@@ -3505,28 +3438,26 @@ extern "C" int sage_b200_picked_precursor(int device, const double* score, const
     if (n == 0) return 0;
     if (int rc = select_device(device)) return rc;
     if (int rc = picked_memory("picked_precursor", n, 0)) return rc;
+    std::vector<uint8_t> flags(n);
+    for (uint64_t i = 0; i < n; i++) flags[i] = decoy[i] ? 1 : 0;
     DevArena A;
-    cudaStream_t st = 0;
+    Stream st;
+    CUDA_TRY(st.create());
     const uint32_t R = (uint32_t)n;
     double* d_in = nullptr;
     float *d_score = nullptr, *d_q = nullptr;
     uint8_t* d_decoy = nullptr;
     uint32_t *d_ix = nullptr, *d_key = nullptr, *d_idx = nullptr;
     unsigned long long* d_passing = nullptr;
-    CUDA_TRY(A.alloc(&d_in, n));
+    CUDA_TRY(A.upload(&d_in, score, n, st));
     CUDA_TRY(A.alloc(&d_score, n));
     CUDA_TRY(A.alloc(&d_q, n));
-    CUDA_TRY(A.alloc(&d_decoy, n));
+    CUDA_TRY(A.upload(&d_decoy, flags.data(), n, st));
     CUDA_TRY(A.alloc(&d_ix, n));
     CUDA_TRY(A.alloc(&d_key, n));
     CUDA_TRY(A.alloc(&d_idx, n));
     CUDA_TRY(A.alloc(&d_passing, 1));
-    std::vector<uint8_t> flags(n);
-    for (uint64_t i = 0; i < n; i++) flags[i] = decoy[i] ? 1 : 0;
-    CUDA_TRY(cudaMemcpyAsync(d_in, score, 8 * n, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_decoy, flags.data(), n, cudaMemcpyHostToDevice, st));
-    k_picked_precursor_rows<<<grid256(n), 256, 0, st>>>(d_in, R, d_score, d_ix, d_key, d_idx);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_picked_precursor_rows, n, st, d_in, R, d_score, d_ix, d_key, d_idx);
     if (int rc = picked_tail(st, A, R, d_score, d_decoy, d_ix, d_key, d_idx, nullptr, nullptr, 0.05f, R, d_q, d_passing)) return rc;
     unsigned long long pass = 0;
     CUDA_TRY(cudaMemcpyAsync(q_value, d_q, 4 * n, cudaMemcpyDeviceToHost, st));
@@ -3554,7 +3485,8 @@ extern "C" int sage_b200_competition_keys(int device, const sage_b200_peptides* 
     const uint64_t nres = P->residue_offsets[P->n_peptides];
     if (int rc = picked_memory("competition_keys", n, 16 * nres + 32 * P->n_peptides)) return rc;
     DevArena A;
-    cudaStream_t st = 0;
+    Stream st;
+    CUDA_TRY(st.create());
     uint32_t *d_key = nullptr, *d_rank = nullptr;
     uint8_t* d_decoy = nullptr;
     CUDA_TRY(A.alloc(&d_key, n));
@@ -3563,31 +3495,14 @@ extern "C" int sage_b200_competition_keys(int device, const sage_b200_peptides* 
     if (int rc = picked_peptide_keys(st, A, P, p, peptide_idx, (uint32_t)n, hash_bits, d_key, d_decoy, nullptr)) return rc;
     uint64_t entries = 0, passing = 0;
     if (int rc = picked_competition(st, A, true, (uint32_t)n, d_key, d_decoy, nullptr, nullptr, true, d_rank, nullptr, &entries, &passing)) return rc;
-    CUDA_TRY(cudaMemcpyAsync(entry_rank, d_rank, 4 * n, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    return 0;
+    return read_back(st, entry_rank, d_rank, 4 * n);
 }
 
 // ================================================================================== protein grouping (protein_grouping.rs; kernels in protein_groups.cuh)
-// Kernel launches over n items; n == 0 launches nothing.
-#define PG_LAUNCH(kernel, n, ...)                                                        \
-    do {                                                                                 \
-        if ((n) > 0) {                                                                   \
-            kernel<<<grid256(n), 256, 0, st>>>(__VA_ARGS__);                             \
-            CUDA_TRY(cudaGetLastError());                                                \
-        }                                                                                \
-    } while (0)
-
-static int pg_read(cudaStream_t st, const void* d, void* h, size_t bytes) {
-    CUDA_TRY(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    return 0;
-}
-
 // out[0..n] = exclusive prefix sum of in[0..n) (in[n] must be 0); returns out[n] in *total.
 static int pg_offsets(cudaStream_t st, DevArena& A, const uint32_t* in, uint32_t* out, uint32_t n, uint32_t* total) {
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, in, out, (int)n + 1, st); }));
-    return pg_read(st, out + n, total, 4);
+    return read_back(st, total, out + n, 4);
 }
 
 struct PgCoverStats {
@@ -3604,34 +3519,30 @@ static int pg_cover(cudaStream_t st, DevArena& A, uint32_t E, uint32_t G, uint32
     uint32_t *ldeg, *rdeg, *loff, *roff, *key_s, *ladj, *radj, *rcov, *rem, *parent, tot = 0;
     uint8_t* active;
     unsigned long long* cnt;
-    CUDA_TRY(A.alloc(&ldeg, G + 1));
-    CUDA_TRY(A.alloc(&rdeg, M + 1));
+    CUDA_TRY(A.zeros(&ldeg, G + 1, st));
+    CUDA_TRY(A.zeros(&rdeg, M + 1, st));
     CUDA_TRY(A.alloc(&loff, G + 1));
     CUDA_TRY(A.alloc(&roff, M + 1));
     CUDA_TRY(A.alloc(&key_s, E));
     CUDA_TRY(A.alloc(&ladj, E));
     CUDA_TRY(A.alloc(&radj, E));
-    CUDA_TRY(A.alloc(&rcov, M));
+    CUDA_TRY(A.zeros(&rcov, M, st));
     CUDA_TRY(A.alloc(&rem, G));
     CUDA_TRY(A.alloc(&parent, G + M));
     CUDA_TRY(A.alloc(&active, G));
-    CUDA_TRY(A.alloc(&cnt, 3));   // forced, greedy picks, covered
-    CUDA_TRY(cudaMemsetAsync(ldeg, 0, 4ull * (G + 1), st));
-    CUDA_TRY(cudaMemsetAsync(rdeg, 0, 4ull * (M + 1), st));
-    CUDA_TRY(cudaMemsetAsync(rcov, 0, 4ull * M, st));
-    CUDA_TRY(cudaMemsetAsync(cnt, 0, 24, st));
-    PG_LAUNCH(k_pg_degrees, E, el, er, E, ldeg, rdeg);
+    CUDA_TRY(A.zeros(&cnt, 3, st));   // forced, greedy picks, covered
+    LAUNCH_N(k_pg_degrees, E, st, el, er, E, ldeg, rdeg);
     if (int rc = pg_offsets(st, A, ldeg, loff, G, &tot)) return rc;
     if (int rc = pg_offsets(st, A, rdeg, roff, M, &tot)) return rc;
     // adjacency of each left node (by a sort on the left end) and of each right node
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, el, key_s, er, ladj, (int)E, 0, 32, st); }));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, er, key_s, el, radj, (int)E, 0, 32, st); }));
-    PG_LAUNCH(k_pg_forced, E, el, er, rdeg, E, lcov);
-    PG_LAUNCH(k_pg_count, G, lcov, G, cnt);
-    PG_LAUNCH(k_pg_cover_rights, E, el, er, lcov, E, rcov);
-    PG_LAUNCH(k_pg_remaining, G, ladj, loff, lcov, rcov, G, rem, active);
-    PG_LAUNCH(k_picked_iota, G + M, G + M, parent);
-    PG_LAUNCH(k_pg_union, E, el, er, lcov, rcov, E, G, parent);
+    LAUNCH_N(k_pg_forced, E, st, el, er, rdeg, E, lcov);
+    LAUNCH_N(k_pg_count, G, st, lcov, G, cnt);
+    LAUNCH_N(k_pg_cover_rights, E, st, el, er, lcov, E, rcov);
+    LAUNCH_N(k_pg_remaining, G, st, ladj, loff, lcov, rcov, G, rem, active);
+    LAUNCH_N(k_picked_iota, G + M, st, G + M, parent);
+    LAUNCH_N(k_pg_union, E, st, el, er, lcov, rcov, E, G, parent);
     // the groups left with edges, by component (ascending group index within one)
     thrust::counting_iterator<uint32_t> it(0);
     uint32_t *act, *comp, *lefts, *uniq, *clen, *coff, *large, *nsel, n_act = 0, n_comp = 0, n_large = 0;
@@ -3639,40 +3550,35 @@ static int pg_cover(cudaStream_t st, DevArena& A, uint32_t E, uint32_t G, uint32
     CUDA_TRY(A.alloc(&act, G));
     CUDA_TRY(A.alloc(&nsel, 1));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, active, act, nsel, (int)G, st); }));
-    if (int rc = pg_read(st, nsel, &n_act, 4)) return rc;
+    if (int rc = read_back(st, &n_act, nsel, 4)) return rc;
     if (n_act) {
         CUDA_TRY(A.alloc(&comp, n_act));
         CUDA_TRY(A.alloc(&lefts, n_act));
         CUDA_TRY(A.alloc(&uniq, n_act));
         CUDA_TRY(A.alloc(&clen, n_act + 1));
         CUDA_TRY(A.alloc(&coff, n_act + 1));
-        PG_LAUNCH(k_pg_comp_of, n_act, parent, act, n_act, comp);
+        LAUNCH_N(k_pg_comp_of, n_act, st, parent, act, n_act, comp);
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, comp, key_s, act, lefts, (int)n_act, 0, 32, st); }));
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRunLengthEncode::Encode(t, b, key_s, uniq, clen, nsel, (int)n_act, st); }));
-        if (int rc = pg_read(st, nsel, &n_comp, 4)) return rc;
+        if (int rc = read_back(st, &n_comp, nsel, 4)) return rc;
         CUDA_TRY(cudaMemsetAsync(clen + n_comp, 0, 4, st));
         if (int rc = pg_offsets(st, A, clen, coff, n_comp, &tot)) return rc;
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceReduce::Max(t, b, clen, uniq, (int)n_comp, st); }));
         uint32_t largest = 0;
-        if (int rc = pg_read(st, uniq, &largest, 4)) return rc;
+        if (int rc = read_back(st, &largest, uniq, 4)) return rc;
         CUDA_TRY(A.alloc(&lflag, n_comp));
         CUDA_TRY(A.alloc(&large, n_comp));
-        PG_LAUNCH(k_pg_large_flag, n_comp, clen, n_comp, lflag);
+        LAUNCH_N(k_pg_large_flag, n_comp, st, clen, n_comp, lflag);
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, lflag, large, nsel, (int)n_comp, st); }));
-        if (int rc = pg_read(st, nsel, &n_large, 4)) return rc;
-        k_pg_greedy_warp<<<(unsigned)((32ull * n_comp + 255) / 256), 256, 0, st>>>(coff, clen, n_comp, lefts, ldeg, ladj, loff, radj, roff, rem, rcov, lcov,
-                                                                                  cnt + 1);
-        CUDA_TRY(cudaGetLastError());
-        if (n_large) {
-            k_pg_greedy_cta<<<n_large, PG_CTA, 0, st>>>(large, coff, clen, lefts, ldeg, ladj, loff, radj, roff, rem, rcov, lcov, cnt + 1);
-            CUDA_TRY(cudaGetLastError());
-        }
+        if (int rc = read_back(st, &n_large, nsel, 4)) return rc;
+        LAUNCH_N(k_pg_greedy_warp, 32ull * n_comp, st, coff, clen, n_comp, lefts, ldeg, ladj, loff, radj, roff, rem, rcov, lcov, cnt + 1);
+        if (n_large) LAUNCH(k_pg_greedy_cta<<<n_large, PG_CTA, 0, st>>>(large, coff, clen, lefts, ldeg, ladj, loff, radj, roff, rem, rcov, lcov, cnt + 1));
         s->components = n_comp;
         s->largest = largest;
     }
-    PG_LAUNCH(k_pg_count, G, lcov, G, cnt + 2);
+    LAUNCH_N(k_pg_count, G, st, lcov, G, cnt + 2);
     unsigned long long c[3];
-    if (int rc = pg_read(st, cnt, c, 24)) return rc;
+    if (int rc = read_back(st, c, cnt, 24)) return rc;
     s->forced = c[0];
     s->greedy = c[1];
     s->covered = c[2];
@@ -3705,14 +3611,13 @@ static int pg_pass(cudaStream_t st, DevArena& A, const PgInputs& in, float thres
     uint32_t *nsel, U = 0;
     uint8_t* mark;
     CUDA_TRY(A.alloc(&nsel, 1));
-    CUDA_TRY(A.alloc(&mark, in.n_pep));
     // 1. the peptide set, ascending PeptideIx
-    CUDA_TRY(cudaMemsetAsync(mark, 0, in.n_pep, st));
-    PG_LAUNCH(k_pg_mark, in.n, in.pep, in.label_ok, in.q, in.n, threshold, mark);
+    CUDA_TRY(A.zeros(&mark, in.n_pep, st));
+    LAUNCH_N(k_pg_mark, in.n, st, in.pep, in.label_ok, in.q, in.n, threshold, mark);
     uint32_t* set;
     CUDA_TRY(A.alloc(&set, in.n_pep));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, mark, set, nsel, (int)in.n_pep, st); }));
-    if (int rc = pg_read(st, nsel, &U, 4)) return rc;
+    if (int rc = read_back(st, &U, nsel, 4)) return rc;
     out->peptides[k] = U;
     uint32_t M = 0, P = 0, G = 0, E = 0, T_pairs = 0, tot = 0;
     uint32_t *pix_of_key = nullptr, *group_of = nullptr, *el = nullptr, *er = nullptr;
@@ -3725,23 +3630,23 @@ static int pg_pass(cudaStream_t st, DevArena& A, const PgInputs& in, float thres
         CUDA_TRY(A.alloc(&len, U + 1));
         CUDA_TRY(A.alloc(&soff, U + 1));
         CUDA_TRY(cudaMemsetAsync(len + U, 0, 4, st));
-        PG_LAUNCH(k_pg_set_len, U, set, in.poff, U, len);
+        LAUNCH_N(k_pg_set_len, U, st, set, in.poff, U, len);
         if (int rc = pg_offsets(st, A, len, soff, U, &T_pairs)) return rc;
         CUDA_TRY(A.alloc(&pair_key, T_pairs));
         CUDA_TRY(A.alloc(&first, NK));
         CUDA_TRY(A.alloc(&flag, NK));
         CUDA_TRY(cudaMemsetAsync(first, 0xFF, 4ull * NK, st));
-        PG_LAUNCH(k_pg_flatten, U, set, soff, in.poff, in.pids, in.pdecoy, U, pair_key, first);
-        PG_LAUNCH(k_pg_key_present, NK, first, NK, flag);
+        LAUNCH_N(k_pg_flatten, U, st, set, soff, in.poff, in.pids, in.pdecoy, U, pair_key, first);
+        LAUNCH_N(k_pg_key_present, NK, st, first, NK, flag);
         CUDA_TRY(A.alloc(&present, NK));
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, flag, present, nsel, (int)NK, st); }));
-        if (int rc = pg_read(st, nsel, &P, 4)) return rc;
+        if (int rc = read_back(st, &P, nsel, 4)) return rc;
         CUDA_TRY(A.alloc(&first_p, P));
         CUDA_TRY(A.alloc(&first_s, P));
         CUDA_TRY(A.alloc(&key_by_pix, P));
-        PG_LAUNCH(k_pg_gather_u32, P, first, present, P, first_p);
+        LAUNCH_N(k_pg_gather_u32, P, st, first, present, P, first_p);
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, first_p, first_s, present, key_by_pix, (int)P, 0, 32, st); }));
-        PG_LAUNCH(k_pg_scatter_rank, P, key_by_pix, P, pix_of_key);
+        LAUNCH_N(k_pg_scatter_rank, P, st, key_by_pix, P, pix_of_key);
         // 3. each peptide's sorted ProteinIx list; meta-peptides = the distinct lists, ranked lexicographically
         uint32_t *pix, *pix_s, *idx, *head, *incl, *mrep;
         CUDA_TRY(A.alloc(&pix, T_pairs));
@@ -3750,17 +3655,17 @@ static int pg_pass(cudaStream_t st, DevArena& A, const PgInputs& in, float thres
         CUDA_TRY(A.alloc(&head, U));
         CUDA_TRY(A.alloc(&incl, U));
         CUDA_TRY(A.alloc(&mrep, U));
-        PG_LAUNCH(k_pg_pair_pix, T_pairs, pair_key, pix_of_key, T_pairs, pix);
+        LAUNCH_N(k_pg_pair_pix, T_pairs, st, pair_key, pix_of_key, T_pairs, pix);
         if (T_pairs)
             CUDA_TRY(A.two_phase([&](void* t, size_t& b) {
                 return cub::DeviceSegmentedSort::SortKeys(t, b, pix, pix_s, (int)T_pairs, (int)U, soff, soff + 1, st);
             }));
-        PG_LAUNCH(k_picked_iota, U, U, idx);
+        LAUNCH_N(k_picked_iota, U, st, U, idx);
         const PgLexLess meta_less{pix_s, soff};
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceMergeSort::StableSortKeys(t, b, idx, (int)U, meta_less, st); }));
-        PG_LAUNCH(k_pg_lex_heads, U, idx, pix_s, soff, U, head);
+        LAUNCH_N(k_pg_lex_heads, U, st, idx, pix_s, soff, U, head);
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, head, incl, (int)U, st); }));
-        if (int rc = pg_read(st, incl + U - 1, &M, 4)) return rc;
+        if (int rc = read_back(st, &M, incl + U - 1, 4)) return rc;
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, idx, head, mrep, nsel, (int)U, st); }));
         if (P) {
             // 4. each protein's evidence: the meta-peptides that hold it, ascending, with multiplicity
@@ -3769,17 +3674,16 @@ static int pg_pass(cudaStream_t st, DevArena& A, const PgInputs& in, float thres
             CUDA_TRY(A.alloc(&mlen, M + 1));
             CUDA_TRY(A.alloc(&moff, M + 1));
             CUDA_TRY(cudaMemsetAsync(mlen + M, 0, 4, st));
-            PG_LAUNCH(k_pg_csr_len, M, mrep, soff, M, mlen);
+            LAUNCH_N(k_pg_csr_len, M, st, mrep, soff, M, mlen);
             if (int rc = pg_offsets(st, A, mlen, moff, M, &TM)) return rc;
-            CUDA_TRY(A.alloc(&pdeg, P + 1));
+            CUDA_TRY(A.zeros(&pdeg, P + 1, st));
             CUDA_TRY(A.alloc(&ev_off, P + 1));
             CUDA_TRY(A.alloc(&pairs, TM));
             CUDA_TRY(A.alloc(&pairs_s, TM));
             CUDA_TRY(A.alloc(&ev, TM));
-            CUDA_TRY(cudaMemsetAsync(pdeg, 0, 4ull * (P + 1), st));
-            PG_LAUNCH(k_pg_meta_pairs, M, mrep, pix_s, soff, moff, M, pairs, pdeg);
+            LAUNCH_N(k_pg_meta_pairs, M, st, mrep, pix_s, soff, moff, M, pairs, pdeg);
             CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, pairs, pairs_s, (int)TM, 0, 64, st); }));
-            PG_LAUNCH(k_pg_low32, TM, pairs_s, TM, ev);
+            LAUNCH_N(k_pg_low32, TM, st, pairs_s, TM, ev);
             if (int rc = pg_offsets(st, A, pdeg, ev_off, P, &tot)) return rc;
             // 5. groups: proteins of equal evidence, ranked by it; members in ascending id; edges (group, each evidence entry)
             uint32_t *pidx, *phead, *pincl, *grep, *gsize, *elen, *eoff;
@@ -3789,33 +3693,32 @@ static int pg_pass(cudaStream_t st, DevArena& A, const PgInputs& in, float thres
             CUDA_TRY(A.alloc(&pincl, P));
             CUDA_TRY(A.alloc(&grep, P));
             CUDA_TRY(A.alloc(&group_of, P));
-            PG_LAUNCH(k_picked_iota, P, P, pidx);
+            LAUNCH_N(k_picked_iota, P, st, P, pidx);
             const PgLexLess group_less{ev, ev_off};
             CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceMergeSort::StableSortKeys(t, b, pidx, (int)P, group_less, st); }));
-            PG_LAUNCH(k_pg_lex_heads, P, pidx, ev, ev_off, P, phead);
+            LAUNCH_N(k_pg_lex_heads, P, st, pidx, ev, ev_off, P, phead);
             CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, phead, pincl, (int)P, st); }));
-            if (int rc = pg_read(st, pincl + P - 1, &G, 4)) return rc;
-            PG_LAUNCH(k_pg_rank_of, P, pidx, pincl, P, group_of);
+            if (int rc = read_back(st, &G, pincl + P - 1, 4)) return rc;
+            LAUNCH_N(k_pg_rank_of, P, st, pidx, pincl, P, group_of);
             CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, pidx, phead, grep, nsel, (int)P, st); }));
-            CUDA_TRY(A.alloc(&gsize, G + 1));
+            CUDA_TRY(A.zeros(&gsize, G + 1, st));
             CUDA_TRY(A.alloc(&T->goff, G + 1));
             CUDA_TRY(A.alloc(&T->members, P));
             CUDA_TRY(A.alloc(&T->gdecoy, G));
             CUDA_TRY(A.alloc(&mem, P));
             CUDA_TRY(A.alloc(&mem_s, P));
-            CUDA_TRY(cudaMemsetAsync(gsize, 0, 4ull * (G + 1), st));
-            PG_LAUNCH(k_pg_members, P, group_of, key_by_pix, P, mem, gsize, T->gdecoy);
+            LAUNCH_N(k_pg_members, P, st, group_of, key_by_pix, P, mem, gsize, T->gdecoy);
             CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, mem, mem_s, (int)P, 0, 64, st); }));
-            PG_LAUNCH(k_pg_low32, P, mem_s, P, T->members);
+            LAUNCH_N(k_pg_low32, P, st, mem_s, P, T->members);
             if (int rc = pg_offsets(st, A, gsize, T->goff, G, &tot)) return rc;
             CUDA_TRY(A.alloc(&elen, G + 1));
             CUDA_TRY(A.alloc(&eoff, G + 1));
             CUDA_TRY(cudaMemsetAsync(elen + G, 0, 4, st));
-            PG_LAUNCH(k_pg_csr_len, G, grep, ev_off, G, elen);
+            LAUNCH_N(k_pg_csr_len, G, st, grep, ev_off, G, elen);
             if (int rc = pg_offsets(st, A, elen, eoff, G, &E)) return rc;
             CUDA_TRY(A.alloc(&el, E));
             CUDA_TRY(A.alloc(&er, E));
-            PG_LAUNCH(k_pg_edges, G, grep, ev, ev_off, eoff, G, el, er);
+            LAUNCH_N(k_pg_edges, G, st, grep, ev, ev_off, eoff, G, el, er);
         }
     }
     T->G = G;
@@ -3838,12 +3741,11 @@ static int pg_pass(cudaStream_t st, DevArena& A, const PgInputs& in, float thres
     // 7. the rows still unannotated
     if (G) {
         unsigned long long* d_ann;
-        CUDA_TRY(A.alloc(&d_ann, 1));
-        CUDA_TRY(cudaMemsetAsync(d_ann, 0, 8, st));
-        PG_LAUNCH(k_pg_lookup, in.n, in.pep, in.n, in.poff, in.pids, in.pdecoy, in.cap_off, pix_of_key, group_of, T->lcov, base, pass_no, pass, count,
-                  scratch, d_ann);
+        CUDA_TRY(A.zeros(&d_ann, 1, st));
+        LAUNCH_N(k_pg_lookup, in.n, st, in.pep, in.n, in.poff, in.pids, in.pdecoy, in.cap_off, pix_of_key, group_of, T->lcov, base, pass_no, pass, count,
+                 scratch, d_ann);
         unsigned long long ann = 0;
-        if (int rc = pg_read(st, d_ann, &ann, 8)) return rc;
+        if (int rc = read_back(st, &ann, d_ann, 8)) return rc;
         out->annotated[k] = ann;
     }
     return 0;
@@ -3896,37 +3798,28 @@ extern "C" int sage_b200_protein_groups(int device, const sage_b200_peptides* P,
     if (int rc = picked_memory("protein_groups", n, 96 * NP + 48 * p->n_names + 8 * cap + 16 * n_pep)) return rc;
     const uint32_t N = (uint32_t)n;
     const bool gen = p->generate_decoys != 0, fma = host_math_variant() != 1;
+    std::vector<uint8_t> pdecoy(n_pep);
+    for (uint64_t q = 0; q < n_pep; q++) pdecoy[q] = P->decoy[q] ? 1 : 0;
     DevArena A;
-    cudaStream_t st = 0;
+    Stream st;
+    CUDA_TRY(st.create());
     Event ev[9];
     for (Event& e : ev) CUDA_TRY(e.create());
     uint32_t *d_pep, *d_poff, *d_pids, *d_count, *d_scratch, *d_csr_len, *d_rows_out;
     uint8_t *d_label, *d_pdecoy, *d_pass;
     float *d_q, *d_score;
     uint64_t *d_cap, *d_out_off;
-    CUDA_TRY(A.alloc(&d_pep, N));
-    CUDA_TRY(A.alloc(&d_poff, n_pep + 1));
-    CUDA_TRY(A.alloc(&d_pids, NP));
-    CUDA_TRY(A.alloc(&d_label, N));
-    CUDA_TRY(A.alloc(&d_pdecoy, n_pep));
-    CUDA_TRY(A.alloc(&d_q, N));
-    CUDA_TRY(A.alloc(&d_score, N));
-    CUDA_TRY(A.alloc(&d_cap, N + 1));
-    CUDA_TRY(A.alloc(&d_pass, N));
-    CUDA_TRY(A.alloc(&d_count, N));
+    CUDA_TRY(A.upload(&d_pep, pep_idx.data(), N, st));
+    CUDA_TRY(A.upload(&d_poff, p->protein_offsets, n_pep + 1, st));
+    CUDA_TRY(A.upload(&d_pids, p->protein_ids, NP, st));
+    CUDA_TRY(A.upload(&d_label, label_ok.data(), N, st));
+    CUDA_TRY(A.upload(&d_pdecoy, pdecoy.data(), n_pep, st));
+    CUDA_TRY(A.upload(&d_q, peptide_q, N, st));
+    CUDA_TRY(A.upload(&d_score, discriminant_score, N, st));
+    CUDA_TRY(A.upload(&d_cap, cap_off.data(), N + 1, st));
+    CUDA_TRY(A.zeros(&d_pass, N, st));
+    CUDA_TRY(A.zeros(&d_count, N, st));
     CUDA_TRY(A.alloc(&d_scratch, cap));
-    std::vector<uint8_t> pdecoy(n_pep);
-    for (uint64_t q = 0; q < n_pep; q++) pdecoy[q] = P->decoy[q] ? 1 : 0;
-    CUDA_TRY(cudaMemcpyAsync(d_pep, pep_idx.data(), 4ull * N, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_poff, p->protein_offsets, 4 * (n_pep + 1), cudaMemcpyHostToDevice, st));
-    if (NP) CUDA_TRY(cudaMemcpyAsync(d_pids, p->protein_ids, 4 * NP, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_label, label_ok.data(), N, cudaMemcpyHostToDevice, st));
-    if (n_pep) CUDA_TRY(cudaMemcpyAsync(d_pdecoy, pdecoy.data(), n_pep, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_q, peptide_q, 4ull * N, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_score, discriminant_score, 4ull * N, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_cap, cap_off.data(), 8ull * (N + 1), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemsetAsync(d_pass, 0, N, st));
-    CUDA_TRY(cudaMemsetAsync(d_count, 0, 4ull * N, st));
     CUDA_TRY(cudaEventRecord(ev[0], st));
     const PgInputs in{N, (uint32_t)n_pep, (uint32_t)p->n_names, d_pep, d_poff, d_pids, d_label, d_pdecoy, d_q, d_cap};
 
@@ -3953,14 +3846,14 @@ extern "C" int sage_b200_protein_groups(int device, const sage_b200_peptides* P,
     CUDA_TRY(A.alloc(&d_csr_len, N + 1));
     CUDA_TRY(A.alloc(&d_out_off, N + 1));
     CUDA_TRY(cudaMemsetAsync(d_csr_len + N, 0, 4, st));
-    PG_LAUNCH(k_pg_fallback, N, d_pep, N, d_poff, d_pass, d_count, d_csr_len);
+    LAUNCH_N(k_pg_fallback, N, st, d_pep, N, d_poff, d_pass, d_count, d_csr_len);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) {
         return cub::DeviceScan::ExclusiveSum(t, b, d_csr_len, d_out_off, (int)N + 1, st);
     }));
     uint64_t n_out = 0;
-    if (int rc = pg_read(st, d_out_off + N, &n_out, 8)) return rc;
+    if (int rc = read_back(st, &n_out, d_out_off + N, 8)) return rc;
     CUDA_TRY(A.alloc(&d_rows_out, n_out));
-    PG_LAUNCH(k_pg_compact_rows, N, d_cap, d_out_off, d_scratch, d_csr_len, N, d_rows_out);
+    LAUNCH_N(k_pg_compact_rows, N, st, d_cap, d_out_off, d_scratch, d_csr_len, N, d_rows_out);
 
     // the group tables of both passes, concatenated
     const uint32_t Gt = T[0].G + T[1].G, Pt = T[0].P + T[1].P;
@@ -3975,7 +3868,7 @@ extern "C" int sage_b200_protein_groups(int device, const sage_b200_peptides* P,
     for (int k = 0, g0 = 0, p0 = 0; k < 2; g0 += T[k].G, p0 += T[k].P, k++) {
         if (!T[k].G) continue;
         CUDA_TRY(cudaMemcpyAsync(goff + g0 + 1, T[k].goff + 1, 4ull * T[k].G, cudaMemcpyDeviceToDevice, st));
-        PG_LAUNCH(k_pg_add, T[k].G, goff + g0 + 1, T[k].G, (uint32_t)p0);
+        LAUNCH_N(k_pg_add, T[k].G, st, goff + g0 + 1, T[k].G, (uint32_t)p0);
         CUDA_TRY(cudaMemcpyAsync(members + p0, T[k].members, 4ull * T[k].P, cudaMemcpyDeviceToDevice, st));
         CUDA_TRY(cudaMemcpyAsync(gdecoy + g0, T[k].gdecoy, T[k].G, cudaMemcpyDeviceToDevice, st));
         CUDA_TRY(cudaMemcpyAsync(gcov + g0, T[k].lcov, T[k].G, cudaMemcpyDeviceToDevice, st));
@@ -3991,9 +3884,9 @@ extern "C" int sage_b200_protein_groups(int device, const sage_b200_peptides* P,
     CUDA_TRY(A.alloc(&gidx_s, Gt));
     CUDA_TRY(A.alloc(&hash, Gt));
     CUDA_TRY(A.alloc(&hash_s, Gt));
-    PG_LAUNCH(k_pg_group_hash, Gt, goff, members, gdecoy, Gt, gen, hash, gidx);
+    LAUNCH_N(k_pg_group_hash, Gt, st, goff, members, gdecoy, Gt, gen, hash, gidx);
     if (Gt) CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, hash, hash_s, gidx, gidx_s, (int)Gt, 0, 64, st); }));
-    PG_LAUNCH(k_pg_group_rep, Gt, goff, members, gdecoy, gen, hash_s, gidx_s, Gt, rep);
+    LAUNCH_N(k_pg_group_rep, Gt, st, goff, members, gdecoy, gen, hash_s, gidx_s, Gt, rep);
     CUDA_TRY(A.alloc(&key, N));
     CUDA_TRY(A.alloc(&side, N));
     CUDA_TRY(A.alloc(&competes, N));
@@ -4005,17 +3898,17 @@ extern "C" int sage_b200_protein_groups(int device, const sage_b200_peptides* P,
     CUDA_TRY(A.alloc(&cq, N));
     CUDA_TRY(A.alloc(&d_pgq, N));
     CUDA_TRY(A.alloc(&nsel, 1));
-    PG_LAUNCH(k_pg_row_keys, N, d_pep, N, d_pass, d_count, d_out_off, d_rows_out, goff, members, gdecoy, rep, d_poff, d_pids, d_pdecoy, gen,
-              (uint32_t)p->n_names, key, side, competes);
+    LAUNCH_N(k_pg_row_keys, N, st, d_pep, N, d_pass, d_count, d_out_off, d_rows_out, goff, members, gdecoy, rep, d_poff, d_pids, d_pdecoy, gen,
+             (uint32_t)p->n_names, key, side, competes);
     thrust::counting_iterator<uint32_t> it(0);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, it, competes, crow, nsel, (int)N, st); }));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, key, competes, ckey, nsel, (int)N, st); }));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, side, competes, cside, nsel, (int)N, st); }));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_score, competes, cscore, nsel, (int)N, st); }));
-    if (int rc = pg_read(st, nsel, &m, 4)) return rc;
+    if (int rc = read_back(st, &m, nsel, 4)) return rc;
     if (int rc = picked_competition(st, A, fma, m, ckey, cside, cscore, nullptr, false, crank, cq, &out->entries, &out->passing)) return rc;
-    PG_LAUNCH(k_pg_fill, N, d_pgq, N, 1.0f);
-    PG_LAUNCH(k_pg_scatter_q, m, crow, cq, m, d_pgq);
+    LAUNCH_N(k_pg_fill, N, st, d_pgq, N, 1.0f);
+    LAUNCH_N(k_pg_scatter_q, m, st, crow, cq, m, d_pgq);
     CUDA_TRY(cudaEventRecord(ev[7], st));
 
     // outputs
@@ -4054,22 +3947,17 @@ extern "C" int sage_b200_bipartite_cover(int device, const uint32_t* left, const
     if (int rc = select_device(device)) return rc;
     if (int rc = picked_memory("bipartite_cover", n_edges, 64 * (n_left + n_right))) return rc;
     DevArena A;
-    cudaStream_t st = 0;
+    Stream st;
+    CUDA_TRY(st.create());
     const uint32_t E = (uint32_t)n_edges, G = (uint32_t)n_left, M = (uint32_t)n_right;
     uint32_t *el, *er;
     uint8_t* lcov;
-    CUDA_TRY(A.alloc(&el, E));
-    CUDA_TRY(A.alloc(&er, E));
+    CUDA_TRY(A.upload(&el, left, E, st));
+    CUDA_TRY(A.upload(&er, right, E, st));
     CUDA_TRY(A.alloc(&lcov, G));
-    if (E) {
-        CUDA_TRY(cudaMemcpyAsync(el, left, 4ull * E, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(er, right, 4ull * E, cudaMemcpyHostToDevice, st));
-    }
     PgCoverStats cs;
     if (int rc = pg_cover(st, A, E, G, M, el, er, lcov, &cs)) return rc;
-    CUDA_TRY(cudaMemcpyAsync(cover, lcov, G, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    return 0;
+    return read_back(st, cover, lcov, G);
 }
 
 #if SAGE_B200_PHASE_CLOCKS
@@ -4194,17 +4082,12 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     sage_b200_digest_info& I = D->info;
     const uint32_t P = (uint32_t)F.acc.size();
     const uint64_t R = F.res.size();
+    DevArena A;
     Stream st;
     CUDA_TRY(st.create());
     Event ev[8];
     for (Event& e : ev) CUDA_TRY(e.create());
-    DevArena A;
     auto done = [&]() { I.peak_device_bytes = A.bytes + D->out.bytes; I.device_bytes = D->out.bytes; };
-    auto read = [&](void* h, const void* d, size_t b) -> int {
-        CUDA_TRY(cudaMemcpyAsync(h, d, b, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        return 0;
-    };
     thrust::counting_iterator<uint32_t> count_it(0);
     uint32_t* d_cnt = nullptr;
     CUDA_TRY(A.alloc(&d_cnt, 1));
@@ -4215,18 +4098,12 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     uint8_t *d_res = nullptr, *d_pdecoy = nullptr;
     uint32_t *d_poff = nullptr, *d_pname = nullptr;
     DgSpec *d_statics = nullptr, *d_vars = nullptr;
-    CUDA_TRY(A.alloc(&d_res, R));
-    CUDA_TRY(A.alloc(&d_poff, P + 1));
-    CUDA_TRY(A.alloc(&d_pdecoy, P));
-    CUDA_TRY(A.alloc(&d_pname, P));
-    CUDA_TRY(A.alloc(&d_statics, statics.size()));
-    CUDA_TRY(A.alloc(&d_vars, vars.size()));
-    CUDA_TRY(cudaMemcpyAsync(d_res, F.res.data(), R, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_poff, F.off.data(), 4ull * (P + 1), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_pdecoy, F.decoy.data(), P, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_pname, prot_name.data(), 4ull * P, cudaMemcpyHostToDevice, st));
-    if (!statics.empty()) CUDA_TRY(cudaMemcpyAsync(d_statics, statics.data(), sizeof(DgSpec) * statics.size(), cudaMemcpyHostToDevice, st));
-    if (!vars.empty()) CUDA_TRY(cudaMemcpyAsync(d_vars, vars.data(), sizeof(DgSpec) * vars.size(), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(A.upload(&d_res, F.res.data(), R, st));
+    CUDA_TRY(A.upload(&d_poff, F.off.data(), P + 1, st));
+    CUDA_TRY(A.upload(&d_pdecoy, F.decoy.data(), P, st));
+    CUDA_TRY(A.upload(&d_pname, prot_name.data(), P, st));
+    CUDA_TRY(A.upload(&d_statics, statics.data(), statics.size(), st));
+    CUDA_TRY(A.upload(&d_vars, vars.data(), vars.size(), st));
     DgParams p = hp;
     p.statics = d_statics;
     p.vars = d_vars;
@@ -4234,30 +4111,24 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
 
     // 1. cleavage sites: count, scan, write
     uint32_t *d_ncut = nullptr, *d_cut_off = nullptr, *d_cuts = nullptr;
-    CUDA_TRY(A.alloc(&d_ncut, P + 1));
+    CUDA_TRY(A.zeros(&d_ncut, P + 1, st));
     CUDA_TRY(A.alloc(&d_cut_off, P + 1));
-    CUDA_TRY(cudaMemsetAsync(d_ncut, 0, 4ull * (P + 1), st));
-    const unsigned gw = (unsigned)((32ull * P + 255) / 256);
-    k_dg_sites<<<gw, 256, 0, st>>>(d_res, d_poff, P, p, d_ncut, nullptr, nullptr);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_sites, 32ull * P, st, d_res, d_poff, P, p, d_ncut, nullptr, nullptr);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_ncut, d_cut_off, (int)(P + 1), st); }));
     uint32_t n_cuts = 0;
-    if (int rc = read(&n_cuts, d_cut_off + P, 4)) return rc;
+    if (int rc = read_back(st, &n_cuts, d_cut_off + P, 4)) return rc;
     CUDA_TRY(A.alloc(&d_cuts, n_cuts));
-    k_dg_sites<<<gw, 256, 0, st>>>(d_res, d_poff, P, p, nullptr, d_cut_off, d_cuts);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_sites, 32ull * P, st, d_res, d_poff, P, p, nullptr, d_cut_off, d_cuts);
     CUDA_TRY(cudaEventRecord(ev[2], st));
 
     // 2. windows: count, scan, write
     uint64_t *d_nwin = nullptr, *d_win_off = nullptr;
-    CUDA_TRY(A.alloc(&d_nwin, P + 1));
+    CUDA_TRY(A.zeros(&d_nwin, P + 1, st));
     CUDA_TRY(A.alloc(&d_win_off, P + 1));
-    CUDA_TRY(cudaMemsetAsync(d_nwin, 0, 8ull * (P + 1), st));
-    k_dg_windows<<<grid256(P), 256, 0, st>>>(d_poff, d_cut_off, d_cuts, P, p, d_nwin, nullptr, nullptr);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_windows, P, st, d_poff, d_cut_off, d_cuts, P, p, d_nwin, nullptr, nullptr);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nwin, d_win_off, (int)(P + 1), st); }));
     uint64_t W64 = 0;
-    if (int rc = read(&W64, d_win_off + P, 8)) return rc;
+    if (int rc = read_back(st, &W64, d_win_off + P, 8)) return rc;
     if (W64 >= 0xFFFFFFFEull) return fail(SAGE_B200_ELIMIT, "digest: %llu windows (2^32 - 2 or more)", (unsigned long long)W64);
     const uint32_t W = (uint32_t)W64;
     I.n_windows = W;
@@ -4266,8 +4137,7 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     if (int rc = dg_memory("window", 100ull * W)) return rc;
     DgWin* d_win = nullptr;
     CUDA_TRY(A.alloc(&d_win, W));
-    k_dg_windows<<<grid256(P), 256, 0, st>>>(d_poff, d_cut_off, d_cuts, P, p, nullptr, d_win_off, d_win);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_windows, P, st, d_poff, d_cut_off, d_cuts, P, p, nullptr, d_win_off, d_win);
     CUDA_TRY(cudaEventRecord(ev[3], st));
 
     // 3. per-protein `seen` and group_digests: sort by hash, exact classes, stable sort by class, keep each protein's first window of a class,
@@ -4282,40 +4152,34 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     CUDA_TRY(A.alloc(&d_idx_s, W));
     CUDA_TRY(A.alloc(&d_rs, W));
     CUDA_TRY(A.alloc(&d_cls, W));
-    const unsigned gW = grid256(W);
-    k_dg_hash<<<gW, 256, 0, st>>>(d_res, d_win, W, d_hash, d_idx);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_hash, W, st, d_res, d_win, W, d_hash, d_idx);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_hash, d_hash_s, d_idx, d_idx_s, (int)W, 0, 64, st); }));
-    k_dg_run_start<<<gW, 256, 0, st>>>(d_hash_s, W, d_rs);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_run_start, W, st, d_hash_s, W, d_rs);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveScan(t, b, d_rs, d_rs, DgMax(), (int)W, st); }));
-    k_dg_class<<<gW, 256, 0, st>>>(d_res, d_win, d_idx_s, d_rs, W, d_cls);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_class, W, st, d_res, d_win, d_idx_s, d_rs, W, d_cls);
     const int cbits = (int)std::max<uint32_t>(1, ceil_log2_u64(W));
     CUDA_TRY(A.alloc(&d_cls_s, W));
     CUDA_TRY(A.alloc(&d_idx2, W));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_cls, d_cls_s, d_idx_s, d_idx2, (int)W, 0, cbits, st); }));
     CUDA_TRY(A.alloc(&d_keep, W));
     CUDA_TRY(A.alloc(&d_key, W));
-    k_dg_seen<<<gW, 256, 0, st>>>(d_win, d_cls_s, d_idx2, d_pdecoy, W, d_keep, d_key);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_seen, W, st, d_win, d_cls_s, d_idx2, d_pdecoy, W, d_keep, d_key);
     CUDA_TRY(A.alloc(&d_key_k, W));
     CUDA_TRY(A.alloc(&d_idx_k, W));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_key, d_keep, d_key_k, d_cnt, (int)W, st); }));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_idx2, d_keep, d_idx_k, d_cnt, (int)W, st); }));
     uint32_t Kc = 0;
-    if (int rc = read(&Kc, d_cnt, 4)) return rc;
+    if (int rc = read_back(st, &Kc, d_cnt, 4)) return rc;
     CUDA_TRY(A.alloc(&d_key3, Kc));
     CUDA_TRY(A.alloc(&d_idx3, Kc));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_key_k, d_key3, d_idx_k, d_idx3, (int)Kc, 0, cbits + 3, st); }));
     CUDA_TRY(A.alloc(&d_head, Kc));
-    k_dg_heads64<<<grid256(Kc), 256, 0, st>>>(d_key3, Kc, d_head);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_heads64, Kc, st, d_key3, Kc, d_head);
     uint32_t* d_gstart = nullptr;
     CUDA_TRY(A.alloc(&d_gstart, Kc + 1));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_head, d_gstart, d_cnt, (int)Kc, st); }));
     uint32_t G = 0;
-    if (int rc = read(&G, d_cnt, 4)) return rc;
+    if (int rc = read_back(st, &G, d_cnt, 4)) return rc;
     I.n_groups = G;
     CUDA_TRY(cudaMemcpyAsync(d_gstart + G, &Kc, 4, cudaMemcpyHostToDevice, st));
     uint32_t *d_gwin = nullptr, *d_gcls = nullptr;
@@ -4323,11 +4187,8 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     CUDA_TRY(A.alloc(&d_gwin, G));
     CUDA_TRY(A.alloc(&d_gcls, G));
     CUDA_TRY(A.alloc(&d_gmeta, G));
-    CUDA_TRY(A.alloc(&d_cls_target, W));
-    CUDA_TRY(cudaMemsetAsync(d_cls_target, 0, W, st));
-    const unsigned gG = grid256(G);
-    k_dg_groups<<<gG, 256, 0, st>>>(d_key3, d_idx3, d_gstart, G, d_gwin, d_gmeta, d_gcls, d_cls_target);
-    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(A.zeros(&d_cls_target, W, st));
+    LAUNCH_N(k_dg_groups, G, st, d_key3, d_idx3, d_gstart, G, d_gwin, d_gmeta, d_gcls, d_cls_target);
     CUDA_TRY(cudaEventRecord(ev[4], st));
 
     // 4. Peptide::try_from, the variable-mod sites, the forms (apply, the mass filter, reverse and the targets filter)
@@ -4341,19 +4202,17 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     CUDA_TRY(A.alloc(&d_nform, G + 1));
     CUDA_TRY(A.alloc(&d_form_off, G + 1));
     CUDA_TRY(A.alloc(&d_revt, G));
-    CUDA_TRY(A.alloc(&d_overflow, 1));
+    CUDA_TRY(A.zeros(&d_overflow, 1, st));
     CUDA_TRY(cudaMemsetAsync(d_nsite + G, 0, 4, st));
     CUDA_TRY(cudaMemsetAsync(d_nform + G, 0, 8, st));
-    CUDA_TRY(cudaMemsetAsync(d_overflow, 0, 4, st));
-    k_dg_group_info<<<gG, 256, 0, st>>>(d_res, d_win, d_gwin, d_gmeta, G, p, d_hash_s, d_idx_s, W, d_gbase, d_nsite, d_nform, d_revt, d_overflow);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_group_info, G, st, d_res, d_win, d_gwin, d_gmeta, G, p, d_hash_s, d_idx_s, W, d_gbase, d_nsite, d_nform, d_revt, d_overflow);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nsite, d_site_off, (int)(G + 1), st); }));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nform, d_form_off, (int)(G + 1), st); }));
     uint32_t n_sites = 0, overflow = 0;
     uint64_t T64 = 0;
-    if (int rc = read(&n_sites, d_site_off + G, 4)) return rc;
-    if (int rc = read(&T64, d_form_off + G, 8)) return rc;
-    if (int rc = read(&overflow, d_overflow, 4)) return rc;
+    if (int rc = read_back(st, &n_sites, d_site_off + G, 4)) return rc;
+    if (int rc = read_back(st, &T64, d_form_off + G, 8)) return rc;
+    if (int rc = read_back(st, &overflow, d_overflow, 4)) return rc;
     if (overflow) return fail(SAGE_B200_ELIMIT, "digest: a peptide has more than 65535 variable-modification sites");
     if (T64 >= (1ull << 31)) return fail(SAGE_B200_ELIMIT, "digest: %llu (peptide, modification combination) candidates (2^31 or more)", (unsigned long long)T64);
     const uint32_t T = (uint32_t)T64;
@@ -4364,17 +4223,15 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     float* d_site_mass = nullptr;
     CUDA_TRY(A.alloc(&d_site_code, n_sites));
     CUDA_TRY(A.alloc(&d_site_mass, n_sites));
-    k_dg_site_fill<<<gG, 256, 0, st>>>(d_res, d_win, d_gwin, d_gmeta, d_site_off, G, p, d_site_code, d_site_mass);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_site_fill, G, st, d_res, d_win, d_gwin, d_gmeta, d_site_off, G, p, d_site_code, d_site_mass);
     DgView V{d_res, d_poff, d_win, d_gwin, d_gmeta, d_site_off, d_site_code, d_site_mass, nullptr, nullptr, p};
     CUDA_TRY(A.alloc(&d_rows, T + 1));
     CUDA_TRY(A.alloc(&d_row_off, T + 1));
     CUDA_TRY(cudaMemsetAsync(d_rows + T, 0, 4, st));
-    k_dg_expand<<<grid256(T), 256, 0, st>>>(V, d_form_off, G, T, d_gbase, d_gcls, d_cls_target, d_revt, d_rows, nullptr, nullptr, nullptr);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_expand, T, st, V, d_form_off, G, T, d_gbase, d_gcls, d_cls_target, d_revt, d_rows, nullptr, nullptr, nullptr);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_rows, d_row_off, (int)(T + 1), st); }));
     uint32_t N = 0;
-    if (int rc = read(&N, d_row_off + T, 4)) return rc;
+    if (int rc = read_back(st, &N, d_row_off + T, 4)) return rc;
     if (N >= 0xFFFFFFFEu) return fail(SAGE_B200_ELIMIT, "digest: 2^32 - 2 or more peptide rows");
     I.n_rows = N;
     if (N == 0) return done(), 0;
@@ -4384,8 +4241,7 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     float* d_fmono = nullptr;
     CUDA_TRY(A.alloc(&d_forms, N));
     CUDA_TRY(A.alloc(&d_fmono, N));
-    k_dg_expand<<<grid256(T), 256, 0, st>>>(V, d_form_off, G, T, d_gbase, d_gcls, d_cls_target, d_revt, d_rows, d_row_off, d_forms, d_fmono);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_expand, T, st, V, d_form_off, G, T, d_gbase, d_gcls, d_cls_target, d_revt, d_rows, d_row_off, d_forms, d_fmono);
     V.forms = d_forms;
     V.form_mono = d_fmono;
     CUDA_TRY(cudaEventRecord(ev[5], st));
@@ -4398,23 +4254,19 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     CUDA_TRY(A.alloc(&d_fidx, N));
     CUDA_TRY(A.alloc(&d_order, N));
     CUDA_TRY(A.alloc(&d_inrun, N));
-    const unsigned gN = grid256(N);
-    k_dg_mono_key<<<gN, 256, 0, st>>>(d_fmono, N, d_mkey, d_fidx);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_mono_key, N, st, d_fmono, N, d_mkey, d_fidx);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_mkey, d_mkey_s, d_fidx, d_order, (int)N, 0, 32, st); }));
-    k_dg_in_run<<<gN, 256, 0, st>>>(d_mkey_s, N, d_inrun);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_in_run, N, st, d_mkey_s, N, d_inrun);
     CUDA_TRY(A.alloc(&d_rpos, N));
     CUDA_TRY(A.alloc(&d_rval, N));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_inrun, d_rpos, d_cnt, (int)N, st); }));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_order, d_inrun, d_rval, d_cnt, (int)N, st); }));
     uint32_t M = 0;
-    if (int rc = read(&M, d_cnt, 4)) return rc;
+    if (int rc = read_back(st, &M, d_cnt, 4)) return rc;
     if (M) {
         const DgRowLess less{V};
         CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceMergeSort::StableSortKeys(t, b, d_rval, (int)M, less, st); }));
-        k_dg_scatter<<<grid256(M), 256, 0, st>>>(d_rpos, d_rval, M, d_order);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH_N(k_dg_scatter, M, st, d_rpos, d_rval, M, d_order);
     }
     CUDA_TRY(cudaEventRecord(ev[6], st));
 
@@ -4422,11 +4274,10 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     uint32_t *d_mhead = nullptr, *d_first = nullptr;
     CUDA_TRY(A.alloc(&d_mhead, N));
     CUDA_TRY(A.alloc(&d_first, N + 1));
-    k_dg_merge_heads<<<gN, 256, 0, st>>>(V, d_order, N, d_mhead);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_merge_heads, N, st, V, d_order, N, d_mhead);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_mhead, d_first, d_cnt, (int)N, st); }));
     uint32_t n_pep = 0;
-    if (int rc = read(&n_pep, d_cnt, 4)) return rc;
+    if (int rc = read_back(st, &n_pep, d_cnt, 4)) return rc;
     CUDA_TRY(cudaMemcpyAsync(d_first + n_pep, &N, 4, cudaMemcpyHostToDevice, st));
     // offsets in 64 bits, so that a table of 2^32 residues or protein references or more is reported rather than wrapped
     uint64_t *d_nres = nullptr, *d_nref = nullptr, *d_res_off64 = nullptr, *d_ref_off64 = nullptr;
@@ -4436,13 +4287,12 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     CUDA_TRY(A.alloc(&d_ref_off64, n_pep + 1));
     CUDA_TRY(cudaMemsetAsync(d_nres + n_pep, 0, 8, st));
     CUDA_TRY(cudaMemsetAsync(d_nref + n_pep, 0, 8, st));
-    k_dg_pep_counts<<<grid256(n_pep), 256, 0, st>>>(V, d_order, d_first, n_pep, d_gstart, d_nres, d_nref);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_pep_counts, n_pep, st, V, d_order, d_first, n_pep, d_gstart, d_nres, d_nref);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nres, d_res_off64, (int)(n_pep + 1), st); }));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nref, d_ref_off64, (int)(n_pep + 1), st); }));
     uint64_t n_res = 0, n_ref = 0;
-    if (int rc = read(&n_res, d_res_off64 + n_pep, 8)) return rc;
-    if (int rc = read(&n_ref, d_ref_off64 + n_pep, 8)) return rc;
+    if (int rc = read_back(st, &n_res, d_res_off64 + n_pep, 8)) return rc;
+    if (int rc = read_back(st, &n_ref, d_ref_off64 + n_pep, 8)) return rc;
     if (n_res > 0xFFFFFFFFull || n_ref >= 0x7FFFFFFFull)
         return fail(SAGE_B200_ELIMIT, "digest: %llu residues / %llu protein references in the table (u32 offsets)", (unsigned long long)n_res,
                     (unsigned long long)n_ref);
@@ -4461,13 +4311,10 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     CUDA_TRY(O.alloc(&D->d_missed, n_pep));
     CUDA_TRY(O.alloc(&D->d_semi, n_pep));
     CUDA_TRY(A.alloc(&d_ids_raw, n_ref));
-    k_dg_u64_to_u32<<<grid256(n_pep + 1), 256, 0, st>>>(d_res_off64, n_pep + 1, D->d_res_off);
-    CUDA_TRY(cudaGetLastError());
-    k_dg_u64_to_u32<<<grid256(n_pep + 1), 256, 0, st>>>(d_ref_off64, n_pep + 1, D->d_ref_off);
-    CUDA_TRY(cudaGetLastError());
-    k_dg_export<<<grid256(n_pep), 256, 0, st>>>(V, d_order, d_first, n_pep, d_gstart, d_idx3, d_pname, D->d_res_off, D->d_ref_off, D->d_seq, D->d_mods,
-                                                D->d_nterm, D->d_cterm, D->d_mono, D->d_decoy, D->d_missed, D->d_semi, d_ids_raw);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH_N(k_dg_u64_to_u32, n_pep + 1, st, d_res_off64, n_pep + 1, D->d_res_off);
+    LAUNCH_N(k_dg_u64_to_u32, n_pep + 1, st, d_ref_off64, n_pep + 1, D->d_ref_off);
+    LAUNCH_N(k_dg_export, n_pep, st, V, d_order, d_first, n_pep, d_gstart, d_idx3, d_pname, D->d_res_off, D->d_ref_off, D->d_seq, D->d_mods,
+             D->d_nterm, D->d_cterm, D->d_mono, D->d_decoy, D->d_missed, D->d_semi, d_ids_raw);
     // proteins.sort_unstable() (database.rs:250): ids are name ranks, so an ascending sort of the ids is the sort of the names
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) {
         return cub::DeviceSegmentedSort::SortKeys(t, b, d_ids_raw, D->d_ids, (int)n_ref, (int)n_pep, D->d_ref_off, D->d_ref_off + 1, st);
@@ -4589,12 +4436,15 @@ extern "C" int sage_b200_digest_export(const sage_b200_digest* D, uint32_t* resi
         return 0;
     }
     CUDA_TRY(cudaSetDevice(D->device));
+    Stream st;
+    CUDA_TRY(st.create());
     struct Copy { void* dst; const void* src; uint64_t bytes; };
     const Copy copies[] = {{residue_offsets, D->d_res_off, 4 * (n + 1)}, {sequence, D->d_seq, I.n_residues}, {modifications, D->d_mods, 4 * I.n_residues},
                            {nterm, D->d_nterm, 4 * n}, {cterm, D->d_cterm, 4 * n}, {monoisotopic, D->d_mono, 4 * n}, {decoy, D->d_decoy, n},
                            {missed_cleavages, D->d_missed, n}, {semi_enzymatic, D->d_semi, n}, {protein_offsets, D->d_ref_off, 4 * (n + 1)},
                            {protein_ids, D->d_ids, 4 * I.n_protein_refs}};
     for (const Copy& c : copies)
-        if (c.dst && c.bytes) CUDA_TRY(cudaMemcpy(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost));
+        if (c.dst && c.bytes) CUDA_TRY(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     return 0;
 }
