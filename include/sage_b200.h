@@ -544,6 +544,59 @@ int sage_b200_digest_export(const sage_b200_digest* d, uint32_t* residue_offsets
                             uint32_t* protein_ids, uint64_t* name_offsets, char* name_bytes);
 void sage_b200_digest_destroy(sage_b200_digest* d);
 
+/* ---------------------------------------------------------------------------------------------------------------------------------------------
+ * Prefilter (database.prefilter = true; runner.rs:104-128, 161-278): the FASTA's proteins are cut into consecutive chunks; each chunk is
+ * digested and indexed, Scorer::quick_score (with report_psms + 1) runs every MS2 spectrum with at least min_peaks peaks against that index,
+ * and only the peptides some spectrum selected are kept. The kept rows of all chunks are merged by reorder_peptides (database.rs:221-258)
+ * and one final index is built from the merged table. Everything after the FASTA parse runs on the device and no table crosses PCIe. The
+ * table is the reference's bit for bit under the definitions of DESIGN.md §15; protein ids are ranks in the names table of the whole FASTA.
+ * create -> get_info -> export / chunk_counts / take_db -> destroy.
+ */
+typedef struct sage_b200_prefilter sage_b200_prefilter;
+
+typedef struct {
+    uint64_t chunk_size;              /* proteins per chunk; 0 = auto_calculate_prefilter_chunk_size (database.rs:142-160) */
+    uint8_t low_memory;               /* prefilter_low_memory: the branch of quick_score (scoring.rs:270) */
+    uint64_t min_peaks;               /* spectra with fewer peaks are not scored (runner.rs:255) */
+} sage_b200_prefilter_params;
+
+typedef struct {
+    uint64_t chunk_size, n_chunks;    /* the chunk size used; chunks digested (0 with the plain build) */
+    uint64_t plain_build;             /* 1: chunk_size >= the protein count, the plain digest was built and nothing was scored (runner.rs:110) */
+    uint64_t n_proteins;              /* proteins kept by the FASTA parser (Fasta::targets) */
+    uint64_t unmodified_peptides;     /* fasta.digest(&enzyme).len() when the chunk size was computed, else 0 */
+    uint64_t n_spectra;               /* spectra scored against each chunk (MS2 with at least min_peaks peaks) */
+    uint64_t rows_digested, rows_kept;/* peptides of the chunk tables, and those kept, over all chunks */
+    uint64_t n_peptides, n_residues, n_protein_refs, n_names, name_bytes;   /* the export's array sizes */
+    uint64_t n_fragments;             /* fragments of the final index */
+    uint64_t device_bytes;            /* HBM the handle holds (the final table and, until taken, the final index) */
+    uint64_t peak_device_bytes;       /* HBM the call held at its peak as counted by the library (the scorer's work buffers are not counted) */
+    float ms_parse;                   /* host wall clock of the FASTA parse, the names table and the argument checks */
+    float ms_count, ms_digest, ms_index, ms_quick_score, ms_compact, ms_merge, ms_final_index;   /* stage times summed over chunks: each stage
+                                         ends with its work finished, so these are wall clock of device work (count: the automatic chunk size) */
+    float ms_spectra_upload;          /* the part of ms_quick_score spent copying the spectra to the device (once per chunk) */
+    float ms_wall;                    /* host wall clock of the create call */
+} sage_b200_prefilter_info;
+
+/* EINVAL (before the device is looked at) for a null required pointer, a null spec array with a nonzero count, a non-finite mod mass,
+ * report_psms == 0, a bad tolerance kind or score type, bucket_size not a power of two, or bad ion kinds; ELIMIT for report_psms + 1 > 64 and
+ * the digest's limits. EINVAL when the automatic chunk size is 0 (the reference panics in `chunks(0)`); ELIMIT when a stage's work buffers
+ * do not fit the device's free memory (checked before it allocates). bucket_size, ion_kinds and min_ion_index are those of
+ * sage_b200_db_build and serve every chunk index and the final index. */
+int sage_b200_prefilter_create(int device, const char* fasta, uint64_t fasta_len, const sage_b200_digest_params* digest, const sage_b200_scorer_params* scorer,
+                               const sage_b200_prefilter_params* params, const sage_b200_spectra* spectra, uint64_t bucket_size, const uint8_t* ion_kinds,
+                               uint64_t n_ion_kinds, uint64_t min_ion_index, sage_b200_prefilter** out);
+int sage_b200_prefilter_get_info(const sage_b200_prefilter* f, sage_b200_prefilter_info* info);
+/* Per chunk, in chunk order: rows of its digest and rows kept ([n_chunks] each; either may be NULL). */
+int sage_b200_prefilter_chunk_counts(const sage_b200_prefilter* f, uint64_t* rows_digested, uint64_t* rows_kept);
+/* The final table, in the arrays and sizes of sage_b200_digest_export. */
+int sage_b200_prefilter_export(const sage_b200_prefilter* f, uint32_t* residue_offsets, uint8_t* sequence, float* modifications, float* nterm, float* cterm,
+                               float* monoisotopic, uint8_t* decoy, uint8_t* missed_cleavages, uint8_t* semi_enzymatic, uint32_t* protein_offsets,
+                               uint32_t* protein_ids, uint64_t* name_offsets, char* name_bytes);
+/* Hands the final index to the caller, who destroys it with sage_b200_db_destroy; EINVAL on a second call. */
+int sage_b200_prefilter_take_db(sage_b200_prefilter* f, sage_b200_db** out);
+void sage_b200_prefilter_destroy(sage_b200_prefilter* f);
+
 /* Page-locked host buffers: spectra/feature arrays placed here are copied by DMA without a staging memcpy. */
 void* sage_b200_host_alloc(size_t bytes);
 /* The same for a batch sage_b200_score_batch_multi cuts into n_devices contiguous blocks: the i-th of n equal parts of the buffer is placed on the

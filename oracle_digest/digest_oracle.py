@@ -36,7 +36,9 @@ def lib():
         build()
         _lib = C.CDLL(_SO)
         _lib.sod_digest.restype = C.c_void_p
-        for f in ("sod_free", "sod_sizes", "sod_export", "sod_db_sizes", "sod_db_export"):
+        _lib.sod_prefilter.restype = C.c_void_p
+        _lib.sod_auto_chunk_size.restype = C.c_uint64
+        for f in ("sod_free", "sod_sizes", "sod_export", "sod_db_sizes", "sod_db_export", "sod_pf_free", "sod_pf_info", "sod_pf_sizes", "sod_pf_export"):
             getattr(_lib, f).restype = None
     return _lib
 
@@ -104,3 +106,41 @@ def protein_lists(t: dict) -> list:
     raw = t["names"].tobytes()
     no, po = t["name_off"], t["prot_off"]
     return [[raw[no[j]:no[j + 1]] for j in range(po[i], po[i + 1])] for i in range(len(po) - 1)]
+
+
+def auto_chunk_size(fasta, **kw) -> int:
+    """Parameters::auto_calculate_prefilter_chunk_size (database.rs:142-160) of FASTA text with OracleDB.from_fasta's keywords (0 where the
+    reference's chunks(0) would panic)."""
+    text = fasta.encode() if isinstance(fasta, str) else bytes(fasta)
+    keep: list = []
+    bp = _build_params(kw, keep)
+    return int(lib().sod_auto_chunk_size(C.c_char_p(text), C.byref(bp)))
+
+
+def prefilter(fasta, spectra: dict, cfg, chunk_size: int = 0, low_memory: bool = True, min_peaks: int = 15, **kw):
+    """The oracle's prefilter (runner.rs:104-128, 161-278) of FASTA text: spectra as OracleDB.score_batch takes them, cfg an oracle
+    ScorerConfig (report_psms as the search's: the chunk scorers add 1), kw OracleDB.from_fasta's keywords. Returns (table, info) with the
+    table of digest() and info = dict(chunk_size, n_chunks, plain_build, rows, kept); None when the chunk size is 0."""
+    text = fasta.encode() if isinstance(fasta, str) else bytes(fasta)
+    keep: list = []
+    bp = _build_params(kw, keep)
+    f32 = lambda x: np.ascontiguousarray(x, np.float32)  # noqa: E731
+    arrs = [np.ascontiguousarray(spectra["peak_off"], np.uint64), f32(spectra["masses"]), f32(spectra["intensities"]), f32(spectra["prec_mz"]),
+            np.ascontiguousarray(spectra["prec_charge"], np.uint8), f32(spectra["iso_lo"]), f32(spectra["iso_hi"]), f32(spectra["tic"])]
+    level = None if spectra.get("level") is None else np.ascontiguousarray(spectra["level"], np.uint8)
+    sp = cfg.to_c()
+    L = lib()
+    h = L.sod_prefilter(C.c_char_p(text), C.byref(bp), C.byref(sp), C.c_uint64(int(chunk_size)), C.c_int(int(bool(low_memory))), C.c_uint64(int(min_peaks)),
+                        C.c_uint64(len(arrs[3])), *[a.ctypes.data_as(C.c_void_p) for a in arrs], None if level is None else level.ctypes.data_as(C.c_void_p))
+    if not h:
+        return None
+    h = C.c_void_p(h)
+    try:
+        head = np.zeros(3, np.uint64)
+        L.sod_pf_info(h, head.ctypes.data_as(C.c_void_p), None, None)
+        rows, kept = np.zeros(int(head[1]), np.uint64), np.zeros(int(head[1]), np.uint64)
+        L.sod_pf_info(h, head.ctypes.data_as(C.c_void_p), rows.ctypes.data_as(C.c_void_p), kept.ctypes.data_as(C.c_void_p))
+        info = dict(chunk_size=int(head[0]), n_chunks=int(head[1]), plain_build=int(head[2]), rows=rows, kept=kept)
+        return _table(L.sod_pf_sizes, L.sod_pf_export, h), info
+    finally:
+        L.sod_pf_free(h)

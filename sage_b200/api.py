@@ -94,6 +94,8 @@ EXPORTED_SYMBOLS = [
     "sage_b200_spectrum_fdr", "sage_b200_kde_build", "sage_b200_device_math", "sage_b200_predict_rt",
     "sage_b200_picked_fdr", "sage_b200_picked_precursor", "sage_b200_competition_keys", "sage_b200_protein_groups", "sage_b200_bipartite_cover",
     "sage_b200_digest_create", "sage_b200_digest_get_info", "sage_b200_digest_export", "sage_b200_digest_destroy",
+    "sage_b200_prefilter_create", "sage_b200_prefilter_get_info", "sage_b200_prefilter_chunk_counts", "sage_b200_prefilter_export",
+    "sage_b200_prefilter_take_db", "sage_b200_prefilter_destroy",
 ]
 
 _lib = None
@@ -123,6 +125,7 @@ def load_library(build: bool = True):
     lib.sage_b200_scorer_destroy.argtypes = [C.c_void_p]
     lib.sage_b200_lfq_destroy.argtypes = [C.c_void_p]
     lib.sage_b200_digest_destroy.argtypes = [C.c_void_p]
+    lib.sage_b200_prefilter_destroy.argtypes = [C.c_void_p]
     _lib = lib
     return lib
 
@@ -420,10 +423,21 @@ class IndexedDatabase:
         return IndexedDatabase(h.value, peptides)
 
     @staticmethod
-    def from_fasta(fasta, *, bucket_size=8192, ion_kinds=("b", "y"), min_ion_index=2, device=0, **digest_args) -> "IndexedDatabase":
+    def from_fasta(fasta, *, bucket_size=8192, ion_kinds=("b", "y"), min_ion_index=2, device=0, prefilter=False, spectra=None, scorer=None,
+                   prefilter_chunk_size=0, prefilter_low_memory=True, min_peaks=15, **digest_args) -> "IndexedDatabase":
         """Builder::make_parameters + Parameters::build (database.rs:96-115, 260) from FASTA text: digest_fasta, then build_from_peptides on
         the digested table. `bucket_size` is rounded up to a power of two. The digest result stays on the db as `.digest` (protein lists,
-        cterm, semi_enzymatic for picked_fdr, protein_groups and the writers)."""
+        cterm, semi_enzymatic for picked_fdr, protein_groups and the writers).
+        prefilter=True: the database prefilter of runner.rs:104-128 (prefilter_fasta) with `spectra` (a SpectraBatch) and `scorer` (a dict of
+        the Scorer keywords, precursor_tol and fragment_tol required); `.digest` is then the PrefilterResult."""
+        if prefilter:
+            if spectra is None or scorer is None:
+                raise ValueError("prefilter=True needs spectra and scorer")
+            r = prefilter_fasta(fasta, spectra, bucket_size=bucket_size, ion_kinds=ion_kinds, min_ion_index=min_ion_index, device=device,
+                                prefilter_chunk_size=prefilter_chunk_size, prefilter_low_memory=prefilter_low_memory, min_peaks=min_peaks,
+                                **dict(scorer), **digest_args)
+            r.db.digest = r
+            return r.db
         if isinstance(bucket_size, bool) or not isinstance(bucket_size, (int, np.integer)) or not 1 <= int(bucket_size) <= 1 << 30:
             raise ValueError(f"bucket_size must be an integer in 1..2^30, got {bucket_size!r}")
         bs = 1 << (int(bucket_size) - 1).bit_length()
@@ -1108,13 +1122,9 @@ def _spec_arrays(mods: dict | None, keep: list, variable: bool):
     return C.cast(specs, C.c_void_p), _ptr(masses), len(items)
 
 
-def digest_fasta(fasta, *, missed_cleavages=0, min_len=5, max_len=50, cleave_at="KR", restrict="P", c_terminal=True, semi_enzymatic=False,
-                 peptide_min_mass=500.0, peptide_max_mass=5000.0, static_mods=None, variable_mods=None, max_variable_mods=2, decoy_tag="rev_",
-                 generate_decoys=True, device=0) -> DigestResult:
-    """Parameters::digest (database.rs:162-258) on the device: FASTA text (str or bytes) to the sorted, merged peptide table. Keywords and
-    defaults are Builder::default()'s. static_mods maps a spec ("C", "^", "[Q", ...) to a mass, variable_mods a spec to a list of masses."""
-    text = fasta.encode() if isinstance(fasta, str) else bytes(fasta)
-    keep: list = []
+def _digest_params(keep: list, missed_cleavages=0, min_len=5, max_len=50, cleave_at="KR", restrict="P", c_terminal=True, semi_enzymatic=False,
+                   peptide_min_mass=500.0, peptide_max_mass=5000.0, static_mods=None, variable_mods=None, max_variable_mods=2, decoy_tag="rev_",
+                   generate_decoys=True) -> CDigestParams:
     p = CDigestParams()
     p.missed_cleavages, p.min_len, p.max_len = int(missed_cleavages), int(min_len), int(max_len)
     p.cleave_at, p.restrict_ = cleave_at.encode(), restrict.encode()
@@ -1123,6 +1133,35 @@ def digest_fasta(fasta, *, missed_cleavages=0, min_len=5, max_len=50, cleave_at=
     p.static_specs, p.static_masses, p.n_static = _spec_arrays(static_mods, keep, False)
     p.variable_specs, p.variable_masses, p.n_variable = _spec_arrays(variable_mods, keep, True)
     p.max_variable_mods, p.decoy_tag, p.generate_decoys = int(max_variable_mods), decoy_tag.encode(), int(bool(generate_decoys))
+    return p
+
+
+def _export_table(export, h, info: dict) -> tuple:
+    """The table of a digest or prefilter handle, exported with `export` into numpy arrays: (Peptides, cterm, semi, prot_off, ids, names)."""
+    n, nres, nref = info["n_peptides"], info["n_residues"], info["n_protein_refs"]
+    a = dict(seq_off=np.empty(n + 1, np.uint32), seq=np.empty(nres, np.uint8), mods=np.empty(nres, np.float32), nterm=np.empty(n, np.float32),
+             cterm=np.empty(n, np.float32), mono=np.empty(n, np.float32), decoy=np.empty(n, np.uint8), missed=np.empty(n, np.uint8),
+             semi=np.empty(n, np.uint8), prot_off=np.empty(n + 1, np.uint32), ids=np.empty(nref, np.uint32),
+             name_off=np.empty(info["n_names"] + 1, np.uint64), names=np.empty(max(1, info["name_bytes"]), np.uint8))
+    t = time.perf_counter()
+    _check(export(h, *[_ptr(a[k]) for k in ("seq_off", "seq", "mods", "nterm", "cterm", "mono", "decoy", "missed", "semi", "prot_off", "ids",
+                                            "name_off", "names")]))
+    info["ms_export"] = (time.perf_counter() - t) * 1e3
+    raw = a["names"].tobytes()
+    no = a["name_off"]
+    names = [raw[no[i]:no[i + 1]].decode("utf-8", errors="surrogateescape") for i in range(len(no) - 1)]
+    pep = Peptides(a["seq_off"], a["seq"], a["mods"], a["nterm"], a["mono"], a["decoy"], a["missed"])
+    return pep, a["cterm"], a["semi"].astype(bool), a["prot_off"], a["ids"], names
+
+
+def digest_fasta(fasta, *, device=0, **digest_args) -> DigestResult:
+    """Parameters::digest (database.rs:162-258) on the device: FASTA text (str or bytes) to the sorted, merged peptide table. Keywords and
+    defaults are Builder::default()'s: missed_cleavages=0, min_len=5, max_len=50, cleave_at="KR", restrict="P", c_terminal=True,
+    semi_enzymatic=False, peptide_min_mass=500.0, peptide_max_mass=5000.0, static_mods=None, variable_mods=None, max_variable_mods=2,
+    decoy_tag="rev_", generate_decoys=True. static_mods maps a spec ("C", "^", "[Q", ...) to a mass, variable_mods a spec to a list of masses."""
+    text = fasta.encode() if isinstance(fasta, str) else bytes(fasta)
+    keep: list = []
+    p = _digest_params(keep, **digest_args)
     lib = load_library()
     h = C.c_void_p()
     _check(lib.sage_b200_digest_create(C.c_int(device), C.c_char_p(text), C.c_uint64(len(text)), C.byref(p), C.byref(h)))
@@ -1130,19 +1169,78 @@ def digest_fasta(fasta, *, missed_cleavages=0, min_len=5, max_len=50, cleave_at=
         ci = CDigestInfo()
         _check(lib.sage_b200_digest_get_info(h, C.byref(ci)))
         info = {k: getattr(ci, k) for k, _ in CDigestInfo._fields_}
-        n, nres, nref = info["n_peptides"], info["n_residues"], info["n_protein_refs"]
-        a = dict(seq_off=np.empty(n + 1, np.uint32), seq=np.empty(nres, np.uint8), mods=np.empty(nres, np.float32), nterm=np.empty(n, np.float32),
-                 cterm=np.empty(n, np.float32), mono=np.empty(n, np.float32), decoy=np.empty(n, np.uint8), missed=np.empty(n, np.uint8),
-                 semi=np.empty(n, np.uint8), prot_off=np.empty(n + 1, np.uint32), ids=np.empty(nref, np.uint32),
-                 name_off=np.empty(info["n_names"] + 1, np.uint64), names=np.empty(max(1, info["name_bytes"]), np.uint8))
-        t = time.perf_counter()
-        _check(lib.sage_b200_digest_export(h, *[_ptr(a[k]) for k in ("seq_off", "seq", "mods", "nterm", "cterm", "mono", "decoy", "missed", "semi",
-                                                                     "prot_off", "ids", "name_off", "names")]))
-        info["ms_export"] = (time.perf_counter() - t) * 1e3
+        table = _export_table(lib.sage_b200_digest_export, h, info)
     finally:
         lib.sage_b200_digest_destroy(h)
-    raw = a["names"].tobytes()
-    no = a["name_off"]
-    names = [raw[no[i]:no[i + 1]].decode("utf-8", errors="surrogateescape") for i in range(len(no) - 1)]
-    pep = Peptides(a["seq_off"], a["seq"], a["mods"], a["nterm"], a["mono"], a["decoy"], a["missed"])
-    return DigestResult(pep, a["cterm"], a["semi"].astype(bool), a["prot_off"], a["ids"], names, info)
+    return DigestResult(*table, info)
+
+
+# ------------------------------------------------------------------------------------------------ prefilter (runner.rs:104-128, 161-278)
+class CPrefilterParams(C.Structure):
+    _fields_ = [("chunk_size", C.c_uint64), ("low_memory", C.c_uint8), ("min_peaks", C.c_uint64)]
+
+
+PREFILTER_COUNTS = ("chunk_size", "n_chunks", "plain_build", "n_proteins", "unmodified_peptides", "n_spectra", "rows_digested", "rows_kept", "n_peptides",
+                    "n_residues", "n_protein_refs", "n_names", "name_bytes", "n_fragments", "device_bytes", "peak_device_bytes")
+PREFILTER_TIMES = ("ms_parse", "ms_count", "ms_digest", "ms_index", "ms_quick_score", "ms_compact", "ms_merge", "ms_final_index", "ms_spectra_upload",
+                   "ms_wall")
+
+
+class CPrefilterInfo(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in PREFILTER_COUNTS] + [(n, C.c_float) for n in PREFILTER_TIMES]
+
+
+@dataclass
+class PrefilterResult(DigestResult):
+    """The prefiltered peptide table in DigestResult's shape (so picked_fdr and protein_groups take it unchanged; protein ids are ranks in the
+    names table of the whole FASTA), the final index over it, and per chunk the rows digested and kept."""
+    db: "IndexedDatabase"
+    chunk_rows: np.ndarray
+    chunk_kept: np.ndarray
+
+
+def prefilter_fasta(fasta, spectra: SpectraBatch, *, precursor_tol: Tolerance, fragment_tol: Tolerance, min_matched_peaks=4, min_isotope_err=0,
+                    max_isotope_err=0, min_precursor_charge=2, max_precursor_charge=4, override_precursor_charge=False, max_fragment_charge=None,
+                    chimera=False, report_psms=1, wide_window=False, annotate_matches=False, score_type=0, min_peaks=15, prefilter_chunk_size=0,
+                    prefilter_low_memory=True, bucket_size=8192, ion_kinds=("b", "y"), min_ion_index=2, device=0, **digest_args) -> PrefilterResult:
+    """The database prefilter (database.prefilter = true, runner.rs:104-128) on the device: the FASTA's proteins in chunks of
+    prefilter_chunk_size (0 = Parameters::auto_calculate_prefilter_chunk_size), each chunk digested and indexed, Scorer::quick_score with
+    report_psms + 1 for every MS2 spectrum of `spectra` with at least min_peaks peaks, the selected peptides of all chunks merged by
+    reorder_peptides, and one index built over them. When the chunk size covers every protein the plain digest and index are built and
+    nothing is scored, as the reference does. The Scorer keywords are Scorer's; the digest keywords are digest_fasta's. bucket_size is rounded
+    up to a power of two."""
+    if isinstance(bucket_size, bool) or not isinstance(bucket_size, (int, np.integer)) or not 1 <= int(bucket_size) <= 1 << 30:
+        raise ValueError(f"bucket_size must be an integer in 1..2^30, got {bucket_size!r}")
+    bs = 1 << (int(bucket_size) - 1).bit_length()
+    text = fasta.encode() if isinstance(fasta, str) else bytes(fasta)
+    keep: list = []
+    dp = _digest_params(keep, **digest_args)
+    sp = CScorerParams()
+    sp.precursor_tol, sp.fragment_tol = precursor_tol._c(), fragment_tol._c()
+    sp.min_matched_peaks = min_matched_peaks
+    sp.min_isotope_err, sp.max_isotope_err = min_isotope_err, max_isotope_err
+    sp.min_precursor_charge, sp.max_precursor_charge = min_precursor_charge, max_precursor_charge
+    sp.override_precursor_charge = int(override_precursor_charge)
+    sp.max_fragment_charge = -1 if max_fragment_charge is None else int(max_fragment_charge)
+    sp.chimera, sp.wide_window, sp.annotate_matches = int(chimera), int(wide_window), int(annotate_matches)
+    sp.score_type, sp.report_psms = int(score_type), int(report_psms)
+    pp = CPrefilterParams(int(prefilter_chunk_size), int(bool(prefilter_low_memory)), int(min_peaks))
+    cs = spectra._c(keep)
+    kinds = _kinds(ion_kinds)
+    lib = load_library()
+    h = C.c_void_p()
+    _check(lib.sage_b200_prefilter_create(C.c_int(device), C.c_char_p(text), C.c_uint64(len(text)), C.byref(dp), C.byref(sp), C.byref(pp), C.byref(cs),
+                                          C.c_uint64(bs), _ptr(kinds), C.c_uint64(len(kinds)), C.c_uint64(int(min_ion_index)), C.byref(h)))
+    try:
+        ci = CPrefilterInfo()
+        _check(lib.sage_b200_prefilter_get_info(h, C.byref(ci)))
+        info = {k: getattr(ci, k) for k, _ in CPrefilterInfo._fields_}
+        table = _export_table(lib.sage_b200_prefilter_export, h, info)
+        rows, kept = np.zeros(info["n_chunks"], np.uint64), np.zeros(info["n_chunks"], np.uint64)
+        _check(lib.sage_b200_prefilter_chunk_counts(h, _ptr(rows), _ptr(kept)))
+        dbh = C.c_void_p()
+        _check(lib.sage_b200_prefilter_take_db(h, C.byref(dbh)))
+    finally:
+        lib.sage_b200_prefilter_destroy(h)
+    db = IndexedDatabase(dbh.value, table[0])
+    return PrefilterResult(*table, info, db, rows, kept)

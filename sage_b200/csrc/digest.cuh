@@ -545,6 +545,11 @@ struct DgRowLess {
     }
 };
 
+__global__ void k_dg_u64_to_u32(const uint64_t* __restrict__ a, uint64_t n, uint32_t* __restrict__ b) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) b[i] = (uint32_t)a[i];
+}
+
 __global__ void k_dg_scatter(const uint32_t* __restrict__ pos, const uint32_t* __restrict__ val, uint32_t M, uint32_t* __restrict__ dst) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < M) dst[pos[i]] = val[i];

@@ -42,6 +42,7 @@
 #include "picked.cuh"
 #include "protein_groups.cuh"
 #include "digest.cuh"
+#include "prefilter.cuh"
 
 using namespace sb;
 
@@ -388,20 +389,59 @@ static uint32_t ceil_log2_u64(uint64_t n) {
     return l;
 }
 
-// Uploads the peptide table and builds the per-peptide ion tables. On return tmp_* hold device copies still needed by db_build.
-static int db_upload_peptides(sage_b200_db* db, const sage_b200_peptides* P, const uint8_t* kinds, uint64_t n_kinds) {
-    if (!P || (P->n_peptides && (!P->residue_offsets || !P->sequence || !P->modifications || !P->nterm || !P->monoisotopic || !P->decoy || !P->missed_cleavages)))
-        return fail(SAGE_B200_EINVAL, "peptides: null array");
+// The ion kinds of an index, validated.
+static int db_set_kinds(sage_b200_db* db, const uint8_t* kinds, uint64_t n_kinds) {
     if (n_kinds == 0 || n_kinds > MAX_KINDS) return fail(SAGE_B200_EINVAL, "ion_kinds: need 1..%d kinds", MAX_KINDS);
-    if (P->n_peptides >= 0xFFFFFFFEull) return fail(SAGE_B200_ELIMIT, "too many peptides for u32 PeptideIx");
-    const uint64_t n = P->n_peptides;
-    db->v.n_pep = (uint32_t)n;
     db->v.n_kinds = (uint32_t)n_kinds;
     for (uint64_t k = 0; k < n_kinds; k++) {
         if (kinds[k] > 5) return fail(SAGE_B200_EINVAL, "ion kind %u out of range", kinds[k]);
         db->v.kinds[k] = kinds[k];
         if (kinds[k] <= 2) db->v.nterm_mask |= 1u << k;
     }
+    return 0;
+}
+
+// The per-peptide arrays of an n-peptide index (mono, length, flags, missed cleavages, ion offsets), allocated and placed in the view.
+static int db_alloc_peptides(sage_b200_db* db, uint64_t n) {
+    int rc;
+    if ((rc = dmalloc(db, &db->d_pep_mono, 4 * n))) return rc;
+    if ((rc = dmalloc(db, &db->d_pep_len, n))) return rc;
+    if ((rc = dmalloc(db, &db->d_pep_flags, n))) return rc;
+    if ((rc = dmalloc(db, &db->d_pep_missed, n))) return rc;
+    if ((rc = dmalloc(db, &db->d_ion_off, 4 * (n + 1)))) return rc;
+    db->v.n_pep = (uint32_t)n;
+    db->v.pep_mono = (const float*)db->d_pep_mono;
+    db->v.pep_len = (const uint8_t*)db->d_pep_len;
+    db->v.pep_flags = (const uint8_t*)db->d_pep_flags;
+    db->v.pep_missed = (const uint8_t*)db->d_pep_missed;
+    db->v.ion_off = (const uint32_t*)db->d_ion_off;
+    return 0;
+}
+
+// The per-peptide ion tables (n_ions entries at the ion offsets already on the device) from the table's device arrays.
+static int db_build_ions(sage_b200_db* db, uint64_t n, uint64_t n_ions, const uint32_t* off, const uint8_t* seq, const float* mods, const float* nterm) {
+    if (int rc = dmalloc(db, &db->d_ions, 4 * n_ions)) return rc;
+    db->v.ions = (const float*)db->d_ions;
+    DevArena A;
+    float* t_res = nullptr;
+    CUDA_TRY(A.alloc(&t_res, sizeof kResidueMass / sizeof(float)));
+    CUDA_TRY(cudaMemcpy(t_res, kResidueMass, sizeof kResidueMass, cudaMemcpyHostToDevice));
+    if (n) {
+        k_build_ions<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, off, seq, mods, nterm, (const float*)db->d_pep_mono, (const uint32_t*)db->d_ion_off,
+                                                           db->v.n_kinds, db->v, (float*)db->d_ions, t_res);
+        CUDA_TRY(cudaGetLastError());
+    }
+    CUDA_TRY(cudaDeviceSynchronize());
+    return 0;
+}
+
+// Uploads the peptide table and builds the per-peptide ion tables.
+static int db_upload_peptides(sage_b200_db* db, const sage_b200_peptides* P, const uint8_t* kinds, uint64_t n_kinds) {
+    if (!P || (P->n_peptides && (!P->residue_offsets || !P->sequence || !P->modifications || !P->nterm || !P->monoisotopic || !P->decoy || !P->missed_cleavages)))
+        return fail(SAGE_B200_EINVAL, "peptides: null array");
+    if (int rc = db_set_kinds(db, kinds, n_kinds)) return rc;
+    if (P->n_peptides >= 0xFFFFFFFEull) return fail(SAGE_B200_ELIMIT, "too many peptides for u32 PeptideIx");
+    const uint64_t n = P->n_peptides;
     const uint64_t nres = n ? P->residue_offsets[n] : 0;
     db->total_residues = nres;
     std::vector<uint8_t> len(n), flags(n);
@@ -417,48 +457,28 @@ static int db_upload_peptides(sage_b200_db* db, const sage_b200_peptides* P, con
         if (acc > 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "ion table exceeds 2^32 entries");
     }
     ion_off[n] = (uint32_t)acc;
-    int rc;
-    if ((rc = dmalloc(db, &db->d_pep_mono, 4 * n))) return rc;
-    if ((rc = dmalloc(db, &db->d_pep_len, n))) return rc;
-    if ((rc = dmalloc(db, &db->d_pep_flags, n))) return rc;
-    if ((rc = dmalloc(db, &db->d_pep_missed, n))) return rc;
-    if ((rc = dmalloc(db, &db->d_ion_off, 4 * (n + 1)))) return rc;
-    if ((rc = dmalloc(db, &db->d_ions, 4 * acc))) return rc;
+    if (int rc = db_alloc_peptides(db, n)) return rc;
     CUDA_TRY(cudaMemcpy(db->d_pep_mono, P->monoisotopic, 4 * n, cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(db->d_pep_len, len.data(), n, cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(db->d_pep_flags, flags.data(), n, cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(db->d_pep_missed, P->missed_cleavages, n, cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(db->d_ion_off, ion_off.data(), 4 * (n + 1), cudaMemcpyHostToDevice));
-    // temporaries for ion generation
+    // device copies of the arrays ion generation reads
     DevArena A;
     uint32_t* t_off = nullptr;
     uint8_t* t_seq = nullptr;
-    float *t_mods = nullptr, *t_nterm = nullptr, *t_res = nullptr;
+    float *t_mods = nullptr, *t_nterm = nullptr;
     CUDA_TRY(A.alloc(&t_off, n + 5));
     CUDA_TRY(A.alloc(&t_seq, nres + 16));
     CUDA_TRY(A.alloc(&t_mods, nres + 4));
     CUDA_TRY(A.alloc(&t_nterm, n + 4));
-    CUDA_TRY(A.alloc(&t_res, sizeof kResidueMass / sizeof(float)));
     if (n) {
         CUDA_TRY(cudaMemcpy(t_off, P->residue_offsets, 4 * (n + 1), cudaMemcpyHostToDevice));
         CUDA_TRY(cudaMemcpy(t_seq, P->sequence, nres, cudaMemcpyHostToDevice));
         CUDA_TRY(cudaMemcpy(t_mods, P->modifications, 4 * nres, cudaMemcpyHostToDevice));
         CUDA_TRY(cudaMemcpy(t_nterm, P->nterm, 4 * n, cudaMemcpyHostToDevice));
     }
-    CUDA_TRY(cudaMemcpy(t_res, kResidueMass, sizeof kResidueMass, cudaMemcpyHostToDevice));
-    db->v.pep_mono = (const float*)db->d_pep_mono;
-    db->v.pep_len = (const uint8_t*)db->d_pep_len;
-    db->v.pep_flags = (const uint8_t*)db->d_pep_flags;
-    db->v.pep_missed = (const uint8_t*)db->d_pep_missed;
-    db->v.ion_off = (const uint32_t*)db->d_ion_off;
-    db->v.ions = (const float*)db->d_ions;
-    if (n) {
-        k_build_ions<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, t_off, t_seq, t_mods, t_nterm, (const float*)db->d_pep_mono, (const uint32_t*)db->d_ion_off,
-                                                           (uint32_t)n_kinds, db->v, (float*)db->d_ions, t_res);
-        CUDA_TRY(cudaGetLastError());
-    }
-    CUDA_TRY(cudaDeviceSynchronize());
-    return 0;
+    return db_build_ions(db, n, acc, t_off, t_seq, t_mods, t_nterm);
 }
 
 // A handle under construction: destroyed (by its C destroy function) unless released to the caller.
@@ -625,26 +645,10 @@ extern "C" int sage_b200_db_create(const sage_b200_peptides* peptides, const sag
     return 0;
 }
 
-extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t bucket_size, const uint8_t* ion_kinds, uint64_t n_ion_kinds,
-                                  uint64_t min_ion_index, int device, sage_b200_db** out) {
-    if (!out || !peptides || !ion_kinds) return fail(SAGE_B200_EINVAL, "db_build: null argument");
-    if (bucket_size == 0 || (bucket_size & (bucket_size - 1)) || bucket_size > (1ull << 30))
-        return fail(SAGE_B200_EINVAL, "bucket_size must be a power of two (Builder::make_parameters rounds up, database.rs:97)");
-    Guard<sage_b200_db> guard(nullptr, sage_b200_db_destroy);
-    if (int rc = db_new(device, guard)) return rc;
-    sage_b200_db* db = guard.get();
-    if (int rc = db_upload_peptides(db, peptides, ion_kinds, n_ion_kinds)) return rc;
-    const uint64_t n = peptides->n_peptides;
-    // fragments kept per peptide: n_kinds * max(0, L-1-min_ion_index)   (database.rs:281-291)
-    std::vector<uint64_t> frag_off(n + 1);
-    uint64_t nf = 0;
-    for (uint64_t i = 0; i < n; i++) {
-        frag_off[i] = nf;
-        const uint64_t L = peptides->residue_offsets[i + 1] - peptides->residue_offsets[i];
-        const uint64_t keep = (L - 1) > min_ion_index ? (L - 1) - min_ion_index : 0;
-        nf += n_ion_kinds * keep;
-    }
-    frag_off[n] = nf;
+// The fragment index of a db whose ion tables are built: fragments kept per peptide at d_off (u64, n + 1; nf in all), the global sort by
+// fragment m/z, bucketing, the per-bucket sort by PeptideIx and the search directories (database.rs:281-365).
+static int db_build_fragments(sage_b200_db* db, const uint64_t* d_off, uint64_t nf, uint64_t bucket_size, uint64_t min_ion_index) {
+    const uint64_t n = db->v.n_pep;
     const uint32_t shift = ceil_log2_u64(bucket_size);
     const uint64_t nb = (nf + bucket_size - 1) / bucket_size;
     if (nb > 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "too many buckets");
@@ -657,7 +661,8 @@ extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t b
     if (int rc = dmalloc(db, &db->d_bucket_min, 4 * nb)) return rc;
     db->v.frag = (const uint2*)db->d_frag;
     db->v.bucket_min = (const float*)db->d_bucket_min;
-    if (nf == 0) { *out = guard.release(); return 0; }
+    if (nf == 0) return 0;
+    if (nf > 0x7FFFFFFFull) return fail(SAGE_B200_ELIMIT, "more than 2^31 fragments: sort in slabs not implemented");
 
     {
         DevArena A;   // freed before the directories are built
@@ -666,15 +671,11 @@ extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t b
         {   // (1) stable LSD radix sort by fragment m/z (par_sort_unstable_by fragment_mz, database.rs:301; ties keep PeptideIx order); its
             // inputs are freed before step (2) allocates
             DevArena S;
-            uint64_t* d_off = nullptr;
             uint32_t *k32a = nullptr, *pa = nullptr;
-            CUDA_TRY(S.alloc(&d_off, n + 1));
-            CUDA_TRY(cudaMemcpy(d_off, frag_off.data(), 8 * (n + 1), cudaMemcpyHostToDevice));
             CUDA_TRY(S.alloc(&k32a, nf)); CUDA_TRY(S.alloc(&pa, nf));
             k_gen_fragments<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, db->v.pep_len, db->v.ion_off, db->v.ions, db->v.n_kinds, db->v, (uint32_t)std::min<uint64_t>(min_ion_index, 0xFFFFFFFFull),
                                                                   nullptr, d_off, k32a, pa);
             CUDA_TRY(cudaGetLastError());
-            if (nf > 0x7FFFFFFFull) return fail(SAGE_B200_ELIMIT, "more than 2^31 fragments: sort in slabs not implemented");
             CUDA_TRY(S.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint32_t*)k32a, k32b, (const uint32_t*)pa, pb, (int)nf); },
                                  16));
         }
@@ -692,7 +693,91 @@ extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t b
         CUDA_TRY(cudaGetLastError());
         CUDA_TRY(cudaDeviceSynchronize());
     }
-    if (int rc = db_build_directories(db)) return rc;
+    return db_build_directories(db);
+}
+
+static int db_check_bucket_size(uint64_t bucket_size) {
+    if (bucket_size == 0 || (bucket_size & (bucket_size - 1)) || bucket_size > (1ull << 30))
+        return fail(SAGE_B200_EINVAL, "bucket_size must be a power of two (Builder::make_parameters rounds up, database.rs:97)");
+    return 0;
+}
+
+extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t bucket_size, const uint8_t* ion_kinds, uint64_t n_ion_kinds,
+                                  uint64_t min_ion_index, int device, sage_b200_db** out) {
+    if (!out || !peptides || !ion_kinds) return fail(SAGE_B200_EINVAL, "db_build: null argument");
+    if (int rc = db_check_bucket_size(bucket_size)) return rc;
+    Guard<sage_b200_db> guard(nullptr, sage_b200_db_destroy);
+    if (int rc = db_new(device, guard)) return rc;
+    sage_b200_db* db = guard.get();
+    if (int rc = db_upload_peptides(db, peptides, ion_kinds, n_ion_kinds)) return rc;
+    const uint64_t n = peptides->n_peptides;
+    // fragments kept per peptide: n_kinds * max(0, L-1-min_ion_index)   (database.rs:281-291)
+    std::vector<uint64_t> frag_off(n + 1);
+    uint64_t nf = 0;
+    for (uint64_t i = 0; i < n; i++) {
+        frag_off[i] = nf;
+        const uint64_t L = peptides->residue_offsets[i + 1] - peptides->residue_offsets[i];
+        const uint64_t keep = (L - 1) > min_ion_index ? (L - 1) - min_ion_index : 0;
+        nf += n_ion_kinds * keep;
+    }
+    frag_off[n] = nf;
+    DevArena A;
+    uint64_t* d_off = nullptr;
+    CUDA_TRY(A.alloc(&d_off, n + 1));
+    CUDA_TRY(cudaMemcpy(d_off, frag_off.data(), 8 * (n + 1), cudaMemcpyHostToDevice));
+    if (int rc = db_build_fragments(db, d_off, nf, bucket_size, min_ion_index)) return rc;
+    *out = guard.release();
+    return 0;
+}
+
+// A peptide table held on the device in the digest's export layout (the prefilter's chunk tables and its merged table).
+struct DevTable {
+    uint64_t n = 0, n_res = 0, n_ref = 0;
+    const uint32_t *res_off = nullptr, *ref_off = nullptr, *ids = nullptr;
+    const uint8_t *seq = nullptr, *decoy = nullptr, *missed = nullptr, *semi = nullptr;
+    const float *mods = nullptr, *nterm = nullptr, *cterm = nullptr, *mono = nullptr;
+    PfRows rows() const { return PfRows{res_off, ref_off, seq, mods, nterm, cterm, mono, decoy, missed, semi, ids}; }
+};
+
+// Parameters::build_from_peptides (database.rs:265-365) from a table already on the device: lengths, flags, ion and fragment offsets come
+// from kernels and scans, the limits are read back once, and nothing crosses PCIe. The table's work must be finished before the call.
+static int db_build_device(const DevTable& T, uint64_t bucket_size, const uint8_t* kinds, uint64_t n_kinds, uint64_t min_ion_index, int device,
+                           sage_b200_db** out) {
+    if (int rc = db_check_bucket_size(bucket_size)) return rc;
+    Guard<sage_b200_db> guard(nullptr, sage_b200_db_destroy);
+    if (int rc = db_new(device, guard)) return rc;
+    sage_b200_db* db = guard.get();
+    if (int rc = db_set_kinds(db, kinds, n_kinds)) return rc;
+    if (T.n >= 0xFFFFFFFEull) return fail(SAGE_B200_ELIMIT, "too many peptides for u32 PeptideIx");
+    const uint64_t n = T.n;
+    db->total_residues = T.n_res;
+    if (int rc = db_alloc_peptides(db, n)) return rc;
+    DevArena A;
+    uint64_t *d_nion = nullptr, *d_ion_off = nullptr, *d_nfrag = nullptr, *d_frag_off = nullptr;
+    uint32_t* d_bad = nullptr;
+    CUDA_TRY(A.zeros(&d_nion, n + 1, 0));
+    CUDA_TRY(A.zeros(&d_nfrag, n + 1, 0));
+    CUDA_TRY(A.alloc(&d_ion_off, n + 1));
+    CUDA_TRY(A.alloc(&d_frag_off, n + 1));
+    CUDA_TRY(A.zeros(&d_bad, 1, 0));
+    LAUNCH_N(k_pf_pep_meta, n, 0, T.res_off, T.decoy, (uint32_t)n, (uint32_t)n_kinds, min_ion_index, (uint8_t*)db->d_pep_len, (uint8_t*)db->d_pep_flags,
+             d_nion, d_nfrag, d_bad);
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nion, d_ion_off, (int)(n + 1)); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nfrag, d_frag_off, (int)(n + 1)); }));
+    uint64_t tail[2] = {0, 0};
+    uint32_t bad = 0;
+    CUDA_TRY(cudaMemcpy(&tail[0], d_ion_off + n, 8, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&tail[1], d_frag_off + n, 8, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&bad, d_bad, 4, cudaMemcpyDeviceToHost));
+    if (bad) return fail(SAGE_B200_ELIMIT, "a peptide has length 0 or over 255 (supported 1..255)");
+    if (tail[0] > 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "ion table exceeds 2^32 entries");
+    LAUNCH_N(k_dg_u64_to_u32, n + 1, 0, d_ion_off, n + 1, (uint32_t*)db->d_ion_off);
+    if (n) {
+        CUDA_TRY(cudaMemcpy(db->d_pep_mono, T.mono, 4 * n, cudaMemcpyDeviceToDevice));
+        CUDA_TRY(cudaMemcpy(db->d_pep_missed, T.missed, n, cudaMemcpyDeviceToDevice));
+    }
+    if (int rc = db_build_ions(db, n, tail[0], T.res_off, T.seq, T.mods, T.nterm)) return rc;
+    if (int rc = db_build_fragments(db, d_frag_off, tail[1], bucket_size, min_ion_index)) return rc;
     *out = guard.release();
     return 0;
 }
@@ -1884,12 +1969,10 @@ extern "C" int sage_b200_score_batch_multi(sage_b200_scorer* const* scorers, int
 
 // Scorer::quick_score over a batch (scoring.rs:255-298), the prefilter used by runner.rs:143-278: keep[PeptideIx] |= peptide identified.
 // prefilter_low_memory != 0: peptides of the report_psms "largest" scored candidates per spectrum (see k_score); == 0: every preliminary hit.
-extern "C" int sage_b200_quick_score(sage_b200_scorer* S, const sage_b200_spectra* sp, int prefilter_low_memory, uint8_t* keep) {
-    if (!S || !keep) return fail(SAGE_B200_EINVAL, "quick_score: null argument");
-    int rc = check_spectra(sp);
-    if (rc) return rc;
-    std::lock_guard<std::mutex> lock(S->mu);
-    CUDA_TRY(cudaSetDevice(S->db->device));
+// quick_score over a batch with the marks left on the device: S->d_keep holds one byte per PeptideIx (nonzero = kept) and every lane is idle
+// on return. The caller holds S->mu and has selected the device.
+static int quick_score_device(sage_b200_scorer* S, const sage_b200_spectra* sp, int prefilter_low_memory) {
+    int rc = 0;
     const size_t npep = S->db->v.n_pep;
     if ((rc = S->d_keep.reserve(npep + 16))) return rc;
     CUDA_TRY(cudaMemset(S->d_keep.p, 0, npep + 16));
@@ -1916,10 +1999,23 @@ extern "C" int sage_b200_quick_score(sage_b200_scorer* S, const sage_b200_spectr
     S->quick_mode = 0;
     L.chunk.loaded = false;
     if (rc) return drain_lanes(S, rc);
+    finish_counters(S);   // lane_finish has waited for the lane's stream: the marks are complete
+    return 0;
+}
+
+// Scorer::quick_score over a batch (scoring.rs:255-298), the prefilter used by runner.rs:143-278: keep[PeptideIx] |= peptide identified.
+// prefilter_low_memory != 0: peptides of the report_psms "largest" scored candidates per spectrum (see k_score); == 0: every preliminary hit.
+extern "C" int sage_b200_quick_score(sage_b200_scorer* S, const sage_b200_spectra* sp, int prefilter_low_memory, uint8_t* keep) {
+    if (!S || !keep) return fail(SAGE_B200_EINVAL, "quick_score: null argument");
+    int rc = check_spectra(sp);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lock(S->mu);
+    CUDA_TRY(cudaSetDevice(S->db->device));
+    if ((rc = quick_score_device(S, sp, prefilter_low_memory))) return rc;
+    const size_t npep = S->db->v.n_pep;
     std::vector<uint8_t> h(npep);
     CUDA_TRY(cudaMemcpy(h.data(), S->d_keep.p, npep, cudaMemcpyDeviceToHost));
     for (size_t i = 0; i < npep; i++) keep[i] |= h[i];
-    finish_counters(S);
     return 0;
 }
 
@@ -4063,10 +4159,6 @@ static int dg_parse_fasta(const char* text, uint64_t len, const std::string& tag
 struct DgMax {
     __device__ uint32_t operator()(uint32_t a, uint32_t b) const { return a > b ? a : b; }
 };
-__global__ void k_dg_u64_to_u32(const uint64_t* __restrict__ a, uint64_t n, uint32_t* __restrict__ b) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) b[i] = (uint32_t)a[i];
-}
 
 static int dg_memory(const char* stage, uint64_t bytes) {
     size_t free_b = 0, total_b = 0;
@@ -4077,11 +4169,17 @@ static int dg_memory(const char* stage, uint64_t bytes) {
     return 0;
 }
 
-static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, const std::vector<DgSpec>& statics, const std::vector<DgSpec>& vars,
-                  const std::vector<uint32_t>& prot_name) {
+// Digests proteins [p0, p1) of the parsed FASTA as a FASTA of their own (its `targets` set, database.rs:186-200, is local to the range) into
+// D's table. prot_name maps each protein of F to its id in the names table. With `seen`, the call stops after the per-protein `seen` stage
+// and writes the number of windows it keeps: fasta.digest(&enzyme).len() of the range (enzyme.rs:310-330, fasta.rs:58-79).
+static int dg_run(sage_b200_digest* D, const DgFasta& F, uint32_t p0, uint32_t p1, const DgParams& hp, const std::vector<DgSpec>& statics,
+                  const std::vector<DgSpec>& vars, const std::vector<uint32_t>& prot_name, uint64_t* seen = nullptr) {
     sage_b200_digest_info& I = D->info;
-    const uint32_t P = (uint32_t)F.acc.size();
-    const uint64_t R = F.res.size();
+    if (seen) *seen = 0;
+    const uint32_t P = p1 - p0;
+    const uint64_t R = F.off[p1] - F.off[p0];
+    std::vector<uint32_t> off(F.off.begin() + p0, F.off.begin() + p1 + 1);
+    for (uint32_t& o : off) o -= F.off[p0];
     DevArena A;
     Stream st;
     CUDA_TRY(st.create());
@@ -4098,10 +4196,10 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     uint8_t *d_res = nullptr, *d_pdecoy = nullptr;
     uint32_t *d_poff = nullptr, *d_pname = nullptr;
     DgSpec *d_statics = nullptr, *d_vars = nullptr;
-    CUDA_TRY(A.upload(&d_res, F.res.data(), R, st));
-    CUDA_TRY(A.upload(&d_poff, F.off.data(), P + 1, st));
-    CUDA_TRY(A.upload(&d_pdecoy, F.decoy.data(), P, st));
-    CUDA_TRY(A.upload(&d_pname, prot_name.data(), P, st));
+    CUDA_TRY(A.upload(&d_res, F.res.data() + F.off[p0], R, st));
+    CUDA_TRY(A.upload(&d_poff, off.data(), P + 1, st));
+    CUDA_TRY(A.upload(&d_pdecoy, F.decoy.data() + p0, P, st));
+    CUDA_TRY(A.upload(&d_pname, prot_name.data() + p0, P, st));
     CUDA_TRY(A.upload(&d_statics, statics.data(), statics.size(), st));
     CUDA_TRY(A.upload(&d_vars, vars.data(), vars.size(), st));
     DgParams p = hp;
@@ -4170,6 +4268,10 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_idx2, d_keep, d_idx_k, d_cnt, (int)W, st); }));
     uint32_t Kc = 0;
     if (int rc = read_back(st, &Kc, d_cnt, 4)) return rc;
+    if (seen) {
+        *seen = Kc;
+        return done(), 0;
+    }
     CUDA_TRY(A.alloc(&d_key3, Kc));
     CUDA_TRY(A.alloc(&d_idx3, Kc));
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_key_k, d_key3, d_idx_k, d_idx3, (int)Kc, 0, cbits + 3, st); }));
@@ -4331,10 +4433,14 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, const DgParams& hp, con
     return 0;
 }
 
-extern "C" int sage_b200_digest_create(int device, const char* fasta, uint64_t fasta_len, const sage_b200_digest_params* p, sage_b200_digest** out) {
-    const auto t0 = std::chrono::steady_clock::now();
-    if (!out || !p || (fasta_len && !fasta)) return fail(SAGE_B200_EINVAL, "digest_create: null argument");
-    *out = nullptr;
+// Builder::make_parameters and Enzyme::new (database.rs:96-115, enzyme.rs:145-184) of the digest parameters, with their argument checks.
+struct DgSetup {
+    DgParams hp{};
+    std::vector<DgSpec> statics, vars;
+    uint64_t n_var_specs = 0;   // distinct valid variable specs: Parameters::variable_mods.len()
+};
+
+static int dg_setup(const sage_b200_digest_params* p, DgSetup& S) {
     if ((p->n_static && (!p->static_specs || !p->static_masses)) || (p->n_variable && (!p->variable_specs || !p->variable_masses)))
         return fail(SAGE_B200_EINVAL, "digest_create: null modification array");
     if (p->max_len > 255) return fail(SAGE_B200_ELIMIT, "digest: max_len %llu > 255 (the library's peptide-length limit)", (unsigned long long)p->max_len);
@@ -4344,8 +4450,7 @@ extern "C" int sage_b200_digest_create(int device, const char* fasta, uint64_t f
     for (uint64_t i = 0; i < p->n_variable; i++)
         if (!p->variable_specs[i] || !std::isfinite(p->variable_masses[i]))
             return fail(SAGE_B200_EINVAL, "digest: variable mod %llu: null spec or non-finite mass", (unsigned long long)i);
-    // Builder::make_parameters and Enzyme::new (database.rs:96-115, enzyme.rs:145-184)
-    DgParams hp{};
+    DgParams& hp = S.hp;
     const std::string cleave_at = p->cleave_at ? p->cleave_at : "", restrict_ = p->restrict_ ? p->restrict_ : "";
     hp.min_len = (uint32_t)std::min<uint64_t>(p->min_len, 256);
     hp.max_len = (uint32_t)p->max_len;
@@ -4367,32 +4472,32 @@ extern "C" int sage_b200_digest_create(int device, const char* fasta, uint64_t f
     hp.min_mass = p->peptide_min_mass;
     hp.max_mass = p->peptide_max_mass;
     auto spec_less = [](const DgSpec& a, const DgSpec& b) { return a.kind != b.kind ? a.kind < b.kind : a.residue < b.residue; };
-    std::vector<DgSpec> statics, vars;
     for (uint64_t i = 0; i < p->n_static; i++) {   // a map keyed by spec: ordered, the last mass of a repeated spec wins
         DgSpec s{};
         if (!dg_parse_spec(p->static_specs[i], s)) continue;
         s.mass = p->static_masses[i];
-        auto it = std::lower_bound(statics.begin(), statics.end(), s, spec_less);
-        if (it != statics.end() && !spec_less(s, *it)) it->mass = s.mass;
-        else statics.insert(it, s);
+        auto it = std::lower_bound(S.statics.begin(), S.statics.end(), s, spec_less);
+        if (it != S.statics.end() && !spec_less(s, *it)) it->mass = s.mass;
+        else S.statics.insert(it, s);
     }
     for (uint64_t i = 0; i < p->n_variable; i++) {
         DgSpec s{};
         if (!dg_parse_spec(p->variable_specs[i], s)) continue;
         s.mass = p->variable_masses[i];
-        vars.push_back(s);
+        S.vars.push_back(s);
     }
-    std::stable_sort(vars.begin(), vars.end(), spec_less);
-    hp.n_static = (uint32_t)statics.size();
-    hp.n_var = (uint32_t)vars.size();
+    std::stable_sort(S.vars.begin(), S.vars.end(), spec_less);
+    for (size_t i = 0; i < S.vars.size(); i++)
+        if (i == 0 || spec_less(S.vars[i - 1], S.vars[i])) S.n_var_specs++;
+    hp.n_static = (uint32_t)S.statics.size();
+    hp.n_var = (uint32_t)S.vars.size();
+    return 0;
+}
 
-    Guard<sage_b200_digest> guard(new sage_b200_digest(), sage_b200_digest_destroy);
-    sage_b200_digest* D = guard.get();
-    D->device = device;
-    DgFasta F;
-    if (int rc = dg_parse_fasta(fasta, fasta_len, p->decoy_tag ? p->decoy_tag : "rev_", p->generate_decoys != 0, F)) return rc;
-    // the names table: distinct accessions in byte order, a protein's id is its accession's rank
-    std::vector<uint32_t> order(F.acc.size()), prot_name(F.acc.size());
+// The names table: distinct accessions in byte order; a protein's id is its accession's rank.
+static void dg_names(const DgFasta& F, sage_b200_digest* D, std::vector<uint32_t>& prot_name) {
+    std::vector<uint32_t> order(F.acc.size());
+    prot_name.assign(F.acc.size(), 0);
     for (uint32_t i = 0; i < order.size(); i++) order[i] = i;
     std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return F.acc[a] < F.acc[b]; });
     D->name_off.push_back(0);
@@ -4407,10 +4512,26 @@ extern "C" int sage_b200_digest_create(int device, const char* fasta, uint64_t f
     I.n_proteins = F.acc.size();
     I.n_names = D->name_off.size() - 1;
     I.name_bytes = D->names.size();
+}
+
+extern "C" int sage_b200_digest_create(int device, const char* fasta, uint64_t fasta_len, const sage_b200_digest_params* p, sage_b200_digest** out) {
+    const auto t0 = std::chrono::steady_clock::now();
+    if (!out || !p || (fasta_len && !fasta)) return fail(SAGE_B200_EINVAL, "digest_create: null argument");
+    *out = nullptr;
+    DgSetup S;
+    if (int rc = dg_setup(p, S)) return rc;
+    Guard<sage_b200_digest> guard(new sage_b200_digest(), sage_b200_digest_destroy);
+    sage_b200_digest* D = guard.get();
+    D->device = device;
+    DgFasta F;
+    if (int rc = dg_parse_fasta(fasta, fasta_len, p->decoy_tag ? p->decoy_tag : "rev_", p->generate_decoys != 0, F)) return rc;
+    std::vector<uint32_t> prot_name;
+    dg_names(F, D, prot_name);
+    sage_b200_digest_info& I = D->info;
     I.ms_parse = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
     if (int rc = select_device(device)) return rc;
     if (!F.acc.empty())
-        if (int rc = dg_run(D, F, hp, statics, vars, prot_name)) return rc;
+        if (int rc = dg_run(D, F, 0, (uint32_t)F.acc.size(), S.hp, S.statics, S.vars, prot_name)) return rc;
     I.ms_wall = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
     *out = guard.release();
     return 0;
@@ -4446,5 +4567,402 @@ extern "C" int sage_b200_digest_export(const sage_b200_digest* D, uint32_t* resi
     for (const Copy& c : copies)
         if (c.dst && c.bytes) CUDA_TRY(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// ================================================================================== prefilter (runner.rs:104-128, 161-238; kernels in prefilter.cuh)
+struct sage_b200_prefilter {
+    int device = 0;
+    sage_b200_digest table;               // the final peptide table and the whole FASTA's names table
+    sage_b200_db* db = nullptr;           // the index over the final table, until the caller takes it
+    std::vector<uint64_t> chunk_rows, chunk_kept;
+    sage_b200_prefilter_info info{};
+};
+
+extern "C" void sage_b200_prefilter_destroy(sage_b200_prefilter* f) {
+    if (!f) return;
+    cudaSetDevice(f->device);
+    sage_b200_db_destroy(f->db);
+    delete f;
+}
+
+// The kept rows of the chunks so far, in chunk order, in the digest's export layout. Rows, residues and protein references each grow
+// geometrically; a growth copies the rows already held.
+struct PfTable {
+    static constexpr int NA = 11;   // res_off, ref_off, nterm, cterm, mono, decoy, missed, semi | seq, mods | ids
+    static constexpr size_t SZ[NA] = {4, 4, 4, 4, 4, 1, 1, 1, 1, 4, 4};
+    void* p[NA] = {};
+    uint64_t n = 0, n_res = 0, n_ref = 0, cap[3] = {0, 0, 0};
+    PfTable() = default;
+    PfTable(const PfTable&) = delete;
+    PfTable& operator=(const PfTable&) = delete;
+    ~PfTable() { for (void* q : p) if (q) cudaFree(q); }
+    static int group(int a) { return a < 8 ? 0 : (a < 10 ? 1 : 2); }
+    uint64_t bytes() const { return (cap[0] + 1) * 23 + cap[1] * 5 + cap[2] * 4; }
+    // Room for `rows` rows, `res` residues and `refs` references in all; the arrays are copied on st.
+    cudaError_t reserve(uint64_t rows, uint64_t res, uint64_t refs, cudaStream_t st) {
+        const uint64_t need[3] = {rows, res, refs}, used[3] = {n, n_res, n_ref};
+        for (int g = 0; g < 3; g++) {
+            if (need[g] <= cap[g] && p[g == 0 ? 0 : (g == 1 ? 8 : 10)]) continue;
+            const uint64_t c = std::max<uint64_t>(std::max<uint64_t>(need[g], 2 * cap[g]), 1024);
+            for (int a = 0; a < NA; a++) {
+                if (group(a) != g) continue;
+                void* q = nullptr;
+                const uint64_t count = g == 0 ? c + 1 : c, keep = g == 0 && a < 2 ? used[0] + 1 : used[g];
+                if (cudaError_t e = cudaMalloc(&q, count * SZ[a])) return e;
+                if (p[a]) {
+                    if (cudaError_t e = cudaMemcpyAsync(q, p[a], keep * SZ[a], cudaMemcpyDeviceToDevice, st)) { cudaFree(q); return e; }
+                    if (cudaError_t e = cudaStreamSynchronize(st)) { cudaFree(q); return e; }
+                    cudaFree(p[a]);
+                }
+                p[a] = q;
+            }
+            cap[g] = c;
+        }
+        return cudaSuccess;
+    }
+    DevTable view() const {
+        DevTable t;
+        t.n = n; t.n_res = n_res; t.n_ref = n_ref;
+        t.res_off = (const uint32_t*)p[0]; t.ref_off = (const uint32_t*)p[1]; t.nterm = (const float*)p[2]; t.cterm = (const float*)p[3];
+        t.mono = (const float*)p[4]; t.decoy = (const uint8_t*)p[5]; t.missed = (const uint8_t*)p[6]; t.semi = (const uint8_t*)p[7];
+        t.seq = (const uint8_t*)p[8]; t.mods = (const float*)p[9]; t.ids = (const uint32_t*)p[10];
+        return t;
+    }
+};
+
+static DevTable dg_table(const sage_b200_digest& D) {
+    DevTable t;
+    t.n = D.info.n_peptides; t.n_res = D.info.n_residues; t.n_ref = D.info.n_protein_refs;
+    t.res_off = D.d_res_off; t.ref_off = D.d_ref_off; t.ids = D.d_ids; t.seq = D.d_seq; t.decoy = D.d_decoy; t.missed = D.d_missed; t.semi = D.d_semi;
+    t.mods = D.d_mods; t.nterm = D.d_nterm; t.cterm = D.d_cterm; t.mono = D.d_mono;
+    return t;
+}
+
+// Appends the rows of chunk table C whose keep byte is set to T (the protein ids are already global), on st. Returns the kept count in *kept.
+static int pf_compact(const DevTable& C, const uint8_t* d_keep, PfTable& T, cudaStream_t st, uint64_t* kept, uint64_t* peak, uint64_t held) {
+    *kept = 0;
+    const uint32_t n = (uint32_t)C.n;
+    if (n == 0) return 0;
+    if (int rc = dg_memory("prefilter compaction", 44ull * (n + 1))) return rc;
+    DevArena A;
+    uint32_t *d_kept = nullptr, *d_row_at = nullptr;
+    uint64_t *d_nres = nullptr, *d_nref = nullptr, *d_res_at = nullptr, *d_ref_at = nullptr;
+    CUDA_TRY(A.zeros(&d_kept, n + 1, st));
+    CUDA_TRY(A.zeros(&d_nres, n + 1, st));
+    CUDA_TRY(A.zeros(&d_nref, n + 1, st));
+    CUDA_TRY(A.alloc(&d_row_at, n + 1));
+    CUDA_TRY(A.alloc(&d_res_at, n + 1));
+    CUDA_TRY(A.alloc(&d_ref_at, n + 1));
+    LAUNCH_N(k_pf_keep_counts, n, st, d_keep, C.res_off, C.ref_off, n, d_kept, d_nres, d_nref);
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_kept, d_row_at, (int)(n + 1), st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nres, d_res_at, (int)(n + 1), st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nref, d_ref_at, (int)(n + 1), st); }));
+    uint32_t k = 0;
+    uint64_t tot[2] = {0, 0};
+    CUDA_TRY(cudaMemcpyAsync(&k, d_row_at + n, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&tot[0], d_res_at + n, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&tot[1], d_ref_at + n, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    const uint64_t rows = T.n + k, res = T.n_res + tot[0], refs = T.n_ref + tot[1];
+    if (rows >= 0xFFFFFFFEull || res > 0xFFFFFFFFull || refs >= 0x7FFFFFFFull)
+        return fail(SAGE_B200_ELIMIT, "prefilter: %llu kept rows / %llu residues / %llu protein references (u32 offsets)", (unsigned long long)rows,
+                    (unsigned long long)res, (unsigned long long)refs);
+    if (k == 0) return 0;
+    if (rows > T.cap[0] || res > T.cap[1] || refs > T.cap[2])
+        if (int rc = dg_memory("prefilter table", 2 * (23ull * rows + 5ull * res + 4ull * refs))) return rc;
+    CUDA_TRY(T.reserve(rows, res, refs, st));
+    *peak = std::max<uint64_t>(*peak, held + T.bytes() + A.bytes);
+    uint32_t *res_off = (uint32_t*)T.p[0], *ref_off = (uint32_t*)T.p[1];
+    LAUNCH_N(k_pf_gather, n, st, C.rows(), n, d_keep, d_row_at, d_res_at, d_ref_at, (uint32_t)T.n, T.n_res, T.n_ref, res_off, ref_off, (uint8_t*)T.p[8],
+             (float*)T.p[9], (float*)T.p[2], (float*)T.p[3], (float*)T.p[4], (uint8_t*)T.p[5], (uint8_t*)T.p[6], (uint8_t*)T.p[7], (uint32_t*)T.p[10]);
+    const uint32_t tail[2] = {(uint32_t)res, (uint32_t)refs};
+    CUDA_TRY(cudaMemcpyAsync(res_off + rows, &tail[0], 4, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(ref_off + rows, &tail[1], 4, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    T.n = rows;
+    T.n_res = res;
+    T.n_ref = refs;
+    *kept = k;
+    return 0;
+}
+
+// reorder_peptides (database.rs:221-258) over the stored rows of T into D's output table: a stable radix sort by total_cmp(mono), a stable
+// merge sort of the equal-mono runs by initial_sort, the adjacent merge, and a segmented sort of each peptide's protein ids.
+static int pf_merge(const PfTable& T, sage_b200_digest* D, cudaStream_t st, uint64_t* peak, uint64_t held) {
+    sage_b200_digest_info& I = D->info;
+    const uint32_t N = (uint32_t)T.n;
+    if (N == 0) return 0;
+    const PfRows rows = T.view().rows();
+    if (int rc = dg_memory("prefilter merge", 64ull * N)) return rc;
+    DevArena A;
+    thrust::counting_iterator<uint32_t> count_it(0);
+    uint32_t *d_cnt = nullptr, *d_mkey = nullptr, *d_mkey_s = nullptr, *d_idx = nullptr, *d_order = nullptr, *d_rpos = nullptr, *d_rval = nullptr;
+    uint8_t* d_inrun = nullptr;
+    CUDA_TRY(A.alloc(&d_cnt, 1));
+    CUDA_TRY(A.alloc(&d_mkey, N));
+    CUDA_TRY(A.alloc(&d_mkey_s, N));
+    CUDA_TRY(A.alloc(&d_idx, N));
+    CUDA_TRY(A.alloc(&d_order, N));
+    CUDA_TRY(A.alloc(&d_inrun, N));
+    LAUNCH_N(k_dg_mono_key, N, st, rows.mono, N, d_mkey, d_idx);
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, d_mkey, d_mkey_s, d_idx, d_order, (int)N, 0, 32, st); }));
+    LAUNCH_N(k_dg_in_run, N, st, d_mkey_s, N, d_inrun);
+    CUDA_TRY(A.alloc(&d_rpos, N));
+    CUDA_TRY(A.alloc(&d_rval, N));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_inrun, d_rpos, d_cnt, (int)N, st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, d_order, d_inrun, d_rval, d_cnt, (int)N, st); }));
+    uint32_t M = 0;
+    if (int rc = read_back(st, &M, d_cnt, 4)) return rc;
+    if (M) {
+        const PfRowLess less{rows};
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceMergeSort::StableSortKeys(t, b, d_rval, (int)M, less, st); }));
+        LAUNCH_N(k_dg_scatter, M, st, d_rpos, d_rval, M, d_order);
+    }
+    uint32_t *d_mhead = nullptr, *d_first = nullptr;
+    CUDA_TRY(A.alloc(&d_mhead, N));
+    CUDA_TRY(A.alloc(&d_first, N + 1));
+    LAUNCH_N(k_pf_merge_heads, N, st, rows, d_order, N, d_mhead);
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, count_it, d_mhead, d_first, d_cnt, (int)N, st); }));
+    uint32_t n_pep = 0;
+    if (int rc = read_back(st, &n_pep, d_cnt, 4)) return rc;
+    CUDA_TRY(cudaMemcpyAsync(d_first + n_pep, &N, 4, cudaMemcpyHostToDevice, st));
+    uint64_t *d_nres = nullptr, *d_nref = nullptr, *d_res_off64 = nullptr, *d_ref_off64 = nullptr;
+    CUDA_TRY(A.zeros(&d_nres, n_pep + 1, st));
+    CUDA_TRY(A.zeros(&d_nref, n_pep + 1, st));
+    CUDA_TRY(A.alloc(&d_res_off64, n_pep + 1));
+    CUDA_TRY(A.alloc(&d_ref_off64, n_pep + 1));
+    LAUNCH_N(k_pf_pep_counts, n_pep, st, rows, d_order, d_first, n_pep, d_nres, d_nref);
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nres, d_res_off64, (int)(n_pep + 1), st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nref, d_ref_off64, (int)(n_pep + 1), st); }));
+    uint64_t n_res = 0, n_ref = 0;
+    CUDA_TRY(cudaMemcpyAsync(&n_res, d_res_off64 + n_pep, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&n_ref, d_ref_off64 + n_pep, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (n_res > 0xFFFFFFFFull || n_ref >= 0x7FFFFFFFull)
+        return fail(SAGE_B200_ELIMIT, "prefilter: %llu residues / %llu protein references in the table (u32 offsets)", (unsigned long long)n_res,
+                    (unsigned long long)n_ref);
+    if (int rc = dg_memory("prefilter output", 5ull * n_res + 30ull * n_pep + 8ull * n_ref)) return rc;
+    DevArena& O = D->out;
+    uint32_t* d_ids_raw = nullptr;
+    CUDA_TRY(O.alloc(&D->d_res_off, n_pep + 1));
+    CUDA_TRY(O.alloc(&D->d_ref_off, n_pep + 1));
+    CUDA_TRY(O.alloc(&D->d_ids, n_ref));
+    CUDA_TRY(O.alloc(&D->d_seq, n_res));
+    CUDA_TRY(O.alloc(&D->d_mods, n_res));
+    CUDA_TRY(O.alloc(&D->d_nterm, n_pep));
+    CUDA_TRY(O.alloc(&D->d_cterm, n_pep));
+    CUDA_TRY(O.alloc(&D->d_mono, n_pep));
+    CUDA_TRY(O.alloc(&D->d_decoy, n_pep));
+    CUDA_TRY(O.alloc(&D->d_missed, n_pep));
+    CUDA_TRY(O.alloc(&D->d_semi, n_pep));
+    CUDA_TRY(A.alloc(&d_ids_raw, n_ref));
+    LAUNCH_N(k_dg_u64_to_u32, n_pep + 1, st, d_res_off64, n_pep + 1, D->d_res_off);
+    LAUNCH_N(k_dg_u64_to_u32, n_pep + 1, st, d_ref_off64, n_pep + 1, D->d_ref_off);
+    LAUNCH_N(k_pf_export, n_pep, st, rows, d_order, d_first, n_pep, D->d_res_off, D->d_ref_off, D->d_seq, D->d_mods, D->d_nterm, D->d_cterm, D->d_mono,
+             D->d_decoy, D->d_missed, D->d_semi, d_ids_raw);
+    // proteins.sort_unstable() (database.rs:250): ids are ranks in the whole FASTA's names table, so an ascending sort of the ids is the sort of
+    // the names across chunks
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) {
+        return cub::DeviceSegmentedSort::SortKeys(t, b, d_ids_raw, D->d_ids, (int)n_ref, (int)n_pep, D->d_ref_off, D->d_ref_off + 1, st);
+    }));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    *peak = std::max<uint64_t>(*peak, held + A.bytes + O.bytes);
+    I.n_peptides = n_pep;
+    I.n_residues = n_res;
+    I.n_protein_refs = n_ref;
+    return 0;
+}
+
+// The spectra runner.rs:252-268 passes to quick_score: masses.len() >= min_peaks && level == 2, gathered into `out`'s arrays.
+struct PfSpectra {
+    std::vector<uint64_t> off{0};
+    std::vector<float> masses, intens, mz, iso_lo, iso_hi, tic;
+    std::vector<uint8_t> charge;
+    sage_b200_spectra s{};
+};
+
+static void pf_filter_spectra(const sage_b200_spectra* sp, uint64_t min_peaks, PfSpectra& F) {
+    for (uint64_t i = 0; i < sp->n; i++) {
+        const uint64_t a = sp->peak_offsets[i], b = sp->peak_offsets[i + 1];
+        if (b - a < min_peaks || (sp->level && sp->level[i] != 2)) continue;
+        F.masses.insert(F.masses.end(), sp->masses + a, sp->masses + b);
+        F.intens.insert(F.intens.end(), sp->intensities + a, sp->intensities + b);
+        F.off.push_back(F.masses.size());
+        F.mz.push_back(sp->precursor_mz[i]);
+        F.charge.push_back(sp->precursor_charge[i]);
+        F.iso_lo.push_back(sp->isolation_lo ? sp->isolation_lo[i] : NAN);
+        F.iso_hi.push_back(sp->isolation_hi ? sp->isolation_hi[i] : NAN);
+        F.tic.push_back(sp->total_ion_current[i]);
+    }
+    F.s.n = F.mz.size();
+    F.s.peak_offsets = F.off.data();
+    F.s.masses = F.masses.data();
+    F.s.intensities = F.intens.data();
+    F.s.precursor_mz = F.mz.data();
+    F.s.precursor_charge = F.charge.data();
+    F.s.isolation_lo = F.iso_lo.data();
+    F.s.isolation_hi = F.iso_hi.data();
+    F.s.total_ion_current = F.tic.data();
+}
+
+static float ms_since(std::chrono::steady_clock::time_point t) { return std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t).count(); }
+
+extern "C" int sage_b200_prefilter_create(int device, const char* fasta, uint64_t fasta_len, const sage_b200_digest_params* dp, const sage_b200_scorer_params* sp,
+                                          const sage_b200_prefilter_params* pp, const sage_b200_spectra* spectra, uint64_t bucket_size, const uint8_t* ion_kinds,
+                                          uint64_t n_ion_kinds, uint64_t min_ion_index, sage_b200_prefilter** out) {
+    const auto t0 = std::chrono::steady_clock::now();
+    if (!out || !dp || !sp || !pp || !ion_kinds || (fasta_len && !fasta)) return fail(SAGE_B200_EINVAL, "prefilter_create: null argument");
+    *out = nullptr;
+    if (int rc = check_spectra(spectra)) return rc;
+    DgSetup S;
+    if (int rc = dg_setup(dp, S)) return rc;
+    if (int rc = db_check_bucket_size(bucket_size)) return rc;
+    if (n_ion_kinds == 0 || n_ion_kinds > MAX_KINDS) return fail(SAGE_B200_EINVAL, "ion_kinds: need 1..%d kinds", MAX_KINDS);
+    for (uint64_t k = 0; k < n_ion_kinds; k++)
+        if (ion_kinds[k] > 5) return fail(SAGE_B200_EINVAL, "ion kind %u out of range", ion_kinds[k]);
+    if (sp->report_psms == 0) return fail(SAGE_B200_EINVAL, "report_psms must be >= 1");
+    if (sp->report_psms + 1ull > (uint64_t)K_MAX / 2)
+        return fail(SAGE_B200_ELIMIT, "prefilter: report_psms + 1 = %llu > %d not supported", sp->report_psms + 1ull, K_MAX / 2);
+    if (sp->precursor_tol.kind < 0 || sp->precursor_tol.kind > 2 || sp->fragment_tol.kind < 0 || sp->fragment_tol.kind > 2)
+        return fail(SAGE_B200_EINVAL, "bad tolerance kind");
+    if (sp->score_type > 1) return fail(SAGE_B200_EINVAL, "bad score_type");
+    Guard<sage_b200_prefilter> guard(new sage_b200_prefilter(), sage_b200_prefilter_destroy);
+    sage_b200_prefilter* PF = guard.get();
+    PF->device = device;
+    PF->table.device = device;
+    sage_b200_prefilter_info& I = PF->info;
+    DgFasta F;
+    if (int rc = dg_parse_fasta(fasta, fasta_len, dp->decoy_tag ? dp->decoy_tag : "rev_", dp->generate_decoys != 0, F)) return rc;
+    std::vector<uint32_t> prot_name;
+    dg_names(F, &PF->table, prot_name);
+    const uint64_t targets = F.acc.size();
+    I.n_proteins = targets;
+    I.ms_parse = ms_since(t0);
+    if (int rc = select_device(device)) return rc;
+
+    // auto_calculate_prefilter_chunk_size (database.rs:142-160)
+    uint64_t chunk = pp->chunk_size;
+    if (chunk == 0) {
+        const auto tc = std::chrono::steady_clock::now();
+        uint64_t total = 0;
+        if (targets) {
+            sage_b200_digest counter;
+            counter.device = device;
+            if (int rc = dg_run(&counter, F, 0, (uint32_t)targets, S.hp, S.statics, S.vars, prot_name, &total)) return rc;
+            I.peak_device_bytes = std::max<uint64_t>(I.peak_device_bytes, counter.info.peak_device_bytes);
+        }
+        I.unmodified_peptides = total;
+        const uint64_t chunk_count = (S.n_var_specs + 1) * (1ull << S.hp.kmax) * total / (1ull << 23);
+        chunk = chunk_count == 0 ? targets : targets / chunk_count;
+        I.ms_count = ms_since(tc);
+        if (chunk == 0 && targets)
+            return fail(SAGE_B200_EINVAL, "prefilter: the automatic chunk size is 0 (%llu proteins, %llu estimated chunks): set a chunk size",
+                        (unsigned long long)targets, (unsigned long long)chunk_count);
+    }
+    I.chunk_size = chunk;
+    if (chunk >= targets) {   // runner.rs:110: the plain build, no quick_score
+        I.plain_build = 1;
+        const auto td = std::chrono::steady_clock::now();
+        if (targets)
+            if (int rc = dg_run(&PF->table, F, 0, (uint32_t)targets, S.hp, S.statics, S.vars, prot_name)) return rc;
+        I.ms_digest = ms_since(td);
+        I.rows_digested = I.rows_kept = PF->table.info.n_peptides;
+        I.peak_device_bytes = std::max<uint64_t>(I.peak_device_bytes, PF->table.info.peak_device_bytes);
+    } else {
+        I.n_chunks = (targets + chunk - 1) / chunk;
+        PfSpectra Q;
+        pf_filter_spectra(spectra, pp->min_peaks, Q);
+        I.n_spectra = Q.s.n;
+        sage_b200_scorer_params qp = *sp;
+        qp.report_psms = sp->report_psms + 1;   // runner.rs:191
+        PfTable T;
+        Stream st;
+        CUDA_TRY(st.create());
+        for (uint64_t c = 0; c < I.n_chunks; c++) {
+            const uint32_t p0 = (uint32_t)(c * chunk), p1 = (uint32_t)std::min<uint64_t>(targets, (c + 1) * chunk);
+            auto t = std::chrono::steady_clock::now();
+            sage_b200_digest D;
+            D.device = device;
+            if (int rc = dg_run(&D, F, p0, p1, S.hp, S.statics, S.vars, prot_name)) return rc;
+            I.ms_digest += ms_since(t);
+            I.peak_device_bytes = std::max<uint64_t>(I.peak_device_bytes, T.bytes() + D.info.peak_device_bytes);
+            const DevTable C = dg_table(D);
+            PF->chunk_rows.push_back(C.n);
+            PF->chunk_kept.push_back(0);
+            I.rows_digested += C.n;
+            if (C.n == 0) continue;
+            t = std::chrono::steady_clock::now();
+            sage_b200_db* cdb = nullptr;
+            if (int rc = db_build_device(C, bucket_size, ion_kinds, n_ion_kinds, min_ion_index, device, &cdb)) return rc;
+            Guard<sage_b200_db> cdb_guard(cdb, sage_b200_db_destroy);
+            I.ms_index += ms_since(t);
+            const uint64_t held = T.bytes() + D.out.bytes + cdb->device_bytes;
+            I.peak_device_bytes = std::max<uint64_t>(I.peak_device_bytes, held);
+            t = std::chrono::steady_clock::now();
+            sage_b200_scorer* sc = nullptr;
+            if (int rc = sage_b200_scorer_create(cdb, &qp, &sc)) return rc;
+            Guard<sage_b200_scorer> sc_guard(sc, sage_b200_scorer_destroy);
+            {
+                std::lock_guard<std::mutex> lock(sc->mu);
+                if (int rc = quick_score_device(sc, &Q.s, pp->low_memory)) return rc;
+            }
+            CUDA_TRY(cudaDeviceSynchronize());   // the keep marks are zeroed on the default stream when no spectrum is scored
+            I.ms_quick_score += ms_since(t);
+            I.ms_spectra_upload += sc->last.ms_h2d;
+            t = std::chrono::steady_clock::now();
+            uint64_t kept = 0;
+            if (int rc = pf_compact(C, sc->d_keep.as<uint8_t>(), T, st, &kept, &I.peak_device_bytes, D.out.bytes + cdb->device_bytes)) return rc;
+            I.ms_compact += ms_since(t);
+            PF->chunk_kept.back() = kept;
+            I.rows_kept += kept;
+        }   // the chunk's digest, index and scorer are freed here
+        const auto tm = std::chrono::steady_clock::now();
+        if (int rc = pf_merge(T, &PF->table, st, &I.peak_device_bytes, T.bytes())) return rc;
+        I.ms_merge = ms_since(tm);
+    }
+    const auto tf = std::chrono::steady_clock::now();
+    if (int rc = db_build_device(dg_table(PF->table), bucket_size, ion_kinds, n_ion_kinds, min_ion_index, device, &PF->db)) return rc;
+    I.ms_final_index = ms_since(tf);
+    const sage_b200_digest_info& O = PF->table.info;
+    I.n_peptides = O.n_peptides;
+    I.n_residues = O.n_residues;
+    I.n_protein_refs = O.n_protein_refs;
+    I.n_names = O.n_names;
+    I.name_bytes = O.name_bytes;
+    I.n_fragments = PF->db->v.n_frag;
+    I.device_bytes = PF->table.out.bytes + PF->db->device_bytes;
+    I.peak_device_bytes = std::max<uint64_t>(I.peak_device_bytes, I.device_bytes);
+    I.ms_wall = ms_since(t0);
+    *out = guard.release();
+    return 0;
+}
+
+extern "C" int sage_b200_prefilter_get_info(const sage_b200_prefilter* f, sage_b200_prefilter_info* info) {
+    if (!f || !info) return fail(SAGE_B200_EINVAL, "prefilter_get_info: null argument");
+    *info = f->info;
+    return 0;
+}
+
+extern "C" int sage_b200_prefilter_chunk_counts(const sage_b200_prefilter* f, uint64_t* rows_digested, uint64_t* rows_kept) {
+    if (!f) return fail(SAGE_B200_EINVAL, "prefilter_chunk_counts: null handle");
+    if (rows_digested && !f->chunk_rows.empty()) memcpy(rows_digested, f->chunk_rows.data(), 8 * f->chunk_rows.size());
+    if (rows_kept && !f->chunk_kept.empty()) memcpy(rows_kept, f->chunk_kept.data(), 8 * f->chunk_kept.size());
+    return 0;
+}
+
+extern "C" int sage_b200_prefilter_export(const sage_b200_prefilter* f, uint32_t* residue_offsets, uint8_t* sequence, float* modifications, float* nterm,
+                                          float* cterm, float* monoisotopic, uint8_t* decoy, uint8_t* missed_cleavages, uint8_t* semi_enzymatic,
+                                          uint32_t* protein_offsets, uint32_t* protein_ids, uint64_t* name_offsets, char* name_bytes) {
+    if (!f) return fail(SAGE_B200_EINVAL, "prefilter_export: null handle");
+    return sage_b200_digest_export(&f->table, residue_offsets, sequence, modifications, nterm, cterm, monoisotopic, decoy, missed_cleavages, semi_enzymatic,
+                                   protein_offsets, protein_ids, name_offsets, name_bytes);
+}
+
+extern "C" int sage_b200_prefilter_take_db(sage_b200_prefilter* f, sage_b200_db** out) {
+    if (!f || !out) return fail(SAGE_B200_EINVAL, "prefilter_take_db: null argument");
+    if (!f->db) return fail(SAGE_B200_EINVAL, "prefilter_take_db: the db was already taken");
+    *out = f->db;
+    f->db = nullptr;
     return 0;
 }
