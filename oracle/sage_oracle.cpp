@@ -302,6 +302,9 @@ static std::vector<Digest> enzyme_digest(const EnzymeParams& e, const std::strin
     std::unordered_set<std::string> seen;
     for (const Site& s : sites) {
         if (s.start > s.end || s.end > n) continue;
+        // sequence.get(start..end) is None off a UTF-8 character boundary
+        auto boundary = [&](size_t i) { return i == 0 || i == n || ((unsigned char)seq[i] & 0xC0) != 0x80; };
+        if (!boundary(s.start) || !boundary(s.end)) continue;
         std::string sub = seq.substr(s.start, s.end - s.start);
         size_t len = sub.size();
         int pos = (s.start == 0) ? (s.end == n ? POS_FULL : POS_NTERM) : (s.end == n ? POS_CTERM : POS_INTERNAL);
@@ -319,18 +322,38 @@ struct Fasta {
     std::string decoy_tag;
     bool generate_decoys;
 };
-static std::string trim(const std::string& s) {
-    size_t a = 0, b = s.size();
-    while (a < b && isspace((unsigned char)s[a])) a++;
-    while (b > a && isspace((unsigned char)s[b - 1])) b--;
-    return s.substr(a, b - a);
+// char::is_whitespace: the UTF-8 byte length of the whitespace character s[0..n), 0 when s[0..n) is not one
+static size_t unicode_space(const unsigned char* s, size_t n) {
+    if (n == 1) return ((s[0] >= 0x09 && s[0] <= 0x0D) || s[0] == 0x20) ? 1 : 0;
+    if (n == 2) return (s[0] == 0xC2 && (s[1] == 0x85 || s[1] == 0xA0)) ? 2 : 0;
+    if (n != 3) return 0;
+    static const char* const three[] = {"\xE1\x9A\x80", "\xE2\x80\xA8", "\xE2\x80\xA9", "\xE2\x80\xAF", "\xE2\x81\x9F", "\xE3\x80\x80"};
+    if (s[0] == 0xE2 && s[1] == 0x80 && s[2] >= 0x80 && s[2] <= 0x8A) return 3;   // U+2000..U+200A
+    for (const char* t : three) if (memcmp(s, t, 3) == 0) return 3;
+    return 0;
 }
+// str::trim: Unicode whitespace at both ends
+static std::string trim(const std::string& str) {
+    const unsigned char* s = (const unsigned char*)str.data();
+    size_t a = 0, b = str.size();
+    for (bool more = true; more;) {
+        more = false;
+        for (size_t k = 1; k <= 3 && !more; k++) if (a + k <= b && unicode_space(s + a, k)) { a += k; more = true; }
+    }
+    for (bool more = true; more;) {
+        more = false;
+        for (size_t k = 1; k <= 3 && !more; k++) if (b >= a + k && unicode_space(s + b - k, k)) { b -= k; more = true; }
+    }
+    return str.substr(a, b - a);
+}
+// u8::is_ascii_whitespace (split_ascii_whitespace): no '\v'
+static bool ascii_space(unsigned char c) { return c == ' ' || c == '\t' || c == '\n' || c == '\f' || c == '\r'; }
 static Fasta fasta_parse(const std::string& contents, const std::string& decoy_tag, bool generate_decoys) {
     Fasta f; f.decoy_tag = decoy_tag; f.generate_decoys = generate_decoys;
     std::string last_id, s;
     auto flush = [&]() {
-        size_t a = 0; while (a < last_id.size() && isspace((unsigned char)last_id[a])) a++;
-        size_t b = a; while (b < last_id.size() && !isspace((unsigned char)last_id[b])) b++;
+        size_t a = 0; while (a < last_id.size() && ascii_space((unsigned char)last_id[a])) a++;
+        size_t b = a; while (b < last_id.size() && !ascii_space((unsigned char)last_id[b])) b++;
         std::string acc = last_id.substr(a, b - a);
         if (acc.find(decoy_tag) == std::string::npos || !generate_decoys) f.targets.push_back({acc, s});
         s.clear();
@@ -1190,7 +1213,19 @@ static BuildParams to_build_params(const so_build_params* p) {
     for (uint64_t i = 0; i < p->n_static; i++) { ModSpec m; if (parse_modspec(p->static_mod_specs[i], m)) st[m] = p->static_mod_masses[i]; }
     for (auto& kv : st) P.static_mods.push_back(kv);
     std::vector<std::pair<ModSpec, float>> var;
-    for (uint64_t i = 0; i < p->n_var; i++) { ModSpec m; if (parse_modspec(p->var_mod_specs[i], m)) var.push_back({m, p->var_mod_masses[i]}); }
+    // validate_var_mods (modification.rs:129-155) is HashMap::insert per spec string: a later string naming the same spec replaces the masses
+    // of the earlier one (entries with equal strings are one string's list)
+    std::vector<std::string> var_str;
+    for (uint64_t i = 0; i < p->n_var; i++) {
+        ModSpec m;
+        if (!parse_modspec(p->var_mod_specs[i], m)) continue;
+        for (size_t j = 0; j < var.size();) {
+            if (!(var[j].first < m) && !(m < var[j].first) && var_str[j] != p->var_mod_specs[i]) { var.erase(var.begin() + j); var_str.erase(var_str.begin() + j); }
+            else j++;
+        }
+        var.push_back({m, p->var_mod_masses[i]});
+        var_str.push_back(p->var_mod_specs[i]);
+    }
     std::stable_sort(var.begin(), var.end(), [](auto& a, auto& b) { return a.first < b.first; });
     P.variable_mods = var;
     P.max_variable_mods = std::max<size_t>((size_t)p->max_variable_mods, 1);

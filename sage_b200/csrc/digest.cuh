@@ -145,8 +145,13 @@ __device__ void dg_for_windows(const DgParams& p, const uint32_t* cuts, uint32_t
         });
 }
 
-// One thread per protein. Pass 1 (out == nullptr) counts the windows that pass the length filter; pass 2 writes them at win_off[prot].
-__global__ void k_dg_windows(const uint32_t* __restrict__ prot_off, const uint32_t* __restrict__ cut_off, const uint32_t* __restrict__ cuts, uint32_t P,
+// str::is_char_boundary of byte offset i in a protein of n bytes: `sequence.get(start..end)` is None for a window that starts or ends inside a
+// multi-byte UTF-8 character (enzyme.rs:316-319), so such a window is never digested, counted or `seen`.
+__device__ __forceinline__ bool dg_char_boundary(const uint8_t* s, uint32_t i, uint32_t n) { return i == 0 || i >= n || (s[i] & 0xC0u) != 0x80u; }
+
+// One thread per protein. Pass 1 (out == nullptr) counts the windows on character boundaries that pass the length filter; pass 2 writes
+// them at win_off[prot].
+__global__ void k_dg_windows(const uint8_t* __restrict__ res, const uint32_t* __restrict__ prot_off, const uint32_t* __restrict__ cut_off, const uint32_t* __restrict__ cuts, uint32_t P,
                              DgParams p, uint64_t* __restrict__ n_win, const uint64_t* __restrict__ win_off, DgWin* __restrict__ out) {
     const uint32_t prot = blockIdx.x * blockDim.x + threadIdx.x;
     if (prot >= P) return;
@@ -157,6 +162,7 @@ __global__ void k_dg_windows(const uint32_t* __restrict__ prot_off, const uint32
         if (s > e || e > n) return;
         const uint32_t len = e - s;
         if (len < p.min_len || len > p.max_len || len == 0) return;
+        if (!dg_char_boundary(res + o, s, n) || !dg_char_boundary(res + o, e, n)) return;
         if (out) {
             const uint32_t pos = s == 0 ? (e == n ? DG_POS_FULL : DG_POS_NTERM) : (e == n ? DG_POS_CTERM : DG_POS_INTERNAL);
             out[at++] = DgWin{o + s, prot, (uint16_t)len, (uint8_t)miss, (uint8_t)((semi ? 1u : 0u) | (pos << 1))};

@@ -4109,18 +4109,31 @@ struct DgFasta {
     std::vector<uint8_t> decoy;
 };
 
-static bool dg_space(uint8_t c) { return c == ' ' || c == '\t' || c == '\n' || c == '\v' || c == '\f' || c == '\r'; }
+// u8::is_ascii_whitespace, the separator of split_ascii_whitespace: no '\v'.
+static bool dg_ascii_space(uint8_t c) { return c == ' ' || c == '\t' || c == '\n' || c == '\f' || c == '\r'; }
 
-// Fasta::parse (fasta.rs:14-56): lines split on '\n' with a trailing '\r' dropped, empty lines skipped, then trimmed; '>' starts a header
-// whose first whitespace-separated token is the accession. A protein is kept when it has residues, and with generate_decoys only when its
-// accession does not contain the decoy tag; without generate_decoys a tagged protein is kept as a decoy.
+// char::is_whitespace (Unicode White_Space), which str::trim strips: the byte length of the whitespace character s[0..n) encodes in UTF-8,
+// or 0 when s[0..n) is not one.
+static size_t dg_utf8_space(const uint8_t* s, size_t n) {
+    if (n == 1) return ((s[0] >= 0x09 && s[0] <= 0x0D) || s[0] == 0x20) ? 1 : 0;
+    if (n == 2) return (s[0] == 0xC2 && (s[1] == 0x85 || s[1] == 0xA0)) ? 2 : 0;   // U+0085, U+00A0
+    if (n != 3) return 0;
+    const uint32_t c = (uint32_t)s[0] << 16 | (uint32_t)s[1] << 8 | s[2];
+    return (c == 0xE19A80 || (c >= 0xE28080 && c <= 0xE2808A) || c == 0xE280A8 || c == 0xE280A9 || c == 0xE280AF || c == 0xE2819F || c == 0xE38080)
+               ? 3 : 0;   // U+1680, U+2000..U+200A, U+2028, U+2029, U+202F, U+205F, U+3000
+}
+
+// Fasta::parse (fasta.rs:14-56): lines split on '\n' with a trailing '\r' dropped, empty lines skipped, then trimmed of Unicode whitespace
+// (str::trim); '>' starts a header whose first token split at ASCII whitespace is the accession. A protein is kept when it has residues,
+// and with generate_decoys only when its accession does not contain the decoy tag; without generate_decoys a tagged protein is kept as a
+// decoy.
 static int dg_parse_fasta(const char* text, uint64_t len, const std::string& tag, bool generate_decoys, DgFasta& F) {
     std::string last_id;
     auto flush = [&]() -> int {
         size_t a = 0;
-        while (a < last_id.size() && dg_space((uint8_t)last_id[a])) a++;
+        while (a < last_id.size() && dg_ascii_space((uint8_t)last_id[a])) a++;
         size_t b = a;
-        while (b < last_id.size() && !dg_space((uint8_t)last_id[b])) b++;
+        while (b < last_id.size() && !dg_ascii_space((uint8_t)last_id[b])) b++;
         std::string acc = last_id.substr(a, b - a);
         const bool tagged = acc.find(tag) != std::string::npos;
         if (tagged && generate_decoys) {
@@ -4140,8 +4153,17 @@ static int dg_parse_fasta(const char* text, uint64_t len, const std::string& tag
         pos = nl ? b + 1 : len + 1;
         if (b > a && text[b - 1] == '\r') b--;
         if (b == a) continue;
-        while (a < b && dg_space((uint8_t)text[a])) a++;
-        while (b > a && dg_space((uint8_t)text[b - 1])) b--;
+        const uint8_t* u = (const uint8_t*)text;
+        for (bool more = true; more;) {
+            more = false;
+            for (size_t k = 1; k <= 3 && !more; k++)
+                if (a + k <= b && dg_utf8_space(u + a, k)) a += k, more = true;
+        }
+        for (bool more = true; more;) {
+            more = false;
+            for (size_t k = 1; k <= 3 && !more; k++)
+                if (b >= a + k && dg_utf8_space(u + b - k, k)) b -= k, more = true;
+        }
         if (b > a && text[a] == '>') {
             if (F.res.size() > F.off.back())
                 if (int rc = flush()) return rc;
@@ -4223,7 +4245,7 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, uint32_t p0, uint32_t p
     uint64_t *d_nwin = nullptr, *d_win_off = nullptr;
     CUDA_TRY(A.zeros(&d_nwin, P + 1, st));
     CUDA_TRY(A.alloc(&d_win_off, P + 1));
-    LAUNCH_N(k_dg_windows, P, st, d_poff, d_cut_off, d_cuts, P, p, d_nwin, nullptr, nullptr);
+    LAUNCH_N(k_dg_windows, P, st, d_res, d_poff, d_cut_off, d_cuts, P, p, d_nwin, nullptr, nullptr);
     CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nwin, d_win_off, (int)(P + 1), st); }));
     uint64_t W64 = 0;
     if (int rc = read_back(st, &W64, d_win_off + P, 8)) return rc;
@@ -4235,7 +4257,7 @@ static int dg_run(sage_b200_digest* D, const DgFasta& F, uint32_t p0, uint32_t p
     if (int rc = dg_memory("window", 100ull * W)) return rc;
     DgWin* d_win = nullptr;
     CUDA_TRY(A.alloc(&d_win, W));
-    LAUNCH_N(k_dg_windows, P, st, d_poff, d_cut_off, d_cuts, P, p, nullptr, d_win_off, d_win);
+    LAUNCH_N(k_dg_windows, P, st, d_res, d_poff, d_cut_off, d_cuts, P, p, nullptr, d_win_off, d_win);
     CUDA_TRY(cudaEventRecord(ev[3], st));
 
     // 3. per-protein `seen` and group_digests: sort by hash, exact classes, stable sort by class, keep each protein's first window of a class,
@@ -4480,11 +4502,22 @@ static int dg_setup(const sage_b200_digest_params* p, DgSetup& S) {
         if (it != S.statics.end() && !spec_less(s, *it)) it->mass = s.mass;
         else S.statics.insert(it, s);
     }
+    // validate_var_mods inserts each spec string's masses into a map keyed by spec (modification.rs:129-155): a later spec string naming the
+    // same spec replaces the masses of the earlier one. Entries with equal spec strings are one string's list.
+    std::vector<const char*> var_str;
     for (uint64_t i = 0; i < p->n_variable; i++) {
         DgSpec s{};
         if (!dg_parse_spec(p->variable_specs[i], s)) continue;
         s.mass = p->variable_masses[i];
+        for (size_t j = 0; j < S.vars.size();)
+            if (!spec_less(S.vars[j], s) && !spec_less(s, S.vars[j]) && strcmp(var_str[j], p->variable_specs[i]) != 0) {
+                S.vars.erase(S.vars.begin() + j);
+                var_str.erase(var_str.begin() + j);
+            } else {
+                j++;
+            }
         S.vars.push_back(s);
+        var_str.push_back(p->variable_specs[i]);
     }
     std::stable_sort(S.vars.begin(), S.vars.end(), spec_less);
     for (size_t i = 0; i < S.vars.size(); i++)
