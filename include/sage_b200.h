@@ -222,6 +222,24 @@ typedef struct {                    /* &[RawSpectrum] flattened (spectrum.rs:81-
 int sage_b200_process_spectra(int device, const sage_b200_processor_params* processor, const sage_b200_raw_spectra* raw, uint64_t* out_peak_offsets,
                               float* out_masses, float* out_intensities, float* out_tic);
 
+/* A batch of RawSpectrum of any MS level (spectrum.rs:81-106) flattened. */
+typedef struct {
+    uint64_t n;
+    const uint64_t* peak_offsets;   /* n+1 */
+    const float* mz;                /* RawSpectrum::mz, in any order */
+    const float* intensity;
+    const uint8_t* level;           /* ms_level, required */
+    const uint8_t* precursor_charge;/* read for level 2 only (as in sage_b200_raw_spectra); may be NULL when no spectrum is level 2 */
+    const float* mobility;          /* per raw peak; NULL = no spectrum of the batch has mobility (the convention of sage_b200_ms1) */
+} sage_b200_raw_batch;
+/* SpectrumProcessor::process (spectrum.rs:338-412) for every level: level 2 as sage_b200_process_spectra (same kernel, same ELIMIT past its
+ * shared-memory budget); other levels keep every peak, mass = mz - PROTON, stably sorted by total_cmp, with no size limit per spectrum.
+ * Outputs are sized for the raw peak count and compacted: out_peak_offsets[n+1]; out_mobilities parallel to out_masses, holding the sorted
+ * mobilities of level-1 spectra when raw->mobility is set, NaN for every other spectrum (whose ProcessedSpectrum::mobilities is empty);
+ * out_tic[n]. Bit for bit the reference's result on x86-64, NaNs included (DESIGN.md §16). */
+int sage_b200_process_raw(int device, const sage_b200_processor_params* processor, const sage_b200_raw_batch* raw, uint64_t* out_peak_offsets,
+                          float* out_masses, float* out_intensities, float* out_mobilities, float* out_tic);
+
 /* tmt::find_reporter_ions (tmt.rs:193-211) over a batch: out[i * n_labels + l] = intensity of the most intense peak of spectrum i within
  * label_tolerance of labels[l] (offset -PROTON, as the reference), 0 where none (the unwrap_or_default of tmt::quantify, tmt.rs:333). */
 int sage_b200_find_reporter_ions(int device, uint64_t n, const uint64_t* peak_offsets, const float* masses, const float* intensities, const float* labels,
@@ -319,6 +337,19 @@ int sage_b200_lfq_create(const sage_b200_db* db, const sage_b200_peptides* pepti
                          const sage_b200_lfq_features* features, uint64_t n_files, const sage_b200_alignment* alignments, sage_b200_lfq** out);
 /* The tracing loop of quantify (lfq.rs:239-287) over one batch. EINVAL for a file_id >= n_files. */
 int sage_b200_lfq_add_ms1(sage_b200_lfq* lfq, const sage_b200_ms1* ms1);
+/* One batch of raw MS1 RawSpectrum: mz in any order. */
+typedef struct {
+    uint64_t n;
+    const uint64_t* peak_offsets;     /* n+1 */
+    const float* mz;
+    const float* intensity;
+    const uint32_t* file_id;          /* < n_files */
+    const float* scan_start_time;
+    const float* mobility;            /* per raw peak; NULL = no spectrum of the batch has mobility */
+} sage_b200_raw_ms1;
+/* add_ms1 of the batch SpectrumProcessor::process makes of raw_ms1: the spectra are processed on the device (as sage_b200_process_raw does
+ * level 1) and traced there; the processed peaks never cross PCIe. Bit for bit equal to add_ms1 of the processed batch. */
+int sage_b200_lfq_add_raw_ms1(sage_b200_lfq* lfq, const sage_b200_raw_ms1* raw_ms1);
 /* summarize_traces + integrate (lfq.rs:447-610) for every touched grid: rows ordered by (id, decoy); areas[row * n_files + file].
  * capacity >= info.n_grids always suffices; *n_rows receives the row count. */
 int sage_b200_lfq_integrate(sage_b200_lfq* lfq, sage_b200_lfq_row* rows, double* areas, uint64_t capacity, uint64_t* n_rows);

@@ -4,5 +4,6 @@ in include/sage_b200.h; this package is the thin Python binding used by the test
 from .api import (DA, PCT, PPM, Feature, IndexedDatabase, Peptides, Precursor, ProcessedSpectrum, Scorer, SpectraBatch, SpectrumProcessor, Tolerance,  # noqa: F401
                   SageB200Error, device_count, FeatureMap, LfqSettings, Ms1Batch, spectrum_fdr, predict_rt, picked_fdr, picked_precursor,
                   competition_keys, protein_groups, protein_group_strings, bipartite_cover,
-                  DigestResult, digest_fasta, PrefilterResult, prefilter_fasta)
+                  DigestResult, digest_fasta, PrefilterResult, prefilter_fasta, RawSpectra, ProcessedBatch, ISOBARIC, tmt_quantify,
+                  tmt_min_deisotope_mz)
 from .build import build_library, library_path  # noqa: F401

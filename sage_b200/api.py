@@ -95,7 +95,7 @@ EXPORTED_SYMBOLS = [
     "sage_b200_picked_fdr", "sage_b200_picked_precursor", "sage_b200_competition_keys", "sage_b200_protein_groups", "sage_b200_bipartite_cover",
     "sage_b200_digest_create", "sage_b200_digest_get_info", "sage_b200_digest_export", "sage_b200_digest_destroy",
     "sage_b200_prefilter_create", "sage_b200_prefilter_get_info", "sage_b200_prefilter_chunk_counts", "sage_b200_prefilter_export",
-    "sage_b200_prefilter_take_db", "sage_b200_prefilter_destroy",
+    "sage_b200_prefilter_take_db", "sage_b200_prefilter_destroy", "sage_b200_process_raw", "sage_b200_lfq_add_raw_ms1",
 ]
 
 _lib = None
@@ -604,8 +604,114 @@ class SpectrumProcessor:
         k = int(out_off[-1])
         return out_off, om[:k].copy(), oi[:k].copy(), tic
 
+    def process_raw(self, batch: "RawSpectra") -> "ProcessedBatch":
+        """process() (spectrum.rs:338-412) of a batch of any MS levels: level 2 as process_batch, other levels keep every peak, sorted."""
+        keep: list = []
+        raw = batch._c(keep)
+        n = len(batch)
+        npk = max(1, int(batch.peak_off[-1] - batch.peak_off[0])) if n else 1
+        pp = CProcessorParams(self.take_top_n, int(self.deisotope), self.min_deisotope_mz)
+        out_off = np.zeros(n + 1, np.uint64)
+        om, oi, ob, tic = np.zeros(npk, np.float32), np.zeros(npk, np.float32), np.zeros(npk, np.float32), np.zeros(n, np.float32)
+        _check(load_library().sage_b200_process_raw(C.c_int(self.device), C.byref(pp), C.byref(raw), _ptr(out_off), _ptr(om), _ptr(oi), _ptr(ob),
+                                                    _ptr(tic)))
+        k = int(out_off[-1])
+        level = np.ascontiguousarray(batch.level, np.uint8).copy()
+        return ProcessedBatch(out_off, om[:k].copy(), oi[:k].copy(), ob[:k].copy(), (level == 1) & (batch.mobility is not None), tic, level)
+
+
+class CRawBatch(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("peak_offsets", C.c_void_p), ("mz", C.c_void_p), ("intensity", C.c_void_p), ("level", C.c_void_p),
+                ("precursor_charge", C.c_void_p), ("mobility", C.c_void_p)]
+
+
+class CRawMs1(C.Structure):
+    _fields_ = [("n", C.c_uint64), ("peak_offsets", C.c_void_p), ("mz", C.c_void_p), ("intensity", C.c_void_p), ("file_id", C.c_void_p),
+                ("scan_start_time", C.c_void_p), ("mobility", C.c_void_p)]
+
+
+def _keep_arr(keep: list, x, dt):
+    if x is None:
+        return None
+    a = np.ascontiguousarray(x, dtype=dt)
+    keep.append(a)
+    return _ptr(a)
+
+
+@dataclass
+class RawSpectra:
+    """A batch of RawSpectrum (spectrum.rs:81-106) of any MS levels, flattened: peaks in any order. precursor_charge (0 = None) is read for
+    level 2 only; mobility (per peak) may be None: then no spectrum of the batch has mobility. file_id and scan_start_time are needed by
+    FeatureMap.add_raw_ms1 only."""
+    peak_off: np.ndarray
+    mz: np.ndarray
+    intensity: np.ndarray
+    level: np.ndarray
+    precursor_charge: np.ndarray | None = None
+    mobility: np.ndarray | None = None
+    file_id: np.ndarray | None = None
+    scan_start_time: np.ndarray | None = None
+
+    def __len__(self):
+        return len(self.level)
+
+    def slice(self, a: int, b: int) -> "RawSpectra":
+        p0, p1 = int(self.peak_off[a]), int(self.peak_off[b])
+        cut = (lambda x, lo, hi: None if x is None else x[lo:hi])
+        return RawSpectra(self.peak_off[a:b + 1] - self.peak_off[a], self.mz[p0:p1], self.intensity[p0:p1], self.level[a:b],
+                          cut(self.precursor_charge, a, b), cut(self.mobility, p0, p1), cut(self.file_id, a, b), cut(self.scan_start_time, a, b))
+
+    def _c(self, keep: list) -> CRawBatch:
+        return CRawBatch(len(self), _keep_arr(keep, self.peak_off, np.uint64), _keep_arr(keep, self.mz, np.float32),
+                         _keep_arr(keep, self.intensity, np.float32), _keep_arr(keep, self.level, np.uint8),
+                         _keep_arr(keep, self.precursor_charge, np.uint8), _keep_arr(keep, self.mobility, np.float32))
+
+
+@dataclass
+class ProcessedBatch:
+    """A batch of ProcessedSpectrum (spectrum.rs:58-79) flattened. mobilities runs parallel to masses and is NaN for a spectrum whose
+    ProcessedSpectrum::mobilities is empty (has_mobilities False: every level but 1, and level 1 without mobility)."""
+    peak_off: np.ndarray
+    masses: np.ndarray
+    intensities: np.ndarray
+    mobilities: np.ndarray
+    has_mobilities: np.ndarray
+    tic: np.ndarray
+    level: np.ndarray
+
+    def __len__(self):
+        return len(self.level)
+
 
 TMT6PLEX = np.float32([126.127726, 127.124761, 128.134436, 129.131471, 130.141145, 131.138180])   # tmt.rs:213-215
+TMT11PLEX = np.float32([126.127726, 127.124761, 127.131081, 128.128116, 128.134436, 129.131471, 129.137790, 130.134825, 130.141145, 131.138180,
+                        131.144499])   # tmt.rs:217-220
+TMT18PLEX = np.float32([126.127726, 127.124761, 127.131081, 128.128116, 128.134436, 129.131471, 129.137790, 130.134825, 130.141145, 131.138180,
+                        131.144500, 132.141535, 132.147855, 133.144890, 133.151210, 134.148245, 134.154565, 135.15160])   # tmt.rs:222-226
+# Isobaric::reporter_masses (tmt.rs:24-34): Tmt10 is the first 10 of the 11-plex, Tmt16 the first 16 of the 18-plex
+ISOBARIC = {"Tmt6": TMT6PLEX, "Tmt10": TMT11PLEX[:10].copy(), "Tmt11": TMT11PLEX, "Tmt16": TMT18PLEX[:16].copy(), "Tmt18": TMT18PLEX}
+
+
+def tmt_min_deisotope_mz(isobaric: str, level: int) -> float:
+    """runner.rs:398-404: with TMT at level 2, the last reporter mass * (1.0 + 20E-6), in f32; 0.0 otherwise (the unwrap_or(0.0))."""
+    if level != 2:
+        return 0.0
+    return float(ISOBARIC[isobaric][-1] * (np.float32(1.0) + np.float32(20e-6)))
+
+
+def tmt_quantify(processed: ProcessedBatch, isobaric: str, level: int, tolerance: Tolerance | None = None, device: int = 0):
+    """tmt::quantify (tmt.rs:314-352): the spectra of `level` (none for level 1) and their reporter intensities through find_reporter_ions
+    (0 where no peak is within tolerance, the unwrap_or_default). Returns (row indices into `processed`, float32 [rows, labels])."""
+    labels = ISOBARIC[isobaric]
+    tolerance = Tolerance.ppm(-20, 20) if tolerance is None else tolerance
+    rows = np.nonzero(np.asarray(processed.level) == level)[0] if level != 1 else np.zeros(0, np.int64)
+    if len(rows) == 0:
+        return rows, np.zeros((0, len(labels)), np.float32)
+    off = np.asarray(processed.peak_off, np.uint64)
+    lens = (off[rows + 1] - off[rows]).astype(np.int64)
+    sub_off = np.concatenate([[0], np.cumsum(lens)]).astype(np.uint64)
+    take = np.concatenate([np.arange(int(off[r]), int(off[r + 1])) for r in rows]) if lens.sum() else np.zeros(0, np.int64)
+    return rows, find_reporter_ions(sub_off, processed.masses[take], processed.intensities[take], labels, tolerance, device)
 
 
 def find_reporter_ions(peak_off, masses, intensities, labels, label_tolerance: Tolerance, device: int = 0) -> np.ndarray:
@@ -748,6 +854,15 @@ class FeatureMap:
         keep: list = []
         cm = batch._c(keep)
         _check(load_library().sage_b200_lfq_add_ms1(self._h, C.byref(cm)))
+
+    def add_raw_ms1(self, batch: RawSpectra):
+        """add_ms1 of process() of a batch of raw MS1 spectra (file_id and scan_start_time set): processed and traced on the device."""
+        if len(batch) and not (np.asarray(batch.level) == 1).all():
+            raise ValueError("add_raw_ms1 takes MS1 spectra only")
+        keep: list = []
+        cr = CRawMs1(len(batch), _keep_arr(keep, batch.peak_off, np.uint64), _keep_arr(keep, batch.mz, np.float32), _keep_arr(keep, batch.intensity, np.float32),
+                     _keep_arr(keep, batch.file_id, np.uint32), _keep_arr(keep, batch.scan_start_time, np.float32), _keep_arr(keep, batch.mobility, np.float32))
+        _check(load_library().sage_b200_lfq_add_raw_ms1(self._h, C.byref(cr)))
 
     def info(self) -> dict:
         ci = CLfqInfo()

@@ -43,6 +43,7 @@
 #include "protein_groups.cuh"
 #include "digest.cuh"
 #include "prefilter.cuh"
+#include "spectra.cuh"
 
 using namespace sb;
 
@@ -2098,6 +2099,15 @@ extern "C" int64_t sage_b200_initial_hits(sage_b200_scorer* S, const sage_b200_s
     return (int64_t)nk;
 }
 
+// k_process_ms2's shared memory for spectra of at most pmax raw peaks (p2: pmax rounded up to a power of two), or ELIMIT past its budget.
+static int ms2_smem(uint32_t pmax, uint32_t& p2, size_t& smem) {
+    p2 = 1;
+    while (p2 < pmax) p2 <<= 1;
+    smem = (size_t)p2 * 12 + (size_t)pmax * (5 * 4 + 2) + 32;
+    if (smem > 200 * 1024) return fail(SAGE_B200_ELIMIT, "spectrum with %u raw peaks exceeds the shared-memory budget of the preprocessing kernel", pmax);
+    return 0;
+}
+
 // SpectrumProcessor::new(take_top_n, deisotope, min_deisotope_mz).process(..) for a batch of centroided MS2 RawSpectrum (spectrum.rs:271-412).
 extern "C" int sage_b200_process_spectra(int device, const sage_b200_processor_params* pr, const sage_b200_raw_spectra* raw, uint64_t* out_peak_offsets,
                                          float* out_masses, float* out_intensities, float* out_tic) {
@@ -2119,9 +2129,8 @@ extern "C" int sage_b200_process_spectra(int device, const sage_b200_processor_p
         pmax = std::max(pmax, off[i + 1] - off[i]);
     }
     uint32_t p2 = 1;
-    while (p2 < pmax) p2 <<= 1;
-    const size_t smem = (size_t)p2 * 12 + (size_t)pmax * (5 * 4 + 2) + 32;
-    if (smem > 200 * 1024) return fail(SAGE_B200_ELIMIT, "spectrum with %u raw peaks exceeds the shared-memory budget of the preprocessing kernel", pmax);
+    size_t smem = 0;
+    if (int rc = ms2_smem(pmax, p2, smem)) return rc;
     DevArena A;
     Stream st;
     CUDA_TRY(st.create());
@@ -2155,6 +2164,161 @@ extern "C" int sage_b200_process_spectra(int device, const sage_b200_processor_p
         w += cnt[i];
         out_peak_offsets[i + 1] = w;
     }
+    return 0;
+}
+
+// Launches the processing of the batch's spectra that are not MS2 (spectra.cuh) on st. `a` points at device arrays; off and level are the
+// host's copies of a.in_off and a.level (level NULL: every spectrum is MS1). Temporaries of the large size class come from A.
+static int raw_launch(cudaStream_t st, DevArena& A, RawArgs a, const uint64_t* off, const uint8_t* level) {
+    std::vector<uint32_t> slot(a.n, 0), large;
+    uint32_t pmax = 0;
+    bool any = false;
+    for (uint32_t s = 0; s < a.n; s++) {
+        if (level && level[s] == 2) continue;
+        any = true;
+        const uint64_t np = off[s + 1] - off[s];
+        if (np > RAW_SMEM_PEAKS) {
+            slot[s] = (uint32_t)large.size();
+            large.push_back(s);
+        } else pmax = std::max(pmax, (uint32_t)np);
+    }
+    if (!any) return 0;
+    uint32_t p2 = 1;
+    while (p2 < pmax) p2 <<= 1;
+    const uint64_t npk = off[a.n] - off[0];
+    const int nl = (int)large.size();
+    uint32_t *d_ids = nullptr, *key_out = nullptr, *val_out = nullptr;
+    if (nl) {
+        uint32_t* d_slot = nullptr;
+        CUDA_TRY(A.upload(&d_slot, slot.data(), a.n, st));
+        CUDA_TRY(A.upload(&d_ids, large.data(), large.size(), st));
+        CUDA_TRY(A.alloc(&a.seg_begin, large.size()));
+        CUDA_TRY(A.alloc(&a.seg_end, large.size()));
+        CUDA_TRY(A.alloc(&a.sort_key, npk));
+        CUDA_TRY(A.alloc(&a.sort_val, npk));
+        CUDA_TRY(A.alloc(&key_out, npk));
+        CUDA_TRY(A.alloc(&val_out, npk));
+        a.large_slot = d_slot;
+    }
+    LAUNCH(k_raw_process<<<a.n, RAW_THREADS, (size_t)p2 * 12, st>>>(a));
+    if (nl) {
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) {
+            return cub::DeviceSegmentedSort::StableSortPairs(t, b, a.sort_key, key_out, a.sort_val, val_out, (int)npk, nl, a.seg_begin, a.seg_end, st);
+        }));
+        a.sort_key = key_out;
+        a.sort_val = val_out;
+        LAUNCH(k_raw_gather_large<<<nl, RAW_THREADS, 0, st>>>(a, d_ids));
+    }
+    return 0;
+}
+
+// SpectrumProcessor::process (spectrum.rs:338-412) for a batch of any MS levels: level 2 through k_process_ms2, the others through spectra.cuh.
+extern "C" int sage_b200_process_raw(int device, const sage_b200_processor_params* pr, const sage_b200_raw_batch* raw, uint64_t* out_peak_offsets,
+                                     float* out_masses, float* out_intensities, float* out_mobilities, float* out_tic) {
+    if (!pr || !raw || !out_peak_offsets || !out_tic) return fail(SAGE_B200_EINVAL, "process_raw: null argument");
+    const uint64_t n = raw->n;
+    if (n && (!raw->peak_offsets || !raw->level)) return fail(SAGE_B200_EINVAL, "process_raw: null array");
+    const uint64_t pk0 = n ? raw->peak_offsets[0] : 0, npk = n ? raw->peak_offsets[n] - pk0 : 0;
+    if (npk && (!raw->mz || !raw->intensity || !out_masses || !out_intensities || !out_mobilities))
+        return fail(SAGE_B200_EINVAL, "process_raw: null peak arrays");
+    if (n > 0x7FFFFFFEull || npk > 0x7FFFFFFFull) return fail(SAGE_B200_ELIMIT, "process_raw: more than 2^31 - 2 spectra or 2^31 - 1 peaks");
+    std::vector<uint64_t> off(n + 1);
+    std::vector<uint32_t> ms2_ids, ms2_off(1, 0), ms2_pos(n, 0);
+    std::vector<uint8_t> ms2_chg;
+    uint32_t pmax2 = 1;
+    for (uint64_t i = 0; i <= n; i++) {
+        if (i < n && raw->peak_offsets[i + 1] < raw->peak_offsets[i])
+            return fail(SAGE_B200_EINVAL, "process_raw: peak_offsets not monotone at spectrum %llu", (unsigned long long)i);
+        off[i] = raw->peak_offsets[i] - pk0;
+    }
+    for (uint64_t i = 0; i < n; i++) {
+        if (raw->level[i] != 2) continue;
+        if (!raw->precursor_charge) return fail(SAGE_B200_EINVAL, "process_raw: spectrum %llu is MS2 and precursor_charge is NULL", (unsigned long long)i);
+        const uint32_t np = (uint32_t)(off[i + 1] - off[i]);
+        ms2_pos[i] = (uint32_t)ms2_ids.size();
+        ms2_ids.push_back((uint32_t)i);
+        ms2_off.push_back(ms2_off.back() + np);
+        ms2_chg.push_back(raw->precursor_charge[i]);
+        pmax2 = std::max(pmax2, np);
+    }
+    uint32_t p2 = 1;
+    size_t smem = 0;
+    if (!ms2_ids.empty()) {
+        if (int rc = ms2_smem(pmax2, p2, smem)) return rc;
+    }
+    out_peak_offsets[0] = 0;
+    if (n == 0) return 0;
+    if (int rc = select_device(device)) return rc;
+    cudaGetLastError();   // a stale non-sticky error left by another user of the runtime must not be blamed on the launches below
+    {
+        // inputs and outputs (28 B per peak), the level-2 copies (16 B per level-2 peak), and the large class's sort (16 B per peak)
+        size_t free_b = 0, total_b = 0;
+        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+        const uint64_t need = npk * 44 + (uint64_t)ms2_off.back() * 16 + n * 64 + (64ull << 20);
+        if (need > free_b) return fail(SAGE_B200_ELIMIT, "process_raw: %llu peaks need about %llu bytes of device memory, %llu free", (unsigned long long)npk,
+                                       (unsigned long long)need, (unsigned long long)free_b);
+    }
+    const uint32_t n2 = (uint32_t)ms2_ids.size();
+    DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
+    RawArgs a{};
+    a.n = (uint32_t)n;
+    uint64_t *d_in_off = nullptr, *d_count = nullptr, *d_out_off = nullptr;
+    float *d_mz = nullptr, *d_int = nullptr, *d_mob = nullptr;
+    uint8_t* d_level = nullptr;
+    CUDA_TRY(A.upload(&d_in_off, off.data(), n + 1, st));
+    CUDA_TRY(A.upload(&d_mz, raw->mz + pk0, npk, st));
+    CUDA_TRY(A.upload(&d_int, raw->intensity + pk0, npk, st));
+    if (raw->mobility) CUDA_TRY(A.upload(&d_mob, raw->mobility + pk0, npk, st));
+    CUDA_TRY(A.upload(&d_level, raw->level, n, st));
+    CUDA_TRY(A.alloc(&d_count, n + 1));
+    CUDA_TRY(A.alloc(&d_out_off, n + 1));
+    CUDA_TRY(A.alloc(&a.out_mass, npk));
+    CUDA_TRY(A.alloc(&a.out_int, npk));
+    CUDA_TRY(A.alloc(&a.out_mob, npk));
+    CUDA_TRY(A.alloc(&a.out_tic, n));
+    uint32_t *d_ms2_ids = nullptr, *d_ms2_off = nullptr, *d_ms2_pos = nullptr, *d_ms2_cnt = nullptr;
+    float *d_ms2_mz = nullptr, *d_ms2_in = nullptr, *d_ms2_om = nullptr, *d_ms2_oi = nullptr, *d_ms2_tic = nullptr;
+    if (n2) {
+        const uint64_t q = ms2_off.back();
+        uint8_t* d_chg = nullptr;
+        CUDA_TRY(A.upload(&d_ms2_ids, ms2_ids.data(), n2, st));
+        CUDA_TRY(A.upload(&d_ms2_off, ms2_off.data(), n2 + 1, st));
+        CUDA_TRY(A.upload(&d_ms2_pos, ms2_pos.data(), n, st));
+        CUDA_TRY(A.upload(&d_chg, ms2_chg.data(), n2, st));
+        CUDA_TRY(A.alloc(&d_ms2_mz, q + 4));
+        CUDA_TRY(A.alloc(&d_ms2_in, q + 4));
+        CUDA_TRY(A.alloc(&d_ms2_om, q + 4));
+        CUDA_TRY(A.alloc(&d_ms2_oi, q + 4));
+        CUDA_TRY(A.alloc(&d_ms2_cnt, n2));
+        CUDA_TRY(A.alloc(&d_ms2_tic, n2));
+        LAUNCH(k_raw_gather_ms2<<<n2, RAW_THREADS, 0, st>>>(n2, d_ms2_ids, d_ms2_off, d_in_off, d_mz, d_int, d_ms2_mz, d_ms2_in));
+        ProcParams pp{(uint32_t)std::min<uint64_t>(pr->take_top_n, 0xFFFFFFFFull), pr->deisotope ? 1u : 0u, pr->min_deisotope_mz};
+        if (int rc = ensure_kernel_attributes(device)) return rc;
+        LAUNCH(k_process_ms2<<<n2, 32, smem, st>>>(pp, n2, d_ms2_off, d_ms2_mz, d_ms2_in, d_chg, pmax2, p2, d_ms2_om, d_ms2_oi, d_ms2_cnt, d_ms2_tic));
+    }
+    LAUNCH_N(k_raw_counts, n + 1, st, (uint32_t)n, d_in_off, d_level, d_ms2_pos, d_ms2_cnt, d_count);
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_count, d_out_off, (int)(n + 1), st); }));
+    if (n2)
+        LAUNCH(k_raw_compact_ms2<<<n2, RAW_THREADS, 0, st>>>(n2, d_ms2_ids, d_ms2_off, d_ms2_cnt, d_ms2_om, d_ms2_oi, d_ms2_tic, d_out_off, a.out_mass,
+                                                               a.out_int, a.out_mob, a.out_tic));
+    a.in_off = d_in_off;
+    a.mz = d_mz;
+    a.intensity = d_int;
+    a.mobility = d_mob;
+    a.level = d_level;
+    a.out_off = d_out_off;
+    if (int rc = raw_launch(st, A, a, off.data(), raw->level)) return rc;
+    if (int rc = read_back(st, out_peak_offsets, d_out_off, 8 * (n + 1))) return rc;
+    const uint64_t kept = out_peak_offsets[n];
+    CUDA_TRY(cudaMemcpyAsync(out_tic, a.out_tic, 4 * n, cudaMemcpyDeviceToHost, st));
+    if (kept) {
+        CUDA_TRY(cudaMemcpyAsync(out_masses, a.out_mass, 4 * kept, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(out_intensities, a.out_int, 4 * kept, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(out_mobilities, a.out_mob, 4 * kept, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
@@ -2292,13 +2456,13 @@ struct sage_b200_lfq {
     uint8_t* d_touched = nullptr;
     sage_b200_alignment* d_align = nullptr;
     std::vector<uint32_t> slot_pep;   // slot -> PeptideIx, ascending
-    DevBuf sp_off, sp_mass, sp_int, sp_mob, sp_file, sp_sst, counts, offsets, cell[2], value[2], tmp, ids, o_present, o_rt, o_sa, o_score, o_areas;
+    DevBuf sp_off, sp_mass, sp_int, sp_mob, raw_mz, raw_int, raw_mob, sp_file, sp_sst, counts, offsets, cell[2], value[2], tmp, ids, o_present, o_rt, o_sa, o_score, o_areas;
     Stream st;
     Event ev[2];
     sage_b200_lfq_info info{};
     uint64_t scratch_bytes() const {
         uint64_t b = 0;
-        for (const DevBuf* d : {&sp_off, &sp_mass, &sp_int, &sp_mob, &sp_file, &sp_sst, &counts, &offsets, &cell[0], &cell[1], &value[0], &value[1], &tmp, &ids,
+        for (const DevBuf* d : {&sp_off, &sp_mass, &sp_int, &sp_mob, &raw_mz, &raw_int, &raw_mob, &sp_file, &sp_sst, &counts, &offsets, &cell[0], &cell[1], &value[0], &value[1], &tmp, &ids,
                                 &o_present, &o_rt, &o_sa, &o_score, &o_areas})
             b += d->cap;
         return b;
@@ -2501,7 +2665,8 @@ extern "C" int sage_b200_lfq_create(const sage_b200_db* db, const sage_b200_pept
 }
 
 // One pass of the tracing loop over spectra [a, b) of the batch (peaks already counted to fit LFQ_CHUNK_PEAKS unless a single spectrum is larger).
-static int lfq_trace_chunk(sage_b200_lfq* L, const sage_b200_ms1* m, uint64_t a, uint64_t b) {
+// raw: m holds raw MS1 spectra (masses are m/z, in any order), uploaded to the raw_* buffers and processed into the sp_* ones first.
+static int lfq_trace_chunk(sage_b200_lfq* L, const sage_b200_ms1* m, uint64_t a, uint64_t b, bool raw) {
     cudaStream_t st = L->st;
     const uint64_t ns = b - a, p0 = m->peak_offsets[a], np = m->peak_offsets[b] - p0;
     std::vector<uint64_t> off(ns + 1);
@@ -2511,15 +2676,32 @@ static int lfq_trace_chunk(sage_b200_lfq* L, const sage_b200_ms1* m, uint64_t a,
         (rc = L->sp_file.reserve(4 * ns)) || (rc = L->sp_sst.reserve(4 * ns)) || (rc = L->counts.reserve(8 * np + 16)) || (rc = L->offsets.reserve(8 * np + 16)) ||
         (m->mobilities && (rc = L->sp_mob.reserve(4 * np + 16))))
         return rc;
+    if (raw && ((rc = L->raw_mz.reserve(4 * np + 16)) || (rc = L->raw_int.reserve(4 * np + 16)) || (m->mobilities && (rc = L->raw_mob.reserve(4 * np + 16)))))
+        return rc;
+    DevBuf &up_mass = raw ? L->raw_mz : L->sp_mass, &up_int = raw ? L->raw_int : L->sp_int, &up_mob = raw ? L->raw_mob : L->sp_mob;
     CUDA_TRY(cudaMemcpyAsync(L->sp_off.p, off.data(), 8 * (ns + 1), cudaMemcpyHostToDevice, st));
     if (np) {
-        CUDA_TRY(cudaMemcpyAsync(L->sp_mass.p, m->masses + p0, 4 * np, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(L->sp_int.p, m->intensities + p0, 4 * np, cudaMemcpyHostToDevice, st));
-        if (m->mobilities) CUDA_TRY(cudaMemcpyAsync(L->sp_mob.p, m->mobilities + p0, 4 * np, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(up_mass.p, m->masses + p0, 4 * np, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(up_int.p, m->intensities + p0, 4 * np, cudaMemcpyHostToDevice, st));
+        if (m->mobilities) CUDA_TRY(cudaMemcpyAsync(up_mob.p, m->mobilities + p0, 4 * np, cudaMemcpyHostToDevice, st));
     }
     CUDA_TRY(cudaMemcpyAsync(L->sp_file.p, m->file_id + a, 4 * ns, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(L->sp_sst.p, m->scan_start_time + a, 4 * ns, cudaMemcpyHostToDevice, st));
     if (np == 0 || L->n_ranges == 0) return 0;
+    if (raw) {   // SpectrumProcessor::process of level 1: every peak is kept, so the processed batch has the raw offsets
+        RawArgs r{};
+        r.n = (uint32_t)ns;
+        r.in_off = r.out_off = L->sp_off.as<uint64_t>();
+        r.mz = L->raw_mz.as<float>();
+        r.intensity = L->raw_int.as<float>();
+        r.mobility = m->mobilities ? L->raw_mob.as<float>() : nullptr;
+        r.out_mass = L->sp_mass.as<float>();
+        r.out_int = L->sp_int.as<float>();
+        r.out_mob = m->mobilities ? L->sp_mob.as<float>() : nullptr;
+        DevArena A;   // the large size class's temporaries
+        if ((rc = raw_launch(st, A, r, off.data(), nullptr))) return rc;
+        if (A.bytes) CUDA_TRY(cudaStreamSynchronize(st));
+    }
 
     LfqTraceArgs t{};
     t.n_spectra = (uint32_t)ns;
@@ -2565,29 +2747,40 @@ static int lfq_trace_chunk(sage_b200_lfq* L, const sage_b200_ms1* m, uint64_t a,
     return 0;
 }
 
-extern "C" int sage_b200_lfq_add_ms1(sage_b200_lfq* L, const sage_b200_ms1* m) {
-    if (!L || !m) return fail(SAGE_B200_EINVAL, "lfq_add_ms1: null argument");
+// add_ms1 and add_raw_ms1 (raw: masses are raw m/z, processed on the device first). `what` names the entry point in errors.
+static int lfq_add(sage_b200_lfq* L, const sage_b200_ms1* m, bool raw, const char* what) {
     std::lock_guard<std::mutex> lock(L->mu);
     if (m->n == 0) return 0;
-    if (!m->peak_offsets || !m->file_id || !m->scan_start_time) return fail(SAGE_B200_EINVAL, "lfq_add_ms1: null array");
-    if (m->peak_offsets[m->n] > m->peak_offsets[0] && (!m->masses || !m->intensities)) return fail(SAGE_B200_EINVAL, "lfq_add_ms1: null peak arrays");
+    if (!m->peak_offsets || !m->file_id || !m->scan_start_time) return fail(SAGE_B200_EINVAL, "%s: null array", what);
+    if (m->peak_offsets[m->n] > m->peak_offsets[0] && (!m->masses || !m->intensities)) return fail(SAGE_B200_EINVAL, "%s: null peak arrays", what);
     for (uint64_t i = 0; i < m->n; i++) {
         if (m->file_id[i] >= L->n_files)
-            return fail(SAGE_B200_EINVAL, "lfq_add_ms1: spectrum %llu has file_id %u >= n_files %u", (unsigned long long)i, m->file_id[i], L->n_files);
-        if (m->peak_offsets[i + 1] < m->peak_offsets[i]) return fail(SAGE_B200_EINVAL, "lfq_add_ms1: peak_offsets not monotone at spectrum %llu", (unsigned long long)i);
+            return fail(SAGE_B200_EINVAL, "%s: spectrum %llu has file_id %u >= n_files %u", what, (unsigned long long)i, m->file_id[i], L->n_files);
+        if (m->peak_offsets[i + 1] < m->peak_offsets[i]) return fail(SAGE_B200_EINVAL, "%s: peak_offsets not monotone at spectrum %llu", what, (unsigned long long)i);
     }
     CUDA_TRY(cudaSetDevice(L->device));
     CUDA_TRY(cudaEventRecord(L->ev[0], L->st));
     for (uint64_t a = 0; a < m->n;) {
         uint64_t b = a + 1;
         while (b < m->n && b - a < 0x7FFFFFull && m->peak_offsets[b + 1] - m->peak_offsets[a] <= LFQ_CHUNK_PEAKS) b++;
-        const int rc = lfq_trace_chunk(L, m, a, b);
+        const int rc = lfq_trace_chunk(L, m, a, b, raw);
         if (rc) return rc;
         a = b;
     }
     L->info.ms1_spectra += m->n;
     L->info.ms1_peaks += m->peak_offsets[m->n] - m->peak_offsets[0];
     return lfq_elapsed(L, L->info.ms_trace);
+}
+
+extern "C" int sage_b200_lfq_add_ms1(sage_b200_lfq* L, const sage_b200_ms1* m) {
+    if (!L || !m) return fail(SAGE_B200_EINVAL, "lfq_add_ms1: null argument");
+    return lfq_add(L, m, false, "lfq_add_ms1");
+}
+
+extern "C" int sage_b200_lfq_add_raw_ms1(sage_b200_lfq* L, const sage_b200_raw_ms1* r) {
+    if (!L || !r) return fail(SAGE_B200_EINVAL, "lfq_add_raw_ms1: null argument");
+    const sage_b200_ms1 m{r->n, r->peak_offsets, r->mz, r->intensity, r->file_id, r->scan_start_time, r->mobility};
+    return lfq_add(L, &m, true, "lfq_add_raw_ms1");
 }
 
 extern "C" int sage_b200_lfq_integrate(sage_b200_lfq* L, sage_b200_lfq_row* rows, double* areas, uint64_t capacity, uint64_t* n_rows) {

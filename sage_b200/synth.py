@@ -487,3 +487,55 @@ def make_rt_psms(pep: Peptides, n: int, n_files: int, seed: int = 0x5E7, mobilit
     if with_truth:
         return rows, fid, dict(rt_true=rt_true, is_true=true, T=T, a=a, b=b)
     return rows, fid
+
+
+def make_raw_spectra(n: int, peaks=(0, 400), levels=(1, 2, 3), order: str = "shuffled", mobility: bool = False, duplicate_fraction: float = 0.1,
+                     mz_range=(100.0, 2000.0), seed: int = 0x5A7):
+    """Synthetic RawSpectrum batch (any levels) for SpectrumProcessor::process: n spectra with a peak count uniform in [peaks[0], peaks[1]],
+    a level drawn from `levels`, log-normal intensities, `duplicate_fraction` of each spectrum's m/z repeating an earlier one of it (with
+    its own intensity, so a stable sort is visible), and peaks in `order`: "sorted" (ascending m/z), "reversed" or "shuffled". With
+    `mobility`, every peak has one (RawSpectrum::mobility is Some for the whole batch). Precursor charges are 0 (None) to 4."""
+    from .api import RawSpectra
+    rng = np.random.default_rng(seed)
+    cnt = rng.integers(peaks[0], peaks[1] + 1, n)
+    off = np.zeros(n + 1, np.uint64)
+    off[1:] = np.cumsum(cnt)
+    mzs, its = [], []
+    for c in cnt:
+        mz = rng.uniform(mz_range[0], mz_range[1], c).astype(np.float32)
+        dup = np.nonzero(rng.random(c) < duplicate_fraction)[0]
+        dup = dup[dup > 0]
+        mz[dup] = mz[rng.integers(0, np.maximum(dup, 1))]
+        if order == "sorted":
+            mz = np.sort(mz, kind="stable")
+        elif order == "reversed":
+            mz = np.sort(mz, kind="stable")[::-1].copy()
+        elif order != "shuffled":
+            raise ValueError(f"order must be sorted, reversed or shuffled, not {order!r}")
+        mzs.append(mz)
+        its.append(np.exp(rng.normal(9.0, 1.5, c)).astype(np.float32))
+    cat = (lambda x: np.concatenate(x).astype(np.float32) if n else np.zeros(0, np.float32))
+    total = int(off[-1])
+    return RawSpectra(off, cat(mzs), cat(its), rng.choice(np.asarray(levels, np.uint8), n).astype(np.uint8), rng.integers(0, 5, n).astype(np.uint8),
+                      rng.uniform(0.6, 1.4, total).astype(np.float32) if mobility else None, np.zeros(n, np.uint32), np.arange(n, dtype=np.float32))
+
+
+def ms1_to_raw(batch, shuffle: bool = False, seed: int = 0x5A8):
+    """The raw MS1 spectra behind an Ms1Batch of make_ms1_runs: m/z = mass + PROTON in f32, every peak's intensity and mobility with it,
+    optionally shuffled inside each spectrum. (Processing them again gives masses within an ulp of the batch's, not the same bits.)"""
+    from .api import RawSpectra
+    off = np.asarray(batch.peak_off, np.uint64)
+    mz = (np.asarray(batch.masses, np.float32) + PROTON).astype(np.float32)
+    it = np.asarray(batch.intensities, np.float32).copy()
+    mob = None if batch.mobilities is None else np.asarray(batch.mobilities, np.float32).copy()
+    if shuffle:
+        rng = np.random.default_rng(seed)
+        perm = np.arange(len(mz))
+        for s in range(len(off) - 1):
+            a, b = int(off[s]), int(off[s + 1])
+            perm[a:b] = a + rng.permutation(b - a)
+        mz, it = mz[perm], it[perm]
+        mob = None if mob is None else mob[perm]
+    n = len(off) - 1
+    return RawSpectra(off.copy(), mz, it, np.ones(n, np.uint8), None, mob, np.asarray(batch.file_id, np.uint32).copy(),
+                      np.asarray(batch.scan_start_time, np.float32).copy())
