@@ -332,42 +332,57 @@ static bool is_pinned(const void* p) {
 }
 
 // ------------------------------------------------------------------------------------------------ db
+// Runs f() (0 or an error code) for work whose failure only turns an optimisation off: the error is cleared and the thread's last error
+// message is kept, since the calling entry point still succeeds.
+template <class F>
+static bool optional_work(F f) {
+    const std::string msg = g_last_error;
+    if (f() == 0) return true;
+    cudaGetLastError();
+    g_last_error = msg;
+    return false;
+}
+
 // One lazily built block-major copy of the fragments: its view and the device arrays behind it.
 template <class View>
 struct BlockIndexSlot {
     View v{};
-    void* d[5] = {};   // the arrays of the current build
+    std::unique_ptr<DevArena> mem;   // the arrays of the current build
     int failed = 0;
     uint64_t bytes = 0;
-    std::vector<void*> retired;   // arrays of earlier builds: another scorer of the same db may still hold a view of them (freed with the db)
+    std::vector<std::unique_ptr<DevArena>> retired;   // arrays of earlier builds: another scorer of the same db may still hold a view of them (freed with the db)
     uint64_t retired_bytes = 0;
-    void free_current() {
-        for (void*& p : d) { if (p) cudaFree(p); p = nullptr; }
-        v = View{};
-        bytes = 0;
-    }
-    void release() {
-        free_current();
-        for (void* p : retired) cudaFree(p);
-        retired.clear();
-        retired_bytes = 0;
-    }
     // A rebuild with another block size keeps the old arrays alive: a chunk of another scorer, queued with the old view, may still run.
     void retire() {
-        for (void*& p : d) { if (p) retired.push_back(p); p = nullptr; }
+        if (mem) retired.push_back(std::move(mem));
         retired_bytes += bytes;
         v = View{};
         bytes = 0;
+    }
+    // build(arena, view, bytes) makes the copy's arrays in a fresh arena and returns 0 once they are finished on the device; only then is
+    // the view published. A failed build frees its arrays and leaves an empty view for good (the kernels then read the page index).
+    template <class F>
+    View rebuild(F build) {
+        retire();
+        std::unique_ptr<DevArena> fresh(new DevArena);
+        View nv{};
+        uint64_t nbytes = 0;
+        if (!optional_work([&] { return build(*fresh, nv, nbytes); })) {
+            failed = 1;
+            return View{};
+        }
+        mem = std::move(fresh);
+        v = nv;
+        bytes = nbytes;
+        return v;
     }
 };
 
 struct sage_b200_db {
     int device = 0;
     DbView v{};
-    void *d_page_grid = nullptr, *d_bucket_lut = nullptr, *d_pep_lut = nullptr;
-    void *d_frag = nullptr, *d_bucket_min = nullptr, *d_pep_mono = nullptr, *d_ion_off = nullptr, *d_ions = nullptr, *d_pep_len = nullptr,
-         *d_pep_flags = nullptr, *d_pep_missed = nullptr;
-    uint64_t total_residues = 0, device_bytes = 0;
+    DevArena mem;   // the arrays the view points at, exact-size
+    uint64_t total_residues = 0;
     int sm_count = 132;   // H100 SXM; replaced by the device's multiProcessorCount in db_new
     // secondary copies of the fragments in peptide-block-major order, built lazily and guarded by wmu: `wide` (WideIndexView: blocks = the
     // open-search count tile, built by the first scorer that meets a wide window) and `narrow` (NarrowIndexView: small blocks, built by the
@@ -376,13 +391,6 @@ struct sage_b200_db {
     mutable BlockIndexSlot<WideIndexView> wide;
     mutable BlockIndexSlot<NarrowIndexView> narrow;
 };
-
-static int dmalloc(sage_b200_db* db, void** p, size_t bytes) {
-    if (bytes == 0) bytes = 16;
-    CUDA_TRY(cudaMalloc(p, bytes));
-    db->device_bytes += bytes;
-    return 0;
-}
 
 static uint32_t ceil_log2_u64(uint64_t n) {
     uint32_t l = 0;
@@ -402,42 +410,45 @@ static int db_set_kinds(sage_b200_db* db, const uint8_t* kinds, uint64_t n_kinds
     return 0;
 }
 
+// The per-peptide arrays of an index, writable (the view holds them read-only).
+struct PeptideArrays {
+    float* mono = nullptr;
+    uint8_t *len = nullptr, *flags = nullptr, *missed = nullptr;
+    uint32_t* ion_off = nullptr;
+};
+
 // The per-peptide arrays of an n-peptide index (mono, length, flags, missed cleavages, ion offsets), allocated and placed in the view.
-static int db_alloc_peptides(sage_b200_db* db, uint64_t n) {
-    int rc;
-    if ((rc = dmalloc(db, &db->d_pep_mono, 4 * n))) return rc;
-    if ((rc = dmalloc(db, &db->d_pep_len, n))) return rc;
-    if ((rc = dmalloc(db, &db->d_pep_flags, n))) return rc;
-    if ((rc = dmalloc(db, &db->d_pep_missed, n))) return rc;
-    if ((rc = dmalloc(db, &db->d_ion_off, 4 * (n + 1)))) return rc;
+static int db_alloc_peptides(sage_b200_db* db, uint64_t n, PeptideArrays& p) {
+    CUDA_TRY(db->mem.alloc(&p.mono, n));
+    CUDA_TRY(db->mem.alloc(&p.len, n));
+    CUDA_TRY(db->mem.alloc(&p.flags, n));
+    CUDA_TRY(db->mem.alloc(&p.missed, n));
+    CUDA_TRY(db->mem.alloc(&p.ion_off, n + 1));
     db->v.n_pep = (uint32_t)n;
-    db->v.pep_mono = (const float*)db->d_pep_mono;
-    db->v.pep_len = (const uint8_t*)db->d_pep_len;
-    db->v.pep_flags = (const uint8_t*)db->d_pep_flags;
-    db->v.pep_missed = (const uint8_t*)db->d_pep_missed;
-    db->v.ion_off = (const uint32_t*)db->d_ion_off;
+    db->v.pep_mono = p.mono;
+    db->v.pep_len = p.len;
+    db->v.pep_flags = p.flags;
+    db->v.pep_missed = p.missed;
+    db->v.ion_off = p.ion_off;
     return 0;
 }
 
-// The per-peptide ion tables (n_ions entries at the ion offsets already on the device) from the table's device arrays.
-static int db_build_ions(sage_b200_db* db, uint64_t n, uint64_t n_ions, const uint32_t* off, const uint8_t* seq, const float* mods, const float* nterm) {
-    if (int rc = dmalloc(db, &db->d_ions, 4 * n_ions)) return rc;
-    db->v.ions = (const float*)db->d_ions;
+// The per-peptide ion tables (n_ions entries at the ion offsets already on the device) from the table's device arrays, finished on st.
+static int db_build_ions(sage_b200_db* db, uint64_t n, uint64_t n_ions, const uint32_t* off, const uint8_t* seq, const float* mods, const float* nterm,
+                         cudaStream_t st) {
+    float* ions = nullptr;
+    CUDA_TRY(db->mem.alloc(&ions, n_ions));
+    db->v.ions = ions;
     DevArena A;
     float* t_res = nullptr;
-    CUDA_TRY(A.alloc(&t_res, sizeof kResidueMass / sizeof(float)));
-    CUDA_TRY(cudaMemcpy(t_res, kResidueMass, sizeof kResidueMass, cudaMemcpyHostToDevice));
-    if (n) {
-        k_build_ions<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, off, seq, mods, nterm, (const float*)db->d_pep_mono, (const uint32_t*)db->d_ion_off,
-                                                           db->v.n_kinds, db->v, (float*)db->d_ions, t_res);
-        CUDA_TRY(cudaGetLastError());
-    }
-    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(A.upload(&t_res, kResidueMass, sizeof kResidueMass / sizeof(float), st));
+    if (n) LAUNCH(k_build_ions<<<(unsigned)((n + 127) / 128), 128, 0, st>>>((uint32_t)n, off, seq, mods, nterm, db->v.pep_mono, db->v.ion_off, db->v.n_kinds, db->v, ions, t_res));
+    CUDA_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
-// Uploads the peptide table and builds the per-peptide ion tables.
-static int db_upload_peptides(sage_b200_db* db, const sage_b200_peptides* P, const uint8_t* kinds, uint64_t n_kinds) {
+// Uploads the peptide table and builds the per-peptide ion tables on st.
+static int db_upload_peptides(sage_b200_db* db, const sage_b200_peptides* P, const uint8_t* kinds, uint64_t n_kinds, cudaStream_t st) {
     if (!P || (P->n_peptides && (!P->residue_offsets || !P->sequence || !P->modifications || !P->nterm || !P->monoisotopic || !P->decoy || !P->missed_cleavages)))
         return fail(SAGE_B200_EINVAL, "peptides: null array");
     if (int rc = db_set_kinds(db, kinds, n_kinds)) return rc;
@@ -458,12 +469,15 @@ static int db_upload_peptides(sage_b200_db* db, const sage_b200_peptides* P, con
         if (acc > 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "ion table exceeds 2^32 entries");
     }
     ion_off[n] = (uint32_t)acc;
-    if (int rc = db_alloc_peptides(db, n)) return rc;
-    CUDA_TRY(cudaMemcpy(db->d_pep_mono, P->monoisotopic, 4 * n, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(db->d_pep_len, len.data(), n, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(db->d_pep_flags, flags.data(), n, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(db->d_pep_missed, P->missed_cleavages, n, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(db->d_ion_off, ion_off.data(), 4 * (n + 1), cudaMemcpyHostToDevice));
+    PeptideArrays p;
+    if (int rc = db_alloc_peptides(db, n, p)) return rc;
+    if (n) {
+        CUDA_TRY(cudaMemcpyAsync(p.mono, P->monoisotopic, 4 * n, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(p.len, len.data(), n, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(p.flags, flags.data(), n, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(p.missed, P->missed_cleavages, n, cudaMemcpyHostToDevice, st));
+    }
+    CUDA_TRY(cudaMemcpyAsync(p.ion_off, ion_off.data(), 4 * (n + 1), cudaMemcpyHostToDevice, st));
     // device copies of the arrays ion generation reads
     DevArena A;
     uint32_t* t_off = nullptr;
@@ -474,12 +488,12 @@ static int db_upload_peptides(sage_b200_db* db, const sage_b200_peptides* P, con
     CUDA_TRY(A.alloc(&t_mods, nres + 4));
     CUDA_TRY(A.alloc(&t_nterm, n + 4));
     if (n) {
-        CUDA_TRY(cudaMemcpy(t_off, P->residue_offsets, 4 * (n + 1), cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMemcpy(t_seq, P->sequence, nres, cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMemcpy(t_mods, P->modifications, 4 * nres, cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMemcpy(t_nterm, P->nterm, 4 * n, cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpyAsync(t_off, P->residue_offsets, 4 * (n + 1), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(t_seq, P->sequence, nres, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(t_mods, P->modifications, 4 * nres, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(t_nterm, P->nterm, 4 * n, cudaMemcpyHostToDevice, st));
     }
-    return db_build_ions(db, n, acc, t_off, t_seq, t_mods, t_nterm);
+    return db_build_ions(db, n, acc, t_off, t_seq, t_mods, t_nterm, st);   // it waits for st: the host and device arrays above outlive the copies
 }
 
 // A handle under construction: destroyed (by its C destroy function) unless released to the caller.
@@ -507,20 +521,17 @@ extern "C" int sage_b200_device_count(void) {
 extern "C" void sage_b200_db_destroy(sage_b200_db* db) {
     if (!db) return;
     cudaSetDevice(db->device);
-    db->wide.release();
-    db->narrow.release();
-    void* ps[] = {db->d_page_grid, db->d_bucket_lut, db->d_pep_lut, db->d_frag, db->d_bucket_min, db->d_pep_mono, db->d_ion_off, db->d_ions, db->d_pep_len, db->d_pep_flags, db->d_pep_missed};
-    for (void* p : ps)
-        if (p) cudaFree(p);
     delete db;
 }
 
-// Search directories over the finished index (see DbView). Skipped (plain binary searches are used) when the shapes do not fit.
-static int db_build_directories(sage_b200_db* db) {
+// Search directories over the finished index (see DbView), built on st. Skipped (plain binary searches are used) when the shapes do not fit.
+static int db_build_directories(sage_b200_db* db, cudaStream_t st) {
     DbView& v = db->v;
     v.page_grid = nullptr; v.bucket_lut = nullptr; v.pep_lut = nullptr;
     if (v.n_frag == 0 || v.n_bucket == 0 || v.n_pep == 0 || (getenv("SAGE_B200_NO_DIRECTORIES") && getenv("SAGE_B200_NO_DIRECTORIES")[0] == '1')) return 0;
     int rc;
+    uint16_t* page_grid = nullptr;
+    uint32_t *bucket_lut = nullptr, *pep_lut = nullptr;
     if (v.bucket_size <= 65535u) {
         // cells per page ~ bucket_size / entries-per-cell: the in-cell search that follows a grid lookup is a chain of dependent loads
         uint32_t epc = 2;   // chosen by A/B on cfg2 against 4..32 entries per cell (+6 % index memory)
@@ -531,49 +542,45 @@ static int db_build_directories(sage_b200_db* db) {
         while (((uint64_t)v.n_pep >> shift) >= cells) shift++;
         const uint32_t gn = (uint32_t)(((uint64_t)v.n_pep - 1) >> shift) + 1;   // cells 0..gn-1 cover every PeptideIx
         const uint64_t total = (uint64_t)v.n_bucket * (gn + 1);
-        if ((rc = dmalloc(db, &db->d_page_grid, 2 * total))) return rc;
-        k_build_page_grid<<<(unsigned)((total + 255) / 256), 256>>>(v, shift, gn, (uint16_t*)db->d_page_grid);
-        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(db->mem.alloc(&page_grid, total));
+        LAUNCH(k_build_page_grid<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(v, shift, gn, page_grid));
         v.grid_shift = shift; v.grid_n = gn;
     }
     float ends[2] = {0.f, 0.f};
-    CUDA_TRY(cudaMemcpy(&ends[0], db->d_bucket_min, 4, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&ends[1], (const float*)db->d_bucket_min + (v.n_bucket - 1), 4, cudaMemcpyDeviceToHost));
+    if ((rc = read_back(st, &ends[0], v.bucket_min, 4))) return rc;
+    if ((rc = read_back(st, &ends[1], v.bucket_min + (v.n_bucket - 1), 4))) return rc;
     bool lut_ok = ends[0] > 0.0f && std::isfinite(ends[0]) && std::isfinite(ends[1]);   // positive finite m/z: float order == total_cmp order
     if (lut_ok) {
         const float w = (ends[1] - ends[0]) / (float)BUCKET_LUT_CELLS;
         const float inv_w = (w > 0.0f && w < 3.0e38f) ? 1.0f / w : 0.0f;
-        if ((rc = dmalloc(db, &db->d_bucket_lut, 4 * BUCKET_LUT_CELLS))) return rc;
-        k_build_bucket_lut<<<BUCKET_LUT_CELLS / 256, 256>>>(v, ends[0], inv_w, (uint32_t*)db->d_bucket_lut);
-        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(db->mem.alloc(&bucket_lut, BUCKET_LUT_CELLS));
+        LAUNCH(k_build_bucket_lut<<<BUCKET_LUT_CELLS / 256, 256, 0, st>>>(v, ends[0], inv_w, bucket_lut));
         v.blut_base = ends[0]; v.blut_inv_w = inv_w;
     }
     // precursor-mass LUT over peptides[].monoisotopic (sorted ascending; needs positive finite ends like the bucket LUT)
     float pe[2] = {0.f, 0.f};
-    CUDA_TRY(cudaMemcpy(&pe[0], db->d_pep_mono, 4, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&pe[1], (const float*)db->d_pep_mono + (v.n_pep - 1), 4, cudaMemcpyDeviceToHost));
+    if ((rc = read_back(st, &pe[0], v.pep_mono, 4))) return rc;
+    if ((rc = read_back(st, &pe[1], v.pep_mono + (v.n_pep - 1), 4))) return rc;
     const float pw = (pe[1] - pe[0]) / (float)PEP_LUT_CELLS;
     bool plut_ok = pe[0] > 0.0f && std::isfinite(pe[1]) && pw > 0.0f && pw < 3.0e38f;
     if (plut_ok) {   // only for a table the reference's binary search is well defined on: ascending, positive, finite
         DevArena A;
         uint32_t* d_bad = nullptr;
         uint32_t h_bad = 1;
-        CUDA_TRY(A.alloc(&d_bad, 1));
-        cudaMemset(d_bad, 0, 4);
-        k_check_ascending<<<(v.n_pep + 255) / 256, 256>>>(v.n_pep, (const float*)db->d_pep_mono, d_bad);
-        cudaMemcpy(&h_bad, d_bad, 4, cudaMemcpyDeviceToHost);
+        CUDA_TRY(A.zeros(&d_bad, 1, st));
+        LAUNCH_N(k_check_ascending, v.n_pep, st, v.n_pep, v.pep_mono, d_bad);
+        if ((rc = read_back(st, &h_bad, d_bad, 4))) return rc;
         plut_ok = h_bad == 0;
     }
     if (plut_ok) {
-        if ((rc = dmalloc(db, &db->d_pep_lut, 4 * (PEP_LUT_CELLS + 1)))) return rc;
-        k_build_pep_lut<<<(PEP_LUT_CELLS + 256) / 256, 256>>>(v, pe[0], 1.0f / pw, (uint32_t*)db->d_pep_lut);
-        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(db->mem.alloc(&pep_lut, PEP_LUT_CELLS + 1));
+        LAUNCH(k_build_pep_lut<<<(PEP_LUT_CELLS + 256) / 256, 256, 0, st>>>(v, pe[0], 1.0f / pw, pep_lut));
         v.plut_base = pe[0]; v.plut_inv_w = 1.0f / pw;
     }
-    CUDA_TRY(cudaDeviceSynchronize());
-    if (plut_ok) v.pep_lut = (const uint32_t*)db->d_pep_lut;
-    if (db->d_page_grid) v.page_grid = (const uint16_t*)db->d_page_grid;
-    if (lut_ok) v.bucket_lut = (const uint32_t*)db->d_bucket_lut;
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (plut_ok) v.pep_lut = pep_lut;
+    if (page_grid) v.page_grid = page_grid;
+    if (lut_ok) v.bucket_lut = bucket_lut;
     return 0;
 }
 
@@ -586,30 +593,30 @@ extern "C" int sage_b200_db_create(const sage_b200_peptides* peptides, const sag
     Guard<sage_b200_db> guard(nullptr, sage_b200_db_destroy);
     if (int rc = db_new(device, guard)) return rc;
     sage_b200_db* db = guard.get();
-    if (int rc = db_upload_peptides(db, peptides, index->ion_kinds, index->n_ion_kinds)) return rc;
+    Stream st;
+    CUDA_TRY(st.create());
+    if (int rc = db_upload_peptides(db, peptides, index->ion_kinds, index->n_ion_kinds, st)) return rc;
     const uint64_t nf = index->n_fragments;
     db->v.n_frag = nf;
     db->v.n_bucket = (uint32_t)index->n_buckets;
     db->v.bucket_size = (uint32_t)index->bucket_size;
-    if (int rc = dmalloc(db, &db->d_frag, 8 * nf + 64)) return rc;
-    if (int rc = dmalloc(db, &db->d_bucket_min, 4 * index->n_buckets)) return rc;
-    {
+    uint2* frag = nullptr;
+    float* bucket_min = nullptr;
+    CUDA_TRY(db->mem.alloc(&frag, nf + 8));
+    CUDA_TRY(db->mem.alloc(&bucket_min, index->n_buckets));
+    if (nf) {
         DevArena A;
-        if (nf) {
-            uint32_t* t_pep = nullptr;
-            float* t_mz = nullptr;
-            CUDA_TRY(A.alloc(&t_pep, nf));
-            CUDA_TRY(A.alloc(&t_mz, nf));
-            // these errors are not sticky: a later synchronize would not report them and the index would be garbage
-            CUDA_TRY(cudaMemcpy(t_pep, index->fragment_peptide, 4 * nf, cudaMemcpyHostToDevice));
-            CUDA_TRY(cudaMemcpy(t_mz, index->fragment_mz, 4 * nf, cudaMemcpyHostToDevice));
-            CUDA_TRY(cudaMemcpy(db->d_bucket_min, index->bucket_min, 4 * index->n_buckets, cudaMemcpyHostToDevice));
-            k_pack_fragments_soa<<<(unsigned)((nf + 255) / 256), 256>>>(nf, t_pep, t_mz, (uint2*)db->d_frag);
-        }
-        CUDA_TRY(cudaDeviceSynchronize());
+        uint32_t* t_pep = nullptr;
+        float* t_mz = nullptr;
+        // these errors are not sticky: a later synchronize would not report them and the index would be garbage
+        CUDA_TRY(A.upload(&t_pep, index->fragment_peptide, nf, st));
+        CUDA_TRY(A.upload(&t_mz, index->fragment_mz, nf, st));
+        CUDA_TRY(cudaMemcpyAsync(bucket_min, index->bucket_min, 4 * index->n_buckets, cudaMemcpyHostToDevice, st));
+        LAUNCH_N(k_pack_fragments_soa, nf, st, nf, t_pep, t_mz, frag);
+        CUDA_TRY(cudaStreamSynchronize(st));
     }
-    db->v.frag = (const uint2*)db->d_frag;
-    db->v.bucket_min = (const float*)db->d_bucket_min;
+    db->v.frag = frag;
+    db->v.bucket_min = bucket_min;
     // IndexedDatabase does not carry min_ion_index (it lives in Parameters, database.rs:128): infer it from the fragment count and
     // verify the index content against the ion table; only then may narrow windows be counted peptide-centrically.
     db->v.pep_centric_ok = 0;
@@ -626,29 +633,29 @@ extern "C" int sage_b200_db_create(const sage_b200_peptides* peptides, const sag
             if (tot == nf) found = (int)m;
             if (tot < nf) break;
         }
-        if (found >= 0) {   // any failure here only leaves the peptide-centric path off
-            DevArena A;
-            uint32_t *acc = nullptr, *mis = nullptr;
-            uint32_t mismatch = 1;
-            if (A.alloc(&acc, 2 * n) == cudaSuccess && A.alloc(&mis, 1) == cudaSuccess && cudaMemset(acc, 0, 8 * n) == cudaSuccess &&
-                cudaMemset(mis, 0, 4) == cudaSuccess) {
-                k_index_signature<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, (uint32_t)n, acc);
-                k_index_verify<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, db->v.pep_len, db->v.ion_off, db->v.ions, db->v.n_kinds, db->v, (uint32_t)found,
-                                                                    acc, mis);
-                if (cudaMemcpy(&mismatch, mis, 4, cudaMemcpyDeviceToHost) != cudaSuccess) mismatch = 1;
-            }
-            cudaGetLastError();
-            if (mismatch == 0) { db->v.min_ion_index = (uint32_t)found; db->v.pep_centric_ok = 1; }
+        uint32_t mismatch = 1;
+        if (found >= 0 && optional_work([&] {   // any failure here only leaves the peptide-centric path off
+                DevArena A;
+                uint32_t *acc = nullptr, *mis = nullptr;
+                CUDA_TRY(A.zeros(&acc, 2 * n, st));
+                CUDA_TRY(A.zeros(&mis, 1, st));
+                LAUNCH_N(k_index_signature, nf, st, nf, db->v.frag, (uint32_t)n, acc);
+                LAUNCH(k_index_verify<<<(unsigned)((n + 127) / 128), 128, 0, st>>>((uint32_t)n, db->v.pep_len, db->v.ion_off, db->v.ions, db->v.n_kinds, db->v,
+                                                                                  (uint32_t)found, acc, mis));
+                return read_back(st, &mismatch, mis, 4);
+            }) && mismatch == 0) {
+            db->v.min_ion_index = (uint32_t)found;
+            db->v.pep_centric_ok = 1;
         }
     }
-    if (int rc = db_build_directories(db)) return rc;
+    if (int rc = db_build_directories(db, st)) return rc;
     *out = guard.release();
     return 0;
 }
 
 // The fragment index of a db whose ion tables are built: fragments kept per peptide at d_off (u64, n + 1; nf in all), the global sort by
-// fragment m/z, bucketing, the per-bucket sort by PeptideIx and the search directories (database.rs:281-365).
-static int db_build_fragments(sage_b200_db* db, const uint64_t* d_off, uint64_t nf, uint64_t bucket_size, uint64_t min_ion_index) {
+// fragment m/z, bucketing, the per-bucket sort by PeptideIx and the search directories (database.rs:281-365), all on st.
+static int db_build_fragments(sage_b200_db* db, const uint64_t* d_off, uint64_t nf, uint64_t bucket_size, uint64_t min_ion_index, cudaStream_t st) {
     const uint64_t n = db->v.n_pep;
     const uint32_t shift = ceil_log2_u64(bucket_size);
     const uint64_t nb = (nf + bucket_size - 1) / bucket_size;
@@ -658,10 +665,12 @@ static int db_build_fragments(sage_b200_db* db, const uint64_t* d_off, uint64_t 
     db->v.bucket_size = (uint32_t)bucket_size;
     db->v.min_ion_index = (uint32_t)std::min<uint64_t>(min_ion_index, 0xFFFFFFFFull);
     db->v.pep_centric_ok = 1;  // the index is generated from the ion table with this filter by construction
-    if (int rc = dmalloc(db, &db->d_frag, 8 * nf + 64)) return rc;
-    if (int rc = dmalloc(db, &db->d_bucket_min, 4 * nb)) return rc;
-    db->v.frag = (const uint2*)db->d_frag;
-    db->v.bucket_min = (const float*)db->d_bucket_min;
+    uint2* frag = nullptr;
+    float* bucket_min = nullptr;
+    CUDA_TRY(db->mem.alloc(&frag, nf + 8));
+    CUDA_TRY(db->mem.alloc(&bucket_min, nb));
+    db->v.frag = frag;
+    db->v.bucket_min = bucket_min;
     if (nf == 0) return 0;
     if (nf > 0x7FFFFFFFull) return fail(SAGE_B200_ELIMIT, "more than 2^31 fragments: sort in slabs not implemented");
 
@@ -674,27 +683,25 @@ static int db_build_fragments(sage_b200_db* db, const uint64_t* d_off, uint64_t 
             DevArena S;
             uint32_t *k32a = nullptr, *pa = nullptr;
             CUDA_TRY(S.alloc(&k32a, nf)); CUDA_TRY(S.alloc(&pa, nf));
-            k_gen_fragments<<<(unsigned)((n + 127) / 128), 128>>>((uint32_t)n, db->v.pep_len, db->v.ion_off, db->v.ions, db->v.n_kinds, db->v, (uint32_t)std::min<uint64_t>(min_ion_index, 0xFFFFFFFFull),
-                                                                  nullptr, d_off, k32a, pa);
-            CUDA_TRY(cudaGetLastError());
-            CUDA_TRY(S.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint32_t*)k32a, k32b, (const uint32_t*)pa, pb, (int)nf); },
+            LAUNCH(k_gen_fragments<<<(unsigned)((n + 127) / 128), 128, 0, st>>>((uint32_t)n, db->v.pep_len, db->v.ion_off, db->v.ions, db->v.n_kinds, db->v,
+                                                                               (uint32_t)std::min<uint64_t>(min_ion_index, 0xFFFFFFFFull), nullptr, d_off, k32a, pa));
+            CUDA_TRY(S.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint32_t*)k32a, k32b, (const uint32_t*)pa, pb, (int)nf, 0, 32, st); },
                                  16));
+            CUDA_TRY(cudaStreamSynchronize(st));
         }
         // (2) bucket minima + (bucket, PeptideIx) keys, then a stable sort inside buckets (database.rs:337-346)
         uint64_t *k64a = nullptr, *k64b = nullptr;
         uint32_t *mza = nullptr, *mzb = nullptr;
         CUDA_TRY(A.alloc(&k64a, nf)); CUDA_TRY(A.alloc(&k64b, nf));
         CUDA_TRY(A.alloc(&mza, nf)); CUDA_TRY(A.alloc(&mzb, nf));
-        k_bucket_keys<<<(unsigned)((nf + 255) / 256), 256>>>(nf, shift, k32b, pb, k64a, mza, (float*)db->d_bucket_min);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH_N(k_bucket_keys, nf, st, nf, shift, k32b, pb, k64a, mza, bucket_min);
         const int end_bit = std::min<int>(64, 32 + (int)ceil_log2_u64(nb + 1) + 1);
-        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)k64a, k64b, (const uint32_t*)mza, mzb, (int)nf, 0, end_bit); },
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)k64a, k64b, (const uint32_t*)mza, mzb, (int)nf, 0, end_bit, st); },
                              16));
-        k_pack_fragments<<<(unsigned)((nf + 255) / 256), 256>>>(nf, k64b, mzb, (uint2*)db->d_frag);
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaDeviceSynchronize());
+        LAUNCH_N(k_pack_fragments, nf, st, nf, k64b, mzb, frag);
+        CUDA_TRY(cudaStreamSynchronize(st));
     }
-    return db_build_directories(db);
+    return db_build_directories(db, st);
 }
 
 static int db_check_bucket_size(uint64_t bucket_size) {
@@ -710,10 +717,14 @@ extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t b
     Guard<sage_b200_db> guard(nullptr, sage_b200_db_destroy);
     if (int rc = db_new(device, guard)) return rc;
     sage_b200_db* db = guard.get();
-    if (int rc = db_upload_peptides(db, peptides, ion_kinds, n_ion_kinds)) return rc;
+    std::vector<uint64_t> frag_off;
+    DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
+    if (int rc = db_upload_peptides(db, peptides, ion_kinds, n_ion_kinds, st)) return rc;
     const uint64_t n = peptides->n_peptides;
     // fragments kept per peptide: n_kinds * max(0, L-1-min_ion_index)   (database.rs:281-291)
-    std::vector<uint64_t> frag_off(n + 1);
+    frag_off.resize(n + 1);
     uint64_t nf = 0;
     for (uint64_t i = 0; i < n; i++) {
         frag_off[i] = nf;
@@ -722,11 +733,9 @@ extern "C" int sage_b200_db_build(const sage_b200_peptides* peptides, uint64_t b
         nf += n_ion_kinds * keep;
     }
     frag_off[n] = nf;
-    DevArena A;
     uint64_t* d_off = nullptr;
-    CUDA_TRY(A.alloc(&d_off, n + 1));
-    CUDA_TRY(cudaMemcpy(d_off, frag_off.data(), 8 * (n + 1), cudaMemcpyHostToDevice));
-    if (int rc = db_build_fragments(db, d_off, nf, bucket_size, min_ion_index)) return rc;
+    CUDA_TRY(A.upload(&d_off, frag_off.data(), n + 1, st));
+    if (int rc = db_build_fragments(db, d_off, nf, bucket_size, min_ion_index, st)) return rc;
     *out = guard.release();
     return 0;
 }
@@ -752,33 +761,35 @@ static int db_build_device(const DevTable& T, uint64_t bucket_size, const uint8_
     if (T.n >= 0xFFFFFFFEull) return fail(SAGE_B200_ELIMIT, "too many peptides for u32 PeptideIx");
     const uint64_t n = T.n;
     db->total_residues = T.n_res;
-    if (int rc = db_alloc_peptides(db, n)) return rc;
+    PeptideArrays p;
+    if (int rc = db_alloc_peptides(db, n, p)) return rc;
     DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
     uint64_t *d_nion = nullptr, *d_ion_off = nullptr, *d_nfrag = nullptr, *d_frag_off = nullptr;
     uint32_t* d_bad = nullptr;
-    CUDA_TRY(A.zeros(&d_nion, n + 1, 0));
-    CUDA_TRY(A.zeros(&d_nfrag, n + 1, 0));
+    CUDA_TRY(A.zeros(&d_nion, n + 1, st));
+    CUDA_TRY(A.zeros(&d_nfrag, n + 1, st));
     CUDA_TRY(A.alloc(&d_ion_off, n + 1));
     CUDA_TRY(A.alloc(&d_frag_off, n + 1));
-    CUDA_TRY(A.zeros(&d_bad, 1, 0));
-    LAUNCH_N(k_pf_pep_meta, n, 0, T.res_off, T.decoy, (uint32_t)n, (uint32_t)n_kinds, min_ion_index, (uint8_t*)db->d_pep_len, (uint8_t*)db->d_pep_flags,
-             d_nion, d_nfrag, d_bad);
-    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nion, d_ion_off, (int)(n + 1)); }));
-    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nfrag, d_frag_off, (int)(n + 1)); }));
+    CUDA_TRY(A.zeros(&d_bad, 1, st));
+    LAUNCH_N(k_pf_pep_meta, n, st, T.res_off, T.decoy, (uint32_t)n, (uint32_t)n_kinds, min_ion_index, p.len, p.flags, d_nion, d_nfrag, d_bad);
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nion, d_ion_off, (int)(n + 1), st); }));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, d_nfrag, d_frag_off, (int)(n + 1), st); }));
     uint64_t tail[2] = {0, 0};
     uint32_t bad = 0;
-    CUDA_TRY(cudaMemcpy(&tail[0], d_ion_off + n, 8, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&tail[1], d_frag_off + n, 8, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(&bad, d_bad, 4, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpyAsync(&tail[0], d_ion_off + n, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&tail[1], d_frag_off + n, 8, cudaMemcpyDeviceToHost, st));
+    if (int rc = read_back(st, &bad, d_bad, 4)) return rc;
     if (bad) return fail(SAGE_B200_ELIMIT, "a peptide has length 0 or over 255 (supported 1..255)");
     if (tail[0] > 0xFFFFFFFFull) return fail(SAGE_B200_ELIMIT, "ion table exceeds 2^32 entries");
-    LAUNCH_N(k_dg_u64_to_u32, n + 1, 0, d_ion_off, n + 1, (uint32_t*)db->d_ion_off);
+    LAUNCH_N(k_dg_u64_to_u32, n + 1, st, d_ion_off, n + 1, p.ion_off);
     if (n) {
-        CUDA_TRY(cudaMemcpy(db->d_pep_mono, T.mono, 4 * n, cudaMemcpyDeviceToDevice));
-        CUDA_TRY(cudaMemcpy(db->d_pep_missed, T.missed, n, cudaMemcpyDeviceToDevice));
+        CUDA_TRY(cudaMemcpyAsync(p.mono, T.mono, 4 * n, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(p.missed, T.missed, n, cudaMemcpyDeviceToDevice, st));
     }
-    if (int rc = db_build_ions(db, n, tail[0], T.res_off, T.seq, T.mods, T.nterm)) return rc;
-    if (int rc = db_build_fragments(db, d_frag_off, tail[1], bucket_size, min_ion_index)) return rc;
+    if (int rc = db_build_ions(db, n, tail[0], T.res_off, T.seq, T.mods, T.nterm, st)) return rc;
+    if (int rc = db_build_fragments(db, d_frag_off, tail[1], bucket_size, min_ion_index, st)) return rc;
     *out = guard.release();
     return 0;
 }
@@ -789,7 +800,7 @@ extern "C" int sage_b200_db_get_info(const sage_b200_db* db, sage_b200_db_info* 
     info->n_ion_kinds = db->v.n_kinds; info->total_residues = db->total_residues; info->device = db->device;
     {   // + the lazily built block-major copies (open search / narrow search), as far as they exist now
         std::lock_guard<std::mutex> lock(db->wmu);
-        info->device_bytes = db->device_bytes + db->wide.bytes + db->narrow.bytes + db->wide.retired_bytes + db->narrow.retired_bytes;
+        info->device_bytes = db->mem.bytes + db->wide.bytes + db->narrow.bytes + db->wide.retired_bytes + db->narrow.retired_bytes;
     }
     return 0;
 }
@@ -797,48 +808,50 @@ extern "C" int sage_b200_db_get_info(const sage_b200_db* db, sage_b200_db_info* 
 extern "C" int sage_b200_db_export_index(const sage_b200_db* db, uint32_t* fragment_peptide, float* fragment_mz, float* bucket_min) {
     if (!db) return fail(SAGE_B200_EINVAL, "db_export_index: null db");
     CUDA_TRY(cudaSetDevice(db->device));
+    DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
     const uint64_t nf = db->v.n_frag;
     if (nf && (fragment_peptide || fragment_mz)) {
-        DevArena A;
         uint32_t* t_pep = nullptr;
         float* t_mz = nullptr;
         CUDA_TRY(A.alloc(&t_pep, nf));
         CUDA_TRY(A.alloc(&t_mz, nf));
-        k_unpack_fragments<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, t_pep, t_mz);
-        CUDA_TRY(cudaDeviceSynchronize());
-        if (fragment_peptide) CUDA_TRY(cudaMemcpy(fragment_peptide, t_pep, 4 * nf, cudaMemcpyDeviceToHost));
-        if (fragment_mz) CUDA_TRY(cudaMemcpy(fragment_mz, t_mz, 4 * nf, cudaMemcpyDeviceToHost));
+        LAUNCH_N(k_unpack_fragments, nf, st, nf, db->v.frag, t_pep, t_mz);
+        if (fragment_peptide) CUDA_TRY(cudaMemcpyAsync(fragment_peptide, t_pep, 4 * nf, cudaMemcpyDeviceToHost, st));
+        if (fragment_mz) CUDA_TRY(cudaMemcpyAsync(fragment_mz, t_mz, 4 * nf, cudaMemcpyDeviceToHost, st));
     }
-    if (bucket_min && db->v.n_bucket) CUDA_TRY(cudaMemcpy(bucket_min, db->d_bucket_min, 4ull * db->v.n_bucket, cudaMemcpyDeviceToHost));
+    if (bucket_min && db->v.n_bucket) CUDA_TRY(cudaMemcpyAsync(bucket_min, db->v.bucket_min, 4ull * db->v.n_bucket, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 
 // Both block-major copies of the fragments start alike: fragments keyed by (PeptideIx / block, m/z), one LSD radix sort, block offsets, and
-// the m/z range of the index. On success *keys / *peps hold the sorted keys and PeptideIx; every temporary is in A.
-static bool sort_block_major(const sage_b200_db* db, DevArena& A, uint32_t block, uint32_t n_block, uint64_t* blk_off, uint64_t** keys, uint32_t** peps,
-                             float& lo, float& hi) {
+// the m/z range of the index, on st. On success *keys / *peps hold the sorted keys and PeptideIx; every temporary is in A.
+static int sort_block_major(const sage_b200_db* db, DevArena& A, cudaStream_t st, uint32_t block, uint32_t n_block, uint64_t* blk_off, uint64_t** keys,
+                            uint32_t** peps, float& lo, float& hi) {
     const uint64_t nf = db->v.n_frag;
-    if (nf > 0x7FFFFFFFull) return false;
+    if (nf > 0x7FFFFFFFull) return fail(SAGE_B200_ELIMIT, "more than 2^31 fragments");
     uint64_t* k_a = nullptr;
     uint32_t *p_a = nullptr, *d_rng = nullptr;
-    if (A.alloc(&k_a, nf) != cudaSuccess || A.alloc(keys, nf) != cudaSuccess || A.alloc(&p_a, nf) != cudaSuccess || A.alloc(peps, nf) != cudaSuccess ||
-        A.alloc(&d_rng, 2) != cudaSuccess)
-        return false;
-    k_wide_keys<<<(unsigned)((nf + 255) / 256), 256>>>(nf, db->v.frag, block, k_a, p_a);
+    CUDA_TRY(A.alloc(&k_a, nf));
+    CUDA_TRY(A.alloc(keys, nf));
+    CUDA_TRY(A.alloc(&p_a, nf));
+    CUDA_TRY(A.alloc(peps, nf));
+    LAUNCH_N(k_wide_keys, nf, st, nf, db->v.frag, block, k_a, p_a);
     int nb_bits = 1;
     while (nb_bits < 32 && (n_block >> nb_bits)) nb_bits++;
-    if (A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)k_a, *keys, (const uint32_t*)p_a, *peps, (int)nf, 0, 32 + nb_bits); },
-                    16) != cudaSuccess)
-        return false;
-    k_wide_block_offsets<<<(n_block + 1 + 255) / 256, 256>>>(nf, *keys, n_block, blk_off);
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)k_a, *keys, (const uint32_t*)p_a, *peps, (int)nf, 0, 32 + nb_bits, st); },
+                         16));
+    LAUNCH_N(k_wide_block_offsets, (uint64_t)n_block + 1, st, nf, *keys, n_block, blk_off);
     // m/z range of the index (positive floats order like their bit patterns)
     const uint32_t rng0[2] = {0xFFFFFFFFu, 0u};
-    if (cudaMemcpy(d_rng, rng0, 8, cudaMemcpyHostToDevice) != cudaSuccess) return false;
-    k_frag_mz_range<<<(unsigned)std::min<uint64_t>((nf + 255) / 256, 4096), 256>>>(nf, db->v.frag, d_rng);
+    CUDA_TRY(A.upload(&d_rng, rng0, 2, st));
+    LAUNCH(k_frag_mz_range<<<(unsigned)std::min<uint64_t>((nf + 255) / 256, 4096), 256, 0, st>>>(nf, db->v.frag, d_rng));
     uint32_t rng[2];
-    if (cudaMemcpy(rng, d_rng, 8, cudaMemcpyDeviceToHost) != cudaSuccess) return false;
+    if (int rc = read_back(st, rng, d_rng, 8)) return rc;
     memcpy(&lo, &rng[0], 4); memcpy(&hi, &rng[1], 4);
-    return true;
+    return 0;
 }
 
 // Directory cells of `cells` equal m/z steps over [lo, hi] (the same for every block): base and inverse width, or inv_w = 0 (every walk
@@ -858,32 +871,32 @@ static WideIndexView build_wide_index(const sage_b200_db* db, BlockIndexSlot<Wid
     if (slot.v.frag != nullptr && slot.v.block == block) return slot.v;
     if (slot.failed || block == 0 || db->v.n_frag == 0 || db->v.n_pep == 0) return WideIndexView{};
     const uint64_t nf = db->v.n_frag;
-    slot.retire();   // a rebuild with another block size (tests, scorers with very different tolerances): see BlockIndexSlot::retire
-    DevArena A;
-    uint64_t* keys = nullptr;
-    uint32_t* peps = nullptr;
-    auto give_up = [&]() { slot.free_current(); cudaGetLastError(); slot.failed = 1; return WideIndexView{}; };
     const uint32_t n_block = (db->v.n_pep + block - 1) / block;
     while (cells > 256 && (uint64_t)n_block * (cells + 1) * 4 > (1024ull << 20)) cells >>= 1;   // at most 1 GB of LUT
-    void *&d_frag = slot.d[0], *&d_blk = slot.d[1], *&d_lut = slot.d[2];
-    if (cudaMalloc(&d_frag, 8 * nf + 64) != cudaSuccess || cudaMalloc(&d_blk, 8 * ((size_t)n_block + 1)) != cudaSuccess ||
-        cudaMalloc(&d_lut, 4 * (size_t)n_block * (cells + 1)) != cudaSuccess)
-        return give_up();
-    float lo, hi;
-    if (!sort_block_major(db, A, block, n_block, (uint64_t*)d_blk, &keys, &peps, lo, hi)) return give_up();
-    k_wide_pack<<<(unsigned)((nf + 255) / 256), 256>>>(nf, keys, peps, (uint2*)d_frag);
-    WideIndexView w{};
-    w.frag = (const uint2*)d_frag; w.blk_off = (const uint64_t*)d_blk; w.lut = (const uint32_t*)d_lut;
-    w.block = block; w.n_block = n_block;
-    set_mz_cells(w, lo, hi, cells);
-    if (w.inv_w > 0.0f) {
+    // a rebuild with another block size (tests, scorers with very different tolerances): see BlockIndexSlot::retire
+    return slot.rebuild([&](DevArena& mem, WideIndexView& w, uint64_t& bytes) -> int {
+        DevArena A;
+        Stream st;
+        CUDA_TRY(st.create());
+        uint2* frag = nullptr;
+        uint64_t *blk = nullptr, *keys = nullptr;
+        uint32_t *lut = nullptr, *peps = nullptr;
+        CUDA_TRY(mem.alloc(&frag, nf + 8));
+        CUDA_TRY(mem.alloc(&blk, (uint64_t)n_block + 1));
+        CUDA_TRY(mem.alloc(&lut, (uint64_t)n_block * (cells + 1)));
+        float lo, hi;
+        if (int rc = sort_block_major(db, A, st, block, n_block, blk, &keys, &peps, lo, hi)) return rc;
+        LAUNCH_N(k_wide_pack, nf, st, nf, keys, peps, frag);
+        w.frag = frag; w.blk_off = blk; w.lut = lut;
+        w.block = block; w.n_block = n_block;
+        set_mz_cells(w, lo, hi, cells);
         const uint64_t total = (uint64_t)n_block * (cells + 1);
-        k_wide_lut<<<(unsigned)((total + 255) / 256), 256>>>(w, (uint32_t*)d_lut);
-    } else if (cudaMemset(d_lut, 0, 4 * (size_t)n_block * (cells + 1)) != cudaSuccess) return give_up();   // degenerate range: every walk starts at the block start
-    if (cudaDeviceSynchronize() != cudaSuccess) return give_up();
-    slot.v = w;
-    slot.bytes = 8 * nf + 8 * ((uint64_t)n_block + 1) + 4ull * n_block * (cells + 1);
-    return w;
+        if (w.inv_w > 0.0f) LAUNCH_N(k_wide_lut, total, st, w, lut);
+        else CUDA_TRY(cudaMemsetAsync(lut, 0, 4 * total, st));   // degenerate range: every walk starts at the block start
+        CUDA_TRY(cudaStreamSynchronize(st));
+        bytes = 8 * nf + 8 * ((uint64_t)n_block + 1) + 4ull * n_block * (cells + 1);
+        return 0;
+    });
 }
 
 static WideIndexView db_wide_index(const sage_b200_db* db, uint32_t block) {
@@ -918,31 +931,33 @@ static NarrowIndexView db_narrow_index(const sage_b200_db* db, uint32_t block, b
     if (slot.v.mz != nullptr && (slot.v.block == block || (!exact && slot.v.block * 2 >= block && slot.v.block <= block * 2))) return slot.v;
     if (slot.failed || block == 0 || block > 65536 || db->v.n_frag == 0 || db->v.n_pep == 0) return NarrowIndexView{};
     const uint64_t nf = db->v.n_frag;
-    slot.retire();
-    DevArena A;
-    uint64_t* keys = nullptr;
-    uint32_t* peps = nullptr;
-    auto give_up = [&]() { slot.free_current(); cudaGetLastError(); slot.failed = 1; return NarrowIndexView{}; };
     const uint32_t n_block = (db->v.n_pep + block - 1) / block;
     const uint32_t cells = narrow_dir_cells(nf, n_block), ngrp = cells / NARROW_GROUP;
-    void *&d_mz = slot.d[0], *&d_pep = slot.d[1], *&d_blk = slot.d[2], *&d_dir = slot.d[3], *&d_grp = slot.d[4];
-    if (cudaMalloc(&d_mz, 4 * nf + 64) != cudaSuccess || cudaMalloc(&d_pep, 2 * nf + 64) != cudaSuccess ||
-        cudaMalloc(&d_blk, 8 * ((size_t)n_block + 1)) != cudaSuccess || cudaMalloc(&d_dir, 2 * (size_t)n_block * cells) != cudaSuccess ||
-        cudaMalloc(&d_grp, 4 * (size_t)n_block * ngrp) != cudaSuccess)
-        return give_up();
-    float lo, hi;
-    if (!sort_block_major(db, A, block, n_block, (uint64_t*)d_blk, &keys, &peps, lo, hi)) return give_up();
-    k_narrow_pack<<<(unsigned)((nf + 255) / 256), 256>>>(nf, keys, peps, block, (float*)d_mz, (uint16_t*)d_pep);
-    NarrowIndexView v{};
-    v.mz = (const float*)d_mz; v.pep = (const uint16_t*)d_pep; v.blk_off = (const uint64_t*)d_blk; v.dir = (const uint16_t*)d_dir;
-    v.grp = (const uint32_t*)d_grp; v.block = block; v.n_block = n_block;
-    set_mz_cells(v, lo, hi, cells);
-    const uint64_t total = (uint64_t)n_block * cells;
-    k_narrow_dir<<<(unsigned)((total + 255) / 256), 256>>>(v, (uint16_t*)d_dir, (uint32_t*)d_grp);
-    if (cudaDeviceSynchronize() != cudaSuccess) return give_up();
-    slot.v = v;
-    slot.bytes = 6 * nf + 128 + 8 * ((uint64_t)n_block + 1) + 2 * total + 4ull * n_block * ngrp;
-    return v;
+    return slot.rebuild([&](DevArena& mem, NarrowIndexView& v, uint64_t& bytes) -> int {
+        DevArena A;
+        Stream st;
+        CUDA_TRY(st.create());
+        float* mz = nullptr;
+        uint16_t *pep = nullptr, *dir = nullptr;
+        uint64_t *blk = nullptr, *keys = nullptr;
+        uint32_t *grp = nullptr, *peps = nullptr;
+        const uint64_t total = (uint64_t)n_block * cells;
+        CUDA_TRY(mem.alloc(&mz, nf + 16));
+        CUDA_TRY(mem.alloc(&pep, nf + 32));
+        CUDA_TRY(mem.alloc(&blk, (uint64_t)n_block + 1));
+        CUDA_TRY(mem.alloc(&dir, total));
+        CUDA_TRY(mem.alloc(&grp, (uint64_t)n_block * ngrp));
+        float lo, hi;
+        if (int rc = sort_block_major(db, A, st, block, n_block, blk, &keys, &peps, lo, hi)) return rc;
+        LAUNCH_N(k_narrow_pack, nf, st, nf, keys, peps, block, mz, pep);
+        v.mz = mz; v.pep = pep; v.blk_off = blk; v.dir = dir;
+        v.grp = grp; v.block = block; v.n_block = n_block;
+        set_mz_cells(v, lo, hi, cells);
+        LAUNCH_N(k_narrow_dir, total, st, v, dir, grp);
+        CUDA_TRY(cudaStreamSynchronize(st));
+        bytes = mem.bytes;
+        return 0;
+    });
 }
 
 // Dynamic shared-memory opt-in of the kernels that need more than 48 KB: set ONCE per device to the device maximum (the attribute is per-function,
@@ -1156,6 +1171,7 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
     if (const char* e = getenv("SAGE_B200_WIDE_VARIANT")) v.wide_variant = (uint32_t)atoi(e);
     v.pep_cap = 0;   // peptide-centric counting of small windows is opt-in: with the dense page grid the index path won on cfg2 at every cap tried
     if (const char* e = getenv("SAGE_B200_PEP_CAP")) v.pep_cap = (uint32_t)std::min<long>(std::max<long>(atol(e), 0), (long)NARROW_CAP);
+    for (Lane& L : s->lanes) CUDA_TRY(L.create());
     {   // lnfact table with the host libm (the reference's f64::ln): Stirling form of scoring.rs:170-177
         const uint32_t N = 4096;
         std::vector<double> tab(N);
@@ -1165,7 +1181,8 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
             tab[n] = x * std::log(x) - x + 0.5 * std::log(x) + 0.5 * std::log(3.14159265358979323846 * 2.0 * x);
         }
         if (int rc = s->d_lnfact.reserve(8 * N)) return rc;
-        CUDA_TRY(cudaMemcpy(s->d_lnfact.p, tab.data(), 8 * N, cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpyAsync(s->d_lnfact.p, tab.data(), 8 * N, cudaMemcpyHostToDevice, s->lanes[0].stream));
+        CUDA_TRY(cudaStreamSynchronize(s->lanes[0].stream));   // both lanes read the table
         v.lnfact_tab = s->d_lnfact.as<double>();
         v.lnfact_n = N;
     }
@@ -1173,7 +1190,6 @@ extern "C" int sage_b200_scorer_create(const sage_b200_db* db, const sage_b200_s
     v.score_fast = 1;
     if (const char* e = getenv("SAGE_B200_SCORE_FAST")) v.score_fast = atoi(e) != 0;
     if (const char* e = getenv("SAGE_B200_SORT")) s->sort_spectra = atoi(e);
-    for (Lane& L : s->lanes) CUDA_TRY(L.create());
     if (const char* e = getenv("SAGE_B200_PIPELINE_CHUNKS")) s->pipeline_chunks = std::max(1, atoi(e));
     if (const char* e = getenv("SAGE_B200_TRACE")) s->trace = e[0] == '1';
     if (const char* e = getenv("SAGE_B200_SCORE_SPLIT")) s->score_split = atoi(e) != 0;
@@ -1250,16 +1266,17 @@ static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 // Peptides per block of the narrow-search copy of the index: the power of two at or above the average precursor window of this scorer
 // (sampled on the device from the peptide masses themselves), 128..4096. A probe then reads one or two short m/z runs. Chosen by A/B of the
 // counting kernels on cfg2 (windows ~180 peptides: 256 best) and cfg3 (windows ~1500: 2048 best), both well ahead of the page index.
+// The sample runs on lane 0's kernel stream.
 static int narrow_block_for(sage_b200_scorer* S) {
     if (S->narrow_block_auto) return 0;
     const uint32_t samples = 4096;
+    cudaStream_t st = S->lanes[0].stream;
     DevArena A;
     unsigned long long* d_sum = nullptr;
     unsigned long long sum = 0;
-    CUDA_TRY(A.alloc(&d_sum, 1));
-    CUDA_TRY(cudaMemset(d_sum, 0, 8));
-    k_window_sample<<<(samples + 255) / 256, 256>>>(S->db->v, S->sv.precursor_tol, samples, d_sum);
-    CUDA_TRY(cudaMemcpy(&sum, d_sum, 8, cudaMemcpyDeviceToHost));
+    CUDA_TRY(A.zeros(&d_sum, 1, st));
+    LAUNCH_N(k_window_sample, samples, st, S->db->v, S->sv.precursor_tol, samples, d_sum);
+    if (int rc = read_back(st, &sum, d_sum, 8)) return rc;
     const double avg = (double)sum / samples;
     uint32_t block = 128;
     while (block < 4096 && (double)block < avg) block <<= 1;
@@ -1432,6 +1449,16 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
         if ((rc = L.d_dbgk.reserve((size_t)n * sv.kparam * 8))) return rc;
         if ((rc = L.d_dbgm.reserve((size_t)n * 16))) return rc;
     }
+    // the small-block copy of the index: built on first use, before this chunk queues
+    // anything (narrow_block_for waits for lane 0's kernel stream); never for wide-window (DIA) scorers
+    // (nor for open-search tolerances, whose windows exceed the warp kernel's cap: the copy would only cost memory)
+    const float ptol_span = std::max(std::fabs(sv.precursor_tol.lo), std::fabs(sv.precursor_tol.hi));
+    const bool narrow_tol = ptol_span <= (sv.precursor_tol.kind == 0 ? 2000.0f : sv.precursor_tol.kind == 1 ? 0.2f : 5.0f);   // ppm / percent / Da
+    NarrowIndexView nv{};
+    if (S->narrow_index && !sv.wide_window && narrow_tol) {
+        if (S->narrow_block == 0 && (rc = narrow_block_for(S))) return rc;
+        nv = db_narrow_index(db, S->narrow_block ? S->narrow_block : S->narrow_block_auto, S->narrow_block != 0);
+    }
     BatchView bv{};
     unsigned char* ds = (unsigned char*)L.d_small.p;
     bv.n = n;
@@ -1503,8 +1530,7 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
     bv.wide_items = L.d_witems.as<uint32_t>();
     bv.wide_cap = C.wide_cap;
     bv.nlist_cap = C.nlist_cap;
-    k_setup_queries<<<(n + 127) / 128, 128, 0, st>>>(db->v, svq, bv, sk_in, sv_in);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_setup_queries<<<(n + 127) / 128, 128, 0, st>>>(db->v, svq, bv, sk_in, sv_in));
     if (sk_in) {
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(L.d_sorttmp.p, sort_tmp, sk_in, sk_out, sv_in, sv_out, (int)n, sort_lo, sort_bits, st));
         bv.order = sv_out;
@@ -1515,50 +1541,34 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
 
     // ---- preliminary scoring. Both kernels are always queued: CTAs whose query belongs to the other kernel (or to nobody) exit at once.
     const size_t rsm = (size_t)sv.kparam * REPLAY_THREADS * 8;
-    // the small-block copy of the index: built on first use; never for wide-window (DIA) scorers
-    // (nor for open-search tolerances, whose windows exceed the warp kernel's cap: the copy would only cost memory)
-    const float ptol_span = std::max(std::fabs(sv.precursor_tol.lo), std::fabs(sv.precursor_tol.hi));
-    const bool narrow_tol = ptol_span <= (sv.precursor_tol.kind == 0 ? 2000.0f : sv.precursor_tol.kind == 1 ? 0.2f : 5.0f);   // ppm / percent / Da
-    NarrowIndexView nv{};
-    if (S->narrow_index && !sv.wide_window && narrow_tol) {
-        if (S->narrow_block == 0 && (rc = narrow_block_for(S))) return rc;
-        nv = db_narrow_index(db, S->narrow_block ? S->narrow_block : S->narrow_block_auto, S->narrow_block != 0);
-    }
     for (uint32_t q = 0; q < C.nparts; q++) {   // one launch per part of the masses copy (a resident batch has one part)
         if (C.nparts > 1) CUDA_TRY(cudaStreamWaitEvent(st, L.ev_part[q], 0));
         const dim3 wgrid((n + WARPQ_WARPS - 1) / WARPQ_WARPS, sv.qmax);
-        if (nv.mz != nullptr) k_prelim_narrow_warp<true><<<wgrid, WARPQ_WARPS * 32, 0, st>>>(db->v, svq, bv, L.d_nlist.as<uint64_t>(), C.part_lo[q], C.part_lo[q + 1], nv);
-        else k_prelim_narrow_warp<false><<<wgrid, WARPQ_WARPS * 32, 0, st>>>(db->v, svq, bv, L.d_nlist.as<uint64_t>(), C.part_lo[q], C.part_lo[q + 1], nv);
-        CUDA_TRY(cudaGetLastError());
+        if (nv.mz != nullptr) LAUNCH(k_prelim_narrow_warp<true><<<wgrid, WARPQ_WARPS * 32, 0, st>>>(db->v, svq, bv, L.d_nlist.as<uint64_t>(), C.part_lo[q], C.part_lo[q + 1], nv));
+        else LAUNCH(k_prelim_narrow_warp<false><<<wgrid, WARPQ_WARPS * 32, 0, st>>>(db->v, svq, bv, L.d_nlist.as<uint64_t>(), C.part_lo[q], C.part_lo[q + 1], nv));
         launches += q > 0;
     }
     if (C.nparts > 1) CUDA_TRY(cudaStreamWaitEvent(st, L.ev_masses, 0));
-    k_prelim_narrow<<<(unsigned)std::min<uint64_t>(C.nitems, (uint64_t)db->sm_count * PRELIM_CTAS), PRELIM_THREADS, pep_smem, st>>>(db->v, svq, bv, C.pmax, L.d_nlist.as<uint64_t>(),
-                                                                                                                         S->narrow_cta ? nv : NarrowIndexView{});
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_prelim_narrow<<<(unsigned)std::min<uint64_t>(C.nitems, (uint64_t)db->sm_count * PRELIM_CTAS), PRELIM_THREADS, pep_smem, st>>>(
+        db->v, svq, bv, C.pmax, L.d_nlist.as<uint64_t>(), S->narrow_cta ? nv : NarrowIndexView{}));
     // the rare queries with >= 2^16 matches, listed by both counting kernels: exact wrapped u16 counts (kernels.cuh: EXACT_TRIGGER). Usually
     // there are none, so the grid is small: the launch costs one short kernel, and a listed query is a whole pass over its window anyway
-    k_prelim_exact<<<(unsigned)std::min<uint64_t>(C.nitems, 8), PRELIM_THREADS, 0, st>>>(db->v, svq, bv, L.d_nlist.as<uint64_t>(), nv);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_prelim_exact<<<(unsigned)std::min<uint64_t>(C.nitems, 8), PRELIM_THREADS, 0, st>>>(db->v, svq, bv, L.d_nlist.as<uint64_t>(), nv));
     CUDA_TRY(cudaEventRecord(L.ev_count_end, st));   // narrow counting kernels done (the open-search kernel, when present, is timed with the replays)
     // narrow windows (<= NARROW_CAP peptides): 32-bit heap keys, half the shared memory
-    k_replay<true><<<(unsigned)((C.nitems + REPLAY_THREADS - 1) / REPLAY_THREADS), REPLAY_THREADS, rsm / 2, st>>>(sv, bv, L.d_nlist.as<uint64_t>(), L.d_nslots.as<ReplaySlot>(),
-                                                                                                                 (uint32_t)C.nitems, nullptr, n);
-    CUDA_TRY(cudaGetLastError());
+    LAUNCH(k_replay<true><<<(unsigned)((C.nitems + REPLAY_THREADS - 1) / REPLAY_THREADS), REPLAY_THREADS, rsm / 2, st>>>(
+        sv, bv, L.d_nlist.as<uint64_t>(), L.d_nslots.as<ReplaySlot>(), (uint32_t)C.nitems, nullptr, n));
     launches += 4;
     if (C.wide_cap) {
         const int ctas = (int)std::min<uint64_t>((uint64_t)db->sm_count * WIDE_CTAS, C.wide_cap);
         const WideIndexView wv = db_wide_index(db, sv.wide_tile);   // built on first use (the first open-search chunk of a scorer is a re-run anyway)
-        k_prelim_wide<<<ctas, WIDE_THREADS, sizeof(WideSmem), st>>>(db->v, sv, bv, (uint32_t)C.nitems, L.d_wlist.as<uint64_t>(), L.d_wslots.as<WideSlot>(), wv);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH(k_prelim_wide<<<ctas, WIDE_THREADS, sizeof(WideSmem), st>>>(db->v, sv, bv, (uint32_t)C.nitems, L.d_wlist.as<uint64_t>(), L.d_wslots.as<WideSlot>(), wv));
         if (wv.frag != nullptr) {   // reference-terms work counters of the queries the block-index path counted (no index entry is read)
-            k_wide_account<<<(C.wide_cap + 7) / 8, 256, 0, st>>>(db->v, sv, bv);
-            CUDA_TRY(cudaGetLastError());
+            LAUNCH(k_wide_account<<<(C.wide_cap + 7) / 8, 256, 0, st>>>(db->v, sv, bv));
             launches++;
         }
-        k_replay<false><<<(unsigned)((C.wide_cap + REPLAY_THREADS - 1) / REPLAY_THREADS), REPLAY_THREADS, rsm, st>>>(
-            sv, bv, L.d_wlist.as<uint64_t>(), L.d_wslots.as<WideSlot>(), C.wide_cap, L.d_counters.as<unsigned long long>() + C_WIDE, 0u);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH(k_replay<false><<<(unsigned)((C.wide_cap + REPLAY_THREADS - 1) / REPLAY_THREADS), REPLAY_THREADS, rsm, st>>>(
+            sv, bv, L.d_wlist.as<uint64_t>(), L.d_wslots.as<WideSlot>(), C.wide_cap, L.d_counters.as<unsigned long long>() + C_WIDE, 0u));
         launches += 2;
     }
     CUDA_TRY(cudaEventRecord(L.ev_replay_end, st));
@@ -1583,25 +1593,20 @@ static int chunk_run(sage_b200_scorer* S, Lane& L, bool dbg) {
         so.hit_t = L.d_hitt.as<float>(); so.hit_cap = C.hits_cap; so.recs = L.d_recs.as<ScoreRec>(); so.hkey = L.d_hkey.as<unsigned long long>(); so.counters = bv.counters;
         // k_score<true> stages the peaks and the hit lists only (no records / order / marks)
         const size_t smem_split = (size_t)(C.pmax + 4) * 8 + (size_t)sv.lcap * 16 + 32;
-        k_score<true><<<n, SCORE_THREADS, smem_split, st>>>(db->v, sv, bv, L.d_features.as<FeatureOut>(), L.d_counts.as<uint32_t>(), C.pmax, nullptr, nullptr, nullptr, 0ull, 0u,
-                                                            nullptr, so);
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH(k_score<true><<<n, SCORE_THREADS, smem_split, st>>>(db->v, sv, bv, L.d_features.as<FeatureOut>(), L.d_counts.as<uint32_t>(), C.pmax, nullptr, nullptr, nullptr,
+                                                                   0ull, 0u, nullptr, so));
         const uint64_t nthr = (uint64_t)n * sv.kparam, nrow = (uint64_t)n * sv.report_psms;
         CUDA_TRY(cudaMemsetAsync(L.d_emit.p, 0xFF, 4 * nrow, st));   // rank slots: RANK_EMPTY
-        k_fold<<<(unsigned)((nthr + 127) / 128), 128, 0, st>>>(db->v, sv, so, n);
-        CUDA_TRY(cudaGetLastError());
-        k_features<<<(unsigned)((nthr + 127) / 128), 128, 0, st>>>(sv, n, so, L.d_emit.as<uint32_t>());
-        CUDA_TRY(cudaGetLastError());
-        k_rows<<<(unsigned)((nrow + 127) / 128), 128, 0, st>>>(db->v, sv, bv, so, L.d_emit.as<uint32_t>(), L.d_counts.as<uint32_t>(), L.d_features.as<FeatureOut>());
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH(k_fold<<<(unsigned)((nthr + 127) / 128), 128, 0, st>>>(db->v, sv, so, n));
+        LAUNCH(k_features<<<(unsigned)((nthr + 127) / 128), 128, 0, st>>>(sv, n, so, L.d_emit.as<uint32_t>()));
+        LAUNCH(k_rows<<<(unsigned)((nrow + 127) / 128), 128, 0, st>>>(db->v, sv, bv, so, L.d_emit.as<uint32_t>(), L.d_counts.as<uint32_t>(), L.d_features.as<FeatureOut>()));
         launches += 4;
     } else {
         C.hits_cap = 0;
-        k_score<false><<<n, SCORE_THREADS, C.smem, st>>>(db->v, sv, bv, L.d_features.as<FeatureOut>(), L.d_counts.as<uint32_t>(), C.pmax,
-                                                        dbg ? L.d_dbgk.as<uint64_t>() : nullptr, dbg ? L.d_dbgm.as<uint32_t>() : nullptr,
-                                                        annotate ? L.d_frags.as<FragmentOut>() : nullptr, (unsigned long long)S->frag_cap, S->quick_mode,
-                                                        S->d_keep.as<uint8_t>(), SplitOut{});
-        CUDA_TRY(cudaGetLastError());
+        LAUNCH(k_score<false><<<n, SCORE_THREADS, C.smem, st>>>(db->v, sv, bv, L.d_features.as<FeatureOut>(), L.d_counts.as<uint32_t>(), C.pmax,
+                                                               dbg ? L.d_dbgk.as<uint64_t>() : nullptr, dbg ? L.d_dbgm.as<uint32_t>() : nullptr,
+                                                               annotate ? L.d_frags.as<FragmentOut>() : nullptr, (unsigned long long)S->frag_cap, S->quick_mode,
+                                                               S->d_keep.as<uint8_t>(), SplitOut{}));
         launches++;
     }
     CUDA_TRY(cudaEventRecord(L.ev_score_end, st));
@@ -1710,7 +1715,7 @@ static int lane_finish(sage_b200_scorer* S, Lane& L) {
             const uint64_t end = hc[C_FRAGS], begin = S->frag_used;
             const uint64_t lim = std::min<uint64_t>(end, S->frag_cap);
             if (lim > begin) {
-                CUDA_TRY(cudaMemcpy(S->frag_dst + begin, L.d_frags.as<sage_b200_fragment>() + begin, (lim - begin) * sizeof(sage_b200_fragment), cudaMemcpyDeviceToHost));
+                if (int rc = read_back(L.stream, S->frag_dst + begin, L.d_frags.as<sage_b200_fragment>() + begin, (lim - begin) * sizeof(sage_b200_fragment))) return rc;
                 T.d2h_bytes += (lim - begin) * sizeof(sage_b200_fragment);
             }
             S->frag_used = end;
@@ -1976,12 +1981,12 @@ static int quick_score_device(sage_b200_scorer* S, const sage_b200_spectra* sp, 
     int rc = 0;
     const size_t npep = S->db->v.n_pep;
     if ((rc = S->d_keep.reserve(npep + 16))) return rc;
-    CUDA_TRY(cudaMemset(S->d_keep.p, 0, npep + 16));
     S->last = sage_b200_counters{};
     S->frag_dst = nullptr;
     CUDA_TRY(idle_lanes(S));
     S->quick_mode = prefilter_low_memory ? 2u : 1u;
-    Lane& L = S->lanes[0];
+    Lane& L = S->lanes[0];   // every chunk runs on lane 0, behind the zeroing of the marks
+    CUDA_TRY(cudaMemsetAsync(S->d_keep.p, 0, npep + 16, L.stream));
     for (int restart = 0; restart < 4; restart++) {
         uint64_t c0 = 0;
         rc = 0;
@@ -1994,13 +1999,14 @@ static int quick_score_device(sage_b200_scorer* S, const sage_b200_spectra* sp, 
         if (rc != SAGE_B200_ERECHUNK) break;
         drain_lanes(S, rc);   // overflowed attempts leave no keep[] marks (k_score), so the marks of the finished chunks stay valid
         S->quick_mode = prefilter_low_memory ? 2u : 1u;
-        CUDA_TRY(cudaMemset(S->d_keep.p, 0, npep + 16));
+        CUDA_TRY(cudaMemsetAsync(S->d_keep.p, 0, npep + 16, L.stream));
     }
     if (rc == SAGE_B200_ERECHUNK) rc = fail(SAGE_B200_ELIMIT, "open search: survivor lists do not fit the arena budget even with the smallest chunks");
     S->quick_mode = 0;
     L.chunk.loaded = false;
     if (rc) return drain_lanes(S, rc);
-    finish_counters(S);   // lane_finish has waited for the lane's stream: the marks are complete
+    CUDA_TRY(cudaStreamSynchronize(L.stream));   // the marks are complete (also when no chunk ran)
+    finish_counters(S);
     return 0;
 }
 
@@ -2015,7 +2021,7 @@ extern "C" int sage_b200_quick_score(sage_b200_scorer* S, const sage_b200_spectr
     if ((rc = quick_score_device(S, sp, prefilter_low_memory))) return rc;
     const size_t npep = S->db->v.n_pep;
     std::vector<uint8_t> h(npep);
-    CUDA_TRY(cudaMemcpy(h.data(), S->d_keep.p, npep, cudaMemcpyDeviceToHost));
+    if ((rc = read_back(S->lanes[0].stream, h.data(), S->d_keep.p, npep))) return rc;
     for (size_t i = 0; i < npep; i++) keep[i] |= h[i];
     return 0;
 }
@@ -2084,8 +2090,8 @@ extern "C" int64_t sage_b200_initial_hits(sage_b200_scorer* S, const sage_b200_s
     L.chunk.loaded = false;
     std::vector<uint64_t> keys(S->sv.kparam);
     uint32_t meta[4] = {0, 0, 0, 0};
-    CUDA_TRY(cudaMemcpy(keys.data(), L.d_dbgk.p, 8 * (size_t)S->sv.kparam, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(meta, L.d_dbgm.p, 16, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpyAsync(keys.data(), L.d_dbgk.p, 8 * (size_t)S->sv.kparam, cudaMemcpyDeviceToHost, L.stream));
+    if ((rc = read_back(L.stream, meta, L.d_dbgm.p, 16))) return rc;
     const uint32_t nk = meta[0];
     for (uint32_t i = 0; i < nk && i < cap; i++) {
         const uint64_t k = keys[i];
@@ -4252,8 +4258,12 @@ extern "C" int sage_b200_bipartite_cover(int device, const uint32_t* left, const
 #if SAGE_B200_PHASE_CLOCKS
 // variant builds only (not declared in the header): cycles per k_score phase summed over CTAs since the last reset
 extern "C" int sage_b200_debug_phase_cycles(unsigned long long* out16, int reset) {
-    if (out16) CUDA_TRY(cudaMemcpyFromSymbol(out16, g_phase, sizeof(unsigned long long) * 16));
-    if (reset) { unsigned long long z[16] = {0}; CUDA_TRY(cudaMemcpyToSymbol(g_phase, z, sizeof z)); }
+    const unsigned long long z[16] = {0};
+    Stream st;
+    CUDA_TRY(st.create());
+    if (out16) CUDA_TRY(cudaMemcpyFromSymbolAsync(out16, g_phase, sizeof z, 0, cudaMemcpyDeviceToHost, st));
+    if (reset) CUDA_TRY(cudaMemcpyToSymbolAsync(g_phase, z, sizeof z, 0, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
     return 0;
 }
 #endif
@@ -5123,7 +5133,7 @@ extern "C" int sage_b200_prefilter_create(int device, const char* fasta, uint64_
             if (int rc = db_build_device(C, bucket_size, ion_kinds, n_ion_kinds, min_ion_index, device, &cdb)) return rc;
             Guard<sage_b200_db> cdb_guard(cdb, sage_b200_db_destroy);
             I.ms_index += ms_since(t);
-            const uint64_t held = T.bytes() + D.out.bytes + cdb->device_bytes;
+            const uint64_t held = T.bytes() + D.out.bytes + cdb->mem.bytes;
             I.peak_device_bytes = std::max<uint64_t>(I.peak_device_bytes, held);
             t = std::chrono::steady_clock::now();
             sage_b200_scorer* sc = nullptr;
@@ -5133,12 +5143,11 @@ extern "C" int sage_b200_prefilter_create(int device, const char* fasta, uint64_
                 std::lock_guard<std::mutex> lock(sc->mu);
                 if (int rc = quick_score_device(sc, &Q.s, pp->low_memory)) return rc;
             }
-            CUDA_TRY(cudaDeviceSynchronize());   // the keep marks are zeroed on the default stream when no spectrum is scored
             I.ms_quick_score += ms_since(t);
             I.ms_spectra_upload += sc->last.ms_h2d;
             t = std::chrono::steady_clock::now();
             uint64_t kept = 0;
-            if (int rc = pf_compact(C, sc->d_keep.as<uint8_t>(), T, st, &kept, &I.peak_device_bytes, D.out.bytes + cdb->device_bytes)) return rc;
+            if (int rc = pf_compact(C, sc->d_keep.as<uint8_t>(), T, st, &kept, &I.peak_device_bytes, D.out.bytes + cdb->mem.bytes)) return rc;
             I.ms_compact += ms_since(t);
             PF->chunk_kept.back() = kept;
             I.rows_kept += kept;
@@ -5157,7 +5166,7 @@ extern "C" int sage_b200_prefilter_create(int device, const char* fasta, uint64_
     I.n_names = O.n_names;
     I.name_bytes = O.name_bytes;
     I.n_fragments = PF->db->v.n_frag;
-    I.device_bytes = PF->table.out.bytes + PF->db->device_bytes;
+    I.device_bytes = PF->table.out.bytes + PF->db->mem.bytes;
     I.peak_device_bytes = std::max<uint64_t>(I.peak_device_bytes, I.device_bytes);
     I.ms_wall = ms_since(t0);
     *out = guard.release();

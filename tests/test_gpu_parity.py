@@ -295,6 +295,52 @@ def test_score_batch_multi_single_process(small):
     assert_features_equal(gf, gc, of, oc, 2, what=f"score_batch_multi over {len(scorers)} scorers / {ndev} device(s)")
 
 
+def test_scorers_on_one_db_in_two_threads(small):
+    """A narrow and an open-search scorer on one fresh db, each scoring from its own thread: both lazily build their block-index copy of the
+    fragments while the other scorer's kernels run. Rows, counts and work counters equal the same searches run one after the other on
+    another fresh db, and the oracle's rows."""
+    import threading
+    from sage_b200.api import COUNTER_U64
+    pep, odb, _, spectra = small
+    kws = (dict(precursor_tol=Tolerance.ppm(-20, 20), fragment_tol=Tolerance.ppm(-20, 20), report_psms=2),
+           dict(precursor_tol=Tolerance.da(-500, 500), fragment_tol=Tolerance.ppm(-20, 20), report_psms=2))
+    subs = (spectra, spectra.slice(0, 400))
+
+    def search(db, kw, sub):
+        sc = Scorer(db, **kw)
+        f, c = sc.score_batch(sub)
+        return f, c, {k: v for k, v in sc.counters().items() if k in COUNTER_U64}
+
+    seq_db = IndexedDatabase.build_from_peptides(pep)
+    seq = [search(seq_db, kw, sub) for kw, sub in zip(kws, subs)]
+    par_db = IndexedDatabase.build_from_peptides(pep)
+    par, errors = [None, None], []
+
+    def run(i):
+        try:
+            par[i] = search(par_db, kws[i], subs[i])
+        except Exception as e:   # re-raised in the main thread
+            errors.append(e)
+
+    threads = [threading.Thread(target=run, args=(i,)) for i in range(2)]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join()
+    assert not errors, errors
+    for (pf, pc, pctr), (sf, sc_, sctr), kw, sub in zip(par, seq, kws, subs):
+        assert np.array_equal(pc, sc_)
+        pv, sv = valid_rows(pf, pc, 2), valid_rows(sf, sc_, 2)
+        for f in pv.dtype.names:
+            if not f.startswith("_"):
+                assert np.array_equal(np.ascontiguousarray(pv[f]).view(np.uint8), np.ascontiguousarray(sv[f]).view(np.uint8)), f
+        assert pctr == sctr
+        of, oc, _, _ = odb.score_batch(oracle_cfg(**kw), sub.as_dict())
+        assert_features_equal(pf, pc, of, oc, 2, what="two threads, one db")
+    assert seq[1][2]["wide_queries"] > 100
+    assert par_db.device_bytes() == seq_db.device_bytes()
+
+
 def test_quick_score_prefilter(small):
     # Scorer::quick_score (scoring.rs:255-298): both branches, incl. isotope fold and unknown charges
     pep, odb, gdb, spectra = small
