@@ -628,6 +628,102 @@ int sage_b200_prefilter_export(const sage_b200_prefilter* f, uint32_t* residue_o
 int sage_b200_prefilter_take_db(sage_b200_prefilter* f, sage_b200_db** out);
 void sage_b200_prefilter_destroy(sage_b200_prefilter* f);
 
+/* ---------------------------------------------------------------------------------------------------------------------------------------------
+ * Result files (runner.rs Runner::run, the CSV writers): the bytes of a Sage output file, formatted on the device as the reference writes
+ * them (csv-core's tab-separated records, quoted only where a field holds '\t', '"', '\r' or '\n'; f32 / f64 in ryu's shortest round-trip
+ * layout; integers as itoa; modification masses as Rust's `{:+}`). The definitions are DESIGN.md §17. One pass measures every record, a
+ * scan places them, a second pass writes them chunk by chunk into at most text_budget bytes of device memory, and each chunk is copied once
+ * to its offset in `out`.
+ *   SAGE_B200_FILE_RESULTS    results.sage.tsv (runner.rs:687-780, 842-884): one record per row, in the caller's order
+ *   SAGE_B200_FILE_PIN        results.sage.pin (runner.rs:938-1120): one record per row; log1p / log1pf are glibc's (the host libm's variant)
+ *   SAGE_B200_FILE_FRAGMENTS  matched_fragments.sage.tsv (runner.rs:782-829, 904-936): one record per fragment of each row, rows in order,
+ *                             fragments[rows[i].fragment_offset .. + fragment_count) in order
+ *   SAGE_B200_FILE_LFQ        lfq.tsv (runner.rs:1182-1240): one record per target row of sage_b200_lfq_integrate, in its order (the
+ *                             reference's order is a HashMap's: the set of records is the reference's, the order is defined here)
+ *   SAGE_B200_FILE_TMT        tmt.tsv (runner.rs:1140-1180): one record per quantified spectrum in the caller's order
+ * Strings the device does not own arrive as CSR byte tables: string i is bytes[offsets[i] .. offsets[i + 1]).
+ */
+#define SAGE_B200_FILE_RESULTS 1
+#define SAGE_B200_FILE_PIN 2
+#define SAGE_B200_FILE_FRAGMENTS 3
+#define SAGE_B200_FILE_LFQ 4
+#define SAGE_B200_FILE_TMT 5
+typedef struct {
+    float ms_upload, ms_measure, ms_scan, ms_write, ms_d2h, ms_total;   /* CUDA-event stage times (write and d2h summed over chunks) */
+    uint64_t h2d_bytes, d2h_bytes, records, chunks;
+} sage_b200_write_stats;
+typedef struct {
+    /* rows: results, pin, fragments */
+    const sage_b200_feature* rows;        /* [n_rows] as the search returns them */
+    const uint64_t* psm_id;               /* [n_rows] Feature::psm_id (the reference takes it from a global counter, so it is the caller's) */
+    uint64_t n_rows;
+    const sage_b200_fragment* fragments;  /* [n_fragments] as sage_b200_score_batch returns them with annotate_matches; kind 0..5 = a b c x y z */
+    uint64_t n_fragments;
+    /* strings: results, pin, tmt (filenames also lfq's header) */
+    const uint64_t* filename_offsets;     /* [n_files + 1] */
+    const char* filename_bytes;
+    uint64_t n_files;
+    const uint64_t* spec_id_offsets;      /* [n_spec_ids + 1] */
+    const char* spec_id_bytes;
+    uint64_t n_spec_ids;
+    /* tmt.tsv */
+    uint64_t n_quant;
+    const uint32_t* quant_file_id;        /* [n_quant] < n_files */
+    const uint32_t* quant_spec_id;        /* [n_quant] < n_spec_ids */
+    const float* ion_injection_time;      /* [n_quant] */
+    const float* peaks;                   /* [n_quant * n_channels] TmtQuant::peaks, row-major */
+    uint64_t n_channels;
+    uint8_t user_labels;                  /* 1: the columns are user_1..n (Isobaric::User), else tmt_1..n */
+    /* the peptide table (results, pin, lfq): the digest's (sage_b200_digest_export) */
+    const sage_b200_peptides* peptides;   /* residue_offsets, sequence, modifications, nterm and decoy are read */
+    const float* cterm;                   /* [n_peptides] NaN = None; NULL = None for every peptide */
+    const uint8_t* semi_enzymatic;        /* [n_peptides]; NULL = 0 */
+    const uint32_t* protein_offsets;      /* [n_peptides + 1] */
+    const uint32_t* protein_ids;          /* each < n_names */
+    const uint64_t* name_offsets;         /* [n_names + 1] the protein names */
+    const char* name_bytes;
+    uint64_t n_names;
+    const char* decoy_tag;                /* NULL = "rev_" */
+    uint8_t generate_decoys;
+    /* results / pin, per row: file and spectrum id, and the post-search columns, each [n_rows] or NULL for Feature's default
+       (scoring.rs:575-592: aligned_rt = rt, predicted 0.0, deltas 0.999, discriminant 0.0, posterior_error and the q-values 1.0) */
+    const uint32_t* file_id;              /* < n_files */
+    const uint32_t* spec_index;           /* < n_spec_ids: the row's Feature::spec_id */
+    const float *discriminant_score, *posterior_error, *spectrum_q;           /* sage_b200_spectrum_fdr */
+    const float *aligned_rt, *predicted_rt, *delta_rt_model, *predicted_ims, *delta_ims_model;   /* sage_b200_predict_rt */
+    const float *peptide_q, *protein_q;                                      /* sage_b200_picked_fdr */
+    /* sage_b200_protein_groups' outputs (results): NULL group_pass = no groups (protein_groups empty). The string rule is the one stated
+       above sage_b200_protein_groups; group ids < n_groups */
+    const uint32_t* num_protein_groups;   /* [n_rows] or NULL = 0 */
+    const float* protein_group_q;         /* [n_rows] or NULL = 1.0 */
+    const uint8_t* group_pass;            /* [n_rows] */
+    const uint64_t* row_group_offsets;    /* [n_rows + 1] */
+    const uint32_t* row_groups;
+    const uint64_t* group_offsets;        /* [n_groups + 1] */
+    const uint32_t* group_members;        /* each < n_names */
+    const uint8_t* group_decoy;           /* [n_groups] */
+    uint64_t n_groups;
+    /* lfq.tsv: sage_b200_lfq_integrate's rows and areas, sage_b200_picked_precursor's q-values */
+    const sage_b200_lfq_row* lfq_rows;    /* [n_lfq] peptide < n_peptides */
+    const double* lfq_areas;              /* [n_lfq * n_files] */
+    const float* lfq_q;                   /* [n_lfq] */
+    uint64_t n_lfq;
+    uint64_t text_budget;                 /* device bytes of text per chunk; 0 = 256 MiB. A test hook: any value gives the same bytes (a chunk
+                                             holds at least one block of 4096 records, so a block larger than the budget is one chunk) */
+    sage_b200_write_stats* stats;         /* optional */
+} sage_b200_write_inputs;
+/* out == NULL: *bytes = the file's size, nothing written. Else: ELIMIT with *bytes set and nothing written when capacity < the size; else the
+ * file is written to out[0 .. *bytes). EINVAL, before the device is looked at, for an unknown file, a null required pointer, a peptide_idx
+ * outside the table, a file id >= n_files, a spectrum index >= n_spec_ids, a fragment range outside the fragment array, a fragment kind
+ * outside 0..5, a protein id >= n_names, a group id >= n_groups or offsets that decrease (these checks read every input once); ELIMIT
+ * beyond 2^32 - 1 records (or rows), or when the work buffers do not fit the device's free memory (checked before allocating; the
+ * message names the byte count). A file with no records is its header alone and needs no device. */
+int sage_b200_write_tsv(int device, int file, const sage_b200_write_inputs* in, char* out, uint64_t capacity, uint64_t* bytes);
+/* Test hook: the per-block FNV-1a 64 hashes of formatted values, each followed by '\n'. format 0: ryu layout of the f32 with bits
+ * first + i; 1: `{:+}` of the same f32; 2: ryu layout of the f64 values[i]. Block b covers values [b * block, (b + 1) * block) of n; hashes[n / block]
+ * (n a multiple of block). */
+int sage_b200_format_hashes(int device, int format, uint64_t first, const double* values, uint64_t n, uint64_t block, uint64_t* hashes);
+
 /* Page-locked host buffers: spectra/feature arrays placed here are copied by DMA without a staging memcpy. */
 void* sage_b200_host_alloc(size_t bytes);
 /* The same for a batch sage_b200_score_batch_multi cuts into n_devices contiguous blocks: the i-th of n equal parts of the buffer is placed on the

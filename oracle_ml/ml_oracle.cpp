@@ -32,6 +32,7 @@
 #include <cstdint>
 #include <cstring>
 #include <map>
+#include <regex>
 #include <set>
 #include <string>
 #include <unordered_map>
@@ -1126,5 +1127,394 @@ uint64_t mo_bipartite_cover(const uint32_t* left, const uint32_t* right, uint64_
     std::copy(c.begin(), c.end(), cover);
     return graph.picks;
 }
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ result files (runner.rs writers)
+// The text of matched_fragments.sage.tsv and tmt.tsv with digits from std::to_chars (libstdc++'s shortest round-trip, closest, ties to even)
+// laid out as ryu::Buffer::format and Rust's `{:+}` do, and csv-core's QuoteStyle::Necessary, in the definitions of DESIGN.md §17. Shares
+// no code with sage_b200/csrc/write.cuh. (fmt_plus above takes std::to_chars' fixed form, which for |x| >= 2^24 can be the exact integer
+// rather than Rust's shortest digits padded with zeros: the writer uses wo_plus.)
+namespace {
+
+// to_chars' shortest scientific form of |x|: its digits into d (returns their count) and the exponent of the last digit into k
+template <class T>
+int wo_digits(T x, char* d, int& k) {
+    char b[64];
+    auto r = std::to_chars(b, b + sizeof b, std::fabs(x), std::chars_format::scientific);
+    int n = 0, i = 0;
+    for (; b[i] != 'e'; i++)
+        if (b[i] != '.') d[n++] = b[i];
+    int e = 0;
+    std::from_chars(b + i + 1 + (b[i + 1] == '+'), r.ptr, e);
+    k = e - (n - 1);
+    return n;
+}
+
+// ryu::Buffer::format of x into o (at least 64 bytes); returns the length
+template <class T>
+int wo_ryu_buf(T x, char* o) {
+    const int T_ = sizeof(T) == 8 ? 16 : 13;
+    auto put = [&](const char* s) { int n = (int)std::strlen(s); std::memcpy(o, s, n); return n; };
+    if (std::isnan(x)) return put("NaN");
+    if (std::isinf(x)) return put(x > 0 ? "inf" : "-inf");
+    if (x == 0) return put(std::signbit(x) ? "-0.0" : "0.0");
+    char d[32];
+    int k, p = 0;
+    const int len = wo_digits(x, d, k), kk = len + k;
+    if (std::signbit(x)) o[p++] = '-';
+    if (0 <= k && kk <= T_) {
+        std::memcpy(o + p, d, len), p += len;
+        for (int i = 0; i < k; i++) o[p++] = '0';
+        o[p++] = '.', o[p++] = '0';
+    } else if (0 < kk && kk <= T_) {
+        std::memcpy(o + p, d, kk), p += kk;
+        o[p++] = '.';
+        std::memcpy(o + p, d + kk, len - kk), p += len - kk;
+    } else if (-5 < kk && kk <= 0) {
+        o[p++] = '0', o[p++] = '.';
+        for (int i = 0; i < -kk; i++) o[p++] = '0';
+        std::memcpy(o + p, d, len), p += len;
+    } else {
+        o[p++] = d[0];
+        if (len > 1) {
+            o[p++] = '.';
+            std::memcpy(o + p, d + 1, len - 1), p += len - 1;
+        }
+        o[p++] = 'e';
+        p = (int)(std::to_chars(o + p, o + 64, kk - 1).ptr - o);
+    }
+    return p;
+}
+
+// Rust's `{:+}` of an f32 into o (at least 64 bytes); returns the length
+int wo_plus_buf(float x, char* o) {
+    if (std::isnan(x)) return std::memcpy(o, "NaN", 3), 3;
+    int p = 0;
+    o[p++] = std::signbit(x) ? '-' : '+';
+    if (std::isinf(x)) return std::memcpy(o + p, "inf", 3), p + 3;
+    if (x == 0) return o[p++] = '0', p;
+    char d[32];
+    int k;
+    const int len = wo_digits(x, d, k), kk = len + k;
+    if (k >= 0) {
+        std::memcpy(o + p, d, len), p += len;
+        for (int i = 0; i < k; i++) o[p++] = '0';
+    } else if (kk > 0) {
+        std::memcpy(o + p, d, kk), p += kk;
+        o[p++] = '.';
+        std::memcpy(o + p, d + kk, len - kk), p += len - kk;
+    } else {
+        o[p++] = '0', o[p++] = '.';
+        for (int i = 0; i < -kk; i++) o[p++] = '0';
+        std::memcpy(o + p, d, len), p += len;
+    }
+    return p;
+}
+
+template <class T>
+std::string wo_ryu(T x) {
+    char o[64];
+    return std::string(o, wo_ryu_buf(x, o));
+}
+std::string wo_plus(float x) {
+    char o[64];
+    return std::string(o, wo_plus_buf(x, o));
+}
+
+std::string wo_field(const char* s, size_t n) {   // csv-core QuoteStyle::Necessary, delimiter '\t'
+    std::string f(s, n);
+    if (f.find_first_of("\t\"\r\n") == std::string::npos) return f;
+    std::string q = "\"";
+    for (char c : f) {
+        if (c == '"') q += '"';
+        q += c;
+    }
+    return q + "\"";
+}
+
+struct WoFragment {
+    int32_t kind, charge, ordinal;
+    float intensity, mz_calculated, mz_experimental;
+};
+
+std::string g_wo_text;
+
+// rec(i) -> record i's text; records split over `threads` host threads and joined in order
+template <class F>
+void wo_records(uint64_t n, int threads, F rec) {
+    threads = std::max(1, threads);
+    std::vector<std::string> part(threads);
+    std::vector<std::thread> th;
+    for (int t = 0; t < threads; t++)
+        th.emplace_back([&, t] {
+            for (uint64_t i = n * t / threads; i < n * (t + 1) / threads; i++) part[t] += rec(i);
+        });
+    for (auto& x : th) x.join();
+    for (auto& p : part) g_wo_text += p;
+}
+
+std::string wo_header(const std::vector<std::string>& f) {
+    std::string h;
+    for (size_t i = 0; i < f.size(); i++) h += (i ? "\t" : "") + wo_field(f[i].data(), f[i].size());
+    return h + "\n";
+}
+
+}  // namespace
+
+extern "C" {
+
+// Per-block FNV-1a 64 of formatted values, each followed by '\n': format 0 ryu f32 (bits first + i), 1 `{:+}` f32, 2 ryu f64 values[i].
+void mo_format_hashes(int format, uint64_t first, const double* values, uint64_t n, uint64_t block, uint64_t* hashes, int threads) {
+    const uint64_t nb = n / block;
+    std::vector<std::thread> th;
+    threads = std::max(1, threads);
+    for (int t = 0; t < threads; t++)
+        th.emplace_back([&, t] {
+            for (uint64_t b = t; b < nb; b += threads) {
+                uint64_t h = 0xcbf29ce484222325ull;
+                for (uint64_t i = b * block; i < (b + 1) * block; i++) {
+                    char s[72];
+                    int n;
+                    if (format == 2) n = wo_ryu_buf(values[i], s);
+                    else {
+                        const uint32_t u = (uint32_t)(first + i);
+                        float x;
+                        std::memcpy(&x, &u, 4);
+                        n = format == 0 ? wo_ryu_buf(x, s) : wo_plus_buf(x, s);
+                    }
+                    s[n++] = '\n';
+                    for (int c = 0; c < n; c++) h = (h ^ (unsigned char)s[c]) * 0x100000001b3ull;
+                }
+                hashes[b] = h;
+            }
+        });
+    for (auto& x : th) x.join();
+}
+
+// One value's text: format 0 ryu f32, 1 `{:+}` f32, 2 ryu f64, 3 csv field of the bytes s[0..n). Returns the length written to out.
+uint64_t mo_format_one(int format, double x, const char* s, uint64_t n, char* out) {
+    std::string r = format == 0 ? wo_ryu((float)x) : format == 1 ? wo_plus((float)x) : format == 2 ? wo_ryu(x) : wo_field(s, n);
+    std::memcpy(out, r.data(), r.size());
+    return r.size();
+}
+
+// matched_fragments.sage.tsv; returns the size, the text is taken with mo_take_text
+uint64_t mo_write_fragments(const uint64_t* psm_id, const uint32_t* frag_offset, const uint32_t* frag_count, uint64_t n_rows, const WoFragment* fr, int threads) {
+    g_wo_text = wo_header({"psm_id", "fragment_type", "fragment_ordinals", "fragment_charge", "fragment_mz_calculated", "fragment_mz_experimental",
+                           "fragment_intensity"});
+    wo_records(n_rows, threads, [&](uint64_t i) {
+        std::string r;
+        for (uint32_t k = 0; k < frag_count[i]; k++) {
+            const WoFragment& f = fr[frag_offset[i] + k];
+            r += std::to_string(psm_id[i]) + "\t" + "abcxyz"[f.kind] + "\t" + std::to_string(f.ordinal) + "\t" + std::to_string(f.charge) + "\t" +
+                 wo_ryu(f.mz_calculated) + "\t" + wo_ryu(f.mz_experimental) + "\t" + wo_ryu(f.intensity) + "\n";
+        }
+        return r;
+    });
+    return g_wo_text.size();
+}
+
+// tmt.tsv
+uint64_t mo_write_tmt(const uint64_t* file_off, const char* file_bytes, const uint64_t* spec_off, const char* spec_bytes, const uint32_t* file_id,
+                      const uint32_t* spec, const float* injection, const float* peaks, uint64_t n, uint64_t n_channels, int user_labels, int threads) {
+    std::vector<std::string> h = {"filename", "scannr", "ion_injection_time"};
+    for (uint64_t c = 0; c < n_channels; c++) h.push_back((user_labels ? "user_" : "tmt_") + std::to_string(c + 1));
+    g_wo_text = wo_header(h);
+    wo_records(n, threads, [&](uint64_t i) {
+        std::string r = wo_field(file_bytes + file_off[file_id[i]], file_off[file_id[i] + 1] - file_off[file_id[i]]) + "\t" +
+                        wo_field(spec_bytes + spec_off[spec[i]], spec_off[spec[i] + 1] - spec_off[spec[i]]) + "\t" + wo_ryu(injection[i]);
+        for (uint64_t c = 0; c < n_channels; c++) r += "\t" + wo_ryu(peaks[i * n_channels + c]);
+        return r + "\n";
+    });
+    return g_wo_text.size();
+}
+
+// The peptide table and names the results / pin / lfq writers read.
+struct WoTable {
+    const uint32_t* res_off;
+    const uint8_t* seq;
+    const float* mods;
+    const float* nterm;
+    const float* cterm;   // NULL = None
+    const uint8_t* decoy;
+    const uint8_t* semi;  // NULL = 0
+    const uint32_t* prot_off;
+    const uint32_t* prot_ids;
+    const uint64_t* name_off;
+    const char* name_bytes;
+    const char* tag;
+    int generate_decoys;
+};
+
+// The post-search columns of results / pin; NULL = Feature's default.
+struct WoColumns {
+    const float *discriminant, *posterior, *spectrum_q, *peptide_q, *protein_q, *protein_group_q, *aligned_rt, *predicted_rt, *delta_rt, *predicted_ims,
+        *delta_ims;
+    const uint32_t* num_groups;
+    const uint8_t* group_pass;   // NULL: no groups
+    const uint64_t* row_group_off;
+    const uint32_t* row_groups;
+    const uint64_t* group_off;
+    const uint32_t* group_members;
+    const uint8_t* group_decoy;
+};
+
+static std::string wo_name(const WoTable& t, uint32_t id) { return std::string(t.name_bytes + t.name_off[id], t.name_bytes + t.name_off[id + 1]); }
+static std::string wo_display(const WoTable& t, uint32_t p) {   // impl Display for Peptide with Rust's `{:+}`
+    std::string out;
+    if (!std::isnan(t.nterm[p])) out += "[" + wo_plus(t.nterm[p]) + "]-";
+    for (uint32_t r = t.res_off[p]; r < t.res_off[p + 1]; r++) {
+        out += (char)t.seq[r];
+        if (t.mods[r] != 0.0f) out += "[" + wo_plus(t.mods[r]) + "]";
+    }
+    if (t.cterm && !std::isnan(t.cterm[p])) out += "-[" + wo_plus(t.cterm[p]) + "]";
+    return out;
+}
+static std::string wo_proteins(const WoTable& t, uint32_t p) {   // Peptide::proteins
+    std::string out;
+    for (uint32_t k = t.prot_off[p]; k < t.prot_off[p + 1]; k++) {
+        if (k > t.prot_off[p]) out += ";";
+        out += (t.decoy[p] && t.generate_decoys ? std::string(t.tag) : std::string()) + wo_name(t, t.prot_ids[k]);
+    }
+    return out;
+}
+static std::string wo_groups(const WoTable& t, const WoColumns& c, uint64_t i, uint32_t p) {
+    if (!c.group_pass) return "";
+    if (!c.group_pass[i]) return wo_proteins(t, p);
+    std::vector<std::string> gs;
+    for (uint64_t k = c.row_group_off[i]; k < c.row_group_off[i + 1]; k++) {
+        const uint32_t g = c.row_groups[k];
+        std::vector<std::string> names;
+        for (uint64_t m = c.group_off[g]; m < c.group_off[g + 1]; m++)
+            names.push_back((c.group_decoy[g] && t.generate_decoys ? std::string(t.tag) : std::string()) + wo_name(t, c.group_members[m]));
+        std::sort(names.begin(), names.end());
+        std::string s;
+        for (size_t j = 0; j < names.size(); j++) s += (j ? "/" : "") + names[j];
+        gs.push_back(s);
+    }
+    std::sort(gs.begin(), gs.end());
+    std::string out;
+    for (size_t j = 0; j < gs.size(); j++) out += (j ? ";" : "") + gs[j];
+    return out;
+}
+static float wo_opt(const float* a, uint64_t i, float d) { return a ? a[i] : d; }
+static std::string wo_str(const uint64_t* off, const char* bytes, uint32_t i) { return std::string(bytes + off[i], bytes + off[i + 1]); }
+
+static const std::vector<std::string> kResultsHeader = {"psm_id", "peptide", "proteins", "protein_groups", "num_proteins", "num_protein_groups", "filename",
+    "scannr", "rank", "label", "expmass", "calcmass", "charge", "peptide_len", "missed_cleavages", "semi_enzymatic", "isotope_error", "precursor_ppm",
+    "fragment_ppm", "hyperscore", "delta_next", "delta_best", "rt", "aligned_rt", "predicted_rt", "delta_rt_model", "ion_mobility", "predicted_mobility",
+    "delta_mobility", "matched_peaks", "longest_b", "longest_y", "longest_y_pct", "matched_intensity_pct", "scored_candidates", "poisson",
+    "sage_discriminant_score", "posterior_error", "spectrum_q", "peptide_q", "protein_q", "protein_group_q", "ms2_intensity"};
+static const std::vector<std::string> kPinHeader = {"SpecId", "Label", "ScanNr", "ExpMass", "CalcMass", "FileName", "retentiontime", "ion_mobility", "rank",
+    "z=2", "z=3", "z=4", "z=5", "z=6", "z=other", "peptide_len", "missed_cleavages", "semi_enzymatic", "isotope_error", "ln(precursor_ppm)", "fragment_ppm",
+    "ln(hyperscore)", "ln(delta_next)", "ln(delta_best)", "aligned_rt", "predicted_rt", "sqrt(delta_rt_model)", "predicted_mobility",
+    "sqrt(delta_mobility)", "matched_peaks", "longest_b", "longest_y", "longest_y_pct", "ln(matched_intensity_pct)", "scored_candidates", "ln(-poisson)",
+    "posterior_error", "Peptide", "Proteins"};
+
+// results.sage.tsv (pin = 0) or results.sage.pin (pin = 1); std::regex gives the pin's ScanNr
+uint64_t mo_write_results(int pin, const Row* rows, const uint64_t* psm_id, const uint32_t* file_id, const uint32_t* spec, uint64_t n, const uint64_t* file_off,
+                          const char* file_bytes, const uint64_t* spec_off, const char* spec_bytes, const WoTable* tab, const WoColumns* cols, int threads) {
+    const WoTable& t = *tab;
+    const WoColumns& c = *cols;
+    g_wo_text = wo_header(pin ? kPinHeader : kResultsHeader);
+    const std::regex scan_re("scan=([0-9]+)");
+    wo_records(n, threads, [&](uint64_t i) {
+        const Row& r = rows[i];
+        const uint32_t p = r.peptide_idx;
+        const std::string fname = wo_field(file_bytes + file_off[file_id[i]], file_off[file_id[i] + 1] - file_off[file_id[i]]);
+        const std::string sid = wo_str(spec_off, spec_bytes, spec[i]);
+        const std::string pep = wo_display(t, p), prots = wo_proteins(t, p);
+        std::vector<std::string> f;
+        auto I = [&](int64_t v) { f.push_back(std::to_string(v)); };
+        const int semi = t.semi ? t.semi[p] : 0;
+        const float aligned = wo_opt(c.aligned_rt, i, r.rt), pred_rt = wo_opt(c.predicted_rt, i, 0.0f), drt = wo_opt(c.delta_rt, i, 0.999f);
+        const float pred_ims = wo_opt(c.predicted_ims, i, 0.0f), dims = wo_opt(c.delta_ims, i, 0.999f), post = wo_opt(c.posterior, i, 1.0f);
+        if (!pin) {
+            I((int64_t)psm_id[i]);
+            f.push_back(wo_field(pep.data(), pep.size()));
+            f.push_back(wo_field(prots.data(), prots.size()));
+            const std::string g = wo_groups(t, c, i, p);
+            f.push_back(wo_field(g.data(), g.size()));
+            I(t.prot_off[p + 1] - t.prot_off[p]);
+            I(c.num_groups ? c.num_groups[i] : 0);
+            f.push_back(fname);
+            f.push_back(wo_field(sid.data(), sid.size()));
+            I(r.rank); I(r.label);
+            f.push_back(wo_ryu(r.expmass)); f.push_back(wo_ryu(r.calcmass));
+            I(r.charge); I(r.peptide_len); I(r.missed_cleavages); I(semi);
+            f.push_back(wo_ryu(r.isotope_error)); f.push_back(wo_ryu(r.delta_mass)); f.push_back(wo_ryu(r.average_ppm));
+            f.push_back(wo_ryu(r.hyperscore)); f.push_back(wo_ryu(r.delta_next)); f.push_back(wo_ryu(r.delta_best));
+            f.push_back(wo_ryu(r.rt)); f.push_back(wo_ryu(aligned)); f.push_back(wo_ryu(pred_rt)); f.push_back(wo_ryu(drt));
+            f.push_back(wo_ryu(r.ims)); f.push_back(wo_ryu(pred_ims)); f.push_back(wo_ryu(dims));
+            I(r.matched_peaks); I(r.longest_b); I(r.longest_y);
+            f.push_back(wo_ryu(r.longest_y_pct)); f.push_back(wo_ryu(r.matched_intensity_pct));
+            I(r.scored_candidates);
+            f.push_back(wo_ryu(r.poisson));
+            f.push_back(wo_ryu(wo_opt(c.discriminant, i, 0.0f))); f.push_back(wo_ryu(post)); f.push_back(wo_ryu(wo_opt(c.spectrum_q, i, 1.0f)));
+            f.push_back(wo_ryu(wo_opt(c.peptide_q, i, 1.0f))); f.push_back(wo_ryu(wo_opt(c.protein_q, i, 1.0f)));
+            f.push_back(wo_ryu(wo_opt(c.protein_group_q, i, 1.0f))); f.push_back(wo_ryu(r.ms2_intensity));
+        } else {
+            std::string scannr = sid;
+            for (auto it = std::sregex_iterator(sid.begin(), sid.end(), scan_re); it != std::sregex_iterator(); ++it) scannr = (*it)[1].str();
+            I((int64_t)psm_id[i]); I(r.label);
+            f.push_back(wo_field(scannr.data(), scannr.size()));
+            f.push_back(wo_ryu(r.expmass)); f.push_back(wo_ryu(r.calcmass));
+            f.push_back(fname);
+            f.push_back(wo_ryu(r.rt)); f.push_back(wo_ryu(r.ims));
+            I(r.rank);
+            for (uint32_t z = 2; z <= 6; z++) I(r.charge == z ? 1 : 0);
+            I((r.charge < 2 || r.charge > 6) ? r.charge : 0);
+            I(r.peptide_len); I(r.missed_cleavages); I(semi);
+            f.push_back(wo_ryu(r.isotope_error));
+            f.push_back(wo_ryu(log1pf(std::fabs(r.delta_mass))));
+            f.push_back(wo_ryu(r.average_ppm));
+            f.push_back(wo_ryu(std::log1p(r.hyperscore))); f.push_back(wo_ryu(std::log1p(r.delta_next))); f.push_back(wo_ryu(std::log1p(r.delta_best)));
+            f.push_back(wo_ryu(aligned)); f.push_back(wo_ryu(pred_rt));
+            const float cl = std::isnan(drt) ? drt : std::min(std::max(drt, 0.001f), 1.0f);
+            f.push_back(wo_ryu(std::sqrt(cl)));
+            f.push_back(wo_ryu(pred_ims)); f.push_back(wo_ryu(dims));
+            I(r.matched_peaks); I(r.longest_b); I(r.longest_y);
+            f.push_back(wo_ryu(r.longest_y_pct)); f.push_back(wo_ryu(log1pf(r.matched_intensity_pct)));
+            I(r.scored_candidates);
+            f.push_back(wo_ryu(std::log1p(-r.poisson)));
+            f.push_back(wo_ryu(post));
+            f.push_back(wo_field(pep.data(), pep.size()));
+            f.push_back(wo_field(prots.data(), prots.size()));
+        }
+        std::string rec;
+        for (size_t k = 0; k < f.size(); k++) rec += (k ? "\t" : "") + f[k];
+        return rec + "\n";
+    });
+    return g_wo_text.size();
+}
+
+// lfq.tsv over sage_b200_lfq_integrate's rows (peptide u32, charge u8, decoy u8, 16 more bytes, spectral_angle f64, score f64)
+struct WoLfqRow {
+    uint32_t peptide;
+    uint8_t charge, decoy;
+    uint16_t pad0;
+    uint32_t rt, pad1;
+    double spectral_angle, score;
+};
+uint64_t mo_write_lfq(const WoLfqRow* rows, const double* areas, const float* q, uint64_t n, const uint64_t* file_off, const char* file_bytes, uint64_t n_files,
+                      const WoTable* tab, int threads) {
+    const WoTable& t = *tab;
+    std::vector<std::string> h = {"peptide", "charge", "proteins", "q_value", "score", "spectral_angle"};
+    for (uint64_t k = 0; k < n_files; k++) h.push_back(wo_str(file_off, file_bytes, (uint32_t)k));
+    g_wo_text = wo_header(h);
+    wo_records(n, threads, [&](uint64_t i) {
+        const WoLfqRow& r = rows[i];
+        if (r.decoy) return std::string();
+        const std::string pep = wo_display(t, r.peptide), prots = wo_proteins(t, r.peptide);
+        std::string rec = wo_field(pep.data(), pep.size()) + "\t" + std::to_string(r.charge ? (int)r.charge : -1) + "\t" + wo_field(prots.data(), prots.size()) +
+                          "\t" + wo_ryu(q[i]) + "\t" + wo_ryu(r.score) + "\t" + wo_ryu(r.spectral_angle);
+        for (uint64_t k = 0; k < n_files; k++) rec += "\t" + wo_ryu(areas[i * n_files + k]);
+        return rec + "\n";
+    });
+    return g_wo_text.size();
+}
+
+void mo_take_text(char* out) { std::memcpy(out, g_wo_text.data(), g_wo_text.size()); }
 
 }  // extern "C"

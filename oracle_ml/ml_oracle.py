@@ -49,6 +49,18 @@ def lib():
         _lib.mo_grouping_text.argtypes = [C.c_void_p]
         _lib.mo_bipartite_cover.restype = C.c_uint64
         _lib.mo_bipartite_cover.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p]
+        _lib.mo_format_hashes.argtypes = [C.c_int, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_int]
+        _lib.mo_format_one.restype = C.c_uint64
+        _lib.mo_format_one.argtypes = [C.c_int, C.c_double, C.c_char_p, C.c_uint64, C.c_void_p]
+        _lib.mo_write_fragments.restype = C.c_uint64
+        _lib.mo_write_fragments.argtypes = [C.c_void_p] * 3 + [C.c_uint64, C.c_void_p, C.c_int]
+        _lib.mo_write_tmt.restype = C.c_uint64
+        _lib.mo_write_tmt.argtypes = [C.c_void_p] * 8 + [C.c_uint64, C.c_uint64, C.c_int, C.c_int]
+        _lib.mo_take_text.argtypes = [C.c_void_p]
+        _lib.mo_write_results.restype = C.c_uint64
+        _lib.mo_write_results.argtypes = [C.c_int] + [C.c_void_p] * 4 + [C.c_uint64] + [C.c_void_p] * 6 + [C.c_int]
+        _lib.mo_write_lfq.restype = C.c_uint64
+        _lib.mo_write_lfq.argtypes = [C.c_void_p] * 3 + [C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int]
     return _lib
 
 
@@ -239,3 +251,124 @@ def bipartite_cover(left, right, n_left, n_right):
     cover = np.zeros(int(n_left), np.uint8)
     picks = lib().mo_bipartite_cover(_p(lft), _p(rgt), len(lft), int(n_left), int(n_right), _p(cover))
     return cover.astype(bool), int(picks)
+
+
+# ------------------------------------------------------------------------------------------------ result files (runner.rs writers)
+def format_hashes(fmt: int, first: int = 0, values=None, n: int = 0, block: int = 1 << 16, threads=None) -> np.ndarray:
+    """Per-block FNV-1a 64 of formatted values (each followed by '\n'): fmt 0 ryu f32 of bits first + i, 1 `{:+}` of that f32, 2 ryu f64."""
+    v = None if values is None else np.ascontiguousarray(values, np.float64)
+    n = len(v) if v is not None else n
+    out = np.zeros(n // block, np.uint64)
+    lib().mo_format_hashes(fmt, first, _p(v), n, block, _p(out), int(threads or default_threads()))
+    return out
+
+
+def format_one(fmt: int, x: float = 0.0, s: bytes = b"") -> str:
+    """One value: fmt 0 ryu f32, 1 `{:+}` f32, 2 ryu f64, 3 the csv field of bytes s."""
+    buf = C.create_string_buffer(2 * len(s) + 128)
+    n = lib().mo_format_one(fmt, float(x), s, len(s), buf)
+    return buf.raw[:n].decode("latin-1")
+
+
+def _take(n: int) -> bytes:
+    buf = C.create_string_buffer(max(n, 1))
+    lib().mo_take_text(buf)
+    return buf.raw[:n]
+
+
+def write_fragments(psm_id, frag_offset, frag_count, fragments, threads=None) -> bytes:
+    """matched_fragments.sage.tsv; fragments: a structured array in sage_b200_fragment's layout."""
+    a = [np.ascontiguousarray(psm_id, np.uint64), np.ascontiguousarray(frag_offset, np.uint32), np.ascontiguousarray(frag_count, np.uint32)]
+    fr = np.ascontiguousarray(fragments)
+    n = lib().mo_write_fragments(_p(a[0]), _p(a[1]), _p(a[2]), len(a[0]), _p(fr), int(threads or default_threads()))
+    return _take(n)
+
+
+def write_tmt(filenames, spec_ids, file_id, spec, injection, peaks, user_labels=False, threads=None) -> bytes:
+    """tmt.tsv; filenames / spec_ids: lists of bytes."""
+    def csr(strs):
+        off = np.concatenate([[0], np.cumsum([len(s) for s in strs])]).astype(np.uint64)
+        return off, np.frombuffer(b"".join(strs) + b"\0", np.uint8)
+    fo, fb = csr(filenames)
+    so, sb = csr(spec_ids)
+    fi, si = np.ascontiguousarray(file_id, np.uint32), np.ascontiguousarray(spec, np.uint32)
+    inj = np.ascontiguousarray(injection, np.float32)
+    pk = np.ascontiguousarray(peaks, np.float32).reshape(len(fi), -1)
+    n = lib().mo_write_tmt(_p(fo), _p(fb), _p(so), _p(sb), _p(fi), _p(si), _p(inj), _p(pk), len(fi), pk.shape[1], int(user_labels),
+                           int(threads or default_threads()))
+    return _take(n)
+
+
+class _WoTable(C.Structure):
+    _fields_ = [(f, C.c_void_p) for f in ("res_off", "seq", "mods", "nterm", "cterm", "decoy", "semi", "prot_off", "prot_ids", "name_off",
+                                          "name_bytes")] + [("tag", C.c_char_p), ("generate_decoys", C.c_int)]
+
+
+_COLS = ("discriminant", "posterior", "spectrum_q", "peptide_q", "protein_q", "protein_group_q", "aligned_rt", "predicted_rt", "delta_rt",
+         "predicted_ims", "delta_ims", "num_groups", "group_pass", "row_group_off", "row_groups", "group_off", "group_members", "group_decoy")
+
+
+class _WoColumns(C.Structure):
+    _fields_ = [(f, C.c_void_p) for f in _COLS]
+
+
+def _csr(strs, keep):
+    bs = [s.encode() if isinstance(s, str) else bytes(s) for s in strs]
+    off = np.concatenate([[0], np.cumsum([len(b) for b in bs], dtype=np.uint64)]).astype(np.uint64)
+    data = np.frombuffer(b"".join(bs) + b"\0", np.uint8)
+    keep += [off, data]
+    return _p(off), _p(data)
+
+
+def _table(digest, decoy_tag, generate_decoys, keep):
+    P = digest.peptides
+    arrs = [np.ascontiguousarray(a, dt) for a, dt in ((P.seq_off, np.uint32), (P.seq, np.uint8), (P.mods, np.float32), (P.nterm, np.float32),
+                                                       (digest.cterm, np.float32), (P.decoy, np.uint8), (digest.semi_enzymatic, np.uint8),
+                                                       (digest.protein_offsets, np.uint32), (digest.protein_ids, np.uint32))]
+    keep += arrs
+    no, nb = _csr(digest.names, keep)
+    tag = decoy_tag.encode()
+    keep.append(tag)
+    return _WoTable(*[_p(a) for a in arrs], no, nb, tag, int(bool(generate_decoys)))
+
+
+def _column(d, key, dt, keep):
+    if d is None or d.get(key) is None:
+        return None
+    a = np.ascontiguousarray(d[key], dt)
+    keep.append(a)
+    return _p(a)
+
+
+def write_results(digest, rows, psm_id, file_id, spec_index, filenames, spec_ids, fdr=None, rt=None, picked=None, groups=None, decoy_tag="rev_",
+                  generate_decoys=True, pin=False, threads=None) -> bytes:
+    """results.sage.tsv (pin=False) or results.sage.pin; the dicts are those of the library's spectrum_fdr, predict_rt, picked_fdr, protein_groups."""
+    keep = []
+    rows = np.ascontiguousarray(rows)
+    t = _table(digest, decoy_tag, generate_decoys, keep)
+    src = dict(discriminant=(fdr, "discriminant_score", np.float32), posterior=(fdr, "posterior_error", np.float32), spectrum_q=(fdr, "spectrum_q", np.float32),
+               peptide_q=(picked, "peptide_q", np.float32), protein_q=(picked, "protein_q", np.float32),
+               protein_group_q=(groups, "protein_group_q", np.float32), aligned_rt=(rt, "aligned_rt", np.float32), predicted_rt=(rt, "predicted_rt", np.float32),
+               delta_rt=(rt, "delta_rt_model", np.float32), predicted_ims=(rt, "predicted_ims", np.float32), delta_ims=(rt, "delta_ims_model", np.float32),
+               num_groups=(groups, "num_protein_groups", np.uint32), group_pass=(groups, "pass", np.uint8), row_group_off=(groups, "row_group_offsets", np.uint64),
+               row_groups=(groups, "row_groups", np.uint32), group_off=(groups, "group_offsets", np.uint64), group_members=(groups, "group_members", np.uint32),
+               group_decoy=(groups, "group_decoy", np.uint8))
+    c = _WoColumns(*[_column(*src[k], keep) for k in _COLS])
+    fo, fb = _csr(filenames, keep)
+    so, sb = _csr(spec_ids, keep)
+    a = [np.ascontiguousarray(psm_id, np.uint64), np.ascontiguousarray(file_id, np.uint32), np.ascontiguousarray(spec_index, np.uint32)]
+    n = lib().mo_write_results(int(pin), _p(rows), _p(a[0]), _p(a[1]), _p(a[2]), len(rows), fo, fb, so, sb, C.byref(t), C.byref(c),
+                               int(threads or default_threads()))
+    return _take(n)
+
+
+def write_lfq(digest, lfq_rows, areas, q_value, filenames, decoy_tag="rev_", generate_decoys=True, threads=None) -> bytes:
+    """lfq.tsv over sage_b200_lfq_integrate's rows (a structured array in sage_b200_lfq_row's layout), areas [n, files] and q-values."""
+    keep = []
+    t = _table(digest, decoy_tag, generate_decoys, keep)
+    r = np.ascontiguousarray(lfq_rows)
+    ar = np.ascontiguousarray(areas, np.float64).reshape(len(r), len(filenames))
+    q = np.ascontiguousarray(q_value, np.float32)
+    fo, fb = _csr(filenames, keep)
+    n = lib().mo_write_lfq(_p(r), _p(ar), _p(q), len(r), fo, fb, len(filenames), C.byref(t), int(threads or default_threads()))
+    return _take(n)

@@ -96,6 +96,7 @@ EXPORTED_SYMBOLS = [
     "sage_b200_digest_create", "sage_b200_digest_get_info", "sage_b200_digest_export", "sage_b200_digest_destroy",
     "sage_b200_prefilter_create", "sage_b200_prefilter_get_info", "sage_b200_prefilter_chunk_counts", "sage_b200_prefilter_export",
     "sage_b200_prefilter_take_db", "sage_b200_prefilter_destroy", "sage_b200_process_raw", "sage_b200_lfq_add_raw_ms1",
+    "sage_b200_write_tsv", "sage_b200_format_hashes",
 ]
 
 _lib = None
@@ -1359,3 +1360,188 @@ def prefilter_fasta(fasta, spectra: SpectraBatch, *, precursor_tol: Tolerance, f
         lib.sage_b200_prefilter_destroy(h)
     db = IndexedDatabase(dbh.value, table[0])
     return PrefilterResult(*table, info, db, rows, kept)
+
+
+# ------------------------------------------------------------------------------------------------ result files (runner.rs writers)
+FILE_RESULTS, FILE_PIN, FILE_FRAGMENTS, FILE_LFQ, FILE_TMT = 1, 2, 3, 4, 5   # SAGE_B200_FILE_*
+
+
+class CWriteStats(C.Structure):
+    _fields_ = [(f, C.c_float) for f in ("ms_upload", "ms_measure", "ms_scan", "ms_write", "ms_d2h", "ms_total")] + [
+        (f, C.c_uint64) for f in ("h2d_bytes", "d2h_bytes", "records", "chunks")]
+
+
+class CWriteInputs(C.Structure):
+    _fields_ = [("rows", C.c_void_p), ("psm_id", C.c_void_p), ("n_rows", C.c_uint64), ("fragments", C.c_void_p), ("n_fragments", C.c_uint64),
+                ("filename_offsets", C.c_void_p), ("filename_bytes", C.c_void_p), ("n_files", C.c_uint64),
+                ("spec_id_offsets", C.c_void_p), ("spec_id_bytes", C.c_void_p), ("n_spec_ids", C.c_uint64),
+                ("n_quant", C.c_uint64), ("quant_file_id", C.c_void_p), ("quant_spec_id", C.c_void_p), ("ion_injection_time", C.c_void_p),
+                ("peaks", C.c_void_p), ("n_channels", C.c_uint64), ("user_labels", C.c_uint8),
+                ("peptides", C.POINTER(CPeptides)), ("cterm", C.c_void_p), ("semi_enzymatic", C.c_void_p), ("protein_offsets", C.c_void_p),
+                ("protein_ids", C.c_void_p), ("name_offsets", C.c_void_p), ("name_bytes", C.c_void_p), ("n_names", C.c_uint64),
+                ("decoy_tag", C.c_char_p), ("generate_decoys", C.c_uint8), ("file_id", C.c_void_p), ("spec_index", C.c_void_p)] + [
+        (f, C.c_void_p) for f in ("discriminant_score", "posterior_error", "spectrum_q", "aligned_rt", "predicted_rt", "delta_rt_model", "predicted_ims",
+                                  "delta_ims_model", "peptide_q", "protein_q", "num_protein_groups", "protein_group_q", "group_pass", "row_group_offsets",
+                                  "row_groups", "group_offsets", "group_members", "group_decoy")] + [
+        ("n_groups", C.c_uint64), ("lfq_rows", C.c_void_p), ("lfq_areas", C.c_void_p), ("lfq_q", C.c_void_p), ("n_lfq", C.c_uint64),
+        ("text_budget", C.c_uint64), ("stats", C.POINTER(CWriteStats))]
+
+
+def _strings(strs, keep: list):
+    """A list of str / bytes as a CSR byte table (offsets [n + 1], bytes)."""
+    bs = [s.encode() if isinstance(s, str) else bytes(s) for s in strs]
+    off = np.concatenate([[0], np.cumsum([len(b) for b in bs], dtype=np.uint64)]).astype(np.uint64)
+    data = np.frombuffer(b"".join(bs) + b"\0", np.uint8)
+    keep += [off, data]
+    return _ptr(off), _ptr(data), len(bs)
+
+
+def _write(file: int, ci: CWriteInputs, device: int, stats: dict | None) -> bytes:
+    lib = load_library()
+    st = CWriteStats()
+    ci.stats = C.pointer(st)
+    size = C.c_uint64()
+    _check(lib.sage_b200_write_tsv(C.c_int(device), C.c_int(file), C.byref(ci), None, C.c_uint64(0), C.byref(size)))
+    buf = np.empty(max(size.value, 1), np.uint8)
+    _check(lib.sage_b200_write_tsv(C.c_int(device), C.c_int(file), C.byref(ci), _ptr(buf), C.c_uint64(size.value), C.byref(size)))
+    if stats is not None:
+        stats.update({f: getattr(st, f) for f, _ in CWriteStats._fields_})
+    return buf[:size.value].tobytes()
+
+
+def write_fragments(rows: np.ndarray, fragments: np.ndarray, psm_id, *, device: int = 0, text_budget: int = 0, stats: dict | None = None) -> bytes:
+    """matched_fragments.sage.tsv (runner.rs write_fragments) on the device: one record per fragment of each row, in row order. rows:
+    FEATURE_DTYPE as Scorer.score_batch returns them with annotate_matches (fragment_offset / fragment_count index `fragments`, FRAGMENT_DTYPE);
+    psm_id: Feature::psm_id of each row. text_budget: device bytes of text per chunk (0 = the library's default)."""
+    rows = np.ascontiguousarray(rows, FEATURE_DTYPE)
+    fragments = np.ascontiguousarray(fragments, FRAGMENT_DTYPE)
+    pid = np.ascontiguousarray(psm_id, np.uint64)
+    if len(pid) != len(rows):
+        raise ValueError("psm_id needs one entry per row")
+    ci = CWriteInputs(rows=_ptr(rows), psm_id=_ptr(pid), n_rows=len(rows), fragments=_ptr(fragments), n_fragments=len(fragments), text_budget=text_budget)
+    return _write(FILE_FRAGMENTS, ci, device, stats)
+
+
+def write_tmt(filenames, spec_ids, file_id, spec, ion_injection_time, peaks, *, user_labels: bool = False, device: int = 0, text_budget: int = 0,
+              stats: dict | None = None) -> bytes:
+    """tmt.tsv (runner.rs write_tmt) on the device. filenames / spec_ids: str or bytes; per quantified spectrum (the rows tmt_quantify returns,
+    in order): file_id into filenames, spec into spec_ids, its ion injection time and peaks [n, channels] (tmt_quantify's intensities).
+    user_labels: the columns are user_1..n (Isobaric::User) instead of tmt_1..n."""
+    keep: list = []
+    fo, fb, nf = _strings(filenames, keep)
+    so, sb, ns = _strings(spec_ids, keep)
+    fi, si = np.ascontiguousarray(file_id, np.uint32), np.ascontiguousarray(spec, np.uint32)
+    inj = np.ascontiguousarray(ion_injection_time, np.float32)
+    pk = np.ascontiguousarray(peaks, np.float32)
+    if pk.ndim != 2 or not (len(fi) == len(si) == len(inj) == pk.shape[0]):
+        raise ValueError("file_id, spec, ion_injection_time and peaks need one entry (row) per quantified spectrum")
+    ci = CWriteInputs(filename_offsets=fo, filename_bytes=fb, n_files=nf, spec_id_offsets=so, spec_id_bytes=sb, n_spec_ids=ns, n_quant=len(fi),
+                      quant_file_id=_ptr(fi), quant_spec_id=_ptr(si), ion_injection_time=_ptr(inj), peaks=_ptr(pk), n_channels=pk.shape[1],
+                      user_labels=int(user_labels), text_budget=text_budget)
+    return _write(FILE_TMT, ci, device, stats)
+
+
+def _digest_table(ci: CWriteInputs, digest: "DigestResult", decoy_tag: str, generate_decoys: bool, keep: list):
+    """The peptide table, its protein lists and names into the inputs (results, pin, lfq)."""
+    cp = digest.peptides._c(keep)
+    keep.append(cp)
+    ci.peptides = C.pointer(cp)
+    cols = [np.ascontiguousarray(digest.cterm, np.float32), np.ascontiguousarray(digest.semi_enzymatic, np.uint8),
+            np.ascontiguousarray(digest.protein_offsets, np.uint32), np.ascontiguousarray(digest.protein_ids, np.uint32)]
+    keep += cols
+    ci.cterm, ci.semi_enzymatic, ci.protein_offsets, ci.protein_ids = (_ptr(c) for c in cols)
+    ci.name_offsets, ci.name_bytes, ci.n_names = _strings(digest.names, keep)
+    tag = decoy_tag.encode()
+    keep.append(tag)
+    ci.decoy_tag, ci.generate_decoys = tag, int(bool(generate_decoys))
+
+
+def _column(ci: CWriteInputs, field: str, d: dict | None, key: str, dt, n: int, keep: list):
+    if d is None or d.get(key) is None:
+        return
+    a = np.ascontiguousarray(d[key], dt)
+    if len(a) != n:
+        raise ValueError(f"{key} needs one value per row")
+    keep.append(a)
+    setattr(ci, field, _ptr(a))
+
+
+def _rows_inputs(digest, rows, psm_id, file_id, spec_index, filenames, spec_ids, fdr, rt, picked, decoy_tag, generate_decoys, text_budget, keep):
+    rows = np.ascontiguousarray(rows, FEATURE_DTYPE)
+    n = len(rows)
+    arrs = [np.ascontiguousarray(x, dt) for x, dt in ((psm_id, np.uint64), (file_id, np.uint32), (spec_index, np.uint32))]
+    if any(len(a) != n for a in arrs):
+        raise ValueError("psm_id, file_id and spec_index need one entry per row")
+    keep += [rows] + arrs
+    ci = CWriteInputs(rows=_ptr(rows), psm_id=_ptr(arrs[0]), n_rows=n, file_id=_ptr(arrs[1]), spec_index=_ptr(arrs[2]), text_budget=text_budget)
+    ci.filename_offsets, ci.filename_bytes, ci.n_files = _strings(filenames, keep)
+    ci.spec_id_offsets, ci.spec_id_bytes, ci.n_spec_ids = _strings(spec_ids, keep)
+    _digest_table(ci, digest, decoy_tag, generate_decoys, keep)
+    for field, d, key in (("discriminant_score", fdr, "discriminant_score"), ("posterior_error", fdr, "posterior_error"), ("spectrum_q", fdr, "spectrum_q"),
+                          ("aligned_rt", rt, "aligned_rt"), ("predicted_rt", rt, "predicted_rt"), ("delta_rt_model", rt, "delta_rt_model"),
+                          ("predicted_ims", rt, "predicted_ims"), ("delta_ims_model", rt, "delta_ims_model"), ("peptide_q", picked, "peptide_q"),
+                          ("protein_q", picked, "protein_q")):
+        _column(ci, field, d, key, np.float32, n, keep)
+    return ci
+
+
+def write_results(digest: "DigestResult", rows: np.ndarray, psm_id, file_id, spec_index, filenames, spec_ids, *, fdr: dict | None = None,
+                  rt: dict | None = None, picked: dict | None = None, groups: dict | None = None, decoy_tag: str = "rev_", generate_decoys: bool = True,
+                  device: int = 0, text_budget: int = 0, stats: dict | None = None) -> bytes:
+    """results.sage.tsv (runner.rs write_features) on the device, one record per row in the given order. digest: the table the rows'
+    PeptideIx index; file_id / spec_index: each row's entry in filenames / spec_ids (Feature::file_id, spec_id); psm_id: Feature::psm_id.
+    fdr, rt, picked, groups: the dicts of spectrum_fdr, predict_rt, picked_fdr and protein_groups over the same rows (None: Feature's defaults;
+    without groups protein_groups is empty and num_protein_groups 0)."""
+    keep: list = []
+    ci = _rows_inputs(digest, rows, psm_id, file_id, spec_index, filenames, spec_ids, fdr, rt, picked, decoy_tag, generate_decoys, text_budget, keep)
+    n = ci.n_rows
+    if groups is not None:
+        _column(ci, "num_protein_groups", groups, "num_protein_groups", np.uint32, n, keep)
+        _column(ci, "protein_group_q", groups, "protein_group_q", np.float32, n, keep)
+        _column(ci, "group_pass", groups, "pass", np.uint8, n, keep)
+        g = [np.ascontiguousarray(groups[k], dt) for k, dt in (("row_group_offsets", np.uint64), ("row_groups", np.uint32), ("group_offsets", np.uint64),
+                                                               ("group_members", np.uint32), ("group_decoy", np.uint8))]
+        keep += g
+        ci.row_group_offsets, ci.row_groups, ci.group_offsets, ci.group_members, ci.group_decoy = (_ptr(a) for a in g)
+        ci.n_groups = len(g[4])
+    return _write(FILE_RESULTS, ci, device, stats)
+
+
+def write_pin(digest: "DigestResult", rows: np.ndarray, psm_id, file_id, spec_index, filenames, spec_ids, *, fdr: dict | None = None,
+              rt: dict | None = None, decoy_tag: str = "rev_", generate_decoys: bool = True, device: int = 0, text_budget: int = 0,
+              stats: dict | None = None) -> bytes:
+    """results.sage.pin (runner.rs write_pin) on the device; the arguments are write_results' (the .pin reads no q-values or groups)."""
+    keep: list = []
+    ci = _rows_inputs(digest, rows, psm_id, file_id, spec_index, filenames, spec_ids, fdr, rt, None, decoy_tag, generate_decoys, text_budget, keep)
+    return _write(FILE_PIN, ci, device, stats)
+
+
+def write_lfq(digest: "DigestResult", quant: dict, q_value, filenames, *, decoy_tag: str = "rev_", generate_decoys: bool = True, device: int = 0,
+              text_budget: int = 0, stats: dict | None = None) -> bytes:
+    """lfq.tsv (runner.rs write_lfq) on the device: quant is FeatureMap.quantify()'s dict, q_value picked_precursor's q-values over its rows.
+    Decoy rows are skipped and Combined rows (charge 0) write charge -1; rows keep quantify's order."""
+    keep: list = []
+    n = len(quant["id"])
+    rows = np.zeros(n, LFQ_ROW_DTYPE)
+    rows["peptide"], rows["charge"], rows["decoy"] = quant["id"], quant["charge"], quant["decoy"]
+    rows["rt"], rows["spectral_angle"], rows["score"] = quant["rt"], quant["spectral_angle"], quant["score"]
+    areas = np.ascontiguousarray(quant["areas"], np.float64).reshape(n, len(filenames))
+    q = np.ascontiguousarray(q_value, np.float32)
+    if len(q) != n:
+        raise ValueError("q_value needs one value per row")
+    keep += [rows, areas, q]
+    ci = CWriteInputs(lfq_rows=_ptr(rows), lfq_areas=_ptr(areas), lfq_q=_ptr(q), n_lfq=n, text_budget=text_budget)
+    ci.filename_offsets, ci.filename_bytes, ci.n_files = _strings(filenames, keep)
+    _digest_table(ci, digest, decoy_tag, generate_decoys, keep)
+    return _write(FILE_LFQ, ci, device, stats)
+
+
+def format_hashes(fmt: int, first: int = 0, values=None, n: int = 0, block: int = 1 << 16, device: int = 0) -> np.ndarray:
+    """Test hook: per-block FNV-1a 64 of values formatted on the device, each followed by '\n'. fmt 0: ryu layout of the f32 with bits
+    first + i (i < n); 1: `{:+}` of that f32; 2: ryu layout of the f64 values."""
+    v = None if values is None else np.ascontiguousarray(values, np.float64)
+    n = len(v) if v is not None else n
+    out = np.zeros(n // block, np.uint64)
+    _check(load_library().sage_b200_format_hashes(C.c_int(device), C.c_int(fmt), C.c_uint64(first), _ptr(v) if v is not None else None, C.c_uint64(n),
+                                                  C.c_uint64(block), _ptr(out)))
+    return out

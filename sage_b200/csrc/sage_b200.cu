@@ -44,6 +44,7 @@
 #include "digest.cuh"
 #include "prefilter.cuh"
 #include "spectra.cuh"
+#include "write.cuh"
 
 using namespace sb;
 
@@ -5200,4 +5201,403 @@ extern "C" int sage_b200_prefilter_take_db(sage_b200_prefilter* f, sage_b200_db*
     *out = f->db;
     f->db = nullptr;
     return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ result files (DESIGN.md §17)
+static constexpr uint64_t WRITE_CUT = 4096;                  // records per block: chunks are cut at block boundaries
+static constexpr uint64_t WRITE_BUDGET = 256ull << 20;      // default device text per chunk
+
+static int write_check_strings(const char* what, const uint64_t* off, const char* bytes, uint64_t n) {
+    if (!off || (!bytes && off[n] > off[0])) return fail(SAGE_B200_EINVAL, "write_tsv: null %s table", what);
+    for (uint64_t i = 0; i < n; i++)
+        if (off[i + 1] < off[i]) return fail(SAGE_B200_EINVAL, "write_tsv: %s offsets decrease at %llu", what, (unsigned long long)i);
+    return 0;
+}
+template <class T>
+static int write_check_ids(const char* what, const T* ids, uint64_t n, uint64_t bound, const char* of) {
+    for (uint64_t i = 0; i < n; i++)
+        if ((uint64_t)ids[i] >= bound)
+            return fail(SAGE_B200_EINVAL, "write_tsv: %s %llu is %llu, %llu %s", what, (unsigned long long)i, (unsigned long long)ids[i], (unsigned long long)bound, of);
+    return 0;
+}
+
+// The peptide table and its protein names (results, pin, lfq).
+static int write_check_peptides(const sage_b200_write_inputs* in) {
+    const sage_b200_peptides* P = in->peptides;
+    if (!P || !P->residue_offsets || !P->nterm || !P->decoy || !in->protein_offsets || (P->n_peptides && (!P->sequence || !P->modifications)))
+        return fail(SAGE_B200_EINVAL, "write_tsv: null peptide table");
+    if (P->n_peptides > (uint64_t)UINT32_MAX) return fail(SAGE_B200_ELIMIT, "write_tsv: more than 2^32 - 1 peptides");
+    for (uint64_t p = 0; p < P->n_peptides; p++)
+        if (P->residue_offsets[p + 1] < P->residue_offsets[p] || in->protein_offsets[p + 1] < in->protein_offsets[p])
+            return fail(SAGE_B200_EINVAL, "write_tsv: peptide offsets decrease at %llu", (unsigned long long)p);
+    const uint64_t n_refs = in->protein_offsets[P->n_peptides] - in->protein_offsets[0];
+    if (in->protein_offsets[0] != 0 || (n_refs && !in->protein_ids)) return fail(SAGE_B200_EINVAL, "write_tsv: bad protein lists");
+    if (int rc = write_check_strings("protein name", in->name_offsets, in->name_bytes, in->n_names)) return rc;
+    return write_check_ids("protein id", in->protein_ids, n_refs, in->n_names, "names");
+}
+
+// Argument checks of one file (no device); n_rec = its records, h2d = the bytes its inputs take on the device.
+static int write_check(int file, const sage_b200_write_inputs* in, uint64_t& n_rec, uint64_t& h2d) {
+    const uint64_t n = in->n_rows;
+    const bool by_row = file == SAGE_B200_FILE_RESULTS || file == SAGE_B200_FILE_PIN || file == SAGE_B200_FILE_FRAGMENTS;
+    if (by_row && n && (!in->rows || !in->psm_id)) return fail(SAGE_B200_EINVAL, "write_tsv: null rows or psm_id");
+    if (n > (uint64_t)UINT32_MAX) return fail(SAGE_B200_ELIMIT, "write_tsv: more than 2^32 - 1 rows");
+    if (file != SAGE_B200_FILE_FRAGMENTS) {
+        if (int rc = write_check_strings("filename", in->filename_offsets, in->filename_bytes, in->n_files)) return rc;
+        h2d += 8 * (in->n_files + 1) + in->filename_offsets[in->n_files] - in->filename_offsets[0];
+    }
+    if (file == SAGE_B200_FILE_RESULTS || file == SAGE_B200_FILE_PIN || file == SAGE_B200_FILE_TMT) {
+        if (int rc = write_check_strings("spectrum id", in->spec_id_offsets, in->spec_id_bytes, in->n_spec_ids)) return rc;
+        h2d += 8 * (in->n_spec_ids + 1) + in->spec_id_offsets[in->n_spec_ids] - in->spec_id_offsets[0];
+    }
+    if (file == SAGE_B200_FILE_RESULTS || file == SAGE_B200_FILE_PIN || file == SAGE_B200_FILE_LFQ) {
+        if (int rc = write_check_peptides(in)) return rc;
+        const sage_b200_peptides* P = in->peptides;
+        h2d += P->n_peptides * 16 + (uint64_t)P->residue_offsets[P->n_peptides] * 5 + 4 * (uint64_t)in->protein_offsets[P->n_peptides] +
+               8 * (in->n_names + 1) + in->name_offsets[in->n_names] - in->name_offsets[0];
+    }
+    if (file == SAGE_B200_FILE_FRAGMENTS) {
+        if (in->n_fragments && !in->fragments) return fail(SAGE_B200_EINVAL, "write_tsv: null fragments");
+        n_rec = 0;
+        for (uint64_t i = 0; i < n; i++) {
+            const sage_b200_feature& r = in->rows[i];
+            if ((uint64_t)r.fragment_offset + r.fragment_count > in->n_fragments)
+                return fail(SAGE_B200_EINVAL, "write_tsv: row %llu's fragments [%u, +%u) lie outside the %llu fragments", (unsigned long long)i, r.fragment_offset,
+                            r.fragment_count, (unsigned long long)in->n_fragments);
+            n_rec += r.fragment_count;
+        }
+        for (uint64_t k = 0; k < in->n_fragments; k++)
+            if ((uint32_t)in->fragments[k].kind > 5) return fail(SAGE_B200_EINVAL, "write_tsv: fragment %llu has kind %d outside 0..5", (unsigned long long)k, in->fragments[k].kind);
+        h2d += n * (sizeof(sage_b200_feature) + 8) + in->n_fragments * sizeof(sage_b200_fragment);
+    } else if (file == SAGE_B200_FILE_TMT) {
+        n_rec = in->n_quant;
+        if (n_rec && (!in->quant_file_id || !in->quant_spec_id || !in->ion_injection_time || (in->n_channels && !in->peaks)))
+            return fail(SAGE_B200_EINVAL, "write_tsv: null TMT input");
+        if (in->n_channels > (uint64_t)UINT32_MAX / 64) return fail(SAGE_B200_ELIMIT, "write_tsv: %llu channels", (unsigned long long)in->n_channels);
+        if (int rc = write_check_ids("record", in->quant_file_id, n_rec, in->n_files, "files")) return rc;
+        if (int rc = write_check_ids("record", in->quant_spec_id, n_rec, in->n_spec_ids, "spectrum ids")) return rc;
+        h2d += n_rec * (12 + 4 * in->n_channels);
+    } else if (file == SAGE_B200_FILE_LFQ) {
+        n_rec = in->n_lfq;
+        if (n_rec && (!in->lfq_rows || !in->lfq_q || (in->n_files && !in->lfq_areas))) return fail(SAGE_B200_EINVAL, "write_tsv: null LFQ input");
+        for (uint64_t i = 0; i < n_rec; i++)
+            if (in->lfq_rows[i].peptide >= in->peptides->n_peptides)
+                return fail(SAGE_B200_EINVAL, "write_tsv: LFQ row %llu has peptide %u outside the table (%llu peptides)", (unsigned long long)i,
+                            in->lfq_rows[i].peptide, (unsigned long long)in->peptides->n_peptides);
+        h2d += n_rec * (sizeof(sage_b200_lfq_row) + 4 + 8 * in->n_files);
+    } else {   // results, pin
+        n_rec = n;
+        if (n && (!in->file_id || !in->spec_index)) return fail(SAGE_B200_EINVAL, "write_tsv: null file_id or spec_index");
+        for (uint64_t i = 0; i < n; i++)
+            if (in->rows[i].peptide_idx >= in->peptides->n_peptides)
+                return fail(SAGE_B200_EINVAL, "write_tsv: row %llu has peptide_idx %u outside the table (%llu peptides)", (unsigned long long)i,
+                            in->rows[i].peptide_idx, (unsigned long long)in->peptides->n_peptides);
+        if (int rc = write_check_ids("row", in->file_id, n, in->n_files, "files")) return rc;
+        if (int rc = write_check_ids("row", in->spec_index, n, in->n_spec_ids, "spectrum ids")) return rc;
+        h2d += n * (sizeof(sage_b200_feature) + 8 + 8 + 4 * 12 + 1);
+        if (file == SAGE_B200_FILE_RESULTS && in->group_pass) {
+            if (!in->row_group_offsets || !in->group_offsets || !in->group_decoy || (n && in->row_group_offsets[n] > in->row_group_offsets[0] && !in->row_groups))
+                return fail(SAGE_B200_EINVAL, "write_tsv: null protein group table");
+            for (uint64_t i = 0; i < n; i++)
+                if (in->row_group_offsets[i + 1] < in->row_group_offsets[i]) return fail(SAGE_B200_EINVAL, "write_tsv: row group offsets decrease at %llu", (unsigned long long)i);
+            for (uint64_t g = 0; g < in->n_groups; g++)
+                if (in->group_offsets[g + 1] < in->group_offsets[g]) return fail(SAGE_B200_EINVAL, "write_tsv: group offsets decrease at %llu", (unsigned long long)g);
+            const uint64_t rg0 = in->row_group_offsets[0], nrg = in->row_group_offsets[n] - rg0;
+            const uint64_t gm0 = in->group_offsets[0], ngm = in->group_offsets[in->n_groups] - gm0;
+            if (rg0 != 0 || gm0 != 0) return fail(SAGE_B200_EINVAL, "write_tsv: group offsets must start at 0");
+            if (ngm && !in->group_members) return fail(SAGE_B200_EINVAL, "write_tsv: null group members");
+            if (int rc = write_check_ids("row group", in->row_groups, nrg, in->n_groups, "groups")) return rc;
+            if (int rc = write_check_ids("group member", in->group_members, ngm, in->n_names, "names")) return rc;
+            h2d += 8 * (n + 1) + 4 * nrg + 9 * (in->n_groups + 1) + 4 * ngm;
+        }
+    }
+    return 0;
+}
+
+// The header record, formatted on the host with the device's field rule.
+static std::string write_header(int file, const sage_b200_write_inputs* in) {
+    std::vector<std::string> f;
+    if (file == SAGE_B200_FILE_RESULTS) {
+        f = {"psm_id", "peptide", "proteins", "protein_groups", "num_proteins", "num_protein_groups", "filename", "scannr", "rank", "label", "expmass",
+             "calcmass", "charge", "peptide_len", "missed_cleavages", "semi_enzymatic", "isotope_error", "precursor_ppm", "fragment_ppm", "hyperscore",
+             "delta_next", "delta_best", "rt", "aligned_rt", "predicted_rt", "delta_rt_model", "ion_mobility", "predicted_mobility", "delta_mobility",
+             "matched_peaks", "longest_b", "longest_y", "longest_y_pct", "matched_intensity_pct", "scored_candidates", "poisson",
+             "sage_discriminant_score", "posterior_error", "spectrum_q", "peptide_q", "protein_q", "protein_group_q", "ms2_intensity"};
+    } else if (file == SAGE_B200_FILE_PIN) {
+        f = {"SpecId", "Label", "ScanNr", "ExpMass", "CalcMass", "FileName", "retentiontime", "ion_mobility", "rank", "z=2", "z=3", "z=4", "z=5", "z=6",
+             "z=other", "peptide_len", "missed_cleavages", "semi_enzymatic", "isotope_error", "ln(precursor_ppm)", "fragment_ppm", "ln(hyperscore)",
+             "ln(delta_next)", "ln(delta_best)", "aligned_rt", "predicted_rt", "sqrt(delta_rt_model)", "predicted_mobility", "sqrt(delta_mobility)",
+             "matched_peaks", "longest_b", "longest_y", "longest_y_pct", "ln(matched_intensity_pct)", "scored_candidates", "ln(-poisson)",
+             "posterior_error", "Peptide", "Proteins"};
+    } else if (file == SAGE_B200_FILE_FRAGMENTS) {
+        f = {"psm_id", "fragment_type", "fragment_ordinals", "fragment_charge", "fragment_mz_calculated", "fragment_mz_experimental", "fragment_intensity"};
+    } else if (file == SAGE_B200_FILE_LFQ) {
+        f = {"peptide", "charge", "proteins", "q_value", "score", "spectral_angle"};
+        for (uint64_t k = 0; k < in->n_files; k++)
+            f.emplace_back(in->filename_bytes + in->filename_offsets[k], in->filename_offsets[k + 1] - in->filename_offsets[k]);
+    } else {
+        f = {"filename", "scannr", "ion_injection_time"};
+        for (uint64_t c = 0; c < in->n_channels; c++) f.push_back((in->user_labels ? "user_" : "tmt_") + std::to_string(c + 1));
+    }
+    std::string out;
+    for (size_t i = 0; i < f.size(); i++) {
+        if (i) out += '\t';
+        wr::Out cnt{nullptr, 0};
+        wr::put_field(cnt, f[i].data(), f[i].size());
+        std::string s(cnt.n, '\0');
+        wr::Out o{&s[0], 0};
+        wr::put_field(o, f[i].data(), f[i].size());
+        out += s;
+    }
+    return out + '\n';
+}
+
+template <int FILE>
+static int write_launch_measure(const wr::WriteArgs& a, uint64_t n, uint64_t* len, cudaStream_t st) {
+    LAUNCH_N(wr::k_write_measure<FILE>, n, st, a, n, len);
+    return 0;
+}
+template <int FILE>
+static int write_launch_text(const wr::WriteArgs& a, uint64_t j0, uint64_t j1, const uint64_t* off, char* text, cudaStream_t st) {
+    LAUNCH_N(wr::k_write_text<FILE>, j1 - j0, st, a, j0, j1, off, text);
+    return 0;
+}
+static int write_measure(int file, const wr::WriteArgs& a, uint64_t n, uint64_t* len, cudaStream_t st) {
+    switch (file) {
+        case SAGE_B200_FILE_RESULTS: return write_launch_measure<SAGE_B200_FILE_RESULTS>(a, n, len, st);
+        case SAGE_B200_FILE_PIN: return write_launch_measure<SAGE_B200_FILE_PIN>(a, n, len, st);
+        case SAGE_B200_FILE_FRAGMENTS: return write_launch_measure<SAGE_B200_FILE_FRAGMENTS>(a, n, len, st);
+        case SAGE_B200_FILE_LFQ: return write_launch_measure<SAGE_B200_FILE_LFQ>(a, n, len, st);
+        default: return write_launch_measure<SAGE_B200_FILE_TMT>(a, n, len, st);
+    }
+}
+static int write_text(int file, const wr::WriteArgs& a, uint64_t j0, uint64_t j1, const uint64_t* off, char* text, cudaStream_t st) {
+    switch (file) {
+        case SAGE_B200_FILE_RESULTS: return write_launch_text<SAGE_B200_FILE_RESULTS>(a, j0, j1, off, text, st);
+        case SAGE_B200_FILE_PIN: return write_launch_text<SAGE_B200_FILE_PIN>(a, j0, j1, off, text, st);
+        case SAGE_B200_FILE_FRAGMENTS: return write_launch_text<SAGE_B200_FILE_FRAGMENTS>(a, j0, j1, off, text, st);
+        case SAGE_B200_FILE_LFQ: return write_launch_text<SAGE_B200_FILE_LFQ>(a, j0, j1, off, text, st);
+        default: return write_launch_text<SAGE_B200_FILE_TMT>(a, j0, j1, off, text, st);
+    }
+}
+
+// A CSR string table on the device with its offsets rebased to 0.
+static int write_upload_strings(DevArena& A, cudaStream_t st, const uint64_t* off, const char* bytes, uint64_t n, uint64_t** d_off, char** d_bytes,
+                                std::vector<uint64_t>& keep) {
+    keep.assign(off, off + n + 1);
+    for (uint64_t& v : keep) v -= off[0];
+    CUDA_TRY(A.upload(d_off, keep.data(), keep.size(), st));
+    CUDA_TRY(A.upload(d_bytes, bytes + off[0], keep.back(), st));
+    return 0;
+}
+// An optional per-row column: NULL stays NULL.
+template <class T>
+static cudaError_t write_upload_opt(DevArena& A, cudaStream_t st, T** d, const T* h, uint64_t n) {
+    if (!h) return cudaSuccess;
+    return A.upload(d, h, n, st);
+}
+
+extern "C" int sage_b200_write_tsv(int device, int file, const sage_b200_write_inputs* in, char* out, uint64_t capacity, uint64_t* bytes) {
+    const auto t_wall = std::chrono::steady_clock::now();
+    if (!in || !bytes) return fail(SAGE_B200_EINVAL, "write_tsv: null argument");
+    if (file < SAGE_B200_FILE_RESULTS || file > SAGE_B200_FILE_TMT) return fail(SAGE_B200_EINVAL, "write_tsv: unknown file %d", file);
+    uint64_t n_rec = 0, h2d = 0;
+    if (int rc = write_check(file, in, n_rec, h2d)) return rc;
+    if (n_rec > (uint64_t)UINT32_MAX) return fail(SAGE_B200_ELIMIT, "write_tsv: %llu records, more than 2^32 - 1", (unsigned long long)n_rec);
+    const std::string header = write_header(file, in);
+    sage_b200_write_stats stats{};
+    stats.records = n_rec;
+    auto finish = [&](uint64_t total) {
+        *bytes = total;
+        stats.ms_total = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_wall).count();
+        if (in->stats) *in->stats = stats;
+        return 0;
+    };
+    if (n_rec == 0) {
+        if (out && capacity < header.size()) {
+            *bytes = header.size();
+            return fail(SAGE_B200_ELIMIT, "write_tsv: the file is %zu bytes, capacity %llu", header.size(), (unsigned long long)capacity);
+        }
+        if (out) memcpy(out, header.data(), header.size());
+        return finish(header.size());
+    }
+
+    if (int rc = select_device(device)) return rc;
+    const uint64_t budget = in->text_budget ? in->text_budget : WRITE_BUDGET;
+    const uint64_t n_cut = (n_rec + WRITE_CUT - 1) / WRITE_CUT;
+    {   // inputs; the fragment file's per-row counts and their scan (16 B per row); lengths and offsets (16 B per record); the cut table; the
+        // scan's storage. The text buffer is checked again once its size is known.
+        size_t free_b = 0, total_b = 0;
+        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+        const uint64_t row_scan = file == SAGE_B200_FILE_FRAGMENTS ? 16 * in->n_rows : 0;
+        const uint64_t need = h2d + row_scan + 16 * (n_rec + 1) + 8 * (n_cut + 1) + (32ull << 20);
+        if (need > free_b) return fail(SAGE_B200_ELIMIT, "write_tsv: %llu records need about %llu bytes of device memory, %llu free", (unsigned long long)n_rec,
+                                       (unsigned long long)need, (unsigned long long)free_b);
+    }
+    DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
+    Event e0, e1, e2, e3;
+    CUDA_TRY(e0.create());
+    CUDA_TRY(e1.create());
+    CUDA_TRY(e2.create());
+    CUDA_TRY(e3.create());
+    CUDA_TRY(cudaEventRecord(e0, st));
+    wr::WriteArgs a{};
+    std::vector<uint64_t> foff, soff, noff;   // rebased offsets: alive until the copies that read them are done
+    const uint64_t n = in->n_rows;
+    if (file != SAGE_B200_FILE_FRAGMENTS)
+        if (int rc = write_upload_strings(A, st, in->filename_offsets, in->filename_bytes, in->n_files, &a.file_off, &a.file_bytes, foff)) return rc;
+    if (file == SAGE_B200_FILE_RESULTS || file == SAGE_B200_FILE_PIN || file == SAGE_B200_FILE_TMT)
+        if (int rc = write_upload_strings(A, st, in->spec_id_offsets, in->spec_id_bytes, in->n_spec_ids, &a.spec_off, &a.spec_bytes, soff)) return rc;
+    if (file == SAGE_B200_FILE_RESULTS || file == SAGE_B200_FILE_PIN || file == SAGE_B200_FILE_LFQ) {
+        const sage_b200_peptides* P = in->peptides;
+        const uint64_t np = P->n_peptides, nres = P->residue_offsets[np], nref = in->protein_offsets[np];
+        CUDA_TRY(A.upload(&a.res_off, P->residue_offsets, np + 1, st));
+        CUDA_TRY(A.upload(&a.seq, (const char*)P->sequence, nres, st));
+        CUDA_TRY(A.upload(&a.mods, P->modifications, nres, st));
+        CUDA_TRY(A.upload(&a.nterm, P->nterm, np, st));
+        CUDA_TRY(A.upload(&a.decoy, P->decoy, np, st));
+        CUDA_TRY(write_upload_opt(A, st, &a.cterm, in->cterm, np));
+        CUDA_TRY(write_upload_opt(A, st, &a.semi, in->semi_enzymatic, np));
+        CUDA_TRY(A.upload(&a.prot_off, in->protein_offsets, np + 1, st));
+        CUDA_TRY(A.upload(&a.prot_ids, in->protein_ids, nref, st));
+        if (int rc = write_upload_strings(A, st, in->name_offsets, in->name_bytes, in->n_names, &a.name_off, &a.name_bytes, noff)) return rc;
+        const char* tag = in->decoy_tag ? in->decoy_tag : "rev_";
+        a.tag_len = (uint32_t)strlen(tag);
+        CUDA_TRY(A.upload(&a.tag, tag, a.tag_len, st));
+        a.generate_decoys = in->generate_decoys != 0;
+    }
+    if (file == SAGE_B200_FILE_RESULTS || file == SAGE_B200_FILE_PIN || file == SAGE_B200_FILE_FRAGMENTS) {
+        CUDA_TRY(A.upload(&a.rows, in->rows, n, st));
+        CUDA_TRY(A.upload(&a.psm_id, in->psm_id, n, st));
+    }
+    if (file == SAGE_B200_FILE_RESULTS || file == SAGE_B200_FILE_PIN) {
+        CUDA_TRY(A.upload(&a.file_id, in->file_id, n, st));
+        CUDA_TRY(A.upload(&a.spec_index, in->spec_index, n, st));
+        CUDA_TRY(write_upload_opt(A, st, &a.discriminant, in->discriminant_score, n));
+        CUDA_TRY(write_upload_opt(A, st, &a.posterior, in->posterior_error, n));
+        CUDA_TRY(write_upload_opt(A, st, &a.spectrum_q, in->spectrum_q, n));
+        CUDA_TRY(write_upload_opt(A, st, &a.peptide_q, in->peptide_q, n));
+        CUDA_TRY(write_upload_opt(A, st, &a.protein_q, in->protein_q, n));
+        CUDA_TRY(write_upload_opt(A, st, &a.aligned_rt, in->aligned_rt, n));
+        CUDA_TRY(write_upload_opt(A, st, &a.predicted_rt, in->predicted_rt, n));
+        CUDA_TRY(write_upload_opt(A, st, &a.delta_rt, in->delta_rt_model, n));
+        CUDA_TRY(write_upload_opt(A, st, &a.predicted_ims, in->predicted_ims, n));
+        CUDA_TRY(write_upload_opt(A, st, &a.delta_ims, in->delta_ims_model, n));
+        a.fma = host_math_variant() != 1;
+    }
+    if (file == SAGE_B200_FILE_RESULTS) {
+        CUDA_TRY(write_upload_opt(A, st, &a.num_groups, in->num_protein_groups, n));
+        CUDA_TRY(write_upload_opt(A, st, &a.protein_group_q, in->protein_group_q, n));
+        if (in->group_pass) {
+            CUDA_TRY(A.upload(&a.group_pass, in->group_pass, n, st));
+            CUDA_TRY(A.upload(&a.row_group_off, in->row_group_offsets, n + 1, st));
+            CUDA_TRY(A.upload(&a.row_groups, in->row_groups, in->row_group_offsets[n], st));
+            CUDA_TRY(A.upload(&a.group_off, in->group_offsets, in->n_groups + 1, st));
+            CUDA_TRY(A.upload(&a.group_members, in->group_members, in->group_offsets[in->n_groups], st));
+            CUDA_TRY(A.upload(&a.group_decoy, in->group_decoy, in->n_groups, st));
+        }
+    }
+    if (file == SAGE_B200_FILE_FRAGMENTS) {
+        uint64_t *counts = nullptr, *row_end = nullptr;
+        CUDA_TRY(A.upload(&a.fragments, in->fragments, in->n_fragments, st));
+        CUDA_TRY(A.alloc(&counts, n));
+        CUDA_TRY(A.alloc(&row_end, n));
+        LAUNCH_N(wr::k_write_fragment_counts, n, st, a.rows, n, counts);
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, counts, row_end, n, st); }));
+        a.row_end = row_end;
+        a.n_rows = (uint32_t)n;
+    }
+    if (file == SAGE_B200_FILE_TMT) {
+        CUDA_TRY(A.upload(&a.quant_file, in->quant_file_id, n_rec, st));
+        CUDA_TRY(A.upload(&a.quant_spec, in->quant_spec_id, n_rec, st));
+        CUDA_TRY(A.upload(&a.injection, in->ion_injection_time, n_rec, st));
+        CUDA_TRY(A.upload(&a.peaks, in->peaks, n_rec * in->n_channels, st));
+        a.n_channels = (uint32_t)in->n_channels;
+    }
+    if (file == SAGE_B200_FILE_LFQ) {
+        CUDA_TRY(A.upload(&a.lfq, in->lfq_rows, n_rec, st));
+        CUDA_TRY(A.upload(&a.lfq_q, in->lfq_q, n_rec, st));
+        CUDA_TRY(A.upload(&a.lfq_areas, in->lfq_areas, n_rec * in->n_files, st));
+        a.n_files = (uint32_t)in->n_files;
+    }
+    CUDA_TRY(cudaEventRecord(e1, st));
+    uint64_t *len = nullptr, *off = nullptr, *d_cuts = nullptr;
+    CUDA_TRY(A.alloc(&len, n_rec));
+    CUDA_TRY(A.alloc(&off, n_rec + 1));
+    CUDA_TRY(A.alloc(&d_cuts, n_cut + 1));
+    if (int rc = write_measure(file, a, n_rec, len, st)) return rc;
+    CUDA_TRY(cudaEventRecord(e2, st));
+    CUDA_TRY(cudaMemsetAsync(off, 0, 8, st));
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, len, off + 1, n_rec, st); }));
+    LAUNCH_N(wr::k_write_cuts, n_cut, st, off, n_rec, WRITE_CUT, n_cut, d_cuts);
+    std::vector<uint64_t> cuts(n_cut + 1);
+    CUDA_TRY(cudaMemcpyAsync(cuts.data(), d_cuts, 8 * (n_cut + 1), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaEventRecord(e3, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaEventElapsedTime(&stats.ms_upload, e0, e1));
+    CUDA_TRY(cudaEventElapsedTime(&stats.ms_measure, e1, e2));
+    CUDA_TRY(cudaEventElapsedTime(&stats.ms_scan, e2, e3));
+    stats.h2d_bytes = h2d;
+    stats.d2h_bytes = 8 * (n_cut + 1);
+    const uint64_t text = cuts[n_cut], total = header.size() + text;
+    if (!out) return finish(total);
+    if (capacity < total) {
+        *bytes = total;
+        return fail(SAGE_B200_ELIMIT, "write_tsv: the file is %llu bytes, capacity %llu", (unsigned long long)total, (unsigned long long)capacity);
+    }
+
+    // chunks: consecutive blocks of WRITE_CUT records while their text fits the budget (a larger block is a chunk of its own)
+    std::vector<uint64_t> chunk_at{0};   // block indices
+    for (uint64_t b = 1; b <= n_cut; b++)
+        if (b == n_cut || cuts[b + 1] - cuts[chunk_at.back()] > budget) chunk_at.push_back(b);
+    uint64_t text_cap = 0;
+    for (size_t c = 0; c + 1 < chunk_at.size(); c++) text_cap = std::max(text_cap, cuts[chunk_at[c + 1]] - cuts[chunk_at[c]]);
+    {
+        size_t free_b = 0, total_b = 0;
+        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+        if (text_cap + (16ull << 20) > free_b)
+            return fail(SAGE_B200_ELIMIT, "write_tsv: a chunk of %llu bytes of text does not fit the %llu bytes of free device memory", (unsigned long long)text_cap,
+                        (unsigned long long)free_b);
+    }
+    char* d_text = nullptr;
+    CUDA_TRY(A.alloc(&d_text, text_cap));
+    memcpy(out, header.data(), header.size());
+    for (size_t c = 0; c + 1 < chunk_at.size(); c++) {
+        const uint64_t j0 = chunk_at[c] * WRITE_CUT, j1 = std::min(n_rec, chunk_at[c + 1] * WRITE_CUT);
+        const uint64_t t0 = cuts[chunk_at[c]], t1 = cuts[chunk_at[c + 1]];
+        CUDA_TRY(cudaEventRecord(e0, st));
+        if (int rc = write_text(file, a, j0, j1, off, d_text, st)) return rc;
+        CUDA_TRY(cudaEventRecord(e1, st));
+        CUDA_TRY(cudaMemcpyAsync(out + header.size() + t0, d_text, t1 - t0, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaEventRecord(e2, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        float ms_w = 0, ms_c = 0;
+        CUDA_TRY(cudaEventElapsedTime(&ms_w, e0, e1));
+        CUDA_TRY(cudaEventElapsedTime(&ms_c, e1, e2));
+        stats.ms_write += ms_w;
+        stats.ms_d2h += ms_c;
+        stats.d2h_bytes += t1 - t0;
+        stats.chunks++;
+    }
+    return finish(total);
+}
+
+extern "C" int sage_b200_format_hashes(int device, int format, uint64_t first, const double* values, uint64_t n, uint64_t block, uint64_t* hashes) {
+    if (format < 0 || format > 2 || !hashes || block == 0 || n % block || (format == 2 && n && !values))
+        return fail(SAGE_B200_EINVAL, "format_hashes: bad argument");
+    if (format < 2 && first + n > (1ull << 32)) return fail(SAGE_B200_EINVAL, "format_hashes: f32 bit patterns beyond 2^32");
+    const uint64_t nb = n / block;
+    if (nb == 0) return 0;
+    if (int rc = select_device(device)) return rc;
+    DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
+    double* d_v = nullptr;
+    uint64_t* d_h = nullptr;
+    if (format == 2) CUDA_TRY(A.upload(&d_v, values, n, st));
+    CUDA_TRY(A.alloc(&d_h, nb));
+    LAUNCH(wr::k_format_hashes<<<(unsigned)((nb + 7) / 8), 256, 0, st>>>(format, first, d_v, block, nb, d_h));
+    return read_back(st, hashes, d_h, 8 * nb);
 }
