@@ -734,6 +734,48 @@ void sage_b200_host_free(void* p);
 /* Message of the last failure on the calling thread. Returns the message length. */
 size_t sage_b200_last_error(char* buf, size_t cap);
 
+/* ---------------------------------------------------------------------------------------------------------------------------------------------
+ * MGF reader (MgfReader::parse, sage-cloudpath mgf.rs:324-370): the bytes of a whole MGF file -> its RawSpectrum list, parsed on the device
+ * (DESIGN.md §18). The text must be UTF-8 (read_to_string); lines are `str::lines`, each `trim`med of Unicode White_Space; numbers are
+ * `str::parse::<f32>`, correctly rounded. A record ends at a line starting "END IONS"; it is dropped when its id is empty, it has no
+ * precursor, no peak, or more m/z than intensities. The first record does not see the header's TOL / TOLU / CHARGE (only QueryData::init
+ * copies them in). create -> get_info -> export (caller-allocated arrays) and/or process -> destroy.
+ */
+typedef struct sage_b200_mgf sage_b200_mgf;
+typedef struct {
+    uint64_t n_bytes, n_lines, n_records;   /* the input; records: END IONS lines after the header */
+    uint64_t n_spectra, n_peaks, n_precursors, id_bytes;   /* the export's array sizes */
+    uint64_t dropped_records;               /* records check_spectrum rejected */
+    uint64_t malformed_lines;               /* peak lines (led by an ASCII digit) whose m/z does not parse, PEPMASS= lines whose m/z does not */
+    uint64_t file_id;
+    uint64_t device_bytes;                  /* HBM the handle holds (the spectra) */
+    uint64_t peak_device_bytes;             /* HBM the create call held at its peak */
+    float ms_h2d, ms_read;                  /* CUDA-event times of the text's upload and of the parse that follows it */
+} sage_b200_mgf_info;
+/* EINVAL for a null out (or text with len > 0), invalid UTF-8 (the message names the first bad byte offset) or no line starting
+ * "BEGIN IONS" (the reference panics); ELIMIT when a stage does not fit the device's free memory (the message names the byte count) or
+ * past 2^31 - 16 records. */
+int sage_b200_mgf_create(int device, const char* text, uint64_t len, uint64_t file_id, sage_b200_mgf** out);
+int sage_b200_mgf_get_info(const sage_b200_mgf* m, sage_b200_mgf_info* info);
+/* Any pointer may be NULL. peak_offsets, precursor_offsets, id_offsets: [n_spectra + 1]; mz, intensity: [n_peaks] in file order;
+ * scan_start_time (RTINSECONDS / 60, else 0) and tic (the f32 sum of the intensities in file order): [n_spectra]. Precursors, [n_precursors]:
+ * every PEPMASS x every charge of the CHARGE list, in that nesting; intensity with its Some flag; charge with its Some flag (Some(0) is a
+ * value); isolation_kind 0 = None, 1 = Da, 2 = ppm with (isolation_lo, isolation_hi) = (-|TOL|, |TOL|). id_bytes: [id_bytes], the TITLEs. */
+int sage_b200_mgf_export(const sage_b200_mgf* m, uint64_t* peak_offsets, float* mz, float* intensity, float* scan_start_time, float* tic,
+                         uint64_t* precursor_offsets, float* precursor_mz, float* precursor_intensity, uint8_t* precursor_intensity_some,
+                         uint8_t* precursor_charge, uint8_t* precursor_charge_some, uint8_t* isolation_kind, float* isolation_lo,
+                         float* isolation_hi, uint64_t* id_offsets, char* id_bytes);
+/* SpectrumProcessor::process (level 2, as sage_b200_process_spectra) of the handle's spectra where they are on the device. Each spectrum's
+ * charge is its first precursor's (None -> 0, which the processor takes as unwrap_or(3)). ELIMIT when a first precursor's charge is
+ * Some(0) (the message names the spectrum), past the processor's shared-memory budget, or past 2^31 - 1 spectra or 2^32 - 16 peaks.
+ * out_offsets[n_spectra + 1]; out_masses / out_intensities sized for n_peaks; out_tic[n_spectra]. */
+int sage_b200_mgf_process(const sage_b200_mgf* m, const sage_b200_processor_params* processor, uint64_t* out_offsets, float* out_masses,
+                          float* out_intensities, float* out_tic);
+void sage_b200_mgf_destroy(sage_b200_mgf* m);
+/* Test hook: out[i], ok[i] = str::parse::<f32> of bytes[offsets[i] .. offsets[i+1]) on the device (ok 0: an Err; out is then 0). EINVAL for
+ * null arrays or decreasing offsets, before any device call. */
+int sage_b200_parse_f32(int device, const char* bytes, const uint64_t* offsets, uint64_t n, float* out, uint8_t* ok);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,5 +5,5 @@ from .api import (DA, PCT, PPM, Feature, IndexedDatabase, Peptides, Precursor, P
                   SageB200Error, device_count, FeatureMap, LfqSettings, Ms1Batch, spectrum_fdr, predict_rt, picked_fdr, picked_precursor,
                   competition_keys, protein_groups, protein_group_strings, bipartite_cover,
                   DigestResult, digest_fasta, PrefilterResult, prefilter_fasta, RawSpectra, ProcessedBatch, ISOBARIC, tmt_quantify,
-                  tmt_min_deisotope_mz)
+                  tmt_min_deisotope_mz, MgfSpectra, read_mgf)
 from .build import build_library, library_path  # noqa: F401

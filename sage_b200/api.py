@@ -97,6 +97,7 @@ EXPORTED_SYMBOLS = [
     "sage_b200_prefilter_create", "sage_b200_prefilter_get_info", "sage_b200_prefilter_chunk_counts", "sage_b200_prefilter_export",
     "sage_b200_prefilter_take_db", "sage_b200_prefilter_destroy", "sage_b200_process_raw", "sage_b200_lfq_add_raw_ms1",
     "sage_b200_write_tsv", "sage_b200_format_hashes",
+    "sage_b200_mgf_create", "sage_b200_mgf_get_info", "sage_b200_mgf_export", "sage_b200_mgf_process", "sage_b200_mgf_destroy", "sage_b200_parse_f32",
 ]
 
 _lib = None
@@ -127,6 +128,7 @@ def load_library(build: bool = True):
     lib.sage_b200_lfq_destroy.argtypes = [C.c_void_p]
     lib.sage_b200_digest_destroy.argtypes = [C.c_void_p]
     lib.sage_b200_prefilter_destroy.argtypes = [C.c_void_p]
+    lib.sage_b200_mgf_destroy.argtypes = [C.c_void_p]
     _lib = lib
     return lib
 
@@ -1545,3 +1547,104 @@ def format_hashes(fmt: int, first: int = 0, values=None, n: int = 0, block: int 
     _check(load_library().sage_b200_format_hashes(C.c_int(device), C.c_int(fmt), C.c_uint64(first), _ptr(v) if v is not None else None, C.c_uint64(n),
                                                   C.c_uint64(block), _ptr(out)))
     return out
+
+
+# ------------------------------------------------------------------------------------------------ MGF reader (mgf.rs)
+class CMgfInfo(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("n_bytes", "n_lines", "n_records", "n_spectra", "n_peaks", "n_precursors", "id_bytes", "dropped_records",
+                                          "malformed_lines", "file_id", "device_bytes", "peak_device_bytes")] + [("ms_h2d", C.c_float), ("ms_read", C.c_float)]
+
+
+MGF_ISOLATION = {0: None, 1: "Da", 2: "ppm"}
+
+
+class MgfSpectra:
+    """MgfReader::parse of one MGF file, read on the device (sage_b200_mgf_*). The spectra stay resident for process(); the arrays below are
+    their exported copies, in the layout of sage_b200_mgf_export: peak_off / mz / intensity, scan_start_time, tic, and the precursor CSR
+    (precursors: prec_off, mz, intensity with intensity_some, charge with charge_some, iso_kind 0 None / 1 Da / 2 ppm, iso_lo, iso_hi)."""
+
+    def __init__(self, handle, info: dict, arrays: dict, device: int):
+        self._h, self.info, self.device = handle, info, device
+        for k, v in arrays.items():
+            setattr(self, k, v)
+        self.precursors = {k: arrays[k] for k in ("prec_off", "prec_mz", "prec_intensity", "prec_intensity_some", "prec_charge", "prec_charge_some",
+                                                  "iso_kind", "iso_lo", "iso_hi")}
+        b = arrays["id_bytes"].tobytes()
+        off = arrays["id_off"]
+        self.ids = [b[int(off[i]):int(off[i + 1])].decode() for i in range(len(off) - 1)]
+
+    def __len__(self):
+        return int(self.info["n_spectra"])
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h and _lib is not None:
+            _lib.sage_b200_mgf_destroy(C.c_void_p(h))
+
+    def first_charge(self) -> np.ndarray:
+        """precursors.first().charge per spectrum as the processor takes it: None -> 0."""
+        first = self.prec_off[:-1].astype(np.int64)
+        return np.where(self.prec_charge_some[first] != 0, self.prec_charge[first], 0).astype(np.uint8)
+
+    def raw(self) -> "RawSpectra":
+        """The spectra as a RawSpectra batch (level 2) for SpectrumProcessor.process_raw."""
+        n = len(self)
+        return RawSpectra(self.peak_off.copy(), self.mz.copy(), self.intensity.copy(), np.full(n, 2, np.uint8), self.first_charge(), None,
+                          np.full(n, self.info["file_id"], np.uint64), self.scan_start_time.copy())
+
+    def process(self, processor: "SpectrumProcessor") -> SpectraBatch:
+        """SpectrumProcessor::process of every spectrum where it is on the device -> a SpectraBatch for Scorer.score_batch. The first
+        precursor gives m/z, charge and the isolation window, which must be in Da (the batch has no other kind)."""
+        n = len(self)
+        first = self.prec_off[:-1].astype(np.int64)
+        ppm = np.nonzero(self.iso_kind[first] == 2)[0]
+        if len(ppm):
+            raise AssertionError(f"spectrum {int(ppm[0])} ({self.ids[int(ppm[0])]!r}) has a ppm isolation window; SpectraBatch holds Da windows only")
+        pp = CProcessorParams(processor.take_top_n, int(processor.deisotope), processor.min_deisotope_mz)
+        npk = max(1, int(self.info["n_peaks"]))
+        off, om, oi, tic = np.zeros(n + 1, np.uint64), np.zeros(npk, np.float32), np.zeros(npk, np.float32), np.zeros(n, np.float32)
+        _check(load_library().sage_b200_mgf_process(C.c_void_p(self._h), C.byref(pp), _ptr(off), _ptr(om), _ptr(oi), _ptr(tic)))
+        k = int(off[-1])
+        da = self.iso_kind[first] == 1
+        nan = np.float32(np.nan)
+        return SpectraBatch(off, om[:k].copy(), oi[:k].copy(), self.prec_mz[first].copy(), self.first_charge(),
+                            np.where(da, self.iso_lo[first], nan).astype(np.float32), np.where(da, self.iso_hi[first], nan).astype(np.float32), tic,
+                            np.full(n, 2, np.uint8), self.scan_start_time.copy(), np.full(n, nan, np.float32))
+
+
+def read_mgf(text, file_id: int = 0, device: int = 0) -> MgfSpectra:
+    """MgfReader::with_file_id(file_id).parse(text) on the device. text: the file's contents as str or bytes (UTF-8)."""
+    data = text.encode("utf-8") if isinstance(text, str) else bytes(text)
+    lib = load_library()
+    h = C.c_void_p()
+    _check(lib.sage_b200_mgf_create(C.c_int(device), data, C.c_uint64(len(data)), C.c_uint64(file_id), C.byref(h)))
+    try:
+        ci = CMgfInfo()
+        _check(lib.sage_b200_mgf_get_info(h, C.byref(ci)))
+        info = {n: getattr(ci, n) for n, _ in CMgfInfo._fields_}
+        n, npk, npr, nid = info["n_spectra"], info["n_peaks"], info["n_precursors"], info["id_bytes"]
+        a = dict(peak_off=np.zeros(n + 1, np.uint64), mz=np.zeros(npk, np.float32), intensity=np.zeros(npk, np.float32),
+                 scan_start_time=np.zeros(n, np.float32), tic=np.zeros(n, np.float32), prec_off=np.zeros(n + 1, np.uint64),
+                 prec_mz=np.zeros(npr, np.float32), prec_intensity=np.zeros(npr, np.float32), prec_intensity_some=np.zeros(npr, np.uint8),
+                 prec_charge=np.zeros(npr, np.uint8), prec_charge_some=np.zeros(npr, np.uint8), iso_kind=np.zeros(npr, np.uint8),
+                 iso_lo=np.zeros(npr, np.float32), iso_hi=np.zeros(npr, np.float32), id_off=np.zeros(n + 1, np.uint64),
+                 id_bytes=np.zeros(nid, np.uint8))
+        _check(lib.sage_b200_mgf_export(h, *[_ptr(a[k]) for k in ("peak_off", "mz", "intensity", "scan_start_time", "tic", "prec_off", "prec_mz",
+                                                                   "prec_intensity", "prec_intensity_some", "prec_charge", "prec_charge_some",
+                                                                   "iso_kind", "iso_lo", "iso_hi", "id_off", "id_bytes")]))
+    except BaseException:
+        lib.sage_b200_mgf_destroy(h)
+        raise
+    return MgfSpectra(h.value, info, a, device)
+
+
+def parse_f32(tokens, device: int = 0) -> tuple[np.ndarray, np.ndarray]:
+    """str::parse::<f32> of each token (str or bytes) on the device -> (values as u32 bits, ok as bool); a failed parse gives bits 0."""
+    bs = [t.encode() if isinstance(t, str) else bytes(t) for t in tokens]
+    n = len(bs)
+    off = np.zeros(n + 1, np.uint64)
+    if n:
+        off[1:] = np.cumsum([len(b) for b in bs])
+    out, ok = np.zeros(max(n, 1), np.float32), np.zeros(max(n, 1), np.uint8)
+    _check(load_library().sage_b200_parse_f32(C.c_int(device), b"".join(bs), _ptr(off), C.c_uint64(n), _ptr(out), _ptr(ok)))
+    return out[:n].view(np.uint32), ok[:n].astype(bool)

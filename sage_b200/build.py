@@ -8,7 +8,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 _SRC = os.path.join(_PKG, "csrc", "sage_b200.cu")
 _DEPS = [os.path.join(_PKG, "csrc", f) for f in ("sage_b200.cu", "kernels.cuh", "lfq.cuh", "fdr.cuh", "device_common.cuh", "glibc_log.cuh", "glibc_log_data.cuh",
                                                        "glibc_math.cuh", "glibc_exp_data.cuh", "rt.cuh", "picked.cuh", "protein_groups.cuh", "digest.cuh",
-                                                       "prefilter.cuh", "spectra.cuh", "write.cuh", "write_pow10.cuh")] + [
+                                                       "prefilter.cuh", "spectra.cuh", "write.cuh", "write_pow10.cuh", "mgf.cuh", "mgf_f32.cuh", "mgf_pow5.cuh")] + [
     os.path.join(os.path.dirname(_PKG), "include", "sage_b200.h")]
 _OUT = os.path.join(_PKG, "lib", "libsage_b200.so")
 

@@ -45,6 +45,7 @@
 #include "prefilter.cuh"
 #include "spectra.cuh"
 #include "write.cuh"
+#include "mgf.cuh"
 
 using namespace sb;
 
@@ -5600,4 +5601,326 @@ extern "C" int sage_b200_format_hashes(int device, int format, uint64_t first, c
     CUDA_TRY(A.alloc(&d_h, nb));
     LAUNCH(wr::k_format_hashes<<<(unsigned)((nb + 7) / 8), 256, 0, st>>>(format, first, d_v, block, nb, d_h));
     return read_back(st, hashes, d_h, 8 * nb);
+}
+
+// ================================================================================== MGF reader (mgf.rs:324-370; kernels in mgf.cuh)
+struct sage_b200_mgf {
+    int device = 0;
+    DevArena out;   // the spectra, exact-size; the text and the line table go with the create call
+    uint64_t *d_peak_off = nullptr, *d_prec_off = nullptr, *d_id_off = nullptr;
+    float *d_mz = nullptr, *d_int = nullptr, *d_rt = nullptr, *d_tic = nullptr;
+    float *d_p_mz = nullptr, *d_p_int = nullptr, *d_p_lo = nullptr, *d_p_hi = nullptr;
+    uint8_t *d_p_int_some = nullptr, *d_p_charge = nullptr, *d_p_charge_some = nullptr, *d_p_iso = nullptr, *d_id = nullptr;
+    sage_b200_mgf_info info{};
+};
+
+extern "C" void sage_b200_mgf_destroy(sage_b200_mgf* m) {
+    if (!m) return;
+    cudaSetDevice(m->device);
+    delete m;
+}
+
+static constexpr uint64_t MGF_SELECT_CHUNK = 1ull << 30;   // items per cub::DeviceSelect call (its item count is an int)
+
+static int mgf_memory(const char* stage, uint64_t bytes) {
+    size_t free_b = 0, total_b = 0;
+    CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
+    if (bytes + (64ull << 20) > free_b)
+        return fail(SAGE_B200_ELIMIT, "mgf_create: the %s stage needs about %llu bytes of device memory, %llu free", stage, (unsigned long long)bytes,
+                    (unsigned long long)free_b);
+    return 0;
+}
+
+static unsigned mgf_grid(uint64_t n) { return (unsigned)std::min<uint64_t>(std::max<uint64_t>(grid256(n), 1), 1u << 20); }
+
+struct MgfIsNewline {
+    const uint8_t* t;
+    __device__ bool operator()(uint64_t i) const { return t[i] == '\n'; }
+};
+struct MgfIsEnd {
+    const MgfLine* L;
+    __device__ bool operator()(uint64_t i) const { return L[i].kind == MGF_END; }
+};
+
+// The indices i in [base, base + n) with pred(i), in order, into out (expect of them).
+template <class Pred>
+static int mgf_select(DevArena& A, cudaStream_t st, uint64_t base, uint64_t n, Pred pred, uint64_t* out, uint64_t expect) {
+    unsigned long long* d_cnt = nullptr;
+    CUDA_TRY(A.alloc(&d_cnt, 1));
+    uint64_t done = 0;
+    for (uint64_t c0 = 0; c0 < n; c0 += MGF_SELECT_CHUNK) {
+        const int m = (int)std::min<uint64_t>(MGF_SELECT_CHUNK, n - c0);
+        thrust::counting_iterator<uint64_t> it(base + c0);
+        CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceSelect::If(t, b, it, out + done, d_cnt, m, pred, st); }));
+        unsigned long long got = 0;
+        if (int rc = read_back(st, &got, d_cnt, 8)) return rc;
+        done += got;
+    }
+    if (done != expect) return fail(SAGE_B200_ECUDA, "mgf_create: selected %llu items, counted %llu", (unsigned long long)done, (unsigned long long)expect);
+    return 0;
+}
+
+static int mgf_scan(DevArena& A, cudaStream_t st, const uint64_t* in, uint64_t* out, uint64_t n) {
+    CUDA_TRY(A.two_phase([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, in, out, (int)n, st); }));
+    return 0;
+}
+
+extern "C" int sage_b200_mgf_create(int device, const char* text, uint64_t len, uint64_t file_id, sage_b200_mgf** out) {
+    if (!out || (len && !text)) return fail(SAGE_B200_EINVAL, "mgf_create: null argument");
+    *out = nullptr;
+    if (len == 0) return fail(SAGE_B200_EINVAL, "mgf_create: no BEGIN IONS line (the file is empty)");
+    if (int rc = select_device(device)) return rc;
+    cudaGetLastError();   // a stale non-sticky error left by another user of the runtime must not be blamed on the launches below
+    Guard<sage_b200_mgf> guard(new sage_b200_mgf(), sage_b200_mgf_destroy);
+    sage_b200_mgf* M = guard.get();
+    M->device = device;
+    sage_b200_mgf_info& I = M->info;
+    I.n_bytes = len;
+    I.file_id = file_id;
+    if (int rc = mgf_memory("text", len + 64)) return rc;
+    DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
+    Event e0, e1, e2;
+    CUDA_TRY(e0.create());
+    CUDA_TRY(e1.create());
+    CUDA_TRY(e2.create());
+    uint8_t* d_text = nullptr;
+    MgfHeader* d_h = nullptr;
+    MgfHeader h{~0ull, 0, 0, 0, 0, 0, ~0ull, 0};
+    CUDA_TRY(A.upload(&d_h, &h, 1, st));
+    CUDA_TRY(cudaEventRecord(e0, st));
+    CUDA_TRY(A.upload(&d_text, (const uint8_t*)text, len, st));
+    CUDA_TRY(cudaEventRecord(e1, st));
+    LAUNCH(k_mgf_bytes<<<mgf_grid(len), 256, 0, st>>>(d_text, len, d_h));
+    if (int rc = read_back(st, &h, d_h, sizeof h)) return rc;
+    if (h.bad_utf8 != ~0ull) return fail(SAGE_B200_EINVAL, "mgf_create: invalid UTF-8 at byte offset %llu", h.bad_utf8);
+    // str::lines: a line per '\n', and one more for text after the last '\n'
+    const uint64_t n_nl = h.n_newline;
+    if (int rc = mgf_memory("line", n_nl * 8 + (n_nl + 1) * sizeof(MgfLine))) return rc;
+    uint64_t* d_nl = nullptr;
+    CUDA_TRY(A.alloc(&d_nl, n_nl));
+    if (int rc = mgf_select(A, st, 0, len, MgfIsNewline{d_text}, d_nl, n_nl)) return rc;
+    uint64_t last_nl = 0;
+    if (n_nl) {
+        if (int rc = read_back(st, &last_nl, d_nl + n_nl - 1, 8)) return rc;
+    }
+    const uint64_t n_lines = n_nl + ((n_nl == 0 || last_nl + 1 < len) ? 1 : 0);
+    I.n_lines = n_lines;
+    MgfLine* d_lines = nullptr;
+    CUDA_TRY(A.alloc(&d_lines, n_lines));
+    LAUNCH(k_mgf_lines<<<mgf_grid(n_lines), 256, 0, st>>>(d_text, len, d_nl, n_nl, n_lines, d_lines, d_h));
+    LAUNCH(k_mgf_scan_lines<<<mgf_grid(n_lines), 256, 0, st>>>(d_lines, n_lines, d_h));
+    if (int rc = read_back(st, &h, d_h, sizeof h)) return rc;
+    if (h.begin_line == ~0ull) return fail(SAGE_B200_EINVAL, "mgf_create: no BEGIN IONS line (mgf.rs panics at lines.next().unwrap())");
+    I.malformed_lines = h.malformed;
+    const uint64_t n_rec = h.n_end;
+    I.n_records = n_rec;
+    if (n_rec > 0x7FFFFFF0ull) return fail(SAGE_B200_ELIMIT, "mgf_create: %llu records, more than 2^31 - 16", (unsigned long long)n_rec);
+    uint64_t counts[4] = {0, 0, 0, 0};   // spectra, peaks, precursors, id bytes
+    uint64_t* at[4] = {nullptr, nullptr, nullptr, nullptr};
+    MgfOut o{};
+    uint64_t* d_end = nullptr;
+    if (n_rec) {
+        if (int rc = mgf_memory("record", n_rec * 8 * 9)) return rc;
+        CUDA_TRY(A.alloc(&d_end, n_rec));
+        if (int rc = mgf_select(A, st, h.begin_line + 1, n_lines - h.begin_line - 1, MgfIsEnd{d_lines}, d_end, n_rec)) return rc;
+        uint64_t* cnt[4];
+        for (int k = 0; k < 4; k++) {
+            CUDA_TRY(A.alloc(&cnt[k], n_rec + 1));
+            CUDA_TRY(A.alloc(&at[k], n_rec + 1));
+        }
+        o.kept = cnt[0];
+        o.n_peaks = cnt[1];
+        o.n_prec = cnt[2];
+        o.id_len = cnt[3];
+        LAUNCH(k_mgf_records<0><<<mgf_grid(n_rec), 256, 0, st>>>(d_text, d_lines, d_end, n_rec, d_h, o));
+        for (int k = 0; k < 4; k++) {
+            if (int rc = mgf_scan(A, st, cnt[k], at[k], n_rec + 1)) return rc;
+            CUDA_TRY(cudaMemcpyAsync(&counts[k], at[k] + n_rec, 8, cudaMemcpyDeviceToHost, st));
+        }
+        CUDA_TRY(cudaStreamSynchronize(st));
+    }
+    const uint64_t n = counts[0], npk = counts[1], npr = counts[2], nid = counts[3];
+    I.n_spectra = n;
+    I.n_peaks = npk;
+    I.n_precursors = npr;
+    I.id_bytes = nid;
+    I.dropped_records = n_rec - n;
+    if (int rc = mgf_memory("output", (npk + 4) * 8 + npr * 24 + nid + (n + 1) * 32)) return rc;
+    CUDA_TRY(M->out.alloc(&M->d_peak_off, n + 1));
+    CUDA_TRY(M->out.alloc(&M->d_prec_off, n + 1));
+    CUDA_TRY(M->out.alloc(&M->d_id_off, n + 1));
+    CUDA_TRY(M->out.alloc(&M->d_mz, npk + 4));
+    CUDA_TRY(M->out.alloc(&M->d_int, npk + 4));
+    CUDA_TRY(M->out.alloc(&M->d_rt, n));
+    CUDA_TRY(M->out.alloc(&M->d_tic, n));
+    CUDA_TRY(M->out.alloc(&M->d_p_mz, npr));
+    CUDA_TRY(M->out.alloc(&M->d_p_int, npr));
+    CUDA_TRY(M->out.alloc(&M->d_p_lo, npr));
+    CUDA_TRY(M->out.alloc(&M->d_p_hi, npr));
+    CUDA_TRY(M->out.alloc(&M->d_p_int_some, npr));
+    CUDA_TRY(M->out.alloc(&M->d_p_charge, npr));
+    CUDA_TRY(M->out.alloc(&M->d_p_charge_some, npr));
+    CUDA_TRY(M->out.alloc(&M->d_p_iso, npr));
+    CUDA_TRY(M->out.alloc(&M->d_id, nid));
+    const uint64_t last[3] = {npk, npr, nid};
+    CUDA_TRY(cudaMemcpyAsync(M->d_peak_off + n, &last[0], 8, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(M->d_prec_off + n, &last[1], 8, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(M->d_id_off + n, &last[2], 8, cudaMemcpyHostToDevice, st));
+    if (n) {
+        o.kept = at[0];
+        o.n_peaks = at[1];
+        o.n_prec = at[2];
+        o.id_len = at[3];
+        o.peak_off = M->d_peak_off;
+        o.prec_off = M->d_prec_off;
+        o.id_off = M->d_id_off;
+        o.mz = M->d_mz;
+        o.intensity = M->d_int;
+        o.rt = M->d_rt;
+        o.tic = M->d_tic;
+        o.p_mz = M->d_p_mz;
+        o.p_int = M->d_p_int;
+        o.p_lo = M->d_p_lo;
+        o.p_hi = M->d_p_hi;
+        o.p_int_some = M->d_p_int_some;
+        o.p_charge = M->d_p_charge;
+        o.p_charge_some = M->d_p_charge_some;
+        o.p_iso = M->d_p_iso;
+        o.id_bytes = M->d_id;
+        LAUNCH(k_mgf_records<1><<<mgf_grid(n_rec), 256, 0, st>>>(d_text, d_lines, d_end, n_rec, d_h, o));
+    }
+    CUDA_TRY(cudaEventRecord(e2, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaEventElapsedTime(&I.ms_h2d, e0, e1));
+    CUDA_TRY(cudaEventElapsedTime(&I.ms_read, e1, e2));
+    I.device_bytes = M->out.bytes;
+    I.peak_device_bytes = M->out.bytes + A.bytes;
+    *out = guard.release();
+    return 0;
+}
+
+extern "C" int sage_b200_mgf_get_info(const sage_b200_mgf* m, sage_b200_mgf_info* info) {
+    if (!m || !info) return fail(SAGE_B200_EINVAL, "mgf_get_info: null argument");
+    *info = m->info;
+    return 0;
+}
+
+extern "C" int sage_b200_mgf_export(const sage_b200_mgf* M, uint64_t* peak_offsets, float* mz, float* intensity, float* scan_start_time, float* tic,
+                                    uint64_t* precursor_offsets, float* precursor_mz, float* precursor_intensity, uint8_t* precursor_intensity_some,
+                                    uint8_t* precursor_charge, uint8_t* precursor_charge_some, uint8_t* isolation_kind, float* isolation_lo,
+                                    float* isolation_hi, uint64_t* id_offsets, char* id_bytes) {
+    if (!M) return fail(SAGE_B200_EINVAL, "mgf_export: null handle");
+    const sage_b200_mgf_info& I = M->info;
+    const uint64_t n = I.n_spectra, npk = I.n_peaks, npr = I.n_precursors;
+    CUDA_TRY(cudaSetDevice(M->device));
+    Stream st;
+    CUDA_TRY(st.create());
+    struct Copy { void* dst; const void* src; uint64_t bytes; };
+    const Copy copies[] = {{peak_offsets, M->d_peak_off, 8 * (n + 1)}, {mz, M->d_mz, 4 * npk}, {intensity, M->d_int, 4 * npk},
+                           {scan_start_time, M->d_rt, 4 * n}, {tic, M->d_tic, 4 * n}, {precursor_offsets, M->d_prec_off, 8 * (n + 1)},
+                           {precursor_mz, M->d_p_mz, 4 * npr}, {precursor_intensity, M->d_p_int, 4 * npr}, {precursor_intensity_some, M->d_p_int_some, npr},
+                           {precursor_charge, M->d_p_charge, npr}, {precursor_charge_some, M->d_p_charge_some, npr}, {isolation_kind, M->d_p_iso, npr},
+                           {isolation_lo, M->d_p_lo, 4 * npr}, {isolation_hi, M->d_p_hi, 4 * npr}, {id_offsets, M->d_id_off, 8 * (n + 1)},
+                           {id_bytes, M->d_id, I.id_bytes}};
+    for (const Copy& c : copies)
+        if (c.dst && c.bytes) CUDA_TRY(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int sage_b200_mgf_process(const sage_b200_mgf* M, const sage_b200_processor_params* pr, uint64_t* out_offsets, float* out_masses,
+                                     float* out_intensities, float* out_tic) {
+    if (!M || !pr || !out_offsets || !out_tic) return fail(SAGE_B200_EINVAL, "mgf_process: null argument");
+    const uint64_t n = M->info.n_spectra, npk = M->info.n_peaks;
+    if (npk && (!out_masses || !out_intensities)) return fail(SAGE_B200_EINVAL, "mgf_process: null peak arrays");
+    out_offsets[0] = 0;
+    if (n == 0) return 0;
+    if (n > 0x7FFFFFFFull || npk > 0xFFFFFFF0ull) return fail(SAGE_B200_ELIMIT, "mgf_process: more than 2^31 - 1 spectra or 2^32 - 16 peaks");
+    CUDA_TRY(cudaSetDevice(M->device));
+    cudaGetLastError();
+    if (int rc = mgf_memory("process", npk * 16 + n * 24)) return rc;
+    DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
+    uint32_t *d_off = nullptr, *d_cnt = nullptr;
+    uint8_t* d_chg = nullptr;
+    unsigned int* d_pmax = nullptr;
+    unsigned long long* d_zero = nullptr;
+    float *d_om = nullptr, *d_oi = nullptr, *d_tic = nullptr, *d_cm = nullptr, *d_ci = nullptr;
+    uint64_t *d_cnt64 = nullptr, *d_out_off = nullptr;
+    const unsigned int pmax0 = 1;
+    const unsigned long long zero0 = ~0ull;
+    CUDA_TRY(A.alloc(&d_off, n + 1));
+    CUDA_TRY(A.alloc(&d_chg, n));
+    CUDA_TRY(A.upload(&d_pmax, &pmax0, 1, st));
+    CUDA_TRY(A.upload(&d_zero, &zero0, 1, st));
+    LAUNCH(k_mgf_process_inputs<<<mgf_grid(n + 1), 256, 0, st>>>(n, M->d_peak_off, M->d_prec_off, M->d_p_charge, M->d_p_charge_some, d_off, d_chg, d_pmax,
+                                                                  d_zero));
+    unsigned int pmax = 0;
+    unsigned long long zero = 0;
+    CUDA_TRY(cudaMemcpyAsync(&pmax, d_pmax, 4, cudaMemcpyDeviceToHost, st));
+    if (int rc = read_back(st, &zero, d_zero, 8)) return rc;
+    if (zero != ~0ull) {
+        uint64_t io[2];
+        if (int rc = read_back(st, io, M->d_id_off + zero, 16)) return rc;
+        std::string id(std::min<uint64_t>(io[1] - io[0], 200), '\0');
+        if (int rc = read_back(st, &id[0], M->d_id + io[0], id.size())) return rc;
+        return fail(SAGE_B200_ELIMIT, "mgf_process: spectrum %llu (\"%s\") has first precursor charge Some(0), which the processor's u8 charge (0 = None) cannot carry",
+                    zero, id.c_str());
+    }
+    uint32_t p2 = 1;
+    size_t smem = 0;
+    if (int rc = ms2_smem(pmax, p2, smem)) return rc;
+    CUDA_TRY(A.alloc(&d_om, npk + 4));
+    CUDA_TRY(A.alloc(&d_oi, npk + 4));
+    CUDA_TRY(A.alloc(&d_cm, npk + 4));
+    CUDA_TRY(A.alloc(&d_ci, npk + 4));
+    CUDA_TRY(A.alloc(&d_cnt, n));
+    CUDA_TRY(A.alloc(&d_tic, n));
+    CUDA_TRY(A.alloc(&d_cnt64, n + 1));
+    CUDA_TRY(A.alloc(&d_out_off, n + 1));
+    ProcParams pp{(uint32_t)std::min<uint64_t>(pr->take_top_n, 0xFFFFFFFFull), pr->deisotope ? 1u : 0u, pr->min_deisotope_mz};
+    if (int rc = ensure_kernel_attributes(M->device)) return rc;
+    LAUNCH(k_process_ms2<<<(unsigned)n, 32, smem, st>>>(pp, (uint32_t)n, d_off, M->d_mz, M->d_int, d_chg, pmax, p2, d_om, d_oi, d_cnt, d_tic));
+    LAUNCH_N(k_mgf_counts64, n + 1, st, n, d_cnt, d_cnt64);
+    if (int rc = mgf_scan(A, st, d_cnt64, d_out_off, n + 1)) return rc;
+    LAUNCH(k_mgf_compact<<<(unsigned)std::min<uint64_t>(n, 1u << 20), 128, 0, st>>>(n, d_off, d_cnt, d_om, d_oi, d_out_off, d_cm, d_ci));
+    if (int rc = read_back(st, out_offsets, d_out_off, 8 * (n + 1))) return rc;
+    const uint64_t kept = out_offsets[n];
+    CUDA_TRY(cudaMemcpyAsync(out_tic, d_tic, 4 * n, cudaMemcpyDeviceToHost, st));
+    if (kept) {
+        CUDA_TRY(cudaMemcpyAsync(out_masses, d_cm, 4 * kept, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(out_intensities, d_ci, 4 * kept, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int sage_b200_parse_f32(int device, const char* bytes, const uint64_t* offsets, uint64_t n, float* out, uint8_t* ok) {
+    if (n == 0) return 0;
+    if (!offsets || !out || !ok) return fail(SAGE_B200_EINVAL, "parse_f32: null argument");
+    for (uint64_t i = 0; i < n; i++)
+        if (offsets[i + 1] < offsets[i]) return fail(SAGE_B200_EINVAL, "parse_f32: offsets decrease at token %llu", (unsigned long long)i);
+    const uint64_t nb = offsets[n] - offsets[0];
+    if (nb && !bytes) return fail(SAGE_B200_EINVAL, "parse_f32: null bytes");
+    if (int rc = select_device(device)) return rc;
+    cudaGetLastError();
+    if (int rc = mgf_memory("parse_f32", nb + n * 13)) return rc;
+    DevArena A;
+    Stream st;
+    CUDA_TRY(st.create());
+    std::vector<uint64_t> off(n + 1);
+    for (uint64_t i = 0; i <= n; i++) off[i] = offsets[i] - offsets[0];
+    uint8_t *d_b = nullptr, *d_ok = nullptr;
+    uint64_t* d_off = nullptr;
+    float* d_out = nullptr;
+    CUDA_TRY(A.upload(&d_b, (const uint8_t*)bytes + offsets[0], nb, st));
+    CUDA_TRY(A.upload(&d_off, off.data(), n + 1, st));
+    CUDA_TRY(A.alloc(&d_out, n));
+    CUDA_TRY(A.alloc(&d_ok, n));
+    LAUNCH(k_mgf_parse_tokens<<<mgf_grid(n), 256, 0, st>>>(d_b, d_off, n, d_out, d_ok));
+    CUDA_TRY(cudaMemcpyAsync(out, d_out, 4 * n, cudaMemcpyDeviceToHost, st));
+    return read_back(st, ok, d_ok, n);
 }

@@ -539,3 +539,23 @@ def ms1_to_raw(batch, shuffle: bool = False, seed: int = 0x5A8):
     n = len(off) - 1
     return RawSpectra(off.copy(), mz, it, np.ones(n, np.uint8), None, mob, np.asarray(batch.file_id, np.uint32).copy(),
                       np.asarray(batch.scan_start_time, np.float32).copy())
+
+
+def write_mgf(batch: SpectraBatch, title: str = "synth", rt=None) -> bytes:
+    """A SpectraBatch as MGF text: one record per spectrum with TITLE, PEPMASS (precursor m/z), CHARGE, RTINSECONDS (when rt is given, f32
+    seconds) and one "mz intensity" line per peak. Every f32 is written in its shortest round-trip form, so MgfReader::parse reads the
+    arrays back bit for bit."""
+    n = len(batch)
+    off = np.asarray(batch.peak_off, np.int64)
+    mz = np.asarray(batch.masses, np.float32).astype("U")
+    it = np.asarray(batch.intensities, np.float32).astype("U")
+    pmz = np.asarray(batch.prec_mz, np.float32).astype("U")
+    rts = None if rt is None else np.asarray(rt, np.float32).astype("U")
+    peaks = np.char.add(np.char.add(mz, " "), it)
+    out = []
+    for s in range(n):
+        head = f"BEGIN IONS\nTITLE={title}.{s}\nPEPMASS={pmz[s]}\nCHARGE={int(batch.prec_charge[s])}+\n"
+        if rts is not None:
+            head += f"RTINSECONDS={rts[s]}\n"
+        out.append(head + "\n".join(peaks[off[s] - off[0]:off[s + 1] - off[0]].tolist()) + "\nEND IONS\n")
+    return "".join(out).encode()
